@@ -6,6 +6,7 @@
 #include <algorithm>
 #include <cmath>
 #include <mutex>
+#include <type_traits>
 
 namespace b200
 {
@@ -164,19 +165,70 @@ static unsigned gcd_u(unsigned a, unsigned b)
     return a;
 }
 
-static int round_up16(double v) { return ((int)std::ceil(v / 16.0)) * 16; }
-static int repair_rounds()
+// SmartResamplerBlock(input, final_samplerate, samplerate) -> (unsigned interpolation, unsigned decimation), smart_resampler.cpp:8-61:
+// a power-of-two decimator by 1 << decim_power first when the input rate is at least twice the final one (power_decim.cpp:13-29),
+// then the rational resampler by the reduced I / D behind it, unless the decimator alone reached the final rate (rational = false)
+struct SmartRatio
 {
-    // a run of r consecutive unconverged junctions needs r rounds; idle rounds cost two empty launches. B200_REPAIR_ROUNDS overrides (profiling).
-    static int v = -1;
-    if (v < 0) {
-        const char *e = getenv("B200_REPAIR_ROUNDS");
-        v = e ? atoi(e) : 8;
+    int decim_power;
+    bool rational;
+    unsigned I, D;
+};
+static SmartRatio smart_resampler_ratio(unsigned interpolation, unsigned decimation)
+{
+    SmartRatio r{0, true, 0, 0};
+    double rsamp_in = decimation, fout = interpolation;
+    if (decimation > interpolation) {
+        const int best_power = (int)floor(log2((double)(decimation / interpolation))); // (unsigned division, as the reference)
+        if (best_power > 0) {
+            r.decim_power = std::min(best_power, PD_NPLANS);
+            rsamp_in = (double)decimation / (double)(1 << r.decim_power);
+        }
+        r.rational = rsamp_in != fout;
+        double t; // "ensure it's all integer" (smart_resampler.cpp:35-40)
+        while (modf(rsamp_in, &t) != 0 || modf(fout, &t) != 0) {
+            rsamp_in *= 10;
+            fout *= 10;
+        }
     }
-    return v;
+    const unsigned g = gcd_u((unsigned)fout, (unsigned)rsamp_in);
+    r.I = (unsigned)fout / g;
+    r.D = (unsigned)rsamp_in / g;
+    return r;
 }
-#define REPAIR_ROUNDS repair_rounds()
 
+// the working window of samples per symbol of the loops (module_psk_demod.cpp:65-70); min_sps / max_sps > 0 replace its ends
+struct SpsWindow
+{
+    float lo, hi;
+};
+static SpsWindow sps_window(int constellation, float min_sps = 0, float max_sps = 0)
+{
+    SpsWindow w{constellation == B200_OQPSK ? 1.6f : 1.1f, constellation == B200_OQPSK ? 2.4f : 4.0f};
+    if (min_sps > 0)
+        w.lo = min_sps;
+    if (max_sps > 0)
+        w.hi = max_sps;
+    return w;
+}
+
+// Calls f(std::integral_constant<int, F>{}) with F the kernels' template index (0 cf32, 1 cs16, 2 cs8) of the sample format fmt.
+template <class Fn> static auto with_fmt(int fmt, Fn &&f)
+{
+    if (fmt == B200_CF32)
+        return f(std::integral_constant<int, 0>{});
+    if (fmt == B200_CS16)
+        return f(std::integral_constant<int, 1>{});
+    return f(std::integral_constant<int, 2>{});
+}
+static int fmt_bytes(int fmt)
+{
+    return with_fmt(fmt, [](auto F) { return RawBytes<F>::v; });
+}
+
+static int round_up16(double v) { return ((int)std::ceil(v / 16.0)) * 16; }
+// a run of r consecutive unconverged junctions needs r rounds; idle rounds cost two empty launches
+constexpr int REPAIR_ROUNDS = 8;
 
 Demod::Demod(const b200_demod_cfg &c) : cfg(c)
 {
@@ -207,51 +259,33 @@ Demod::Demod(const b200_demod_cfg &c) : cfg(c)
         B200_REQUIRE(c.constellation == B200_BPSK, B200_EINVAL, "For carrier mode, constellation must be BPSK!");
         B200_REQUIRE(c.carrier_pll_bw > 0 && c.carrier_pll_bw < 0.5f && c.carrier_pll_max_offset > 0, B200_EINVAL, "carrier_pll_bw / carrier_pll_max_offset out of range");
     }
-    // MAX_SPS = 10 for pm_demod ("we do NOT want to resample unless really necessary", module_pm_demod.cpp:56)
-    const float lo = c.constellation == B200_OQPSK ? 1.6f : 1.1f, hi = pm ? 10.0f : (c.constellation == B200_OQPSK ? 2.4f : 4.0f);
-    B200_REQUIRE(sps >= lo * 0.999f && sps <= hi * 1.001f, B200_EINVAL,
-                 "samples per symbol %.4f outside [%.1f, %.1f]: set final_samplerate (b200_demod_final_samplerate) so that the front-end resampler runs", sps, lo,
-                 hi);
+    SpsWindow win = sps_window(c.constellation);
+    if (pm) // MAX_SPS = 10 for pm_demod ("we do NOT want to resample unless really necessary", module_pm_demod.cpp:56)
+        win.hi = 10.0f;
+    B200_REQUIRE(sps >= win.lo * 0.999f && sps <= win.hi * 1.001f, B200_EINVAL,
+                 "samples per symbol %.4f outside [%.1f, %.1f]: set final_samplerate (b200_demod_final_samplerate) so that the front-end resampler runs", sps,
+                 win.lo, win.hi);
     if (c.final_samplerate > 0 && (long)c.final_samplerate != fs && c.front_resample != 2) {
-        // SmartResamplerBlock(input, final_samplerate, d_samplerate) -> (unsigned interpolation, unsigned decimation), smart_resampler.cpp:8-61
         const unsigned interpolation = (unsigned)final_fs, decimation = (unsigned)fs;
         B200_REQUIRE(interpolation > 0, B200_EINVAL, "final_samplerate too small");
-        double rsamp_in = decimation, fout = interpolation;
-        bool rational = true;
-        if (decimation > interpolation) {
-            const int best_power = (int)floor(log2((double)(decimation / interpolation))); // (unsigned division, as the reference)
-            if (best_power > 0) { // power-of-two decimator first: smart_resampler.cpp:22-29, power_decim.cpp:13-29
-                const int best_decim = std::min<int>(1 << best_power, 1 << PD_NPLANS);
-                rsamp_in = (double)decimation / (double)best_decim;
-                const PdPlan &plan = PD_PLANS[(int)log2((double)best_decim) - 1];
-                for (int i = 0; i < plan.nstages; i++) {
-                    DecimStage st;
-                    st.D = plan.stages[i].decimation;
-                    st.nt = plan.stages[i].ntaps;
-                    st.taps_rev.resize(st.nt);
-                    for (int k = 0; k < st.nt; k++)
-                        st.taps_rev[k] = PD_TAPS[plan.stages[i].offset + st.nt - 1 - k]; // decimating_fir.cpp:30: reversed
-                    decim.push_back(std::move(st));
-                }
-                decim_total = best_decim;
+        const SmartRatio r = smart_resampler_ratio(interpolation, decimation);
+        if (r.decim_power > 0) {
+            const PdPlan &plan = PD_PLANS[r.decim_power - 1];
+            for (int i = 0; i < plan.nstages; i++) {
+                DecimStage st;
+                st.D = plan.stages[i].decimation;
+                st.nt = plan.stages[i].ntaps;
+                st.taps_rev.resize(st.nt);
+                for (int k = 0; k < st.nt; k++)
+                    st.taps_rev[k] = PD_TAPS[plan.stages[i].offset + st.nt - 1 - k]; // decimating_fir.cpp:30: reversed
+                decim.push_back(std::move(st));
             }
-            rational = rsamp_in != fout;
-            if (rational) {
-                double t; // "ensure it's all integer" (smart_resampler.cpp:35-40)
-                while (modf(rsamp_in, &t) != 0 || modf(fout, &t) != 0) {
-                    rsamp_in *= 10;
-                    fout *= 10;
-                }
-            }
+            decim_total = 1 << r.decim_power;
         }
-        if (rational) {
-            unsigned I = (unsigned)fout, D = (unsigned)rsamp_in;
-            const unsigned g = gcd_u(I, D);
-            I /= g;
-            D /= g;
-            rs_I = (int)I;
-            rs_D = (int)D;
-            rs_nt = design_resampler_bank(I, D, rs_bank);
+        if (r.rational) {
+            rs_I = (int)r.I;
+            rs_D = (int)r.D;
+            rs_nt = design_resampler_bank(r.I, r.D, rs_bank);
             B200_REQUIRE(rs_nt <= RS_MAX_TAPS, B200_EUNSUPPORTED, "resampler arm of %d taps exceeds the built maximum %d", rs_nt, RS_MAX_TAPS);
             resamp = true;
         } else if (c.iq_swap && decim.empty() && !pm_after) {
@@ -295,16 +329,12 @@ Demod::Demod(const b200_demod_cfg &c) : cfg(c)
         // carrier PLL warm-up: the loop is linear (its detector is the input's own phase minus the loop phase), two copies approach each
         // other like exp(-n * bw * 1.5): 24 / bw samples bring any start state below float resolution of the phase
         Wp = round_up16(24.0 / (pm ? c.pm_pll_bw : c.carrier_pll_bw));
-        if (const char *e = getenv("B200_PLL_WARMUP_SCALE")) // tuning hook
-            Wp = round_up16(Wp * atof(e));
     }
     design_rrc(1, final_fs, (double)(int)rs, c.rrc_alpha, c.rrc_taps, rrc);
     design_mm_bank(bank);
     // Costas warm-up: 24 loop time constants for orders 2/4; the order-8 detector has about a third of the gain (measured on the
     // psk8 signal: 0.94 % of the samples off by >1e-5 with 24/bw, 0.10 % with 48/bw, 0.015 % with 96/bw)
     Wc = round_up16((c.constellation == B200_8PSK ? 72.0 : 24.0) / c.pll_bw);
-    if (const char *e = getenv("B200_COSTAS_WARMUP_SCALE")) // tuning hook
-        Wc = round_up16(Wc * atof(e));
     // M&M warm-up: the timing loop has to land on the sequential trajectory to ~1e-4 sample. Its time constant is 1/(gain_mu * K)
     // symbols with a TED gain K that falls with the samples per symbol (the pulse slope per sample) and is about half as large for
     // BPSK (one rail), i.e. ~ sps^2 in samples. Measured on 2^21-sample signals: QPSK sps 2.57 with 70/gain_mu samples sits at the
@@ -318,20 +348,14 @@ Demod::Demod(const b200_demod_cfg &c) : cfg(c)
         // 1e-6: tests/floors.py); the error falls by e per ~1200 samples: 87.5/gain_mu -> 4e-5 (0.7 %)
         Wm = round_up16((c.constellation == B200_BPSK ? 240.0 : 87.5) * scale / c.clock_gain_mu);
     }
-    if (const char *e = getenv("B200_MM_WARMUP_SCALE")) // tuning hook
-        Wm = round_up16(Wm * atof(e));
     // gear shift (k_costas / k_mm): the first quarter of a warm-up runs first order at 4x the gain
     Gc = (Wc / 4) & ~15;
     Gm = (Wm / 4) & ~15;
-    if (const char *e = getenv("B200_GEAR_SCALE")) { // tuning hook: fraction of the warm-up
-        Gc = (int)(Wc * atof(e)) & ~15;
-        Gm = (int)(Wm * atof(e)) & ~15;
-    }
     // junction tolerances (a junction outside them is repaired = re-run as the exact sequential continuation). Orders 2 / 4 on
     // non-offset signals: converged segments sit within 6e-6 rad of their predecessor (float rounding noise of two loops on the same
     // trajectory), so 1e-5 only catches real stragglers and bounds the output error of a junction to ~1e-5 |v|. The OQPSK / 8PSK
     // detectors leave 0.1-0.4 % of the warm-ups ~1e-3 off (hang-ups near the unstable lock point); a junction that far off seeds
-    // sign-decision events in the segment (a 7e-3 rad kick each), hence 2e-5 there too. Environment: tuning hooks
+    // sign-decision events in the segment (a 7e-3 rad kick each), hence 2e-5 there too.
     if (order == 2 || (order == 4 && c.constellation != B200_OQPSK)) {
         tol_cphase = 1e-5f;
         tol_cfreq = 2e-6f;
@@ -340,32 +364,19 @@ Demod::Demod(const b200_demod_cfg &c) : cfg(c)
         tol_cfreq = 4e-6f;
     }
     tol_mm = 0.01f; // samples (1.3 interpolator arms)
-    if (const char *e = getenv("B200_COSTAS_TOL"))
-        tol_cphase = (float)atof(e);
-    if (const char *e = getenv("B200_COSTAS_FTOL"))
-        tol_cfreq = (float)atof(e);
-    if (const char *e = getenv("B200_MM_TOL"))
-        tol_mm = (float)atof(e);
     int dev_sms = 132;
     cudaDeviceGetAttribute(&dev_sms, cudaDevAttrMultiProcessorCount, c.device);
-    seg_ctas = 3;
-    if (const char *e = getenv("B200_SEG_CTAS")) // tuning hook: resident CTAs of the loop kernels per SM the segment count aims at
-        seg_ctas = std::max(1, atoi(e));
-    seg_cap_threads = dev_sms * seg_ctas * SEG_THREADS;
-
-
+    seg_cap_threads = dev_sms * 3 * SEG_THREADS; // the segment count aims at 3 resident CTAs of the loop kernels per SM
     {
         // in a pipelined chain the demodulator of batch i runs next to the decoder of batch i-1 and is the longer of the two: its
-        // kernels take freed SM slots first (B200_STREAM_PRIORITY=0 disables, for A/B measurements)
+        // kernels take freed SM slots first
         int lo = 0, hi = 0;
         B200_CUDA(cudaDeviceGetStreamPriorityRange(&lo, &hi));
-        const char *e = getenv("B200_STREAM_PRIORITY");
-        B200_CUDA(cudaStreamCreateWithPriority(&stream, cudaStreamNonBlocking, (e && atoi(e) == 0) ? lo : hi));
+        B200_CUDA(cudaStreamCreateWithPriority(&stream, cudaStreamNonBlocking, hi));
     }
     for (auto &e : ev)
         B200_CUDA(cudaEventCreate(&e));
-    const int fmt_bytes = c.format == B200_CF32 ? 8 : (c.format == B200_CS16 ? 4 : 2);
-    raw.alloc((size_t)max_batch * fmt_bytes + 64);
+    raw.alloc((size_t)max_batch * fmt_bytes(c.format) + 64);
     B200_CUDA(cudaStreamCreateWithFlags(&copy_stream, cudaStreamNonBlocking));
     for (auto &p : pf)
         B200_CUDA(cudaEventCreateWithFlags(&p.done, cudaEventDisableTiming));
@@ -384,16 +395,12 @@ Demod::Demod(const b200_demod_cfg &c) : cfg(c)
     {
         // one wave of resident warps, each owning a range of tiles (k_agc_fir_w: 4 independent warps per CTA, 11.5 KB of smem)
         int per_sm = 0;
-        if (c.format == B200_CF32 || resamp || c.dc_block || !decim.empty())
-            B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_agc_fir_w<0, false, false>, 32 * FW_WARPS, 0));
-        else if (c.format == B200_CS16)
-            B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_agc_fir_w<1, false, false>, 32 * FW_WARPS, 0));
-        else
-            B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_agc_fir_w<2, false, false>, 32 * FW_WARPS, 0));
+        const int agc_fmt = (resamp || c.dc_block || !decim.empty()) ? B200_CF32 : c.format;
+        with_fmt(agc_fmt, [&](auto F) {
+            B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_agc_fir_w<F, false, false>, 32 * FW_WARPS, 0));
+        });
         fir_ctas = std::max(1, per_sm) * dev_sms;
         fir_warps = fir_ctas * FW_WARPS;
-        if (const char *e = getenv("B200_FIR_BULK")) // measured variant: raw chunks by 1-D bulk copy (TMA) instead of register prefetch
-            fir_bulk = atoi(e) != 0;
         if (const char *e = getenv("B200_AGC_WARM_TILES")) // 0 forces the exact (scanned-seed) pass: test hook
             agc_warm_max = std::max(0, atoi(e));
     }
@@ -466,15 +473,7 @@ Demod::Demod(const b200_demod_cfg &c) : cfg(c)
     B200_CUDA(cudaMemcpyAsync(d_bank.p, bank.data(), 128 * 8 * sizeof(float), cudaMemcpyHostToDevice, stream));
     B200_CUDA(cudaMallocHost((void **)&h_total, sizeof(long)));
     B200_CUDA(cudaMallocHost((void **)&h_state, sizeof(DemodDevState)));
-    // initial loop state: AGC gain 1 (module_demod_base.cpp:207), Costas 0/0, M&M mu / omega (clock_recovery_mm.cpp:11)
-    memset(h_state, 0, sizeof(DemodDevState));
-    h_state->gain[0] = h_state->gain[1] = 1.0f;
-    h_state->gain2[0] = h_state->gain2[1] = 1.0f;
-    for (int i = 0; i < 2; i++) {
-        h_state->mm[i].mu = c.clock_mu;
-        h_state->mm[i].omega = sps;
-    }
-    B200_CUDA(cudaMemcpyAsync(st.p, h_state, sizeof(DemodDevState), cudaMemcpyHostToDevice, stream));
+    init_state();
     bufA.zero(stream);
     bufB.zero(stream);
     B200_CUDA(cudaFuncSetAttribute(k_mm<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, MM_SMEM_BYTES));
@@ -509,19 +508,25 @@ Demod::~Demod()
         cudaStreamDestroy(stream);
 }
 
-void Demod::reset()
+// initial loop state, uploaded on the stream: AGC gain 1 (module_demod_base.cpp:207), Costas 0/0, M&M mu / omega (clock_recovery_mm.cpp:11)
+void Demod::init_state()
 {
-    DeviceGuard g(cfg.device);
-    B200_CUDA(cudaStreamSynchronize(stream));
     memset(h_state, 0, sizeof(DemodDevState));
     h_state->gain[0] = h_state->gain[1] = 1.0f;
     h_state->gain2[0] = h_state->gain2[1] = 1.0f;
-    pm_pos = fs_pos = 0;
     for (int i = 0; i < 2; i++) {
         h_state->mm[i].mu = cfg.clock_mu;
         h_state->mm[i].omega = sps;
     }
     B200_CUDA(cudaMemcpyAsync(st.p, h_state, sizeof(DemodDevState), cudaMemcpyHostToDevice, stream));
+}
+
+void Demod::reset()
+{
+    DeviceGuard g(cfg.device);
+    B200_CUDA(cudaStreamSynchronize(stream));
+    init_state();
+    pm_pos = fs_pos = 0;
     B200_CUDA(cudaStreamSynchronize(stream));
     parity = 0;
     last_n = last_syms = 0;
@@ -563,45 +568,28 @@ template <int FMT> static void launch_front(Demod &d, const void *raw, long n, i
     ctl.warm_max = d.agc_warm_max;
     ctl.max_gain = u.max_gain;
     const int *need = d.agc_need.p + (ctl.epoch & 1);
-    const bool dump = u.dump != nullptr;
+    const auto fir = u.dump ? k_agc_fir_w<FMT, true, false> : k_agc_fir_w<FMT, false, false>;
     for (int pass = 0; pass < 2; pass++) {
         ctl.seeded = pass;
         if (pass) { // exact pass: returns at once unless the fast pass asked for it
             k_agc_compose<FMT><<<std::min(ntiles, d.fir_ctas * 2), FIR_THREADS, 0, d.stream>>>(raw, n, u.rate, need, ntiles, d.tile_map.p);
             k_agc_scan<<<1, 1024, 0, d.stream>>>(d.tile_map.p, ntiles, u.gain_in, need, d.seeds.p, &S->agc_exact);
         }
-        if (dump)
-            k_agc_fir_w<FMT, true, false><<<grid, 32 * FW_WARPS, 0, d.stream>>>(raw, n, u.rate, u.gain_in, R, ctl, taps, u.tail_in, u.tail_out, u.fir_out, u.dump,
-                                                                              u.gain_out, &S->flags);
-        else if (d.fir_bulk)
-            k_agc_fir_w<FMT, false, false, true><<<grid, 32 * FW_WARPS, 0, d.stream>>>(raw, n, u.rate, u.gain_in, R, ctl, taps, u.tail_in, u.tail_out, u.fir_out,
-                                                                                     nullptr, u.gain_out, &S->flags);
-        else
-            k_agc_fir_w<FMT, false, false><<<grid, 32 * FW_WARPS, 0, d.stream>>>(raw, n, u.rate, u.gain_in, R, ctl, taps, u.tail_in, u.tail_out, u.fir_out, nullptr,
-                                                                               u.gain_out, &S->flags);
+        fir<<<grid, 32 * FW_WARPS, 0, d.stream>>>(raw, n, u.rate, u.gain_in, R, ctl, taps, u.tail_in, u.tail_out, u.fir_out, u.dump, u.gain_out, &S->flags);
     }
     // clamp pass: the gain reached max_gain somewhere in this batch (silent input), so the unclamped maps above do not describe
     // the reference's loop; redo the stage with the clamped ones. All three launches return at once otherwise.
     ctl.seeded = 1;
     k_agc_compose3<FMT><<<std::min(ntiles, d.fir_ctas * 2), FIR_THREADS, 0, d.stream>>>(raw, n, u.rate, (double)u.max_gain, &S->flags, ntiles, d.tile_map3.p);
     k_agc_scan3<<<1, 1024, 0, d.stream>>>(d.tile_map3.p, ntiles, u.gain_in, &S->flags, d.seeds.p);
-    if (dump)
-        k_agc_fir_w<FMT, true, true><<<grid, 32 * FW_WARPS, 0, d.stream>>>(raw, n, u.rate, u.gain_in, R, ctl, taps, u.tail_in, u.tail_out, u.fir_out, u.dump,
-                                                                         u.gain_out, &S->flags);
-    else
-        k_agc_fir_w<FMT, false, true><<<grid, 32 * FW_WARPS, 0, d.stream>>>(raw, n, u.rate, u.gain_in, R, ctl, taps, u.tail_in, u.tail_out, u.fir_out, nullptr,
-                                                                          u.gain_out, &S->flags);
+    const auto fir_clamp = u.dump ? k_agc_fir_w<FMT, true, true> : k_agc_fir_w<FMT, false, true>;
+    fir_clamp<<<grid, 32 * FW_WARPS, 0, d.stream>>>(raw, n, u.rate, u.gain_in, R, ctl, taps, u.tail_in, u.tail_out, u.fir_out, u.dump, u.gain_out, &S->flags);
     d.launches += 7;
 }
 static void launch_front_fmt(Demod &d, int fmt, const void *raw, long n, FirTaps taps, const AgcUnit &u)
 {
     const int ntiles = (int)((n + FIR_TILE - 1) / FIR_TILE);
-    if (fmt == B200_CF32)
-        launch_front<0>(d, raw, n, ntiles, taps, u);
-    else if (fmt == B200_CS16)
-        launch_front<1>(d, raw, n, ntiles, taps, u);
-    else
-        launch_front<2>(d, raw, n, ntiles, taps, u);
+    with_fmt(fmt, [&](auto F) { launch_front<F>(d, raw, n, ntiles, taps, u); });
 }
 
 // FreqShiftBlock / PMToBPSK: see k_rotator. pos = samples the rotator has seen before this batch.
@@ -609,13 +597,22 @@ void Demod::run_rotator(const void *src, int fmt, long n, int iq_swap, int imag_
 {
     const unsigned grid = (unsigned)((n + 8 * 256 - 1) / (8 * 256));
     const unsigned long long turn0 = pos * dturn; // mod 2^64 = mod one turn
-    if (fmt == B200_CF32)
-        k_rotator<0><<<grid, 256, 0, stream>>>(src, n, iq_swap, imag_only, turn0, dturn, dst);
-    else if (fmt == B200_CS16)
-        k_rotator<1><<<grid, 256, 0, stream>>>(src, n, iq_swap, imag_only, turn0, dturn, dst);
-    else
-        k_rotator<2><<<grid, 256, 0, stream>>>(src, n, iq_swap, imag_only, turn0, dturn, dst);
+    with_fmt(fmt, [&](auto F) { k_rotator<F><<<grid, 256, 0, stream>>>(src, n, iq_swap, imag_only, turn0, dturn, dst); });
     launches++;
+}
+
+// CorrectIQBlock (utils/correct_iq.cpp:18-35, alpha correct_iq.h:24) over n samples at src: per-tile maps, their scan from the carried
+// accumulator acc_in, then the output and the accumulator after the batch (acc_out)
+void Demod::run_dc(const void *src, int fmt, int iq_swap, long n, const float2 *acc_in, float2 *acc_out, float2 *dst)
+{
+    const int nt = (int)((n + FIR_TILE - 1) / FIR_TILE);
+    const float alpha = 0.0001f, beta = 1.0f - alpha;
+    with_fmt(fmt, [&](auto F) {
+        k_dc_tile<F><<<nt, FIR_THREADS, 0, stream>>>(src, n, iq_swap, alpha, beta, dc_map.p);
+        k_dc_scan<<<1, 1024, 0, stream>>>(dc_map.p, nt, acc_in, dc_seeds.p);
+        k_dc_apply<F><<<nt, FIR_THREADS, 0, stream>>>(src, n, iq_swap, alpha, beta, dc_seeds.p, dst, acc_out);
+    });
+    launches += 3;
 }
 
 // pm_demod: PLLCarrierTrackingBlock over the AGC output (pm_agc -> pm_pll; junction check / repair rounds as for the Costas loop, with
@@ -669,12 +666,7 @@ float2 *Demod::stage_costas(long n, int L, int nseg, int cur, int nxt, bool mate
         // psk_demod carrier mode (module_psk_demod.cpp:109-112,121): carrier PLL on the RRC output, then CorrectIQBlock; the Costas loop
         // reads the result (written back over the RRC output)
         run_pll(fir_out, pm_pll.p, n, cfg.carrier_pll_bw, cfg.carrier_pll_max_offset, cur, nxt);
-        const int nt = (int)((n + FIR_TILE - 1) / FIR_TILE);
-        const float alpha = 0.0001f, beta = 1.0f - alpha; // correct_iq.h:24, correct_iq.cpp:9
-        k_dc_tile<0><<<nt, FIR_THREADS, 0, stream>>>(pm_pll.p, n, 0, alpha, beta, dc_map.p);
-        k_dc_scan<<<1, 1024, 0, stream>>>(dc_map.p, nt, &S->dc_acc3[cur], dc_seeds.p);
-        k_dc_apply<0><<<nt, FIR_THREADS, 0, stream>>>(pm_pll.p, n, 0, alpha, beta, dc_seeds.p, fir_out, &S->dc_acc3[nxt]);
-        launches += 3;
+        run_dc(pm_pll.p, B200_CF32, 0, n, &S->dc_acc3[cur], &S->dc_acc3[nxt], fir_out);
     }
     if (order) {
         CostasParams P;
@@ -687,25 +679,16 @@ float2 *Demod::stage_costas(long n, int L, int nseg, int cur, int nxt, bool mate
         }
         P.fmin = -cfg.costas_max_offset;
         P.fmax = cfg.costas_max_offset;
-#define B200_COSTAS_LAUNCH(grid, ...)                                                                                                       \
-    do {                                                                                                                                    \
-        if (order == 2)                                                                                                                     \
-            k_costas<2><<<grid, SEG_THREADS, COSTAS_SMEM_BYTES, stream>>>(__VA_ARGS__);                                                      \
-        else if (order == 4)                                                                                                                \
-            k_costas<4><<<grid, SEG_THREADS, COSTAS_SMEM_BYTES, stream>>>(__VA_ARGS__);                                                      \
-        else                                                                                                                                \
-            k_costas<8><<<grid, SEG_THREADS, COSTAS_SMEM_BYTES, stream>>>(__VA_ARGS__);                                                      \
-    } while (0)
-        B200_COSTAS_LAUNCH(nblk, fir_out, n, L, Wc, Gc, nseg, P, S->costas[cur], cos_out, crec.p, nullptr, nullptr);
+        const auto costas = order == 2 ? k_costas<2> : (order == 4 ? k_costas<4> : k_costas<8>);
+        costas<<<nblk, SEG_THREADS, COSTAS_SMEM_BYTES, stream>>>(fir_out, n, L, Wc, Gc, nseg, P, S->costas[cur], cos_out, crec.p, nullptr, nullptr);
         k_costas_fix<<<1, 1024, 0, stream>>>(crec.p, nseg, order, tol_cphase, tol_cfreq, quad.p, S->costas[nxt], &S->costas_unconv, repair.p + 1, repair.p, 0,
                                              &S->repairs);
         for (int round = 1; round <= REPAIR_ROUNDS; round++) { // both kernels return at once when no junction is flagged
-            B200_COSTAS_LAUNCH(8, fir_out, n, L, Wc, Gc, nseg, P, S->costas[cur], cos_out, crec.p, repair.p + 1, repair.p);
+            costas<<<8, SEG_THREADS, COSTAS_SMEM_BYTES, stream>>>(fir_out, n, L, Wc, Gc, nseg, P, S->costas[cur], cos_out, crec.p, repair.p + 1, repair.p);
             k_costas_fix<<<1, 1024, 0, stream>>>(crec.p, nseg, order, tol_cphase, tol_cfreq, quad.p, S->costas[nxt], &S->costas_unconv, repair.p + 1, repair.p,
                                                  round, &S->repairs);
             launches += 2;
         }
-#undef B200_COSTAS_LAUNCH
         if (!materialise && !cfg.post_costas_dc) {
             // fused: the clock recovery rotates (and, for OQPSK, delays) its input rows itself
             k_mm_prep<<<1, 32, 0, stream>>>(bufB.p, n, L, order, quad.p, S->mm_hist[cur], S->mm_hist[nxt]);
@@ -720,14 +703,9 @@ float2 *Demod::stage_costas(long n, int L, int nseg, int cur, int nxt, bool mate
         launches += 3;
         if (cfg.post_costas_dc) {
             // CorrectIQBlock on the loop's output (module_psk_demod.cpp:127-134); the clock recovery's 8-sample history are ITS outputs
-            const int nt = (int)((n + FIR_TILE - 1) / FIR_TILE);
-            const float alpha = 0.0001f, beta = 1.0f - alpha;
-            k_dc_tile<0><<<nt, FIR_THREADS, 0, stream>>>(mmin + 16, n, 0, alpha, beta, dc_map.p);
-            k_dc_scan<<<1, 1024, 0, stream>>>(dc_map.p, nt, &S->dc_acc2[cur], dc_seeds.p);
-            k_dc_apply<0><<<nt, FIR_THREADS, 0, stream>>>(mmin + 16, n, 0, alpha, beta, dc_seeds.p, pdc_out.p + 16, &S->dc_acc2[nxt]);
+            run_dc(mmin + 16, B200_CF32, 0, n, &S->dc_acc2[cur], &S->dc_acc2[nxt], pdc_out.p + 16);
             B200_CUDA(cudaMemcpyAsync(pdc_out.p + 16 - MM_HIST, S->pdc_hist[cur], MM_HIST * sizeof(float2), cudaMemcpyDeviceToDevice, stream));
             B200_CUDA(cudaMemcpyAsync(S->pdc_hist[nxt], pdc_out.p + 16 + n - MM_HIST, MM_HIST * sizeof(float2), cudaMemcpyDeviceToDevice, stream));
-            launches += 3;
             mmin = pdc_out.p;
         }
     } else if (!materialise) {
@@ -747,18 +725,7 @@ void Demod::stage_mm(float2 *mmin, long n, int L, int nseg, int cur, int nxt, in
 {
     DemodDevState *S = st.p;
     const int nblk = (nseg + SEG_THREADS - 1) / SEG_THREADS;
-#define B200_MM_LAUNCH(grid, ...)                                                                                                           \
-    do {                                                                                                                                    \
-        if (cfg.clock_recovery == 1) {                                                                                                      \
-            if (strict)                                                                                                                     \
-                k_mm<true, true><<<grid, SEG_THREADS, MM_SMEM_BYTES, stream>>>(__VA_ARGS__);                                                 \
-            else                                                                                                                            \
-                k_mm<false, true><<<grid, SEG_THREADS, MM_SMEM_BYTES, stream>>>(__VA_ARGS__);                                                \
-        } else if (strict)                                                                                                                  \
-            k_mm<true, false><<<grid, SEG_THREADS, MM_SMEM_BYTES, stream>>>(__VA_ARGS__);                                                    \
-        else                                                                                                                                \
-            k_mm<false, false><<<grid, SEG_THREADS, MM_SMEM_BYTES, stream>>>(__VA_ARGS__);                                                   \
-    } while (0)
+    const auto mm = cfg.clock_recovery == 1 ? (strict ? k_mm<true, true> : k_mm<false, true>) : (strict ? k_mm<true, false> : k_mm<false, false>);
     MMParams MP;
     MP.omega_mid = sps;
     MP.omega_limit = cfg.clock_omega_limit * sps;
@@ -766,17 +733,18 @@ void Demod::stage_mm(float2 *mmin, long n, int L, int nseg, int cur, int nxt, in
     MP.mu_gain = cfg.clock_gain_mu;
     const int cap = slot_cap_for(L);
     B200_REQUIRE((size_t)nseg * cap <= slots.n, B200_ENOMEM, "internal: symbol slot storage too small");
-    B200_MM_LAUNCH(nblk, mmin, n, L, Wm, Gm, nseg, MP, &S->mm[cur], &S->mm[nxt], d_bank.p, slots.p, cap, mrec.p, nullptr, nullptr, mm_quad, mm_rot, mm_oqpsk);
+    mm<<<nblk, SEG_THREADS, MM_SMEM_BYTES, stream>>>(mmin, n, L, Wm, Gm, nseg, MP, &S->mm[cur], &S->mm[nxt], d_bank.p, slots.p, cap, mrec.p, nullptr, nullptr,
+                                                    mm_quad, mm_rot, mm_oqpsk);
     k_mm_scan<<<1, 1024, 0, stream>>>(mrec.p, nseg, tol_mm, offs.p, &S->mm_unconv, cap, &S->flags, repair.p + 1, repair.p, 0, &S->repairs);
     for (int round = 1; round <= REPAIR_ROUNDS; round++) {
-        B200_MM_LAUNCH(8, mmin, n, L, Wm, Gm, nseg, MP, &S->mm[cur], &S->mm[nxt], d_bank.p, slots.p, cap, mrec.p, repair.p + 1, repair.p, mm_quad, mm_rot, mm_oqpsk);
+        mm<<<8, SEG_THREADS, MM_SMEM_BYTES, stream>>>(mmin, n, L, Wm, Gm, nseg, MP, &S->mm[cur], &S->mm[nxt], d_bank.p, slots.p, cap, mrec.p, repair.p + 1, repair.p,
+                                                     mm_quad, mm_rot, mm_oqpsk);
         k_mm_scan<<<1, 1024, 0, stream>>>(mrec.p, nseg, tol_mm, offs.p, &S->mm_unconv, cap, &S->flags, repair.p + 1, repair.p, round, &S->repairs);
         launches += 2;
     }
     k_mm_compact<<<std::min(nseg, 132 * 8), 256, 0, stream>>>(slots.p, cap, mrec.p, offs.p, nseg, pm ? 2 : (bps == 1), sym_out.p, sdst);
     k_snr_m2m4<<<1, 1024, 0, stream>>>(sym_out.p, offs.p + nseg, 0.001f, S->snr_y[cur], S->snr_y[nxt]); // M2M4SNREstimator(alpha = 0.001)
     launches += 4;
-#undef B200_MM_LAUNCH
 }
 
 // SmartResamplerBlock (module_demod_base.cpp:203-204; behind PMToBPSK for pm_demod with resample_after_pll): power-of-two decimator
@@ -791,12 +759,9 @@ void Demod::front_resample(const void *&d_raw, long &n, int &front_fmt, int &rs_
             J = (n - stg.inc + stg.D - 1) / stg.D;
         B200_REQUIRE(J >= 64, B200_ESTATE, "batch of %ld samples decimates to %ld: push at least %d samples", n_in, J, 64 * decim_total + 4096);
         const unsigned grid = (unsigned)((std::max<long>(J, stg.nt) + 255) / 256);
-        if (front_fmt == B200_CF32)
-            k_decim_fir<0><<<grid, 256, 0, stream>>>(d_raw, n, rs_swap, stg.tail[cur].p, stg.tail[nxt].p, stg.d_taps.p, stg.nt, stg.D, stg.inc, J, stg.out.p);
-        else if (front_fmt == B200_CS16)
-            k_decim_fir<1><<<grid, 256, 0, stream>>>(d_raw, n, rs_swap, stg.tail[cur].p, stg.tail[nxt].p, stg.d_taps.p, stg.nt, stg.D, stg.inc, J, stg.out.p);
-        else
-            k_decim_fir<2><<<grid, 256, 0, stream>>>(d_raw, n, rs_swap, stg.tail[cur].p, stg.tail[nxt].p, stg.d_taps.p, stg.nt, stg.D, stg.inc, J, stg.out.p);
+        with_fmt(front_fmt, [&](auto F) {
+            k_decim_fir<F><<<grid, 256, 0, stream>>>(d_raw, n, rs_swap, stg.tail[cur].p, stg.tail[nxt].p, stg.d_taps.p, stg.nt, stg.D, stg.inc, J, stg.out.p);
+        });
         launches++;
         stg.inc = stg.inc + J * stg.D - n;
         d_raw = stg.out.p;
@@ -812,12 +777,10 @@ void Demod::front_resample(const void *&d_raw, long &n, int &front_fmt, int &rs_
             J = ((n - rs_inc) * I - rs_ctr + D - 1) / D;
         B200_REQUIRE(J >= 64 && J <= max_work, B200_ESTATE, "batch of %ld samples resamples to %ld: outside [64, %ld]", n, J, max_work);
         const unsigned grid = (unsigned)((J + RS_THREADS - 1) / RS_THREADS);
-        if (front_fmt == B200_CF32)
-            k_resample<0><<<grid, RS_THREADS, 0, stream>>>(d_raw, n, rs_swap, S->rs_tail[cur], S->rs_tail[nxt], d_rs_bank.p, rs_I, rs_D, rs_nt, rs_inc, rs_ctr, J, rs_out.p);
-        else if (front_fmt == B200_CS16)
-            k_resample<1><<<grid, RS_THREADS, 0, stream>>>(d_raw, n, rs_swap, S->rs_tail[cur], S->rs_tail[nxt], d_rs_bank.p, rs_I, rs_D, rs_nt, rs_inc, rs_ctr, J, rs_out.p);
-        else
-            k_resample<2><<<grid, RS_THREADS, 0, stream>>>(d_raw, n, rs_swap, S->rs_tail[cur], S->rs_tail[nxt], d_rs_bank.p, rs_I, rs_D, rs_nt, rs_inc, rs_ctr, J, rs_out.p);
+        with_fmt(front_fmt, [&](auto F) {
+            k_resample<F><<<grid, RS_THREADS, 0, stream>>>(d_raw, n, rs_swap, S->rs_tail[cur], S->rs_tail[nxt], d_rs_bank.p, rs_I, rs_D, rs_nt, rs_inc, rs_ctr, J,
+                                                          rs_out.p);
+        });
         launches++;
         const long c_end = rs_ctr + J * D;
         rs_inc = rs_inc + c_end / I - n;
@@ -843,22 +806,7 @@ long Demod::process(const void *d_raw, long n, int8_t *soft_dst)
     int rs_swap = cfg.iq_swap;
     if (cfg.dc_block) {
         // CorrectIQBlock sits right behind the reader (module_demod_base.cpp:113-120): (iq_swap ->) dc block -> (resampler ->) AGC
-        const int nt = (int)((n + FIR_TILE - 1) / FIR_TILE);
-        const float alpha = 0.0001f, beta = 1.0f - alpha; // correct_iq.h:24, correct_iq.cpp:9
-#define B200_DC(F)                                                                                                                          \
-    do {                                                                                                                                    \
-        k_dc_tile<F><<<nt, FIR_THREADS, 0, stream>>>(d_raw, n, cfg.iq_swap, alpha, beta, dc_map.p);                                         \
-        k_dc_scan<<<1, 1024, 0, stream>>>(dc_map.p, nt, &S->dc_acc[cur], dc_seeds.p);                                                        \
-        k_dc_apply<F><<<nt, FIR_THREADS, 0, stream>>>(d_raw, n, cfg.iq_swap, alpha, beta, dc_seeds.p, dc_out.p, &S->dc_acc[nxt]);            \
-    } while (0)
-        if (cfg.format == B200_CF32)
-            B200_DC(0);
-        else if (cfg.format == B200_CS16)
-            B200_DC(1);
-        else
-            B200_DC(2);
-#undef B200_DC
-        launches += 3;
+        run_dc(d_raw, cfg.format, cfg.iq_swap, n, &S->dc_acc[cur], &S->dc_acc[nxt], dc_out.p);
         d_raw = dc_out.p;
         front_fmt = B200_CF32;
         rs_swap = 0; // already applied
@@ -1025,15 +973,15 @@ void Demod::prefetch_host(const void *h_raw, long n)
 {
     B200_REQUIRE(n <= max_batch && n >= 64, B200_ESTATE, "prefetch of %ld samples outside [64, max_batch %ld]", n, max_batch);
     DeviceGuard g(cfg.device);
-    const int fmt_bytes = cfg.format == B200_CF32 ? 8 : (cfg.format == B200_CS16 ? 4 : 2);
+    const int bytes = fmt_bytes(cfg.format);
     if (!raw2.p)
-        raw2.alloc((size_t)max_batch * fmt_bytes + 64);
+        raw2.alloc((size_t)max_batch * bytes + 64);
     Prefetch *slot = !pf[0].valid ? &pf[0] : (!pf[1].valid ? &pf[1] : nullptr);
     B200_REQUIRE(slot != nullptr, B200_ESTATE, "two prefetched batches are already pending: push one first");
     // the staging buffer no pending prefetch occupies (pushes may come in any order, so a blind alternation could overwrite one)
     const Prefetch *other = slot == &pf[0] ? &pf[1] : &pf[0];
     slot->buf = (other->valid && other->buf == 0) ? 1 : 0;
-    B200_CUDA(cudaMemcpyAsync(slot->buf ? raw2.p : raw.p, h_raw, (size_t)n * fmt_bytes, cudaMemcpyHostToDevice, copy_stream));
+    B200_CUDA(cudaMemcpyAsync(slot->buf ? raw2.p : raw.p, h_raw, (size_t)n * bytes, cudaMemcpyHostToDevice, copy_stream));
     B200_CUDA(cudaEventRecord(slot->done, copy_stream));
     slot->ptr = h_raw;
     slot->n = n;
@@ -1055,16 +1003,16 @@ long Demod::push_host(const void *h_raw, long n, int8_t *soft_dst)
         hit->valid = false;
         return process(hit->buf ? raw2.p : raw.p, n, soft_dst);
     }
-    const int fmt_bytes = cfg.format == B200_CF32 ? 8 : (cfg.format == B200_CS16 ? 4 : 2);
+    const int bytes = fmt_bytes(cfg.format);
     // no pending prefetch may target the buffer we copy into
     unsigned char *dst = (pf[0].valid && pf[0].buf == 0) || (pf[1].valid && pf[1].buf == 0) ? nullptr : raw.p;
     if (!dst) {
         if (!raw2.p)
-            raw2.alloc((size_t)max_batch * fmt_bytes + 64);
+            raw2.alloc((size_t)max_batch * bytes + 64);
         B200_REQUIRE(!((pf[0].valid && pf[0].buf == 1) || (pf[1].valid && pf[1].buf == 1)), B200_ESTATE, "both staging buffers hold prefetched batches");
         dst = raw2.p;
     }
-    B200_CUDA(cudaMemcpyAsync(dst, h_raw, (size_t)n * fmt_bytes, cudaMemcpyHostToDevice, stream));
+    B200_CUDA(cudaMemcpyAsync(dst, h_raw, (size_t)n * bytes, cudaMemcpyHostToDevice, stream));
     return process(dst, n, soft_dst);
 }
 
@@ -1170,11 +1118,8 @@ double b200_demod_final_samplerate(double samplerate, double symbolrate, int con
     // module_demod_base.cpp:59-80 with its types: long d_samplerate, int d_symbolrate, float MIN_SPS / MAX_SPS / final_samplerate
     const long d_samplerate = (long)samplerate;
     const int d_symbolrate = (int)symbolrate;
-    float MIN_SPS = constellation == B200_OQPSK ? 1.6f : 1.1f, MAX_SPS = constellation == B200_OQPSK ? 2.4f : 4.0f; // module_psk_demod.cpp:65-70
-    if (min_sps > 0)
-        MIN_SPS = min_sps;
-    if (max_sps > 0)
-        MAX_SPS = max_sps;
+    const SpsWindow win = sps_window(constellation, min_sps, max_sps);
+    const float MIN_SPS = win.lo, MAX_SPS = win.hi;
     if (d_symbolrate <= 0 || d_samplerate <= 0)
         return samplerate;
     const float input_sps = (float)d_samplerate / (float)d_symbolrate;
@@ -1195,43 +1140,27 @@ int b200_demod_resample_decision(double samplerate, double symbolrate, int const
 {
     const long d_samplerate = (long)samplerate;
     const int d_symbolrate = (int)symbolrate;
-    float MIN_SPS = constellation == B200_OQPSK ? 1.6f : 1.1f, MAX_SPS = constellation == B200_OQPSK ? 2.4f : 4.0f;
-    if (min_sps > 0)
-        MIN_SPS = min_sps;
-    if (max_sps > 0)
-        MAX_SPS = max_sps;
+    const SpsWindow win = sps_window(constellation, min_sps, max_sps);
     if (d_symbolrate <= 0 || d_samplerate <= 0)
         return 0;
     const float input_sps = (float)d_samplerate / (float)d_symbolrate;
-    return (input_sps > MAX_SPS || input_sps < MIN_SPS) ? 1 : 0;
+    return (input_sps > win.hi || input_sps < win.lo) ? 1 : 0;
 }
 int b200_demod_resampler_bank(double samplerate, double final_samplerate, float *out, long cap, int *ntaps, int *interp, int *decim)
 {
     return guarded([&] {
         B200_REQUIRE(out && ntaps && interp && decim, B200_EINVAL, "NULL argument");
-        // the same reduction as the constructor: SmartResamplerBlock(final, input) -> RationalResamplerBlock::set_ratio
-        unsigned interpolation = (unsigned)(float)final_samplerate, decimation = (unsigned)(long)samplerate;
+        // the constructor's reduction: the rational part behind the power-of-two decimator -> RationalResamplerBlock::set_ratio
+        const unsigned interpolation = (unsigned)(float)final_samplerate, decimation = (unsigned)(long)samplerate;
         B200_REQUIRE(interpolation > 0 && decimation > 0, B200_EINVAL, "rates must be positive");
-        if (decimation > interpolation) { // the rational part behind the power-of-two decimator (smart_resampler.cpp:17-44)
-            const int best_power = (int)floor(log2((double)(decimation / interpolation)));
-            double rsamp_in = decimation, fout = interpolation, t;
-            if (best_power > 0)
-                rsamp_in = (double)decimation / (double)std::min<int>(1 << best_power, 1 << PD_NPLANS);
-            while (modf(rsamp_in, &t) != 0 || modf(fout, &t) != 0) {
-                rsamp_in *= 10;
-                fout *= 10;
-            }
-            interpolation = (unsigned)fout;
-            decimation = (unsigned)rsamp_in;
-        }
-        const unsigned g = gcd_u(interpolation, decimation);
+        const SmartRatio r = smart_resampler_ratio(interpolation, decimation);
         std::vector<float> bank;
-        const int nt = design_resampler_bank(interpolation / g, decimation / g, bank);
+        const int nt = design_resampler_bank(r.I, r.D, bank);
         B200_REQUIRE((long)bank.size() <= cap, B200_ESTATE, "output buffer too small: need %zu floats", bank.size());
         memcpy(out, bank.data(), bank.size() * sizeof(float));
         *ntaps = nt;
-        *interp = (int)(interpolation / g);
-        *decim = (int)(decimation / g);
+        *interp = (int)r.I;
+        *decim = (int)r.D;
     });
 }
 int b200_demod_debug_stage(b200_demod *h, int stage, float *out, long cap_samples)
@@ -1272,16 +1201,10 @@ int b200_demod_debug_convert(b200_demod *h, const void *host_iq, long n, float *
         Demod &d = *h->d;
         B200_REQUIRE(n > 0 && n <= d.max_batch, B200_ESTATE, "sample count outside (0, max_batch]");
         DeviceGuard g(d.cfg.device);
-        const int fmt_bytes = d.cfg.format == B200_CF32 ? 8 : (d.cfg.format == B200_CS16 ? 4 : 2);
-        B200_CUDA(cudaMemcpyAsync(d.raw.p, host_iq, (size_t)n * fmt_bytes, cudaMemcpyHostToDevice, d.stream));
+        B200_CUDA(cudaMemcpyAsync(d.raw.p, host_iq, (size_t)n * fmt_bytes(d.cfg.format), cudaMemcpyHostToDevice, d.stream));
         float2 *out = d.bufB.p + 16;
         const unsigned blocks = (unsigned)((n + 8 * 256 - 1) / (8 * 256));
-        if (d.cfg.format == B200_CF32)
-            k_convert_only<0><<<blocks, 256, 0, d.stream>>>(d.raw.p, n, out);
-        else if (d.cfg.format == B200_CS16)
-            k_convert_only<1><<<blocks, 256, 0, d.stream>>>(d.raw.p, n, out);
-        else
-            k_convert_only<2><<<blocks, 256, 0, d.stream>>>(d.raw.p, n, out);
+        with_fmt(d.cfg.format, [&](auto F) { k_convert_only<F><<<blocks, 256, 0, d.stream>>>(d.raw.p, n, out); });
         B200_CUDA(cudaMemcpyAsync(host_out, out, n * sizeof(float2), cudaMemcpyDeviceToHost, d.stream));
         B200_CUDA(cudaStreamSynchronize(d.stream));
     });

@@ -421,9 +421,6 @@ static void viterbi_segment(Fec &f, long c0, long nch, std::vector<OutChunk> &ou
             if (lost)
                 break;
         }
-        if (getenv("B200_DEBUG_FEC"))
-            fprintf(stderr, "[fec] segment chunks [%ld, %ld): accepted %d, vit_state %d, invalid %d, last ber %.3f, redo rounds list %zu\n", c, c + n, accepted,
-                    f.vit_state, f.invalid, f.last_ber, f.h_redo.size());
         f.main_next_start = f.h_rec[accepted - 1].next_start;
         f.enc_state = f.h_rec[accepted - 1].enc_tail;
         out_base += accepted;
@@ -884,8 +881,6 @@ void Fec::process()
                         nosync_runs = 0;
                 }
             }
-            if (getenv("B200_DEBUG_FEC"))
-                fprintf(stderr, "[fec] process: chunks from %ld: %ld decoded, deframer events %d, redo_from %ld, nosync_runs %d\n", c, nout, h_counters[1], redo_from, nosync_runs);
             if (redo_from >= 0 && redo_from < nout - 1) {
                 // roll back to just after output chunk redo_from, with the Viterbi forced to IDLE
                 replays++;

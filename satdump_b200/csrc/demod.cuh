@@ -570,29 +570,7 @@ template <int FMT> struct FwState
     float2 *xs;        // the warp's strip
     const float2 *xrd; // this lane's FIR window: xidx(8 * lane + c) = 10 * lane + xidx(c)
     int lane, c_last;
-    // BULK variant (1-D TMA): the warp's two raw-chunk buffers and their mbarriers (shared-space addresses), the first / one-past-last
-    // chunk fetched that way
-    unsigned rawbuf0, bar0; // buffer b at rawbuf0 + b * chunk bytes, its barrier at bar0 + 8 b
-    int c_bulk0, c_bulk1;
 };
-
-// ---- 1-D bulk copy (TMA, cp.async.bulk -> UBLKCP) of a raw chunk into shared memory, completion on an mbarrier
-__device__ __forceinline__ void mbar_init(unsigned bar, unsigned count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count)); }
-__device__ __forceinline__ void mbar_expect_tx(unsigned bar, unsigned bytes)
-{
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(unsigned dst, const void *src, unsigned bytes, unsigned bar)
-{
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src), "r"(bytes), "r"(bar)
-                 : "memory");
-}
-__device__ __forceinline__ void mbar_wait(unsigned bar, unsigned parity)
-{
-    asm volatile("{\n.reg .pred p;\nB200_MBAR_WAIT:\nmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n@p bra B200_MBAR_DONE;\nbra B200_MBAR_WAIT;\nB200_MBAR_DONE:\n}" ::"r"(bar),
-                 "r"(parity)
-                 : "memory");
-}
 
 // the 31-tap FIR of one chunk out of the warp's strip: lane -> outputs 8*lane .. 8*lane+7; y[n] = sum_j x[n-30+j] * h[30-j], oldest first
 // (fir.cpp:74-83). One scalar FFMA per (re or im) x real tap MAC, the tap a broadcast register operand; the output pairs are packed into
@@ -629,7 +607,7 @@ __device__ __forceinline__ void fw_fir8(const float2 *xrd, const FirTaps &taps, 
 
 // One chunk of k_agc_fir_w. FAST: every sample of the chunk exists, none belongs to the stream tail, output wanted, no dump, no clamp:
 // no per-sample conditions, and the conversion's power-of-two factor S rides in the gain (raw_convert_scaled).
-template <int FMT, bool DUMP, bool CLAMP, bool FAST, bool BULK = false>
+template <int FMT, bool DUMP, bool CLAMP, bool FAST>
 __device__ __forceinline__ void fw_chunk(FwState<FMT> &st, RawRegs<FMT> &rr, int c, bool out, const FirTaps &taps, float2 *__restrict__ tail_out,
                                          float2 *__restrict__ fir_out, float2 *__restrict__ agc_dump, float *__restrict__ gain_out,
                                          int *__restrict__ flags)
@@ -640,45 +618,17 @@ __device__ __forceinline__ void fw_chunk(FwState<FMT> &st, RawRegs<FMT> &rr, int
     const long s0 = (long)c * FW_CH + 8 * lane;
     constexpr float S = FAST ? RawScale<FMT>::v : 1.0f;
     float2 x[8];
-    if (FAST && BULK) {
-        // the chunk's raw bytes were brought to shared memory by one bulk copy (issued a chunk ahead by lane 0); start the next one
-        constexpr unsigned RAWB = FW_CH * RawBytes<FMT>::v;
-        const int k = c - st.c_bulk0;
-        if (c + 1 < st.c_bulk1 && lane == 0) {
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            const unsigned nb = (unsigned)(k + 1) & 1u;
-            mbar_expect_tx(st.bar0 + 8u * nb, RAWB);
-            bulk_g2s(st.rawbuf0 + nb * RAWB, reinterpret_cast<const unsigned char *>(st.raw) + (long)(c + 1) * RAWB, RAWB, st.bar0 + 8u * nb);
-        }
-        const unsigned cb = (unsigned)k & 1u;
-        mbar_wait(st.bar0 + 8u * cb, (unsigned)(k >> 1) & 1u);
-        const unsigned a = st.rawbuf0 + cb * RAWB + lane * (8 * RawBytes<FMT>::v);
-        if constexpr (FMT == 1) {
-            asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(rr.a.x), "=r"(rr.a.y), "=r"(rr.a.z), "=r"(rr.a.w) : "r"(a));
-            asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(rr.b.x), "=r"(rr.b.y), "=r"(rr.b.z), "=r"(rr.b.w) : "r"(a + 16));
-        } else if constexpr (FMT == 2) {
-            asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(rr.a.x), "=r"(rr.a.y), "=r"(rr.a.z), "=r"(rr.a.w) : "r"(a));
-        } else {
-#pragma unroll
-            for (int i = 0; i < 4; i++)
-                asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(rr.v[i].x), "=f"(rr.v[i].y), "=f"(rr.v[i].z), "=f"(rr.v[i].w) : "r"(a + 16 * i));
-        }
-        raw_convert_scaled<FMT>(rr, x);
-        if (FMT != 0 && c + 1 == st.c_bulk1 && c + 1 < st.c_last && s0 + FW_CH + 8 <= N) // the general body after the last bulk chunk reads registers
-            raw_fetch<FMT>(st.raw, s0 + FW_CH, rr);
-    } else {
-        if (FAST || s0 + 8 <= N) {
-            if (FMT == 0) // cf32: 16 registers of raw data are too many to hold across a chunk
-                raw_fetch<FMT>(st.raw, s0, rr);
-            if (FAST)
-                raw_convert_scaled<FMT>(rr, x);
-            else
-                raw_convert<FMT>(rr, x);
-        } else
-            load8_ragged<FMT>(st.raw, s0, N, x);
-        if (FMT != 0 && c + 1 < st.c_last && s0 + FW_CH + 8 <= N) // the next chunk's loads fly under this chunk's arithmetic
-            raw_fetch<FMT>(st.raw, s0 + FW_CH, rr);
-    }
+    if (FAST || s0 + 8 <= N) {
+        if (FMT == 0) // cf32: 16 registers of raw data are too many to hold across a chunk
+            raw_fetch<FMT>(st.raw, s0, rr);
+        if (FAST)
+            raw_convert_scaled<FMT>(rr, x);
+        else
+            raw_convert<FMT>(rr, x);
+    } else
+        load8_ragged<FMT>(st.raw, s0, N, x);
+    if (FMT != 0 && c + 1 < st.c_last && s0 + FW_CH + 8 <= N) // the next chunk's loads fly under this chunk's arithmetic
+        raw_fetch<FMT>(st.raw, s0 + FW_CH, rr);
     EB inc{0.f, 0.f};
     float incC = (float)AGC_NO_CLAMP;
     float e[8]; // rate * |sample|: the step map of sample q is g -> g * (1 - e[q]) + rate
@@ -809,16 +759,13 @@ __device__ __forceinline__ void fw_chunk(FwState<FMT> &st, RawRegs<FMT> &rr, int
     }
 }
 
-template <int FMT, bool DUMP, bool CLAMP, bool BULK = false>
+template <int FMT, bool DUMP, bool CLAMP>
 __global__ void __launch_bounds__(32 * FW_WARPS, 8) k_agc_fir_w(const void *__restrict__ raw, long N, float rate, const float *__restrict__ gain_in, int R,
                                                                   const AgcCtl ctl, const FirTaps taps, const float2 *__restrict__ tail_in,
                                                                   float2 *__restrict__ tail_out, float2 *__restrict__ fir_out,
                                                                   float2 *__restrict__ agc_dump, float *__restrict__ gain_out, int *__restrict__ flags)
 {
     __shared__ __align__(16) float2 xs_all[FW_WARPS][FW_BUF_F2];
-    constexpr unsigned RAWB = FW_CH * RawBytes<FMT>::v;
-    __shared__ __align__(128) unsigned char rawbuf_all[BULK ? FW_WARPS : 1][2][BULK ? RAWB : 16];
-    __shared__ __align__(8) unsigned long long bar_all[BULK ? FW_WARPS : 1][2];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     float2 *xs = xs_all[warp];
     int *need = ctl.need + (ctl.epoch & 1);
@@ -896,17 +843,7 @@ __global__ void __launch_bounds__(32 * FW_WARPS, 8) k_agc_fir_w(const void *__re
     RawRegs<FMT> rr;
     if (FMT != 0 && (long)c0 * FW_CH + 8 * lane + 8 <= N)
         raw_fetch<FMT>(raw, (long)c0 * FW_CH + 8 * lane, rr);
-    FwState<FMT> st{raw, N, rate, ctl.max_gain, G, xs, &xs[10 * lane], lane, c_last, 0u, 0u, 0, 0};
-    if (BULK) {
-        st.rawbuf0 = (unsigned)__cvta_generic_to_shared(&rawbuf_all[warp][0][0]);
-        st.bar0 = (unsigned)__cvta_generic_to_shared(&bar_all[warp][0]);
-        if (lane == 0) {
-            mbar_init(st.bar0, 1);
-            mbar_init(st.bar0 + 8u, 1);
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        }
-        __syncwarp();
-    }
+    FwState<FMT> st{raw, N, rate, ctl.max_gain, G, xs, &xs[10 * lane], lane, c_last};
     // [c0, c_first): history only; [c_first, c_fast): every sample exists, none is in the stream tail -> the branch-free body;
     // the rest (the batch's last chunks; all of them in the dump / clamp instantiations): the general body
     int c = c0;
@@ -914,17 +851,9 @@ __global__ void __launch_bounds__(32 * FW_WARPS, 8) k_agc_fir_w(const void *__re
         fw_chunk<FMT, DUMP, CLAMP, false>(st, rr, c, false, taps, tail_out, fir_out, agc_dump, gain_out, flags);
     if (!DUMP && !CLAMP) {
         const int c_fast = (int)min((long)c_last, max(0L, (N - 32) / FW_CH)); // (c + 1) * FW_CH + 32 <= N
-        if (BULK && c < c_fast) { // first chunk of the bulk-copied stretch
-            st.c_bulk0 = c;
-            st.c_bulk1 = c_fast;
-            if (lane == 0) {
-                mbar_expect_tx(st.bar0, RAWB);
-                bulk_g2s(st.rawbuf0, reinterpret_cast<const unsigned char *>(raw) + (long)c * RAWB, RAWB, st.bar0);
-            }
-        }
 #pragma unroll 1
         for (; c < c_fast; c++)
-            fw_chunk<FMT, false, false, true, BULK>(st, rr, c, true, taps, tail_out, fir_out, agc_dump, gain_out, flags);
+            fw_chunk<FMT, false, false, true>(st, rr, c, true, taps, tail_out, fir_out, agc_dump, gain_out, flags);
     }
     for (; c < c_last; c++)
         fw_chunk<FMT, DUMP, CLAMP, false>(st, rr, c, true, taps, tail_out, fir_out, agc_dump, gain_out, flags);

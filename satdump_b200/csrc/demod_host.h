@@ -59,6 +59,7 @@ class Demod
     void prefetch_host(const void *h_raw, long nsamples);
     void stats(b200_demod_stats *out);
     void reset(); // back to the state of a freshly created demodulator (new stream)
+    void init_state(); // the initial DemodDevState, into h_state and (on the stream) st
     // stages of process(), also run alone by the stage-isolated parity hook
     float2 *stage_costas(long n, int L, int nseg, int cur, int nxt, bool materialise);
     // front-end resampler (power-of-two decimator stages + rational resampler) over n samples at d_raw: updates them to its output
@@ -68,6 +69,8 @@ class Demod
     // PLLCarrierTrackingBlock (segmented, junction check + repair rounds) over n samples: in -> out
     void run_pll(const float2 *in, float2 *out, long n, float bw, float max_offset, int cur, int nxt);
     void run_rotator(const void *src, int fmt, long n, int iq_swap, int imag_only, unsigned long long dturn, unsigned long long pos, float2 *dst);
+    // CorrectIQBlock over n samples: src -> dst, carried accumulator acc_in -> acc_out
+    void run_dc(const void *src, int fmt, int iq_swap, long n, const float2 *acc_in, float2 *acc_out, float2 *dst);
     const uint8_t *mm_quad = nullptr; // set by stage_costas when the clock recovery applies the rotation (/ OQPSK delay) itself
     int mm_rot = 0, mm_oqpsk = 0;
     void stage_mm(float2 *mmin, long n, int L, int nseg, int cur, int nxt, int8_t *sdst, bool strict);
@@ -91,7 +94,6 @@ class Demod
     cudaStream_t copy_stream = nullptr;
     struct Prefetch { const void *ptr = nullptr; long n = 0; int buf = 0; bool valid = false; cudaEvent_t done = nullptr; long seq = 0; } pf[2];
     long pf_seq = 0;
-    int pf_next_buf = 0;
     DevBuf<float2> bufA, bufB, agc_dump, fir_dump, slots, sym_out;
     DevBuf<int8_t> soft;
     DevBuf<Affine3> tile_map3;     // clamp pass (silent input): per-tile maps with the max_gain clamp
@@ -101,7 +103,6 @@ class Demod
     DevBuf<int> agc_need;          // [2] raised by the fast pass when a range cannot prove its seed
     unsigned agc_epoch = 0;
     int fir_ctas = 0;              // resident k_agc_fir_w CTAs on the device
-    bool fir_bulk = false;         // B200_FIR_BULK=1: the bulk-copy (TMA) variant of the raw prefetch
     int fir_warps = 0;             // ... and their warps: one range of tiles each (one wave)
     // front-end resampler (RationalResamplerBlock) / iq_swap pass
     bool resamp = false;
@@ -142,7 +143,6 @@ class Demod
     DemodDevState *h_state = nullptr; // pinned snapshot for stats
     cudaEvent_t ev[4];
     int Wc, Wm, Gc = 0, Gm = 0, seg_cap_threads; // warm-up lengths, gear-shift parts of them
-    int seg_ctas = 3; // resident CTAs of the loop kernels per SM the segment count aims at
     // pm_demod / freq_shift
     bool pm = false, pm_after = false;   // PMDemodModule's chain; its resampler sits behind the PLL ("resample_after_pll")
     int Wp = 0;                          // carrier PLL warm-up

@@ -101,7 +101,6 @@ def main():
             r.get("chain_costas", {}).get("max", 0), r["chain_mm"].get("gt1e5", -1), r["chain_mm"].get("max", -1), r.get("chain_soft"),
             cj["repairs"], cj["costas_unconv"], cj["mm_unconv"]), flush=True)
         g.close()
-    res["env"] = {k: v for k, v in os.environ.items() if k.startswith("B200_")}
     os.makedirs(os.path.dirname(out_path) or ".", exist_ok=True)
     with open(out_path, "w") as f:
         json.dump(res, f, indent=1)

@@ -21,7 +21,7 @@ for name in sys.argv[2:] or ["bpsk_half"]:
     sps = n / sy.size
     top = np.argsort(-d)[:2000]
     big = np.sort(top[d[top] > 1.5e-2])
-    print(name, "L", L, "symbols >1.5e-2:", big.size, "max %.3e" % d.max(), "tol env", os.environ.get("B200_MM_TOL"))
+    print(name, "L", L, "symbols >1.5e-2:", big.size, "max %.3e" % d.max())
     # cluster the big deviations into events
     ev = []
     for i in big:

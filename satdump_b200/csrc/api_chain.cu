@@ -70,7 +70,7 @@ struct Chain
                     stash_frames(); // the old stream's decoded frames stay pullable
                     f->reset();
                 }
-                f->push_device(src, nb);
+                f->push(src, nb, cudaMemcpyDeviceToDevice);
                 f->process();
                 DeviceGuard g(f->cfg.device);
                 B200_CUDA(cudaEventRecord(e1, f->stream));
@@ -340,7 +340,7 @@ int b200_chain_last_timing(b200_chain *h, float *ms, int n)
         ms[4] = c.f->t_vit;
         ms[5] = c.f->t_frames;
         ms[0] = ms[1] + ms[2] + ms[3] + ms[4] + ms[5];
-        ms[6] = c.f->t_vit_main;               // k_vit_main alone (sum over its launches in the last push)
+        ms[6] = c.f->t_vit_main;               // k_vit_acs3 alone (sum over its launches in the last push)
         ms[7] = (float)c.f->last_main_chunks;  // chunks those launches decoded
         ms[8] = c.t_total;                     // CUDA-event time from the start of the push (before any H2D) to the last kernel
     });

@@ -51,6 +51,15 @@ Fec::Fec(const b200_fec_cfg &c) : cfg(c)
     B200_REQUIRE(c.kind == B200_FEC_METOP || c.kind == B200_FEC_CCSDS || c.kind == B200_FEC_SIMPLE, B200_EINVAL, "unknown decoder kind %d", c.kind);
     B200_REQUIRE(c.max_soft >= 65536, B200_EINVAL, "max_soft must be >= 65536");
     memset(&geom, 0, sizeof(geom));
+    if (c.kind != B200_FEC_METOP) {
+        B200_REQUIRE(c.cadu_size >= 64 && c.cadu_size <= 65536, B200_EINVAL, "cadu_size out of range");
+        B200_REQUIRE(c.cadu_size % 8 == 0, B200_EINVAL, "cadu_size must be a multiple of 8 (frame padding is not built)");
+        B200_REQUIRE(c.rs_i >= 0 && c.rs_i <= RS_MAX_I, B200_EINVAL, "rs_i out of range (0..%d)", RS_MAX_I);
+        B200_REQUIRE(c.rs_i == 0 || c.cadu_size / 8 >= 4 + 255 * c.rs_i, B200_EINVAL, "cadu_size too small for rs_i interleaved codewords");
+        B200_REQUIRE(c.rs_fill_bytes <= 0, B200_EINVAL, "rs_fill_bytes (shortened codes) is not built");
+        if (cfg.asm_sync == 0)
+            cfg.asm_sync = 0x1ACFFC1D;
+    }
     if (c.kind == B200_FEC_METOP) {
         // module_metop_ahrpt_decoder.cpp:10,17-25: 16384-byte chunks, r=3/4, phases {0,90}, deframer SYNCED threshold 18, RS223 I=4
         geom.rate34 = 1;
@@ -71,11 +80,6 @@ Fec::Fec(const b200_fec_cfg &c) : cfg(c)
         spec_steps = VIT_SPEC_STEPS_34;
     } else if (c.kind == B200_FEC_SIMPLE) {
         // module_ccsds_simple_psk_decoder.cpp:19-98: one loop iteration = cadu_size soft bytes -> cadu_size bits
-        B200_REQUIRE(c.cadu_size >= 64 && c.cadu_size <= 65536, B200_EINVAL, "cadu_size out of range");
-        B200_REQUIRE(c.cadu_size % 8 == 0, B200_EINVAL, "cadu_size must be a multiple of 8 (frame padding is not built)");
-        B200_REQUIRE(c.rs_i >= 0 && c.rs_i <= RS_MAX_I, B200_EINVAL, "rs_i out of range (0..%d)", RS_MAX_I);
-        B200_REQUIRE(c.rs_i == 0 || c.cadu_size / 8 >= 4 + 255 * c.rs_i, B200_EINVAL, "cadu_size too small for rs_i interleaved codewords");
-        B200_REQUIRE(c.rs_fill_bytes <= 0, B200_EINVAL, "rs_fill_bytes (shortened codes) is not built");
         B200_REQUIRE(c.constellation == B200_BPSK || c.constellation == B200_QPSK, B200_EINVAL, "CCSDS Simple PSK Decoder : invalid constellation type!");
         geom.rate34 = 0;
         geom.chunk = c.cadu_size;
@@ -83,15 +87,8 @@ Fec::Fec(const b200_fec_cfg &c) : cfg(c)
         nphases = 1; ph0 = ph1 = 0; nswap = 1;
         st_synced = 12;
         spec_steps = 0;
-        if (cfg.asm_sync == 0)
-            cfg.asm_sync = 0x1ACFFC1D;
     } else {
         // module_ccsds_conv_concat_decoder.cpp:16-131
-        B200_REQUIRE(c.cadu_size >= 64 && c.cadu_size <= 65536, B200_EINVAL, "cadu_size out of range");
-        B200_REQUIRE(c.cadu_size % 8 == 0, B200_EINVAL, "cadu_size must be a multiple of 8 (frame padding is not built)");
-        B200_REQUIRE(c.rs_i >= 0 && c.rs_i <= RS_MAX_I, B200_EINVAL, "rs_i out of range (0..%d)", RS_MAX_I);
-        B200_REQUIRE(c.rs_i == 0 || c.cadu_size / 8 >= 4 + 255 * c.rs_i, B200_EINVAL, "cadu_size too small for rs_i interleaved codewords");
-        B200_REQUIRE(c.rs_fill_bytes <= 0, B200_EINVAL, "rs_fill_bytes (shortened codes) is not built");
         geom.rate34 = 0;
         geom.chunk = std::max(c.cadu_size, 8192);
         B200_REQUIRE(geom.chunk % 2 == 0, B200_EINVAL, "chunk size must be even");
@@ -116,8 +113,6 @@ Fec::Fec(const b200_fec_cfg &c) : cfg(c)
         nswap = c.constellation == B200_OQPSK ? 2 : 1;
         st_synced = 12;
         spec_steps = VIT_SPEC_STEPS_12;
-        if (cfg.asm_sync == 0)
-            cfg.asm_sync = 0x1ACFFC1D;
     }
     geom.dec_stride = (geom.F + 6 + 7) & ~7;
     geom.bit_words = (geom.F + 31) / 32 + 1;
@@ -185,24 +180,9 @@ Fec::Fec(const b200_fec_cfg &c) : cfg(c)
     RsTables T;
     build_rs_tables(T);
     B200_CUDA(cudaMemcpyAsync(tables.p, &T, sizeof(T), cudaMemcpyHostToDevice, stream));
-    fifo.zero(stream);
     rec.zero(stream);
-    if (punc) {
-        bdep.zero(stream);   // (the reference's member array: zero-initialised by the harness; never cleared afterwards)
-        vitbuf.zero(stream);
-    }
-    h_dstate[0].state = 2;
-    h_dstate[0].inversion = h_dstate[0].good = h_dstate[0].bad = 0;
-    h_dstate[0].pos = 32; // the FIFO starts with 32 zero bits = the deframer's empty shifter
-    h_dstate[0].frame_pay = -1;
-    B200_CUDA(cudaMemcpyAsync(dstate.p, h_dstate, sizeof(DefrState), cudaMemcpyHostToDevice, stream));
-    if (simple) {
-        h_dstate2 = h_dstate[0];
-        fifo2.zero(stream);
-        slice_carry.zero(stream);
-        B200_CUDA(cudaMemcpyAsync(dstate2.p, h_dstate, sizeof(DefrState), cudaMemcpyHostToDevice, stream));
-    }
-    const int fr_smem = (int)sizeof(RsTables) + ((cadu_bytes + 15) & ~15) + RS_MAX_I * 704;
+    start_stream(fifo.n * sizeof(uint32_t));
+    fr_smem = (int)sizeof(RsTables) + ((cadu_bytes + 15) & ~15) + RS_MAX_I * 704;
     B200_CUDA(cudaFuncSetAttribute(k_frames, cudaFuncAttributeMaxDynamicSharedMemorySize, fr_smem));
     B200_CUDA(cudaStreamSynchronize(stream));
 }
@@ -225,72 +205,73 @@ Fec::~Fec()
         cudaStreamDestroy(stream);
 }
 
-void Fec::push_host(const int8_t *h, long n)
+void Fec::push(const int8_t *src, long n, cudaMemcpyKind kind)
 {
     B200_REQUIRE(n <= append_room(), B200_ESTATE, "push of %ld soft bytes exceeds the FIFO room %ld (max_soft too small)", n, append_room());
     DeviceGuard g(cfg.device);
-    B200_CUDA(cudaMemcpyAsync(append_ptr(), h, n, cudaMemcpyHostToDevice, stream));
+    B200_CUDA(cudaMemcpyAsync(append_ptr(), src, n, kind, stream));
     commit(n);
     process();
 }
-void Fec::push_device(const int8_t *d, long n)
-{
-    B200_REQUIRE(n <= append_room(), B200_ESTATE, "push of %ld soft bytes exceeds the FIFO room %ld (max_soft too small)", n, append_room());
-    DeviceGuard g(cfg.device);
-    B200_CUDA(cudaMemcpyAsync(append_ptr(), d, n, cudaMemcpyDeviceToDevice, stream));
-    commit(n);
-    process();
-}
-
-constexpr int ACS_DEC_MODE = 0; // decision store of k_vit_acs3: lane 0 writes each step's two ballot words to a shared-memory row (measured fastest: tests/tools/bench_acs.cu)
 
 struct OutChunk { long soft_chunk; int next_start, enc_tail, invalid_after, state_after; VitIdleState idle_st; };
 
-// Optimistic parallel decode of n consecutive decoder windows (chunks c .. c+n-1 of `src`, f.geom.chunk bytes apart) into chunk_bits[out_base ..]:
-// start-state speculation, ACS, parallel chainback (+ checks and serial fallback), BER counters, and the redo rounds for chunks whose
-// speculated start state was wrong. Leaves the per-chunk records in f.h_rec[0 .. n).
-static void decode_range(Fec &f, const int8_t *src, long c, int n, long out_base)
+constexpr int WPB = 4; // warps per block of the one-warp-per-chunk kernels (k_vit_acs3 indexes its warps by blockIdx.x * 4)
+
+// An adaptive window follows the channel: many misses in a launch (> 2 % of its chunks) double it up to `cap`; 32 launches in a row
+// with almost none (< 0.2 %) halve it back towards `base`. It shrinks slowly because one doubling squares the miss probability, so
+// the shorter window would fail again at once on the same channel.
+static void adapt_window(int &win, int &clean, double miss_frac, int base, int cap)
 {
-    B200_CUDA(cudaMemcpyAsync(f.start_state.p, &f.main_next_start, sizeof(int), cudaMemcpyHostToDevice, f.stream));
-    const int wpb = 4, nb_main = (n + wpb - 1) / wpb;
-    if (n > 1) {
-        k_vit_spec<<<(n - 1 + wpb - 1) / wpb, 32 * wpb, 0, f.stream>>>(src, c, n, f.geom, f.hyp, f.spec_steps, f.start_state.p);
-        f.launches++;
+    if (miss_frac > 0.02) {
+        win = std::min(cap, win * 2);
+        clean = 0;
+    } else if (miss_frac < 0.002 && ++clean >= 32) {
+        win = std::max(base, win / 2);
+        clean = 0;
     }
+}
+
+// One decode pass: ACS, parallel chainback (+ check and serial fallback) and BER counters of `n` chunks of the range of `nrange`
+// chunks at c of `src` (all of them, or the ones in `qlist`; the BER check runs on `nber` chunks, or on the ones in `ber_list`). The
+// records of the whole range come back to f.h_rec. Returns the number of chunks chained back serially.
+static int decode_pass(Fec &f, const int8_t *src, long c, int nrange, long out_base, int n, const int *qlist, int nber, const int *ber_list)
+{
     B200_CUDA(cudaEventRecord(f.evm[0], f.stream));
-    k_vit_acs3<true, ACS_DEC_MODE><<<nb_main, 32 * wpb, 0, f.stream>>>(src, c, n, f.geom, f.hyp, f.start_state.p, f.dec.p, f.rec.p, nullptr);
+    k_vit_acs3<<<(n + WPB - 1) / WPB, 32 * WPB, 0, f.stream>>>(src, c, n, f.geom, f.hyp, f.start_state.p, f.dec.p, f.rec.p, qlist);
     B200_CUDA(cudaEventRecord(f.evm[1], f.stream));
-    {
-        const long nthr = (long)n * f.tb_blocks;
-        B200_CUDA(cudaMemsetAsync(f.tb_list.p, 0, sizeof(int), f.stream));
-        k_vit_tb<<<(unsigned)((nthr + 127) / 128), 128, 0, f.stream>>>(n, f.tb_blocks, f.geom, f.dec.p, f.chunk_bits.p, out_base, f.rec.p, f.tb_edges.p, nullptr, f.tb_overlap);
-        k_vit_tb_check<<<(n + 255) / 256, 256, 0, f.stream>>>(n, f.tb_blocks, f.tb_edges.p, f.tb_list.p, n, nullptr);
-        k_vit_tb_serial<<<(n + 127) / 128, 128, 0, f.stream>>>(f.tb_list.p, n, f.geom, f.dec.p, f.chunk_bits.p, out_base, f.rec.p); // (threads beyond the list return at once)
-        f.launches += 3;
-    }
-    k_vit_ber<<<nb_main, 32 * wpb, 0, f.stream>>>(src, c, n, f.geom, f.hyp, f.chunk_bits.p, out_base, f.enc_state, f.rec.p, nullptr);
-    f.launches += 2;
-    B200_CUDA(cudaMemcpyAsync(f.h_rec, f.rec.p, sizeof(VitRec) * n, cudaMemcpyDeviceToHost, f.stream));
+    const long nthr = (long)n * f.tb_blocks;
+    B200_CUDA(cudaMemsetAsync(f.tb_list.p, 0, sizeof(int), f.stream));
+    k_vit_tb<<<(unsigned)((nthr + 127) / 128), 128, 0, f.stream>>>(n, f.tb_blocks, f.geom, f.dec.p, f.chunk_bits.p, out_base, f.rec.p, f.tb_edges.p, qlist, f.tb_overlap);
+    k_vit_tb_check<<<(n + 255) / 256, 256, 0, f.stream>>>(n, f.tb_blocks, f.tb_edges.p, f.tb_list.p, nrange, qlist);
+    k_vit_tb_serial<<<(n + 127) / 128, 128, 0, f.stream>>>(f.tb_list.p, nrange, f.geom, f.dec.p, f.chunk_bits.p, out_base, f.rec.p); // (threads beyond the list return at once)
+    k_vit_ber<<<(nber + WPB - 1) / WPB, 32 * WPB, 0, f.stream>>>(src, c, nber, f.geom, f.hyp, f.chunk_bits.p, out_base, f.enc_state, f.rec.p, ber_list);
+    f.launches += 5;
+    B200_CUDA(cudaMemcpyAsync(f.h_rec, f.rec.p, sizeof(VitRec) * nrange, cudaMemcpyDeviceToHost, f.stream));
     int tb_redone = 0;
     B200_CUDA(cudaMemcpyAsync(&tb_redone, f.tb_list.p, sizeof(int), cudaMemcpyDeviceToHost, f.stream));
     B200_CUDA(cudaStreamSynchronize(f.stream));
     f.tb_serial_total += tb_redone;
-    if (n > 64) { // the chainback warm-up follows the channel like the speculation window does
-        const double frac = (double)tb_redone / (double)n;
-        if (frac > 0.02) {
-            f.tb_overlap = std::min(TB_OVERLAP_MAX, f.tb_overlap * 2);
-            f.tb_clean = 0;
-        } else if (frac < 0.002 && ++f.tb_clean >= 32) { // (slowly back: one doubling squares the miss probability, so the
-            f.tb_overlap = std::max(TB_OVERLAP, f.tb_overlap / 2); //  shorter window would fail again at once on the same channel)
-            f.tb_clean = 0;
-        }
+    float ms = 0;
+    cudaEventElapsedTime(&ms, f.evm[0], f.evm[1]);
+    f.t_vit_main += ms;
+    return tb_redone;
+}
+
+// Optimistic parallel decode of n consecutive decoder windows (chunks c .. c+n-1 of `src`, f.geom.chunk bytes apart) into chunk_bits[out_base ..]:
+// start-state speculation, one decode pass, and the redo rounds for chunks whose speculated start state was wrong. Leaves the per-chunk
+// records in f.h_rec[0 .. n).
+static void decode_range(Fec &f, const int8_t *src, long c, int n, long out_base)
+{
+    B200_CUDA(cudaMemcpyAsync(f.start_state.p, &f.main_next_start, sizeof(int), cudaMemcpyHostToDevice, f.stream));
+    if (n > 1) {
+        k_vit_spec<<<(n - 1 + WPB - 1) / WPB, 32 * WPB, 0, f.stream>>>(src, c, n, f.geom, f.hyp, f.spec_steps, f.start_state.p);
+        f.launches++;
     }
-    {
-        float ms = 0;
-        cudaEventElapsedTime(&ms, f.evm[0], f.evm[1]);
-        f.t_vit_main += ms;
-        f.last_main_chunks += n;
-    }
+    const int tb_redone = decode_pass(f, src, c, n, out_base, n, nullptr, n, nullptr);
+    f.last_main_chunks += n;
+    if (n > 64) // the chainback warm-up follows the channel like the speculation window does
+        adapt_window(f.tb_overlap, f.tb_clean, (double)tb_redone / (double)n, TB_OVERLAP, TB_OVERLAP_MAX);
     // Start states that were speculated wrong (k_vit_spec: common at low SNR, where 768 steps do not always pin the state): those
     // chunks alone are decoded again from the state their predecessor really left. A chunk's end state almost never depends on its
     // start state, so one round normally settles it; a round that changes a successor's start state is followed by another.
@@ -301,19 +282,9 @@ static void decode_range(Fec &f, const int8_t *src, long c, int n, long out_base
                 f.h_redo.push_back(i);
                 f.h_start[i] = f.h_rec[i - 1].next_start;
             }
-        if (round == 0 && n > 64) {
-            // the speculation window follows the channel: many wrong guesses (low SNR: the survivors of 768 steps have not all
-            // merged) -> twice the window for the next launch; almost none -> back towards the default
-            const double frac = (double)f.h_redo.size() / (double)n;
-            const int base = f.geom.rate34 ? VIT_SPEC_STEPS_34 : VIT_SPEC_STEPS_12, top = (f.geom.F / 32) * 32;
-            if (frac > 0.02) {
-                f.spec_steps = std::min(top, f.spec_steps * 2);
-                f.spec_clean = 0;
-            } else if (frac < 0.002 && ++f.spec_clean >= 32) {
-                f.spec_steps = std::max(base, f.spec_steps / 2);
-                f.spec_clean = 0;
-            }
-        }
+        if (round == 0 && n > 64) // wrong guesses: the survivors of the speculation window had not all merged (low SNR)
+            adapt_window(f.spec_steps, f.spec_clean, (double)f.h_redo.size() / (double)n, f.geom.rate34 ? VIT_SPEC_STEPS_34 : VIT_SPEC_STEPS_12,
+                         (f.geom.F / 32) * 32);
         if (f.h_redo.empty())
             break;
         const int m = (int)f.h_redo.size();
@@ -331,23 +302,7 @@ static void decode_range(Fec &f, const int8_t *src, long c, int n, long out_base
             B200_CUDA(cudaMemcpyAsync(f.start_state.p + i, &f.h_start[i], sizeof(int), cudaMemcpyHostToDevice, f.stream));
         B200_CUDA(cudaMemcpyAsync(f.redo_list.p, f.h_redo.data(), sizeof(int) * m, cudaMemcpyHostToDevice, f.stream));
         B200_CUDA(cudaMemcpyAsync(f.redo_list.p + n, f.h_redo_ber.data(), sizeof(int) * mb, cudaMemcpyHostToDevice, f.stream));
-        B200_CUDA(cudaEventRecord(f.evm[0], f.stream));
-        k_vit_acs3<true, ACS_DEC_MODE><<<(m + wpb - 1) / wpb, 32 * wpb, 0, f.stream>>>(src, c, m, f.geom, f.hyp, f.start_state.p, f.dec.p, f.rec.p, f.redo_list.p);
-        B200_CUDA(cudaEventRecord(f.evm[1], f.stream));
-        const long nthr = (long)m * f.tb_blocks;
-        B200_CUDA(cudaMemsetAsync(f.tb_list.p, 0, sizeof(int), f.stream));
-        k_vit_tb<<<(unsigned)((nthr + 127) / 128), 128, 0, f.stream>>>(m, f.tb_blocks, f.geom, f.dec.p, f.chunk_bits.p, out_base, f.rec.p, f.tb_edges.p, f.redo_list.p, f.tb_overlap);
-        k_vit_tb_check<<<(m + 255) / 256, 256, 0, f.stream>>>(m, f.tb_blocks, f.tb_edges.p, f.tb_list.p, n, f.redo_list.p);
-        k_vit_tb_serial<<<(m + 127) / 128, 128, 0, f.stream>>>(f.tb_list.p, n, f.geom, f.dec.p, f.chunk_bits.p, out_base, f.rec.p);
-        k_vit_ber<<<(mb + wpb - 1) / wpb, 32 * wpb, 0, f.stream>>>(src, c, mb, f.geom, f.hyp, f.chunk_bits.p, out_base, f.enc_state, f.rec.p, f.redo_list.p + n);
-        f.launches += 5;
-        B200_CUDA(cudaMemcpyAsync(f.h_rec, f.rec.p, sizeof(VitRec) * n, cudaMemcpyDeviceToHost, f.stream));
-        B200_CUDA(cudaMemcpyAsync(&tb_redone, f.tb_list.p, sizeof(int), cudaMemcpyDeviceToHost, f.stream));
-        B200_CUDA(cudaStreamSynchronize(f.stream));
-        f.tb_serial_total += tb_redone;
-        float ms = 0;
-        cudaEventElapsedTime(&ms, f.evm[0], f.evm[1]);
-        f.t_vit_main += ms;
+        decode_pass(f, src, c, n, out_base, m, f.redo_list.p, mb, f.redo_list.p + n);
     }
 }
 
@@ -372,7 +327,6 @@ static void viterbi_segment(Fec &f, long c0, long nch, std::vector<OutChunk> &ou
                 B200_CUDA(cudaStreamSynchronize(f.stream));
                 *f.h_idle = f.h_idle2->o;
                 if (f.h_idle2->fallback_chunk >= 0) {
-                    f.idle_fallbacks++;
                     const long c2 = c + f.h_idle2->fallback_chunk;
                     k_vit_idle<<<1, 32, 0, f.stream>>>(f.softbuf.p, c2, (int)(nch - c2), f.geom, f.nswap, f.nphases, f.ph0, f.ph1, f.cfg.ber_thresold,
                                                       f.h_idle2->o.st, f.idle_dec.p, f.idle_out.p);
@@ -573,7 +527,6 @@ void Fec::deframe_and_rs(long new_bits)
         fc.rs_nroots = cfg.rs_type == 1 ? 16 : 32;
         fc.rs_fcr = cfg.rs_type == 1 ? 120 : 112;
         fc.sync = cfg.asm_sync;
-        const int fr_smem = (int)sizeof(RsTables) + ((cadu_bytes + 15) & ~15) + RS_MAX_I * 704;
         const bool filter = cfg.rs_usecheck && cfg.rs_i > 0;
         uint8_t *dst = filter ? frames_tmp.p : frames_out.p + out_frames * cadu_bytes;
         k_frames<<<std::min(nf, 132 * 8), 256, fr_smem, stream>>>(fifo.p, frames.p, nf, fc, tables.p, dst, rs_err.p);
@@ -610,18 +563,18 @@ void Fec::deframe_and_rs(long new_bits)
     defr_state_now = h_dstate->state;
 }
 
-// back to the state of a freshly created decoder (new stream), keeping all allocations
-void Fec::reset()
+// The state a new stream starts from: the lock machines, the punctured decoder's sliding buffer and the deframers (the FIFO starts
+// with 32 zero bits = the deframer's empty shifter; the first `fifo_bytes` of each bit FIFO are cleared). The statistics and the
+// adaptive windows (spec_steps, tb_overlap) carry over.
+void Fec::start_stream(size_t fifo_bytes)
 {
-    DeviceGuard g(cfg.device);
-    B200_CUDA(cudaStreamSynchronize(stream));
     soft_have = 0;
     fifo_bits = 32;
     vit_state = 0; invalid = 0; main_next_start = -1; enc_state = 0; nrzm_last = 0; nosync_runs = 0;
     in_buffer = 0; changing_shift = 0; is_first = got_extra = false; buf_value = 128; test_bit_len = 0; pdec_start = -1;
     if (punc) {
-        B200_CUDA(cudaMemsetAsync(bdep.p, 0, bdep.n, stream));
-        B200_CUDA(cudaMemsetAsync(vitbuf.p, 0, vitbuf.n, stream));
+        bdep.zero(stream);   // (the reference's member array: zero-initialised by the harness; never cleared afterwards)
+        vitbuf.zero(stream);
     }
     hyp = VitHyp{0, 0, 0};
     idle_st = VitIdleState{-1, 0};
@@ -629,7 +582,7 @@ void Fec::reset()
     defr_state_now = 2;
     out_frames = 0;
     last_bits0 = last_nbits = 0;
-    B200_CUDA(cudaMemsetAsync(fifo.p, 0, 64, stream));
+    B200_CUDA(cudaMemsetAsync(fifo.p, 0, fifo_bytes, stream));
     h_dstate[0].state = 2;
     h_dstate[0].inversion = h_dstate[0].good = h_dstate[0].bad = 0;
     h_dstate[0].pos = 32;
@@ -641,10 +594,18 @@ void Fec::reset()
         defr_state2 = 2;
         slice_par = 0;
         total_chunks = 0; // the hard-decision stage knows the stream's very first chunk by this count
-        B200_CUDA(cudaMemsetAsync(fifo2.p, 0, 64, stream));
-        B200_CUDA(cudaMemsetAsync(slice_carry.p, 0, sizeof(int) * 4, stream));
+        B200_CUDA(cudaMemsetAsync(fifo2.p, 0, fifo_bytes, stream));
+        slice_carry.zero(stream);
         B200_CUDA(cudaMemcpyAsync(dstate2.p, h_dstate, sizeof(DefrState), cudaMemcpyHostToDevice, stream));
     }
+}
+
+// back to the state of a freshly created decoder (new stream), keeping all allocations
+void Fec::reset()
+{
+    DeviceGuard g(cfg.device);
+    B200_CUDA(cudaStreamSynchronize(stream));
+    start_stream(64);
     B200_CUDA(cudaStreamSynchronize(stream));
 }
 
@@ -658,8 +619,9 @@ void Fec::swap_unit()
     std::swap(defr_state_now, defr_state2);
 }
 
-// keep from the open frame's payload, or the 31 bits of shifter history
-void Fec::compact_fifo()
+// Compacts the bit FIFO: keeps from the open frame's payload, or the 31 bits of shifter history. `sync`: wait for the upload of the
+// pinned deframer mirror when one was queued (swap_unit() overwrites the mirror next).
+void Fec::compact_fifo(bool sync)
 {
     DefrState S = *h_dstate;
     long keep = S.frame_pay >= 0 ? S.frame_pay : S.pos - 31;
@@ -675,107 +637,44 @@ void Fec::compact_fifo()
         fifo_bits -= keep_al;
         *h_dstate = S;
         B200_CUDA(cudaMemcpyAsync(dstate.p, h_dstate, sizeof(DefrState), cudaMemcpyHostToDevice, stream));
-        B200_CUDA(cudaStreamSynchronize(stream)); // swap_unit() reuses the pinned mirror right away
+        if (sync)
+            B200_CUDA(cudaStreamSynchronize(stream));
     }
 }
 
-// ccsds_simple_psk_decoder: module_ccsds_simple_psk_decoder.cpp:144-296 over every complete cadu_size-byte chunk of the soft FIFO
-void Fec::process_simple()
+// Saves the main deframer (device state into its slot 1, host mirror) and the frame counters, for a rollback by rewind().
+Fec::Mark Fec::mark()
 {
-    DeviceGuard g(cfg.device);
-    const int n = geom.chunk;
-    const long nch = soft_have / n;
-    B200_REQUIRE(nch <= max_chunks, B200_ESTATE, "internal: too many chunks");
-    const bool qpsk = cfg.constellation == B200_QPSK, two = qpsk && !cfg.nrzm;
-    compact_fifo();
-    if (two) {
-        swap_unit();
-        compact_fifo();
-        swap_unit();
-    }
-    last_bits0 = fifo_bits;
-    last_nbits = 0;
-    t_frames = 0;
-    t_vit_main = 0;
-    last_main_chunks = 0;
-    B200_CUDA(cudaEventRecord(ev[0], stream));
-    if (nch > 0) {
-        B200_REQUIRE(((fifo_bits + nch * (long)n + 64) >> 5) + 2 < (long)fifo.n, B200_ESTATE, "internal: bit FIFO too small");
-        SliceCfg P;
-        P.n = n;
-        P.bit_words = geom.bit_words;
-        P.qpsk = qpsk;
-        P.nrzm = cfg.nrzm;
-        P.swap_iq = cfg.qpsk_swap_iq;
-        P.swap_diff = cfg.qpsk_swap_diff;
-        P.delay = cfg.oqpsk_delay;
-        const long words = nch * ((n + 31) / 32);
-        k_slice<<<(unsigned)std::min<long>((words + 255) / 256, 132 * 16), 256, 0, stream>>>(softbuf.p, nch, P, total_chunks, slice_carry.p + 2 * slice_par,
-                                                                                         slice_carry.p + 2 * (slice_par ^ 1), two ? chunk_bits2.p : nullptr,
-                                                                                         chunk_bits.p);
-        slice_par ^= 1;
-        launches++;
-        const bool bpsk_nrzm = !qpsk && cfg.nrzm;
-        // one pass over chunks [c0, c0 + m): second deframer first, then the main one (the order of one reference iteration)
-        auto run = [&](long c0, long m) {
-            int nfa = 0;
-            if (two) {
-                swap_unit();
-                k_bits_append<<<1024, 256, 0, stream>>>(chunk_bits2.p + c0 * geom.bit_words, m, n, geom.bit_words, 0, 0, fifo.p, fifo_bits);
-                launches++;
-                deframe_and_rs(m * (long)n);
-                nfa = last_nf;
-                swap_unit();
-            }
-            int last_raw = 0;
-            if (bpsk_nrzm) {
-                uint32_t w;
-                const int k = n - 1;
-                B200_CUDA(cudaMemcpyAsync(&w, chunk_bits.p + (c0 + m - 1) * geom.bit_words + (k >> 5), 4, cudaMemcpyDeviceToHost, stream));
-                B200_CUDA(cudaStreamSynchronize(stream));
-                last_raw = (w >> (31 - (k & 31))) & 1;
-            }
-            k_bits_append<<<1024, 256, 0, stream>>>(chunk_bits.p + c0 * geom.bit_words, m, n, geom.bit_words, bpsk_nrzm, nrzm_last, fifo.p, fifo_bits);
-            launches++;
-            deframe_and_rs(m * (long)n);
-            if (bpsk_nrzm)
-                nrzm_last = last_raw;
-            return std::make_pair(nfa, last_nf);
-        };
-        if (!two || nch == 1)
-            run(0, nch);
-        else {
-            // both deframers finding frames in the same call is all but impossible for a real signal; if it happens the
-            // reference's output order is per iteration, so redo this call one chunk at a time
-            B200_CUDA(cudaMemcpyAsync(dstate.p + 1, dstate.p, sizeof(DefrState), cudaMemcpyDeviceToDevice, stream));
-            B200_CUDA(cudaMemcpyAsync(dstate2.p + 1, dstate2.p, sizeof(DefrState), cudaMemcpyDeviceToDevice, stream));
-            const DefrState h0 = h_dstate[0], h1 = h_dstate2;
-            const long fb0 = fifo_bits, fb1 = fifo_bits2, of0 = out_frames, tf0 = total_frames, rc0 = rs_corrected, rf0 = rs_failed;
-            const int ds0 = defr_state_now, ds1 = defr_state2;
-            const auto r = run(0, nch);
-            if (r.first > 0 && r.second > 0) {
-                replays++;
-                B200_CUDA(cudaMemcpyAsync(dstate.p, dstate.p + 1, sizeof(DefrState), cudaMemcpyDeviceToDevice, stream));
-                B200_CUDA(cudaMemcpyAsync(dstate2.p, dstate2.p + 1, sizeof(DefrState), cudaMemcpyDeviceToDevice, stream));
-                h_dstate[0] = h0;
-                h_dstate2 = h1;
-                fifo_bits = fb0;
-                fifo_bits2 = fb1;
-                out_frames = of0;
-                total_frames = tf0;
-                rs_corrected = rc0;
-                rs_failed = rf0;
-                defr_state_now = ds0;
-                defr_state2 = ds1;
-                for (long c = 0; c < nch; c++)
-                    run(c, 1);
-            }
-        }
-        total_bits += nch * (long)n;
-        last_nbits += nch * (long)n;
-    }
-    total_chunks += nch;
-    const long used = nch * (long)n, left = soft_have - used;
+    B200_CUDA(cudaMemcpyAsync(dstate.p + 1, dstate.p, sizeof(DefrState), cudaMemcpyDeviceToDevice, stream));
+    return Mark{h_dstate[0], fifo_bits, out_frames, total_frames, rs_corrected, rs_failed, defr_state_now};
+}
+void Fec::rewind(const Mark &m)
+{
+    B200_CUDA(cudaMemcpyAsync(dstate.p, dstate.p + 1, sizeof(DefrState), cudaMemcpyDeviceToDevice, stream));
+    h_dstate[0] = m.h_dstate;
+    fifo_bits = m.fifo_bits;
+    out_frames = m.out_frames;
+    total_frames = m.total_frames;
+    rs_corrected = m.rs_corrected;
+    rs_failed = m.rs_failed;
+    defr_state_now = m.defr_state_now;
+}
+
+// the last of the `nbits` hard bits of chunk q of chunk_bits (NRZ-M decodes the next bit against it)
+int Fec::last_raw_bit(long q, int nbits)
+{
+    uint32_t w;
+    const int k = nbits - 1;
+    B200_CUDA(cudaMemcpyAsync(&w, chunk_bits.p + q * geom.bit_words + (k >> 5), 4, cudaMemcpyDeviceToHost, stream));
+    B200_CUDA(cudaStreamSynchronize(stream));
+    return (w >> (31 - (k & 31))) & 1;
+}
+
+// Keeps the undecoded tail of the soft FIFO behind the `used` bytes. The regions overlap only if left > used; chunks are large, so
+// then the copy goes through the head of the decision buffer.
+void Fec::keep_soft_tail(long used)
+{
+    const long left = soft_have - used;
     if (used > 0 && left > 0) {
         if (left <= used)
             B200_CUDA(cudaMemcpyAsync(softbuf.p, softbuf.p + used, left, cudaMemcpyDeviceToDevice, stream));
@@ -785,70 +684,93 @@ void Fec::process_simple()
         }
     }
     soft_have = left;
-    B200_CUDA(cudaEventRecord(ev[1], stream));
-    B200_CUDA(cudaStreamSynchronize(stream));
-    B200_CUDA(cudaGetLastError());
-    cudaEventElapsedTime(&t_vit, ev[0], ev[1]);
-    t_vit -= t_frames;
 }
 
-void Fec::process()
+// ccsds_simple_psk_decoder: module_ccsds_simple_psk_decoder.cpp:144-296 over the nch complete cadu_size-byte chunks of the soft FIFO
+void Fec::decode_simple(long nch)
 {
-    if (cfg.kind == B200_FEC_SIMPLE)
-        return process_simple();
-    DeviceGuard g(cfg.device);
-    const long nch = soft_have / geom.chunk;
-    B200_REQUIRE(nch <= max_chunks, B200_ESTATE, "internal: too many chunks");
-    // (lazy, so that b200_fec_debug_bits can still read the previous push's bits until now)
-    // compact the bit FIFO: keep from the open frame's payload, or the 31 bits of shifter history
-    {
-        DefrState S = *h_dstate;
-        long keep = S.frame_pay >= 0 ? S.frame_pay : S.pos - 31;
-        keep = std::max<long>(0, std::min<long>(keep, fifo_bits));
-        const long keep_al = keep & ~31L;
-        if (keep_al > 0) {
-            const long nwords = ((fifo_bits - keep_al) + 31) / 32 + 1;
-            k_words_move<<<1, 1024, 0, stream>>>(fifo.p, fifo.p + keep_al / 32, nwords);
+    if (nch == 0)
+        return;
+    const int n = geom.chunk;
+    const bool qpsk = cfg.constellation == B200_QPSK, two = two_deframers();
+    B200_REQUIRE(((fifo_bits + nch * (long)n + 64) >> 5) + 2 < (long)fifo.n, B200_ESTATE, "internal: bit FIFO too small");
+    SliceCfg P;
+    P.n = n;
+    P.bit_words = geom.bit_words;
+    P.qpsk = qpsk;
+    P.nrzm = cfg.nrzm;
+    P.swap_iq = cfg.qpsk_swap_iq;
+    P.swap_diff = cfg.qpsk_swap_diff;
+    P.delay = cfg.oqpsk_delay;
+    const long words = nch * ((n + 31) / 32);
+    k_slice<<<(unsigned)std::min<long>((words + 255) / 256, 132 * 16), 256, 0, stream>>>(softbuf.p, nch, P, total_chunks, slice_carry.p + 2 * slice_par,
+                                                                                     slice_carry.p + 2 * (slice_par ^ 1), two ? chunk_bits2.p : nullptr,
+                                                                                     chunk_bits.p);
+    slice_par ^= 1;
+    launches++;
+    const bool bpsk_nrzm = !qpsk && cfg.nrzm;
+    // one pass over chunks [c0, c0 + m): second deframer first, then the main one (the order of one reference iteration)
+    auto run = [&](long c0, long m) {
+        int nfa = 0;
+        if (two) {
+            swap_unit();
+            k_bits_append<<<1024, 256, 0, stream>>>(chunk_bits2.p + c0 * geom.bit_words, m, n, geom.bit_words, 0, 0, fifo.p, fifo_bits);
             launches++;
-            S.pos -= keep_al;
-            if (S.frame_pay >= 0)
-                S.frame_pay -= keep_al;
-            fifo_bits -= keep_al;
-            *h_dstate = S;
-            B200_CUDA(cudaMemcpyAsync(dstate.p, h_dstate, sizeof(DefrState), cudaMemcpyHostToDevice, stream));
+            deframe_and_rs(m * (long)n);
+            nfa = last_nf;
+            swap_unit();
+        }
+        const int last_raw = bpsk_nrzm ? last_raw_bit(c0 + m - 1, n) : 0;
+        k_bits_append<<<1024, 256, 0, stream>>>(chunk_bits.p + c0 * geom.bit_words, m, n, geom.bit_words, bpsk_nrzm, nrzm_last, fifo.p, fifo_bits);
+        launches++;
+        deframe_and_rs(m * (long)n);
+        if (bpsk_nrzm)
+            nrzm_last = last_raw;
+        return std::make_pair(nfa, last_nf);
+    };
+    if (!two || nch == 1)
+        run(0, nch);
+    else {
+        // both deframers finding frames in the same call is all but impossible for a real signal; if it happens the
+        // reference's output order is per iteration, so redo this call one chunk at a time
+        const Mark m0 = mark();
+        B200_CUDA(cudaMemcpyAsync(dstate2.p + 1, dstate2.p, sizeof(DefrState), cudaMemcpyDeviceToDevice, stream));
+        const DefrState h1 = h_dstate2;
+        const long fb1 = fifo_bits2;
+        const int ds1 = defr_state2;
+        const auto r = run(0, nch);
+        if (r.first > 0 && r.second > 0) {
+            replays++;
+            rewind(m0);
+            B200_CUDA(cudaMemcpyAsync(dstate2.p, dstate2.p + 1, sizeof(DefrState), cudaMemcpyDeviceToDevice, stream));
+            h_dstate2 = h1;
+            fifo_bits2 = fb1;
+            defr_state2 = ds1;
+            for (long c = 0; c < nch; c++)
+                run(c, 1);
         }
     }
-    last_bits0 = fifo_bits;
-    last_nbits = 0;
-    t_frames = 0;
-    t_vit_main = 0;
-    last_main_chunks = 0;
-    B200_CUDA(cudaEventRecord(ev[0], stream));
-    float acc_frames_ms = 0;
+    total_bits += nch * (long)n;
+    last_nbits += nch * (long)n;
+}
+
+// metop_ahrpt_decoder / ccsds_conv_concat_decoder: Viterbi (or its depunctured form) -> NRZ-M -> deframer -> RS over the nch soft
+// chunks of the FIFO
+void Fec::decode_conv(long nch)
+{
     long c = 0;
     std::vector<OutChunk> outs;
     while (c < nch) {
-        // snapshot for the (rare) MetOp "deframer stuck in NOSYNC -> viterbi.reset()" rollback
-        B200_CUDA(cudaMemcpyAsync(dstate.p + 1, dstate.p, sizeof(DefrState), cudaMemcpyDeviceToDevice, stream));
-        const long fifo_bits0 = fifo_bits, out_frames0 = out_frames, total_frames0 = total_frames, rs_c0 = rs_corrected, rs_f0 = rs_failed;
-        const int nosync0 = nosync_runs;
-        const long seg_end = nch;
+        const Mark m0 = mark(); // for the (rare) MetOp "deframer stuck in NOSYNC -> viterbi.reset()" rollback
         if (punc)
-            punc_segment(*this, c, seg_end, outs);
+            punc_segment(*this, c, nch, outs);
         else
-            viterbi_segment(*this, c, seg_end, outs);
+            viterbi_segment(*this, c, nch, outs);
         const long nout = (long)outs.size();
-        long next_c = seg_end;
+        long next_c = nch;
         if (nout > 0) {
             B200_REQUIRE(((fifo_bits + nout * geom.F + 64) >> 5) + 2 < (long)fifo.n, B200_ESTATE, "internal: bit FIFO too small");
-            int last_raw = 0;
-            if (cfg.nrzm) {
-                uint32_t w;
-                const int k = geom.F - 1;
-                B200_CUDA(cudaMemcpyAsync(&w, chunk_bits.p + (nout - 1) * geom.bit_words + (k >> 5), 4, cudaMemcpyDeviceToHost, stream));
-                B200_CUDA(cudaStreamSynchronize(stream));
-                last_raw = (w >> (31 - (k & 31))) & 1;
-            }
+            const int last_raw = cfg.nrzm ? last_raw_bit(nout - 1, geom.F) : 0;
             k_bits_append<<<1024, 256, 0, stream>>>(chunk_bits.p, nout, geom.F, geom.bit_words, cfg.nrzm, nrzm_last, fifo.p, fifo_bits);
             launches++;
             deframe_and_rs(nout * (long)geom.F);
@@ -864,7 +786,7 @@ void Fec::process()
                     st = snap.state;
                 }
                 for (long k = 0; k < nout; k++) {
-                    const long end = fifo_bits0 + (k + 1) * (long)geom.F; // exclusive
+                    const long end = m0.fifo_bits + (k + 1) * (long)geom.F; // exclusive
                     while (ei < ne && h_events[ei].pos < end)
                         st = h_events[ei++].state;
                     if (st == 2) {
@@ -885,12 +807,7 @@ void Fec::process()
                 // roll back to just after output chunk redo_from, with the Viterbi forced to IDLE
                 replays++;
                 const OutChunk &oc = outs[redo_from];
-                B200_CUDA(cudaMemcpyAsync(dstate.p, dstate.p + 1, sizeof(DefrState), cudaMemcpyDeviceToDevice, stream));
-                fifo_bits = fifo_bits0;
-                out_frames = out_frames0;
-                total_frames = total_frames0;
-                rs_corrected = rs_c0;
-                rs_failed = rs_f0;
+                rewind(m0);
                 deframe_and_rs((redo_from + 1) * (long)geom.F);
                 vit_state = 0;
                 main_next_start = oc.next_start;
@@ -899,7 +816,6 @@ void Fec::process()
                 invalid = oc.invalid_after;
                 nosync_runs = 0;
                 next_c = oc.soft_chunk + 1;
-                if (cfg.nrzm) { /* METOP has no NRZ-M */ }
                 total_bits += (redo_from + 1) * (long)geom.F;
                 last_nbits += (redo_from + 1) * (long)geom.F;
             } else {
@@ -910,29 +826,41 @@ void Fec::process()
                 total_bits += nout * (long)geom.F;
                 last_nbits += nout * (long)geom.F;
             }
-            (void)nosync0;
         }
         c = next_c;
     }
-    total_chunks += nch;
-    // keep the undecoded tail of the soft FIFO
-    const long used = nch * (long)geom.chunk, left = soft_have - used;
-    if (used > 0 && left > 0) {
-        // regions may overlap only if left > used; chunks are large, so copy through the head of the decision buffer when needed
-        if (left <= used)
-            B200_CUDA(cudaMemcpyAsync(softbuf.p, softbuf.p + used, left, cudaMemcpyDeviceToDevice, stream));
-        else {
-            B200_CUDA(cudaMemcpyAsync(dec.p, softbuf.p + used, left, cudaMemcpyDeviceToDevice, stream));
-            B200_CUDA(cudaMemcpyAsync(softbuf.p, dec.p, left, cudaMemcpyDeviceToDevice, stream));
-        }
+}
+
+void Fec::process()
+{
+    DeviceGuard g(cfg.device);
+    const long nch = soft_have / geom.chunk;
+    B200_REQUIRE(nch <= max_chunks, B200_ESTATE, "internal: too many chunks");
+    // (lazy, so that b200_fec_debug_bits can still read the previous push's bits until now)
+    const bool simple = cfg.kind == B200_FEC_SIMPLE;
+    compact_fifo(simple);
+    if (two_deframers()) {
+        swap_unit();
+        compact_fifo(true);
+        swap_unit();
     }
-    soft_have = left;
+    last_bits0 = fifo_bits;
+    last_nbits = 0;
+    t_frames = 0;
+    t_vit_main = 0;
+    last_main_chunks = 0;
+    B200_CUDA(cudaEventRecord(ev[0], stream));
+    if (simple)
+        decode_simple(nch);
+    else
+        decode_conv(nch);
+    total_chunks += nch;
+    keep_soft_tail(nch * (long)geom.chunk);
     B200_CUDA(cudaEventRecord(ev[1], stream));
     B200_CUDA(cudaStreamSynchronize(stream));
     B200_CUDA(cudaGetLastError());
     cudaEventElapsedTime(&t_vit, ev[0], ev[1]);
     t_vit -= t_frames; // ev[0]..ev[1] spans both stages
-    (void)acc_frames_ms;
 }
 
 long Fec::pull(uint8_t *host_out, long cap)
@@ -975,10 +903,6 @@ struct b200_fec
 {
     Fec *f;
 };
-namespace b200
-{
-Fec *fec_of(b200_fec *h) { return h->f; }
-}
 
 extern "C" {
 b200_fec *b200_fec_create(const b200_fec_cfg *cfg)
@@ -1001,14 +925,14 @@ int b200_fec_push_soft(b200_fec *h, const int8_t *host_soft, long n)
 {
     return guarded([&] {
         B200_REQUIRE(h && host_soft && n >= 0, B200_EINVAL, "bad argument");
-        h->f->push_host(host_soft, n);
+        h->f->push(host_soft, n, cudaMemcpyHostToDevice);
     });
 }
 int b200_fec_push_soft_device(b200_fec *h, const int8_t *dev_soft, long n)
 {
     return guarded([&] {
         B200_REQUIRE(h && dev_soft && n >= 0, B200_EINVAL, "bad argument");
-        h->f->push_device(dev_soft, n);
+        h->f->push(dev_soft, n, cudaMemcpyDeviceToDevice);
     });
 }
 int b200_fec_pull_frames(b200_fec *h, uint8_t *out, long cap, long *nbytes)

@@ -110,9 +110,6 @@ __device__ __forceinline__ int vit_symbols(const int8_t *__restrict__ c, int t, 
 }
 
 __device__ __forceinline__ int parity_u32(unsigned x) { return __popc(x) & 1; }
-
-// One warp: `nsteps` ACS steps starting at step t0. Lane i holds X[i] (xl) and X[i+32] (xh). Decisions (ballot words
-// D0: new state 2i chose predecessor i+32, D1: new state 2i+1 chose i+32) go to dec[2*(t-tdec0)] when dec != nullptr.
 #endif // B200_DEFINE_KERNELS
 struct AcsLane { int mask0, mask1; };
 #ifdef B200_DEFINE_KERNELS
@@ -246,52 +243,11 @@ __global__ void __launch_bounds__(128) k_vit_spec(const int8_t *__restrict__ sof
     if (lane == 0) start_state[w + 1] = st;
 }
 
-// ---------------------------------------------------------------- main decode, part 1: ACS (one warp per chunk)
 #endif // B200_DEFINE_KERNELS
 struct VitRec { int start_used, next_start, ber_errors, ber_total, enc_tail, end_state, pad1, pad2; };
 #ifdef B200_DEFINE_KERNELS
 
-// start_state[q]: >= 0 biased start (63 everywhere, 0 at that state), -1: unbiased all-31 (first call ever).
-// Writes the survivor decisions (two ballot words per trellis step) and the first-minimum end state.
-__global__ void __launch_bounds__(128) k_vit_acs(const int8_t *__restrict__ soft, long chunk0, int nchunks, VitGeom g, VitHyp h,
-                                                  const int *__restrict__ start_state, uint2 *__restrict__ dec, VitRec *__restrict__ rec)
-{
-    const int q = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (q >= nchunks) return;
-    const int8_t *c = soft + (chunk0 + q) * (long)g.chunk;
-    uint2 *d = dec + (long)q * g.dec_stride;
-    const Acs2Lane L = acs2_lane_consts(lane);
-    const int ss = start_state[q];
-    unsigned xl2, xh2, D0, D1;
-    acs2_init(ss, lane, xl2, xh2);
-    const int steps = g.F + 6;
-    for (int t0 = 0; t0 < steps; t0 += 32) {
-        // lane j prepares step t0+j (symbol fetch incl. rotate / soft->u8 / depuncture, then the 4-entry metric table)
-        const int tm = t0 + lane;
-        const unsigned mine = tm < steps ? metric_table(vit_symbols(c, tm, g, h, g.chunk, 128)) : 0u;
-        if (t0 + 32 <= steps) {
-#pragma unroll
-            for (int j = 0; j < 32; j++) {
-                acs2_step(__shfl_sync(0xffffffffu, mine, j), L, lane, xl2, xh2, D0, D1);
-                if (lane == 0) d[t0 + j] = make_uint2(D0, D1);
-            }
-        } else {
-            for (int j = 0; j < steps - t0; j++) {
-                acs2_step(__shfl_sync(0xffffffffu, mine, j), L, lane, xl2, xh2, D0, D1);
-                if (lane == 0) d[t0 + j] = make_uint2(D0, D1);
-            }
-        }
-    }
-    const int st = acs2_endstate(xl2, xh2, lane);
-    if (lane == 0) {
-        VitRec r = rec[q];
-        r.start_used = ss;
-        r.end_state = st;
-        rec[q] = r;
-    }
-}
-
-// ---------------------------------------------------------------- ACS, DPX form (production kernel)
+// ---------------------------------------------------------------- main decode, part 1: ACS, DPX form (one warp per chunk)
 // Same arithmetic as acs2_step with the metrics held as X << 8 in each 16-bit field (low byte 0): VIADD.16x2 adds per field modulo 2^16,
 // which IS the reference's uint8 wrap (volk_k7_r2_generic_fixed.h:108-111), so no mask is needed; VIMNMX.U16x2 with predicate outputs
 // returns the minima and both decisions in one instruction (min(Sh, Sl) prefers Sh on ties = the reference's "m0 >= m1 picks m1",
@@ -325,33 +281,6 @@ __device__ __forceinline__ void acs3_step(unsigned w, const Acs3Lane L, int lane
     xl2 = __byte_perm(a, 0u, L.selX);
     xh2 = __byte_perm(b, 0u, L.selX);
 }
-// the same step without the ballots: the lane's own two decisions as predicates (for the transposed decision store of k_vit_acs3)
-__device__ __forceinline__ void acs3_step_p(unsigned w, const Acs3Lane L, int lane, unsigned &xl2, unsigned &xh2, bool &p_lo, bool &p_hi)
-{
-    const unsigned mb = __byte_perm(w, 0u, L.selM);
-    const unsigned Ml = mb * 0xFFFF0001u + 0x3F000000u;
-    const unsigned Mh = mb * 0x0000FFFFu + 0x00003F00u;
-    const unsigned Sl = __vadd2(xl2, Ml), Sh = __vadd2(xh2, Mh);
-    unsigned Y = __vibmin_u16x2(Sh, Sl, &p_hi, &p_lo);
-    const unsigned mn2 = __reduce_min_sync(0xffffffffu, __vminu2(Y, __byte_perm(Y, 0u, 0x1032u)));
-    Y -= mn2;
-    const unsigned a = __shfl_sync(0xffffffffu, Y, lane >> 1);
-    const unsigned b = __shfl_sync(0xffffffffu, Y, (lane >> 1) + 16);
-    xl2 = __byte_perm(a, 0u, L.selX);
-    xh2 = __byte_perm(b, 0u, L.selX);
-}
-// 32 x 32 bit-matrix transpose across the warp: in: lane i holds row i; out: lane r holds column r (bit i = row i's bit r). Five
-// butterfly stages of one shuffle each.
-__device__ __forceinline__ unsigned warp_transpose32(unsigned x, int lane)
-{
-#pragma unroll
-    for (int sft = 16; sft >= 1; sft >>= 1) {
-        const unsigned m = sft == 16 ? 0x0000FFFFu : (sft == 8 ? 0x00FF00FFu : (sft == 4 ? 0x0F0F0F0Fu : (sft == 2 ? 0x33333333u : 0x55555555u)));
-        const unsigned y = __shfl_xor_sync(0xffffffffu, x, sft);
-        x = (lane & sft) ? ((x & ~m) | ((y & ~m) >> sft)) : ((x & m) | ((y & m) << sft));
-    }
-    return x;
-}
 __device__ __forceinline__ void acs3_init(int ss, int lane, unsigned &xl2, unsigned &xh2)
 {
     const unsigned l = ss < 0 ? 31u : (lane == ss ? 0u : 63u), h = ss < 0 ? 31u : (lane + 32 == ss ? 0u : 63u);
@@ -364,12 +293,12 @@ __device__ __forceinline__ int acs3_endstate(unsigned xl2, unsigned xh2, int lan
     return (int)(__reduce_min_sync(0xffffffffu, min(k0, k1)) & 63);
 }
 
-// One warp per chunk like k_vit_acs. Per batch of 32 trellis steps: every lane prepares the metric table word of one step (next
-// batch's symbol loads are issued one batch ahead), the 32 words are exchanged through shared memory (8 broadcast LDS.128 per lane
-// instead of one SHFL per step: the kernel is bound by the SM's shuffle / vote / reduce port, not by the ALUs), and the two decision
-// words of a step go to a per-warp shared-memory row (one STS by lane 0; DEC_SEL: kept by lane j in registers instead) that leaves
-// as one coalesced 256-byte store per 32 steps.
-template <bool MET_SMEM, int DEC_MODE> // DEC_MODE 0: STS row buffer, 1: lane j keeps step j (SEL), 2: per-lane bit accumulators + warp transpose
+// start_state[q]: >= 0 biased start (63 everywhere, 0 at that state), -1: unbiased all-31 (first call ever). Writes the survivor
+// decisions (two ballot words per trellis step) and the first-minimum end state. Per batch of 32 trellis steps: every lane prepares
+// the metric table word of one step (next batch's symbol loads are issued one batch ahead), the 32 words are exchanged through shared
+// memory (8 broadcast LDS.128 per lane instead of one SHFL per step: the kernel is bound by the SM's shuffle / vote / reduce port, not
+// by the ALUs), and the two decision words of a step go to a per-warp shared-memory row (one STS by lane 0) that leaves as one
+// coalesced 256-byte store per 32 steps.
 __global__ void __launch_bounds__(128) k_vit_acs3(const int8_t *__restrict__ soft, long chunk0, int nchunks, VitGeom g, VitHyp h,
                                                    const int *__restrict__ start_state, uint2 *__restrict__ dec, VitRec *__restrict__ rec,
                                                    const int *__restrict__ qlist)
@@ -395,45 +324,22 @@ __global__ void __launch_bounds__(128) k_vit_acs3(const int8_t *__restrict__ sof
         const int tn = t0 + 32 + lane;
         next = tn < steps ? metric_table(vit_symbols(c, tn, g, h, nlim, 128)) : 0u; // consumed one batch later
         uint2 *row = srow[wib][par];
-        unsigned k0 = 0, k1 = 0;
         if (t0 + 32 <= steps) {
             unsigned w[32];
-            if (MET_SMEM) {
-                smet[wib][par][lane] = mine;
-                __syncwarp();
+            smet[wib][par][lane] = mine;
+            __syncwarp();
 #pragma unroll
-                for (int v = 0; v < 8; v++) {
-                    const uint4 u = reinterpret_cast<const uint4 *>(smet[wib][par])[v];
-                    w[4 * v] = u.x; w[4 * v + 1] = u.y; w[4 * v + 2] = u.z; w[4 * v + 3] = u.w;
-                }
+            for (int v = 0; v < 8; v++) {
+                const uint4 u = reinterpret_cast<const uint4 *>(smet[wib][par])[v];
+                w[4 * v] = u.x; w[4 * v + 1] = u.y; w[4 * v + 2] = u.z; w[4 * v + 3] = u.w;
             }
-            if (DEC_MODE == 2) {
 #pragma unroll
-                for (int j = 0; j < 32; j++) {
-                    bool p_lo, p_hi;
-                    acs3_step_p(MET_SMEM ? w[j] : __shfl_sync(0xffffffffu, mine, j), L, lane, xl2, xh2, p_lo, p_hi);
-                    k0 = k0 * 2u + (p_lo ? 1u : 0u); // step j ends up at bit 31 - j
-                    k1 = k1 * 2u + (p_hi ? 1u : 0u);
-                }
-                k0 = warp_transpose32(k0, lane);     // lane r: the ballot word of step 31 - r
-                k1 = warp_transpose32(k1, lane);
-                d[t0 + 31 - lane] = make_uint2(k0, k1);
-            } else {
-#pragma unroll
-                for (int j = 0; j < 32; j++) {
-                    acs3_step(MET_SMEM ? w[j] : __shfl_sync(0xffffffffu, mine, j), L, lane, xl2, xh2, D0, D1);
-                    if (DEC_MODE == 1) {
-                        if (lane == j) { k0 = D0; k1 = D1; }
-                    } else if (lane == 0)
-                        row[j] = make_uint2(D0, D1);
-                }
-                if (DEC_MODE == 1)
-                    d[t0 + lane] = make_uint2(k0, k1);
-                else {
-                    __syncwarp();
-                    d[t0 + lane] = row[lane];
-                }
+            for (int j = 0; j < 32; j++) {
+                acs3_step(w[j], L, lane, xl2, xh2, D0, D1);
+                if (lane == 0) row[j] = make_uint2(D0, D1);
             }
+            __syncwarp();
+            d[t0 + lane] = row[lane];
         } else {
             const int nn = steps - t0;
             for (int j = 0; j < nn; j++) {

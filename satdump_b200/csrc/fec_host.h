@@ -21,19 +21,18 @@ class Fec
     int8_t *append_ptr() { return softbuf.p + soft_have; }
     long append_room() const { return (long)softbuf.n - soft_have; }
     void commit(long n) { soft_have += n; total_soft += n; }
-    void push_host(const int8_t *h, long n);
-    void push_device(const int8_t *d, long n);
+    void push(const int8_t *src, long n, cudaMemcpyKind kind); // append n soft bytes from host or device memory, then process()
     void process(); // decode every complete chunk in the FIFO
-    void process_simple(); // kind B200_FEC_SIMPLE: hard decisions -> deframer(s) -> RS
     long pull(uint8_t *host_out, long cap);
     void stats(b200_fec_stats *o);
 
     b200_fec_cfg cfg;
     VitGeom geom;
     int cadu_bytes, nphases, ph0, ph1, nswap, st_synced, spec_steps;
+    int fr_smem = 0; // dynamic shared memory of k_frames
     cudaStream_t stream = nullptr;
-    cudaEvent_t ev[3];
-    float t_vit = 0, t_frames = 0, t_vit_main = 0; // ms of the last process(): whole Viterbi stage, deframe+RS, k_vit_main alone
+    cudaEvent_t ev[2];
+    float t_vit = 0, t_frames = 0, t_vit_main = 0; // ms of the last process(): whole Viterbi stage, deframe+RS, k_vit_acs3 alone
     cudaEvent_t evm[2], evf[2];
     long last_main_chunks = 0;
     void reset();
@@ -72,7 +71,6 @@ class Fec
     DevBuf<VitIdleOut> idle_out;
     DevBuf<VitIdle2Out> idle2_out;
     VitIdle2Out *h_idle2 = nullptr;
-    long idle_fallbacks = 0;
     DevBuf<DefrState> dstate;
     DevBuf<DefrEvent> devents;
     DevBuf<FrameRec> frames;
@@ -86,8 +84,10 @@ class Fec
     DefrState h_dstate2{};
     long fifo_bits2 = 32;
     int defr_state2 = 2, slice_par = 0, last_nf = 0;
+    // QPSK without NRZ-M runs the second deframer
+    bool two_deframers() const { return cfg.kind == B200_FEC_SIMPLE && cfg.constellation == B200_QPSK && !cfg.nrzm; }
     void swap_unit();
-    void compact_fifo();
+    void compact_fifo(bool sync);
     // pinned host mirrors
     VitRec *h_rec = nullptr;
     VitIdleOut *h_idle = nullptr;
@@ -109,7 +109,15 @@ class Fec
     long total_soft = 0, total_chunks = 0, total_bits = 0, total_frames = 0, rs_corrected = 0, rs_failed = 0, replays = 0, launches = 0;
 
   private:
-    long decode_chunks(long c0, long nch, bool single_step);
+    // the main deframer and the frame counters at a point a pass may have to roll back to
+    struct Mark { DefrState h_dstate; long fifo_bits, out_frames, total_frames, rs_corrected, rs_failed; int defr_state_now; };
+    Mark mark();
+    void rewind(const Mark &m);
+    void start_stream(size_t fifo_bytes);
+    void decode_simple(long nch);
+    void decode_conv(long nch);
+    int last_raw_bit(long q, int nbits);
+    void keep_soft_tail(long used);
     void deframe_and_rs(long new_bits);
 };
 

@@ -75,13 +75,26 @@ def test_baseline_size_properties(built):
 
 
 def test_reset_starts_a_new_stream(built):
-    cfg, raw, _ = signal("metop_ahrpt", 21)
-    n = nsamples(raw, cfg)
-    ch = gpu_chain(cfg, n)
-    a = ch.push(raw).frames()
-    ch.reset()
-    b = ch.push(raw).frames()
-    assert a.shape[0] > 0 and np.array_equal(a, b)
+    """One decoder of each kind (MetOp, CCSDS r=1/2, punctured, two deframers, NRZ-M): reset() after an odd-length part of another
+    signal, i.e. mid-frame and mid-lock, and the next stream gives exactly the frames of a fresh chain."""
+    from satdump_b200 import capi
+    from tests.common import demod_kwargs
+    for name in ["metop_ahrpt", "bpsk_half", "qpsk_p34", "qpsk_simple", "bpsk_simple"]:
+        cfg, raw, _ = signal(name, 21)
+        _, other, _ = signal(name, 21, seed=2)
+        n = nsamples(raw, cfg)
+        per = 1 if cfg.fmt == "cf32" else 2
+
+        def chain():
+            return capi.Chain(capi.demod_cfg(max_batch=n, **demod_kwargs(cfg)), capi.fec_cfg_for(cfg, 2 * n))
+
+        want = chain().push(raw).frames()
+        ch = chain()
+        lead = (n // 2) | 1
+        assert ch.push(other[:lead * per]).frames().shape[0] > 0, name
+        ch.reset()
+        got = ch.push(raw).frames()
+        assert want.shape[0] > 0 and got.shape == want.shape and np.array_equal(got, want), name
 
 
 def test_prefetched_host_batches_equal_plain_pushes(built):

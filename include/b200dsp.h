@@ -15,6 +15,7 @@
  *   b200_fec_*     the decoder modules
  *                    plugins/noaa_metop_support/metop/module_metop_ahrpt_decoder.cpp:34-90      (kind METOP)
  *                    src-core/pipeline/modules/ccsds/module_ccsds_conv_concat_decoder.cpp:140-200 (kind CCSDS, r=1/2)
+ *                    src-core/pipeline/modules/ccsds/module_ccsds_ldpc_decoder.cpp:134-277       (kind LDPC, ldpc_rate "7/8")
  *   b200_chain_*   both modules joined the way Pipeline::run joins them with a byte FIFO
  *                    src-core/pipeline/pipeline_run.cpp:44-117 — here the int8 soft stream never leaves HBM.
  *   b200_demux_*   the step behind the decoder: CADUs -> CCSDS space packets
@@ -45,7 +46,7 @@ enum { B200_BPSK = 0, B200_QPSK = 1, B200_OQPSK = 2, B200_8PSK = 3, B200_NONE = 
 /* baseband_format (common/dsp/io/baseband_type.h:7-21) */
 enum { B200_CF32 = 0, B200_CS16 = 1, B200_CS8 = 2 };
 /* decoder kind */
-enum { B200_FEC_METOP = 0, B200_FEC_CCSDS = 1, B200_FEC_SIMPLE = 2 };
+enum { B200_FEC_METOP = 0, B200_FEC_CCSDS = 1, B200_FEC_SIMPLE = 2, B200_FEC_LDPC = 3 };
 /* debug stage ids for b200_demod_debug_stage */
 enum { B200_STAGE_AGC = 0, B200_STAGE_FIR = 1, B200_STAGE_COSTAS = 2, B200_STAGE_RESAMP = 3, B200_STAGE_DC = 4, B200_STAGE_MM = 5,
        B200_STAGE_PLL = 6 /* pm_demod: PLLCarrierTrackingBlock output */, B200_STAGE_PM = 7 /* pm_demod: PMToBPSK output */ };
@@ -122,6 +123,17 @@ typedef struct b200_fec_cfg
     int oqpsk_delay;          /* simple: "oqpsk_delay" (:29)                                          */
     int conv_rate;            /* ccsds: "conv_rate" (module_ccsds_conv_concat_decoder.cpp:33,99-117): 0 = "1/2" (Viterbi1_2); 2, 3, 5, 7 = "2/3",
                                  "3/4", "5/6", "7/8" (Viterbi_Depunc, common/codings/viterbi/viterbi_punc.cpp + depunc.h)           */
+    /* kind B200_FEC_LDPC = ccsds_ldpc_decoder (module_ccsds_ldpc_decoder.cpp:19-124): correlator on the 32-bit ASM 0x1ACFFC1D over
+       8192-soft-byte frames, phase fix, derandomiser ("derandomize"), CCSDS C2 (8176, 7154) LDPC decoder, 1024-byte CADUs.
+       "constellation": B200_BPSK / QPSK / OQPSK. Built: ldpc_rate 7. Device memory: about 7 bytes per max_soft byte (FIFO, fp32
+       correlator scores, their syncword indices, decoder input, CADUs), so max_soft = 2^30 (the limit) takes about 7 GiB.            */
+    int ldpc_rate;            /* 7 = "7/8" (C2). 1, 2, 4 = "1/2", "2/3", "4/5" (AR4JA): rejected                                         */
+    int ldpc_block_size;      /* "ldpc_block_size" of the AR4JA codes (not built)                                                         */
+    int ldpc_iterations;      /* "ldpc_iterations"                                                                                        */
+    int ldpc2;                /* "ldpc2" (the labrador decoder): rejected                                                                 */
+    int internal_stream;      /* "internal_stream": the 7136 info bits of every codeword go through BPSK_CCSDS_Deframer(internal_cadu_size,
+                                 internal_asm) and its frames are the output (cadu_bytes = internal_cadu_size / 8; no RS)               */
+    int internal_cadu_size;   /* "internal_cadu_size" bits, a multiple of 8 (frame padding is rejected); asm_sync carries "internal_asm"  */
 } b200_fec_cfg;
 
 typedef struct b200_demod_stats
@@ -155,6 +167,12 @@ typedef struct b200_fec_stats
     long tb_serial;           /* chunks whose parallel chainback blocks disagreed and were chained back serially (part of replays) */
     int spec_steps;           /* current length of the start-state speculation window (adapts to the channel) */
     int tb_overlap;           /* current warm-up length of the parallel chainback blocks (adapts to the channel) */
+    /* ccsds_ldpc_decoder (module stats keys, module_ccsds_ldpc_decoder.cpp:279-295), of the last frame decoded */
+    int correlator_lock;      /* "correlator_lock": the ASM was found at the expected place (pos 0); "lock_state" SYNCED / NOSYNC.
+                                 internal_stream: deframer_state above is "deframer_state" (deframer_lock = SYNCED)                   */
+    float correlator_corr;    /* "correlator_corr": the correlator's best score                                                       */
+    int ldpc_corr;            /* "ldpc_corr": info positions whose decoded bit differs from the sign of the input                     */
+    long ldpc_resyncs;        /* frames so far whose ASM was not at the expected place (the frame walk shifted)                       */
 } b200_fec_stats;
 
 typedef struct b200_demod b200_demod;
@@ -226,6 +244,20 @@ int b200_fec_debug_bits(b200_fec *f, uint8_t *host_out, long cap, long *n_out);
 int b200_fec_get_stats(b200_fec *f, b200_fec_stats *out);
 int b200_fec_cadu_bytes(b200_fec *f);
 int b200_fec_chunk_size(b200_fec *f);
+/* ccsds_ldpc_decoder: one record per frame of the LAST push, in stream order */
+typedef struct b200_ldpc_frame
+{
+    long offset;              /* stream offset (soft bytes since create / reset) of the frame's first byte                           */
+    int pos;                  /* the correlator's position in the window read before it (0 = locked)                                */
+    float cor;                /* correlator_corr                                                                                    */
+    int phase, swap;          /* the phase ambiguity fixed (0..3 = 0, 90, 180, 270 degrees) and the OQPSK re-delay / IQ swap         */
+    int ldpc_corr;
+} b200_ldpc_frame;
+int b200_fec_debug_ldpc_frames(b200_fec *f, b200_ldpc_frame *out, long cap, long *n_out);
+/* ccsds_ldpc_decoder only (B200_EINVAL for the other kinds): elapsed device milliseconds of the last push (CUDA events on the decoder's
+   stream): [0] correlation, [1] frame walk, [2] gather, [3] decode + CADU repack (+ internal_stream: bit append, deframer, frames),
+   [4] the whole push */
+int b200_fec_ldpc_timing(b200_fec *f, float *ms_out, int n);
 
 /* ---- fused chain: raw IQ -> CADUs, soft stream stays in HBM ---------------------------------------- */
 b200_chain *b200_chain_create(const b200_demod_cfg *dcfg, const b200_fec_cfg *fcfg);

@@ -6,7 +6,7 @@
 //
 //   loader()                          the one symbol SatDump dlsym()s (core/plugin.cpp:15-33)
 //   B200DSPSupport::init()            on SatDumpStartedEvent (fired after every plugin registered its modules, init.cpp:163) the
-//                                     entries "psk_demod", "pm_demod", "metop_ahrpt_decoder", "ccsds_conv_concat_decoder" and "ccsds_simple_psk_decoder" of
+//                                     entries "psk_demod", "pm_demod", "metop_ahrpt_decoder", "ccsds_conv_concat_decoder", "ccsds_simple_psk_decoder" and "ccsds_ldpc_decoder" of
 //                                     satdump::pipeline::modules_registry (module.h:210, looked up first-match by id, module.cpp:129-135)
 //                                     get their factory replaced, so existing pipelines instantiate the CUDA modules.
 //                                     Set B200_DSP_REGISTER_ONLY=1 to register "<id>_b200" ids instead and leave the originals alone.
@@ -211,7 +211,22 @@ namespace b200plugin
         }
         nlohmann::json getModuleStats() override
         {
-            nlohmann::json v; // keys of MetOpAHRPTDecoderModule::getModuleStats (module_metop_ahrpt_decoder.cpp:92-104)
+            nlohmann::json v;
+            if (stage->getID() == "ccsds_ldpc_decoder") // CCSDSLDPCDecoderModule::getModuleStats (module_ccsds_ldpc_decoder.cpp:279-295)
+            {
+                const int ds = stage->deframer_state.load();
+                if (stage->cfg.internal_stream)
+                {
+                    v["deframer_lock"] = ds == 12;
+                    v["deframer_state"] = ds == 2 ? "NOSYNC" : (ds == 6 ? "SYNCING" : "SYNCED");
+                }
+                v["correlator_lock"] = stage->correlator_lock.load() != 0;
+                v["correlator_corr"] = stage->correlator_corr.load();
+                v["ldpc_corr"] = stage->ldpc_corr.load();
+                v["lock_state"] = stage->correlator_lock.load() ? "SYNCED" : "NOSYNC";
+                return v;
+            }
+            // keys of MetOpAHRPTDecoderModule::getModuleStats (module_metop_ahrpt_decoder.cpp:92-104)
             v["deframer_lock"] = stage->deframer_state.load() > 6;
             v["viterbi_ber"] = stage->viterbi_ber.load();
             v["viterbi_lock"] = stage->viterbi_lock.load();
@@ -246,14 +261,15 @@ public:
 
     static void registerHandler(const satdump::pipeline::RegisterModulesEvent &evt)
     {
-        for (const char *id : {"psk_demod", "pm_demod", "metop_ahrpt_decoder", "ccsds_conv_concat_decoder", "ccsds_simple_psk_decoder"})
+        for (const char *id : {"psk_demod", "pm_demod", "metop_ahrpt_decoder", "ccsds_conv_concat_decoder", "ccsds_simple_psk_decoder", "ccsds_ldpc_decoder"})
             evt.modules_registry.push_back({std::string(id) + "_b200", nlohmann::json(), factory(id)});
     }
 
     static void patchHandler(const satdump::SatDumpStartedEvent &)
     {
         for (auto &e : satdump::pipeline::modules_registry)
-            if (e.id == "psk_demod" || e.id == "pm_demod" || e.id == "metop_ahrpt_decoder" || e.id == "ccsds_conv_concat_decoder" || e.id == "ccsds_simple_psk_decoder")
+            if (e.id == "psk_demod" || e.id == "pm_demod" || e.id == "metop_ahrpt_decoder" || e.id == "ccsds_conv_concat_decoder" || e.id == "ccsds_simple_psk_decoder" ||
+                e.id == "ccsds_ldpc_decoder")
             {
                 e.inst = factory(e.id);
                 logger->info("b200_dsp_support: module " + e.id + " now runs on the B200 path");

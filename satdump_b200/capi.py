@@ -23,7 +23,7 @@ SYMBOLS = [
     "b200_demod_create", "b200_demod_destroy", "b200_demod_push_iq", "b200_demod_push_iq_device", "b200_demod_pull_soft",
     "b200_demod_pull_symbols", "b200_demod_debug_stage", "b200_demod_debug_convert", "b200_demod_debug_run_stage", "b200_demod_debug_junctions", "b200_demod_reset", "b200_demod_prefetch_iq", "b200_demod_last_timing", "b200_demod_get_stats", "b200_demod_get_taps",
     "b200_fec_create", "b200_fec_destroy", "b200_fec_push_soft", "b200_fec_push_soft_device", "b200_fec_pull_frames",
-    "b200_fec_debug_bits", "b200_fec_get_stats", "b200_fec_cadu_bytes", "b200_fec_chunk_size",
+    "b200_fec_debug_bits", "b200_fec_get_stats", "b200_fec_cadu_bytes", "b200_fec_chunk_size", "b200_fec_debug_ldpc_frames", "b200_fec_ldpc_timing",
     "b200_chain_create", "b200_chain_destroy", "b200_chain_push_iq", "b200_chain_push_iq_device", "b200_chain_prefetch_iq", "b200_chain_pull_frames",
     "b200_chain_frames_device", "b200_chain_get_stats", "b200_chain_last_timing", "b200_chain_reset",
     "b200_chain_set_pipelined", "b200_chain_sync", "b200_chain_span_begin", "b200_chain_span_end",
@@ -49,7 +49,9 @@ class FecCfg(C.Structure):
                 ("ber_thresold", C.c_float), ("nrzm", C.c_int), ("derandomize", C.c_int), ("derand_after_rs", C.c_int),
                 ("derand_start", C.c_int), ("rs_i", C.c_int), ("rs_dualbasis", C.c_int), ("rs_fill_bytes", C.c_int),
                 ("rs_usecheck", C.c_int), ("rs_type", C.c_int), ("iq_invert", C.c_int), ("asm_sync", C.c_uint),
-                ("device", C.c_int), ("max_soft", C.c_long), ("qpsk_swap_iq", C.c_int), ("qpsk_swap_diff", C.c_int), ("oqpsk_delay", C.c_int), ("conv_rate", C.c_int)]
+                ("device", C.c_int), ("max_soft", C.c_long), ("qpsk_swap_iq", C.c_int), ("qpsk_swap_diff", C.c_int), ("oqpsk_delay", C.c_int), ("conv_rate", C.c_int),
+                ("ldpc_rate", C.c_int), ("ldpc_block_size", C.c_int), ("ldpc_iterations", C.c_int), ("ldpc2", C.c_int), ("internal_stream", C.c_int),
+                ("internal_cadu_size", C.c_int)]
 
 
 class DemuxCfg(C.Structure):
@@ -77,7 +79,12 @@ class FecStats(C.Structure):
     _fields_ = [("soft_in", C.c_long), ("chunks", C.c_long), ("bits_out", C.c_long), ("frames_out", C.c_long),
                 ("viterbi_state", C.c_int), ("viterbi_ber", C.c_float), ("deframer_state", C.c_int), ("rs_corrected", C.c_long),
                 ("rs_failed", C.c_long), ("replays", C.c_long), ("kernel_launches", C.c_long), ("start_redone", C.c_long), ("tb_serial", C.c_long),
-                ("spec_steps", C.c_int), ("tb_overlap", C.c_int)]
+                ("spec_steps", C.c_int), ("tb_overlap", C.c_int),
+                ("correlator_lock", C.c_int), ("correlator_corr", C.c_float), ("ldpc_corr", C.c_int), ("ldpc_resyncs", C.c_long)]
+
+
+class LdpcFrame(C.Structure):
+    _fields_ = [("offset", C.c_long), ("pos", C.c_int), ("cor", C.c_float), ("phase", C.c_int), ("swap", C.c_int), ("ldpc_corr", C.c_int)]
 
 
 class B200Error(RuntimeError):
@@ -127,6 +134,8 @@ def lib():
         L.b200_fec_get_stats.argtypes = [vp, C.POINTER(FecStats)]
         L.b200_fec_cadu_bytes.argtypes = [vp]
         L.b200_fec_chunk_size.argtypes = [vp]
+        L.b200_fec_debug_ldpc_frames.argtypes = [vp, C.POINTER(LdpcFrame), cl, C.POINTER(cl)]
+        L.b200_fec_ldpc_timing.argtypes = [vp, vp, ci]
         L.b200_chain_create.restype = vp
         L.b200_chain_create.argtypes = [C.POINTER(DemodCfg), C.POINTER(FecCfg)]
         L.b200_chain_destroy.argtypes = [vp]
@@ -225,11 +234,31 @@ def ccsds_cfg(constellation, cadu_size, ber_thresold, outsync_after, rs_i, nrzm=
                   0, 0, 0, {"1/2": 0, "2/3": 2, "3/4": 3, "5/6": 5, "7/8": 7}[conv_rate])
 
 
+LDPC_RATES = {"1/2": 1, "2/3": 2, "4/5": 4, "7/8": 7}
+
+
+def ldpc_cfg(constellation, ldpc_rate="7/8", ldpc_iterations=10, derandomize=True, internal_stream=False, internal_cadu_size=0,
+             internal_asm=0x1ACFFC1D, ldpc_block_size=0, ldpc2=False, device=0, max_soft=1 << 24):
+    """ccsds_ldpc_decoder (module_ccsds_ldpc_decoder.cpp:19-124). Built: ldpc_rate "7/8" (the C2 code) without internal_stream; the
+    library refuses the other options by name."""
+    if ldpc_rate not in LDPC_RATES:
+        raise ValueError(f"Invalid LDPC code rate {ldpc_rate}")
+    cfg = FecCfg()
+    cfg.kind, cfg.constellation, cfg.derandomize, cfg.asm_sync, cfg.device, cfg.max_soft = 3, CONST[constellation], int(derandomize), internal_asm, device, max_soft
+    cfg.cadu_size = internal_cadu_size if internal_stream else 8192  # bits of one output frame
+    cfg.ldpc_rate, cfg.ldpc_block_size, cfg.ldpc_iterations, cfg.ldpc2 = LDPC_RATES[ldpc_rate], ldpc_block_size, ldpc_iterations, int(ldpc2)
+    cfg.internal_stream, cfg.internal_cadu_size = int(internal_stream), internal_cadu_size
+    return cfg
+
+
 def fec_cfg_for(sig, max_soft, device=0):
     """The decoder configuration that goes with a satdump_b200.synth.SignalCfg (metop_ahrpt_decoder / ccsds_conv_concat_decoder /
     ccsds_simple_psk_decoder parameters of the shipped pipeline JSONs)."""
     if sig.decoder == "metop":
         return metop_cfg(sig.ber_thresold, sig.outsync_after, device=device, max_soft=max_soft)
+    if sig.decoder == "ldpc":
+        return ldpc_cfg(sig.constellation, internal_stream=bool(sig.internal_cadu_size), internal_cadu_size=sig.internal_cadu_size,
+                        internal_asm=sig.internal_asm, device=device, max_soft=max_soft)
     if sig.decoder == "simple":
         return simple_cfg(sig.constellation, (4 + 255 * sig.interleave) * 8, sig.interleave, nrzm=sig.nrzm, qpsk_swap_iq=sig.constellation == "qpsk",
                           device=device, max_soft=max_soft)
@@ -409,6 +438,25 @@ class Fec:
         _chk(lib().b200_fec_get_stats(self.h, C.byref(s)))
         return _struct_dict(s)
 
+    def ldpc_frames(self):
+        """ccsds_ldpc_decoder: one record per frame of the last push (LdpcFrame fields) as int64 [n, 7] = offset, pos, cor (float32 bits),
+        phase, swap, ldpc_corr, correlator_locked."""
+        cap = int(self._n) // 8192 + 4
+        recs = (LdpcFrame * cap)()
+        n = C.c_long(0)
+        _chk(lib().b200_fec_debug_ldpc_frames(self.h, recs, cap, C.byref(n)))
+        out = np.zeros((n.value, 7), np.int64)
+        for k in range(n.value):
+            r = recs[k]
+            out[k] = [r.offset, r.pos, int(np.float32(r.cor).view(np.uint32)), r.phase, r.swap, r.ldpc_corr, int(r.pos == 0)]
+        return out
+
+    def timing(self):
+        """ccsds_ldpc_decoder: device milliseconds of the last push: correlation, walk, gather, decode (+ repack), whole push."""
+        ms = np.zeros(5, np.float32)
+        _chk(lib().b200_fec_ldpc_timing(self.h, ms.ctypes.data, 5))
+        return dict(zip(["corr", "walk", "gather", "decode", "push"], ms.tolist()))
+
 
 class Chain:
     """Demodulator + decoder of one stream on one GPU; the soft stream stays in HBM."""
@@ -418,7 +466,7 @@ class Chain:
         self.h = lib().b200_chain_create(C.byref(dcfg), C.byref(fcfg))
         if not self.h:
             raise B200Error(-1 if "device" not in last_error().lower() else -2, last_error())
-        self.cadu_bytes = (fcfg.cadu_size + 7) // 8 if fcfg.kind == 1 else 1024
+        self.cadu_bytes = (fcfg.cadu_size + 7) // 8 if fcfg.kind in (1, 3) else 1024
 
     def close(self):
         if getattr(self, "h", None):

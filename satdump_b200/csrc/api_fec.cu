@@ -48,9 +48,14 @@ void build_rs_tables(RsTables &T)
 
 Fec::Fec(const b200_fec_cfg &c) : cfg(c)
 {
-    B200_REQUIRE(c.kind == B200_FEC_METOP || c.kind == B200_FEC_CCSDS || c.kind == B200_FEC_SIMPLE, B200_EINVAL, "unknown decoder kind %d", c.kind);
+    B200_REQUIRE(c.kind == B200_FEC_METOP || c.kind == B200_FEC_CCSDS || c.kind == B200_FEC_SIMPLE || c.kind == B200_FEC_LDPC, B200_EINVAL,
+                 "unknown decoder kind %d", c.kind);
     B200_REQUIRE(c.max_soft >= 65536, B200_EINVAL, "max_soft must be >= 65536");
     memset(&geom, 0, sizeof(geom));
+    if (c.kind == B200_FEC_LDPC) {
+        ldpc_init();
+        return;
+    }
     if (c.kind != B200_FEC_METOP) {
         B200_REQUIRE(c.cadu_size >= 64 && c.cadu_size <= 65536, B200_EINVAL, "cadu_size out of range");
         B200_REQUIRE(c.cadu_size % 8 == 0, B200_EINVAL, "cadu_size must be a multiple of 8 (frame padding is not built)");
@@ -192,6 +197,7 @@ Fec::~Fec()
     DeviceGuard g(cfg.device);
     if (stream)
         cudaStreamSynchronize(stream);
+    ldpc_free();
     for (auto &e : ev)
         cudaEventDestroy(e);
     for (auto &e : evm)
@@ -600,11 +606,43 @@ void Fec::start_stream(size_t fifo_bytes)
     }
 }
 
+// The deframer and frame stage behind another decoder (ccsds_ldpc_decoder's internal_stream): storage for `max_new_bits` new bits per
+// push, as the constructor allocates it for the convolutional decoders; cfg holds the deframer's cadu_size / asm_sync, rs_i = 0.
+void Fec::deframer_storage(long max_new_bits)
+{
+    fifo.alloc((size_t)((max_new_bits + 2L * cfg.cadu_size + 4096) / 32 + 8));
+    dstate.alloc(2);
+    devents.alloc(4096);
+    max_frames_push = max_new_bits / cfg.cadu_size + 4;
+    frames.alloc(max_frames_push);
+    frames_out.alloc((size_t)(2 * max_frames_push + 4) * cadu_bytes);
+    frames_tmp.alloc(1);
+    rs_err.alloc((size_t)max_frames_push + 4);
+    frame_dst.alloc((size_t)max_frames_push + 4);
+    counters.alloc(8);
+    tables.alloc(1);
+    B200_CUDA(cudaMallocHost((void **)&h_counters, sizeof(int) * 8));
+    B200_CUDA(cudaMallocHost((void **)&h_dstate, sizeof(DefrState) * 2));
+    B200_CUDA(cudaMallocHost((void **)&h_events, sizeof(DefrEvent) * 4096));
+    B200_CUDA(cudaMallocHost((void **)&h_rs_err, sizeof(int) * (max_frames_push + 4)));
+    RsTables T;
+    build_rs_tables(T);
+    B200_CUDA(cudaMemcpyAsync(tables.p, &T, sizeof(T), cudaMemcpyHostToDevice, stream));
+    fr_smem = (int)sizeof(RsTables) + ((cadu_bytes + 15) & ~15) + RS_MAX_I * 704;
+    B200_CUDA(cudaFuncSetAttribute(k_frames, cudaFuncAttributeMaxDynamicSharedMemorySize, fr_smem));
+    start_stream(fifo.n * sizeof(uint32_t));
+    B200_CUDA(cudaStreamSynchronize(stream));
+}
+
 // back to the state of a freshly created decoder (new stream), keeping all allocations
 void Fec::reset()
 {
     DeviceGuard g(cfg.device);
     B200_CUDA(cudaStreamSynchronize(stream));
+    if (ldpc) {
+        ldpc_reset();
+        return;
+    }
     start_stream(64);
     B200_CUDA(cudaStreamSynchronize(stream));
 }
@@ -834,6 +872,10 @@ void Fec::decode_conv(long nch)
 void Fec::process()
 {
     DeviceGuard g(cfg.device);
+    if (ldpc) {
+        ldpc_process();
+        return;
+    }
     const long nch = soft_have / geom.chunk;
     B200_REQUIRE(nch <= max_chunks, B200_ESTATE, "internal: too many chunks");
     // (lazy, so that b200_fec_debug_bits can still read the previous push's bits until now)
@@ -894,6 +936,8 @@ void Fec::stats(b200_fec_stats *o)
     o->spec_steps = spec_steps;
     o->tb_overlap = tb_overlap;
     o->kernel_launches = launches;
+    if (ldpc)
+        ldpc_stats(o);
 }
 
 } // namespace b200
@@ -972,4 +1016,19 @@ int b200_fec_get_stats(b200_fec *h, b200_fec_stats *out)
 }
 int b200_fec_cadu_bytes(b200_fec *h) { return h ? h->f->cadu_bytes : B200_EINVAL; }
 int b200_fec_chunk_size(b200_fec *h) { return h ? h->f->geom.chunk : B200_EINVAL; }
+int b200_fec_debug_ldpc_frames(b200_fec *h, b200_ldpc_frame *out, long cap, long *n_out)
+{
+    return guarded([&] {
+        B200_REQUIRE(h && out && n_out, B200_EINVAL, "NULL argument");
+        *n_out = h->f->ldpc_frames(out, cap);
+    });
+}
+int b200_fec_ldpc_timing(b200_fec *h, float *ms_out, int n)
+{
+    return guarded([&] {
+        B200_REQUIRE(h && ms_out, B200_EINVAL, "NULL argument");
+        B200_REQUIRE(h->f->ldpc, B200_EINVAL, "not an LDPC decoder (kind B200_FEC_LDPC)");
+        h->f->ldpc_timing(ms_out, n);
+    });
+}
 }

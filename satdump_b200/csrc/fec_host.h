@@ -11,6 +11,7 @@ namespace b200
 {
 
 struct DefrEvent { long pos; int state; int pad; };
+struct Ldpc; // ccsds_ldpc_decoder's state (api_ldpc.cu)
 
 class Fec
 {
@@ -36,6 +37,10 @@ class Fec
     cudaEvent_t evm[2], evf[2];
     long last_main_chunks = 0;
     void reset();
+    // ccsds_ldpc_decoder (B200_FEC_LDPC): set up by the constructor instead of the Viterbi / deframer storage
+    Ldpc *ldpc = nullptr;
+    long ldpc_frames(b200_ldpc_frame *out, long cap); // records of the last push
+    void ldpc_timing(float *ms, int n);
 
     // device storage
     DevBuf<int8_t> softbuf;
@@ -119,6 +124,12 @@ class Fec
     int last_raw_bit(long q, int nbits);
     void keep_soft_tail(long used);
     void deframe_and_rs(long new_bits);
+    void ldpc_init();
+    void deframer_storage(long max_new_bits); // bit FIFO, deframer and frame stage of LDPC's internal_stream (api_fec.cu)
+    void ldpc_free();
+    void ldpc_reset();
+    void ldpc_process();
+    void ldpc_stats(b200_fec_stats *o);
 };
 
 void build_rs_tables(RsTables &T);

@@ -10,7 +10,7 @@ using namespace b200host;
 int main(int argc, char **argv)
 {
     if (argc < 5) {
-        fprintf(stderr, "usage: %s <metop_ahrpt|jpss_hrd|npp_hrd|simple_bpsk|simple_qpsk|pm_bpsk> baseband <input> <output_hint> [--fused] [--key value ...]\n", argv[0]);
+        fprintf(stderr, "usage: %s <metop_ahrpt|jpss_hrd|npp_hrd|simple_bpsk|simple_qpsk|pm_bpsk|ldpc_qpsk|landsat> baseband <input> <output_hint> [--fused] [--key value ...]\n", argv[0]);
         return 2;
     }
     const std::string pipe = argv[1], level = argv[2], in = argv[3], out = argv[4];
@@ -39,6 +39,18 @@ int main(int argc, char **argv)
         fp = Params{{"constellation", "bpsk"}, {"cadu_size", "8192"}, {"viterbi_ber_thresold", "0.3"}, {"viterbi_outsync_after", "20"}, {"derandomize", "true"},
                     {"rs_i", "4"}, {"rs_type", "rs223"}};
         dec = "ccsds_conv_concat_decoder";
+    } else if (pipe == "ldpc_qpsk" || pipe == "landsat") { // psk_demod -> ccsds_ldpc_decoder, rate 7/8: FengYun-3 MERSI / GOES-R raw data
+        // (FengYun-3.json:530-548, GOES.json:532-560) and LandSat 8/9 with its inner stream (LandSat.json:35-63); rates from the command line
+        const bool ls = pipe == "landsat";
+        dp = Params{{"constellation", ls ? "oqpsk" : "qpsk"}, {"symbolrate", ls ? "2000000" : "3000000"}, {"rrc_alpha", ls ? "0.5" : "0.35"},
+                    {"pll_bw", ls ? "0.002" : "0.003"}};
+        fp = Params{{"constellation", ls ? "oqpsk" : "qpsk"}, {"ldpc_rate", "7/8"}, {"ldpc_iterations", "10"}, {"derandomize", "true"}};
+        if (ls) {
+            fp.set("internal_stream", "true");
+            fp.set("internal_cadu_size", "8272");
+            fp.set("internal_asm", "352EF853");
+        }
+        dec = "ccsds_ldpc_decoder";
     } else {
         fprintf(stderr, "unknown pipeline %s\n", pipe.c_str());
         return 2;

@@ -256,6 +256,31 @@ b200_demod_cfg pm_demod_cfg_from_params(const Params &p, bool &is_bpsk)
 b200_fec_cfg fec_cfg_from_params(const std::string &id, const Params &p)
 {
     b200_fec_cfg c{};
+    if (id == "ccsds_ldpc_decoder") { // module_ccsds_ldpc_decoder.cpp:19-124
+        c.kind = B200_FEC_LDPC;
+        c.device = (int)p.num("b200_device", 0);
+        const std::string con = p.str("constellation");
+        if (con == "bpsk") c.constellation = B200_BPSK;
+        else if (con == "qpsk") c.constellation = B200_QPSK;
+        else if (con == "oqpsk") c.constellation = B200_OQPSK;
+        else throw ModuleError("CCSDS LDPC Decoder : invalid constellation type!");
+        c.derandomize = p.flag("derandomize", true);
+        const std::string rate = p.str("ldpc_rate");
+        if (rate == "1/2") c.ldpc_rate = 1;
+        else if (rate == "2/3") c.ldpc_rate = 2;
+        else if (rate == "4/5") c.ldpc_rate = 4;
+        else if (rate == "7/8") c.ldpc_rate = 7;
+        else throw ModuleError("Invalid LDPC code rate " + rate);
+        c.ldpc_block_size = (int)p.num("ldpc_block_size", 0);
+        c.ldpc_iterations = (int)p.num("ldpc_iterations");
+        c.ldpc2 = p.flag("ldpc2", false);
+        // d_internal_stream / d_cadu_size (:33-34): internal_cadu_size is read whenever internal_stream is given
+        c.internal_stream = p.flag("internal_stream", false);
+        c.internal_cadu_size = p.has("internal_stream") ? (int)p.num("internal_cadu_size") : 0;
+        c.asm_sync = p.has("internal_asm") ? (unsigned)std::stoul(p.str("internal_asm"), nullptr, 16) : 0x1ACFFC1D; // (:102-104)
+        c.cadu_size = c.internal_stream ? c.internal_cadu_size : 8192; // what one output frame holds
+        return c; // ("ccsds": .cadu / .frm output naming, :123, in FecStage::process)
+    }
     if (id != "ccsds_simple_psk_decoder") {
         c.outsync_after = (int)p.num("viterbi_outsync_after");
         c.ber_thresold = (float)p.num("viterbi_ber_thresold");
@@ -538,6 +563,9 @@ void FecStage::process()
             viterbi_ber = st.viterbi_ber;
             deframer_state = st.deframer_state;
             frames_written = st.frames_out;
+            correlator_lock = st.correlator_lock;
+            correlator_corr = st.correlator_corr;
+            ldpc_corr = st.ldpc_corr;
         }
     }
     if (fin)

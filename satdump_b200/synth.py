@@ -13,6 +13,7 @@ All coding is written from the CCSDS definitions (GF(256) poly 0x187, generator 
 dual basis, PN h(x)=x^8+x^7+x^5+x^3+1); tests/test_synth.py cross-checks every encoder against the
 reference's own encoders (oracle/_ref) and checks that the reference receiver recovers the payload.
 """
+import functools
 from dataclasses import dataclass, field
 
 import numpy as np
@@ -203,9 +204,15 @@ class SignalCfg:
     # (pm_index * d(t), no subcarrier): carrier PLL -> DC blocker -> Costas loop
     has_carrier: bool = False
     carrier_pll_bw: float = 0.001
+    # ccsds_ldpc_decoder (decoder "ldpc", rate 7/8 C2 code): 0 = the decoder writes the LDPC frames' CADUs; > 0 = "internal_stream": the info
+    # bits carry inner CADUs of this many bits that start with internal_asm
+    internal_cadu_size: int = 0
+    internal_asm: int = 0x1ACFFC1D
 
     @property
     def cadu_bytes(self):
+        if self.decoder == "ldpc":
+            return self.internal_cadu_size // 8 if self.internal_cadu_size else 1024
         return 4 + 255 * self.interleave
 
     @property
@@ -271,6 +278,14 @@ CONFIGS = {
     # C5: DVB-S2 front half AGC->RRC->M&M, cs8, 45 Msym/s @ 90 MS/s (sps 2.0), alpha 0.25 (DVB_Test.json:132-137), REC_ALPHA 1.7e-3
     "dvbs2_front": SignalCfg(name="dvbs2_front", samplerate=90e6, symbolrate=45000000, constellation="qpsk", conv="none", interleave=4,
                              rrc_alpha=0.25, fmt="cs8", decoder="none", clock_alpha=1.7e-3, carrier_rad=0.0, phase0=0.0, esn0_db=12.0),
+    # psk_demod -> ccsds_ldpc_decoder (rate 7/8 C2 code, 10 iterations): QPSK at 2 samples per symbol in cs8 (FengYun-3 MERSI / GOES-R
+    # raw-data shape, FengYun-3.json:530-548, GOES.json:532-560)
+    "ldpc_qpsk": SignalCfg(name="ldpc_qpsk", samplerate=6e6, symbolrate=3000000, constellation="qpsk", conv="ldpc", rrc_alpha=0.35, fmt="cs8",
+                           decoder="ldpc", esn0_db=12.0),
+    # LandSat-like (LandSat.json:35-63): OQPSK, internal_stream with 8272-bit inner CADUs behind the ASM 0x352EF853; 3 samples per symbol,
+    # above OQPSK's MAX_SPS 2.4, so the front-end resampler runs (6 -> 4.8 MS/s)
+    "ldpc_landsat": SignalCfg(name="ldpc_landsat", samplerate=6e6, symbolrate=2000000, constellation="oqpsk", conv="ldpc", rrc_alpha=0.5, fmt="cs16",
+                              decoder="ldpc", esn0_db=12.0, pll_bw=0.002, internal_cadu_size=8272, internal_asm=0x352EF853),
 }
 
 
@@ -299,6 +314,13 @@ def qpsk_diff_encode(dibits, swap=True):
 
 
 def make_bitstream(cfg: SignalCfg, nframes, seed):
+    if cfg.decoder == "ldpc":  # nframes LDPC frames
+        if cfg.internal_cadu_size:
+            info, clear = ldpc_inner_frames(nframes, cfg.internal_cadu_size, cfg.internal_asm, seed)
+            tx, _, _ = ldpc_frames(nframes, seed, info=info)
+        else:
+            tx, _, clear = ldpc_frames(nframes, seed)
+        return tx.reshape(-1), clear
     rng = np.random.default_rng(seed)
     payload = rng.integers(0, 256, size=(nframes, cfg.interleave * 223), dtype=np.uint8)
     tx, clear = build_cadus(payload, cfg.interleave)
@@ -406,6 +428,8 @@ def modulate(cfg: SignalCfg, coded, seed, nsamples=None, device="cpu"):
 
 def frames_for_samples(cfg: SignalCfg, nsamples):
     bps = 1 if cfg.constellation == "bpsk" else 2
+    if cfg.decoder == "ldpc":  # LDPC frames of 8192 bits
+        return int(nsamples * bps / (cfg.samplerate / cfg.symbolrate) / 8192) + 2
     rate = {"1/2": 0.5, "3/4": 0.75, "none": 1.0, "p2/3": 2 / 3, "p3/4": 0.75, "p5/6": 5 / 6, "p7/8": 7 / 8}[cfg.conv]
     bits_per_sample = bps * rate / (cfg.samplerate / cfg.symbolrate)
     return int(nsamples * bits_per_sample / (cfg.cadu_bytes * 8)) + 4
@@ -529,3 +553,123 @@ def craft_leftover_frames(mpdu, variant=0, vcid=9, cadu_size=1024):
         if p < 2047:
             d(f)[p + 4], d(f)[p + 5] = 0, 30
     return fr
+
+
+# ---- CCSDS C2 LDPC (8176, 7154), the code behind ccsds_ldpc_decoder's ldpc_rate "7/8" -----------------------------------------------
+LDPC_CIRC, LDPC_BX, LDPC_BY = 511, 16, 2
+LDPC_N, LDPC_ROWS, LDPC_SHORT = 8176, 1022, 18  # code length, parity checks, leading positions that are always 0 (not sent)
+LDPC_INFO = 7154 - LDPC_SHORT                   # info bits sent per codeword (7136)
+
+
+@functools.lru_cache(maxsize=1)
+def ldpc_c2_offsets():
+    """The circulant offsets of satdump_b200/csrc/ldpc_c2_table.inc (tools/gen_ldpc_c2_table.py) as int [2, 16, 2]."""
+    import os
+    import re
+    src = open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "csrc", "ldpc_c2_table.inc")).read()
+    nums = [int(v) for v in re.findall(r"\d+", src.split("= {", 1)[1])]
+    return np.array(nums, np.int64).reshape(LDPC_BY, LDPC_BX, 2)
+
+
+@functools.lru_cache(maxsize=1)
+def ldpc_c2_cols():
+    """H's rows (row block 0's 511 rows, then row block 1's) as the ascending column indices of their 32 ones: int [1022, 32]."""
+    off = ldpc_c2_offsets()
+    r = np.arange(LDPC_CIRC)
+    cols = np.zeros((LDPC_ROWS, 2 * LDPC_BX), np.int64)
+    for y in range(LDPC_BY):
+        for x in range(LDPC_BX):
+            a, b = (off[y, x, 0] + r) % LDPC_CIRC, (off[y, x, 1] + r) % LDPC_CIRC
+            cols[y * LDPC_CIRC:(y + 1) * LDPC_CIRC, 2 * x] = LDPC_CIRC * x + np.minimum(a, b)
+            cols[y * LDPC_CIRC:(y + 1) * LDPC_CIRC, 2 * x + 1] = LDPC_CIRC * x + np.maximum(a, b)
+    return cols
+
+
+def ldpc_c2_h():
+    H = np.zeros((LDPC_ROWS, LDPC_N), np.uint8)
+    H[np.repeat(np.arange(LDPC_ROWS), 2 * LDPC_BX), ldpc_c2_cols().reshape(-1)] = 1
+    return H
+
+
+@functools.lru_cache(maxsize=1)
+def _ldpc_parity_solver():
+    """Gaussian elimination of H's parity part (columns 7154..8175, rank 1020) over GF(2): the pivot columns and the row operations
+    that turn a syndrome into their values (the two non-pivot parity positions are set to 0)."""
+    H = ldpc_c2_h()
+    A = np.concatenate([H[:, 7154:], np.eye(LDPC_ROWS, dtype=np.uint8)], axis=1)
+    piv_cols, r = [], 0
+    for c in range(LDPC_ROWS):
+        rows = np.nonzero(A[r:, c])[0]
+        if rows.size == 0:
+            continue
+        p = r + rows[0]
+        A[[r, p]] = A[[p, r]]
+        hit = np.nonzero(A[:, c])[0]
+        hit = hit[hit != r]
+        A[hit] ^= A[r]
+        piv_cols.append(c)
+        r += 1
+    return np.array(piv_cols), A[:r, LDPC_ROWS:].astype(np.int64)
+
+
+def ldpc_c2_encode(info):
+    """info: uint8 [n, 7136] -> codewords uint8 [n, 8176] with H c = 0: 18 zeros, the info bits, 1022 parity bits."""
+    info = np.atleast_2d(np.asarray(info, np.uint8))
+    n = info.shape[0]
+    H = ldpc_c2_h().astype(np.int64)
+    cw = np.zeros((n, LDPC_N), np.uint8)
+    cw[:, LDPC_SHORT:7154] = info
+    syn = (cw[:, :7154].astype(np.int64) @ H[:, :7154].T) % 2
+    piv, E = _ldpc_parity_solver()
+    cw[:, 7154 + piv] = ((syn @ E.T) % 2).astype(np.uint8)
+    assert not ((cw.astype(np.int64) @ H.T) % 2).any(), "H c != 0"
+    return cw
+
+
+def ldpc_pn_bits(n):
+    """The CCSDS pseudo-random sequence one bit per entry (period 255), as derand_ccsds_soft applies it to the 8160 code soft bytes."""
+    return np.resize(np.unpackbits(ccsds_pn(32))[:255], n)
+
+
+def ldpc_frames(nframes, seed=0, info=None):
+    """(tx bits uint8 [n, 8192] = ASM + PN-randomised (code bits 18..8175 + 2 zero fill bits), codewords [n, 8176], the CADUs the decoder
+    writes for them [n, 1024]: the ASM 0x1ACFFC1D as a little-endian uint32, then the 8158 code bits and the 2 zero fill bits)."""
+    if info is None:
+        info = np.random.default_rng(seed).integers(0, 2, (nframes, LDPC_INFO), dtype=np.uint8)
+    cw = ldpc_c2_encode(info)
+    sent = np.concatenate([cw[:, LDPC_SHORT:], np.zeros((cw.shape[0], 2), np.uint8)], axis=1)
+    asm = np.unpackbits(np.frombuffer(ASM, np.uint8))
+    tx = np.concatenate([np.tile(asm, (cw.shape[0], 1)), sent ^ ldpc_pn_bits(8160)[None, :]], axis=1)
+    cadu = np.concatenate([np.tile(np.array([0x1D, 0xFC, 0xCF, 0x1A], np.uint8), (cw.shape[0], 1)), np.packbits(sent, axis=1)], axis=1)
+    return tx, cw, cadu
+
+
+def ldpc_soft(tx_bits, constellation, amp=60.0, sigma=0.0, rot=0, q_late=False, seed=0):
+    """int8 soft stream of the bit stream as psk_demod writes it: bit 1 -> +amp. BPSK: one byte per bit (rot 0 / 2 = 0 / 180 degrees).
+    QPSK / OQPSK: (I, Q) pairs of consecutive bits, the symbols rotated by rot * 90 degrees; q_late: Q lags I by one symbol."""
+    b = np.asarray(tx_bits, np.uint8).reshape(-1).astype(np.float64) * 2 - 1
+    rng = np.random.default_rng(seed)
+    if constellation == "bpsk":
+        s = b * (-1 if rot == 2 else 1) * amp
+    else:
+        z = (b[0::2] + 1j * b[1::2]) * np.exp(1j * np.pi / 2 * rot)
+        I, Q = np.round(z.real), np.round(z.imag)
+        if q_late:
+            Q = np.concatenate([[0.0], Q[:-1]])
+        s = np.empty(2 * I.size)
+        s[0::2], s[1::2] = I * amp, Q * amp
+    if sigma:
+        s = s + rng.normal(0, sigma, s.size)
+    return np.clip(np.round(s), -127, 127).astype(np.int8)
+
+
+def ldpc_inner_frames(nframes, cadu_size, asm, seed):
+    """internal_stream: inner CADUs of cadu_size bits (asm + random bits) packed back to back into the 7136 info bits of nframes codewords.
+    Returns (info uint8 [nframes, 7136], the whole inner frames the info bits carry, uint8 [k, cadu_size / 8])."""
+    rng = np.random.default_rng(seed + 1)
+    total = nframes * LDPC_INFO
+    k = total // cadu_size
+    asm_bits = np.unpackbits(np.frombuffer(int(asm).to_bytes(4, "big"), np.uint8))
+    inner = np.concatenate([np.tile(asm_bits, (k, 1)), rng.integers(0, 2, (k, cadu_size - 32), dtype=np.uint8)], axis=1)
+    bits = np.concatenate([inner.reshape(-1), rng.integers(0, 2, total - k * cadu_size, dtype=np.uint8)])
+    return bits.reshape(nframes, LDPC_INFO), np.packbits(inner, axis=1)

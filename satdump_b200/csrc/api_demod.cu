@@ -721,7 +721,8 @@ float2 *Demod::stage_costas(long n, int L, int nseg, int cur, int nxt, bool mate
 }
 
 // M&M clock recovery over mmin (+ stitching, repair rounds, compaction and the int8 quantiser). `strict`: test hook, see k_mm.
-void Demod::stage_mm(float2 *mmin, long n, int L, int nseg, int cur, int nxt, int8_t *sdst, bool strict)
+// all_symbols: every symbol lands in sym_out (b200_demod_pull_symbols reads them); otherwise only the tail the SNR estimate reads.
+void Demod::stage_mm(float2 *mmin, long n, int L, int nseg, int cur, int nxt, int8_t *sdst, bool strict, bool all_symbols)
 {
     DemodDevState *S = st.p;
     const int nblk = (nseg + SEG_THREADS - 1) / SEG_THREADS;
@@ -742,7 +743,8 @@ void Demod::stage_mm(float2 *mmin, long n, int L, int nseg, int cur, int nxt, in
         k_mm_scan<<<1, 1024, 0, stream>>>(mrec.p, nseg, tol_mm, offs.p, &S->mm_unconv, cap, &S->flags, repair.p + 1, repair.p, round, &S->repairs);
         launches += 2;
     }
-    k_mm_compact<<<std::min(nseg, 132 * 8), 256, 0, stream>>>(slots.p, cap, mrec.p, offs.p, nseg, pm ? 2 : (bps == 1), sym_out.p, sdst);
+    k_mm_compact<<<std::min(nseg, 132 * 8), 256, 0, stream>>>(slots.p, cap, mrec.p, offs.p, nseg, pm ? 2 : (bps == 1), all_symbols ? 1 : 0, sym_out.p,
+                                                              sdst);
     k_snr_m2m4<<<1, 1024, 0, stream>>>(sym_out.p, offs.p + nseg, 0.001f, S->snr_y[cur], S->snr_y[nxt]); // M2M4SNREstimator(alpha = 0.001)
     launches += 4;
 }
@@ -866,7 +868,8 @@ long Demod::process(const void *d_raw, long n, int8_t *soft_dst)
     const int nseg = (int)((n + L - 1) / L);
     float2 *mmin = stage_costas(n, L, nseg, cur, nxt, cfg.keep_stages != 0);
     B200_CUDA(cudaEventRecord(ev[2], stream));
-    stage_mm(mmin, n, L, nseg, cur, nxt, soft_dst ? soft_dst : soft.p, false);
+    // a caller-supplied soft destination (the fused chain) consumes the soft stream only: its demodulator's symbols are never pulled
+    stage_mm(mmin, n, L, nseg, cur, nxt, soft_dst ? soft_dst : soft.p, false, soft_dst == nullptr);
     B200_CUDA(cudaEventRecord(ev[3], stream));
     B200_CUDA(cudaMemcpyAsync(h_total, offs.p + nseg, sizeof(long), cudaMemcpyDeviceToHost, stream));
     B200_CUDA(cudaMemcpyAsync(h_state, st.p, sizeof(DemodDevState), cudaMemcpyDeviceToHost, stream));
@@ -950,7 +953,7 @@ long Demod::debug_run_stage(int stage, const float *h_in, long n, int mode, floa
         B200_CUDA(cudaMemcpyAsync(mmin + 16, h_in, n * sizeof(float2), cudaMemcpyHostToDevice, stream));
         last_L = L;
         last_nseg = nseg;
-        stage_mm(mmin, n, L, nseg, 0, 1, soft.p, strict);
+        stage_mm(mmin, n, L, nseg, 0, 1, soft.p, strict, true);
         B200_CUDA(cudaMemcpyAsync(h_total, offs.p + nseg, sizeof(long), cudaMemcpyDeviceToHost, stream));
         B200_CUDA(cudaStreamSynchronize(stream));
         count = *h_total;

@@ -2159,26 +2159,44 @@ __device__ __forceinline__ int8_t soft_quant(float x)
 }
 
 // ---------------------------------------------------------------- K3c: compact per-segment symbol slots -> contiguous symbols + int8 soft
+constexpr int SNR_WINDOW = 1024 * 64; // symbols at the end of a batch that k_snr_m2m4 reads (one CTA, 64 per thread)
+// all_symbols == 0: only the last SNR_WINDOW symbols go to sym_out (the soft stream is the batch's only consumer-visible output, and the
+// SNR estimate needs no more), which saves 8 of the 18 bytes per symbol this pass moves. Each thread loads MC_UNROLL slots before it
+// stores anything, so enough loads are in flight to keep HBM busy.
+constexpr int MC_UNROLL = 4;
 __global__ void __launch_bounds__(256) k_mm_compact(const float2 *__restrict__ slots, int cap, const MMRec *__restrict__ rec,
-                                                   const long *__restrict__ offs, int nseg, int bpsk, float2 *__restrict__ sym_out,
-                                                   int8_t *__restrict__ soft_out)
+                                                   const long *__restrict__ offs, int nseg, int bpsk, int all_symbols,
+                                                   float2 *__restrict__ sym_out, int8_t *__restrict__ soft_out)
 {
+    const long keep0 = all_symbols ? 0 : offs[nseg] - SNR_WINDOW; // symbols from here on are written to sym_out
     for (int s = blockIdx.x; s < nseg; s += gridDim.x) {
         const int sk = rec[s].skip;
         const int c = min(rec[s].count, cap) - sk;
         const long o = offs[s];
         const float2 *src = slots + (long)s * cap + sk;
-        for (int i = threadIdx.x; i < c; i += blockDim.x) {
-            float2 v = src[i];
-            if (sym_out)
-                sym_out[o + i] = v;
-            if (bpsk) // 1: psk_demod's BPSK, real * 50 (module_psk_demod.cpp:199-205); 2: pm_demod, real * 100 (module_pm_demod.cpp:141-144)
-                soft_out[o + i] = soft_quant(v.x * (bpsk == 2 ? 100.0f : 50.0f));
-            else {
-                char2 q;
-                q.x = soft_quant(v.x * 100.0f);
-                q.y = soft_quant(v.y * 100.0f);
-                reinterpret_cast<char2 *>(soft_out)[o + i] = q;
+        for (int i0 = threadIdx.x; i0 < c; i0 += MC_UNROLL * blockDim.x) {
+            float2 v[MC_UNROLL];
+#pragma unroll
+            for (int j = 0; j < MC_UNROLL; j++) {
+                const int i = i0 + j * blockDim.x;
+                if (i < c)
+                    v[j] = src[i];
+            }
+#pragma unroll
+            for (int j = 0; j < MC_UNROLL; j++) {
+                const int i = i0 + j * blockDim.x;
+                if (i >= c)
+                    break;
+                if (o + i >= keep0)
+                    sym_out[o + i] = v[j];
+                if (bpsk) // 1: psk_demod's BPSK, real * 50 (module_psk_demod.cpp:199-205); 2: pm_demod, real * 100 (module_pm_demod.cpp:141-144)
+                    soft_out[o + i] = soft_quant(v[j].x * (bpsk == 2 ? 100.0f : 50.0f));
+                else {
+                    char2 q;
+                    q.x = soft_quant(v[j].x * 100.0f);
+                    q.y = soft_quant(v[j].y * 100.0f);
+                    reinterpret_cast<char2 *>(soft_out)[o + i] = q;
+                }
             }
         }
     }
@@ -2195,8 +2213,8 @@ __global__ void __launch_bounds__(1024) k_snr_m2m4(const float2 *__restrict__ sy
     __shared__ double red[2][32];
     const long n = *total;
     const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
-    const int RUN = 64;
-    const long M = min(n, 1024L * RUN), base = n - M;
+    const int RUN = SNR_WINDOW / 1024;
+    const long M = min(n, (long)SNR_WINDOW), base = n - M;
     const double beta = (double)(float)(1.0 - (double)alpha), al = (double)alpha;
     const long i0 = (long)t * RUN, i1 = min(M, i0 + RUN);
     double a1 = 0.0, a2 = 0.0;

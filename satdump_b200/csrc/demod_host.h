@@ -73,7 +73,7 @@ class Demod
     void run_dc(const void *src, int fmt, int iq_swap, long n, const float2 *acc_in, float2 *acc_out, float2 *dst);
     const uint8_t *mm_quad = nullptr; // set by stage_costas when the clock recovery applies the rotation (/ OQPSK delay) itself
     int mm_rot = 0, mm_oqpsk = 0;
-    void stage_mm(float2 *mmin, long n, int L, int nseg, int cur, int nxt, int8_t *sdst, bool strict);
+    void stage_mm(float2 *mmin, long n, int L, int nseg, int cur, int nxt, int8_t *sdst, bool strict, bool all_symbols);
     long debug_run_stage(int stage, const float *h_in, long n, int mode, float *h_out, long cap);
     int last_L = 0, last_nseg = 0;          // segmentation of the last batch (b200_demod_debug_junctions)
     int dbg_costas_unconv = 0, dbg_mm_unconv = 0, dbg_repairs = 0; // of the last debug_run_stage

@@ -572,16 +572,16 @@ template <int FMT> static void launch_front(Demod &d, const void *raw, long n, i
     for (int pass = 0; pass < 2; pass++) {
         ctl.seeded = pass;
         if (pass) { // exact pass: returns at once unless the fast pass asked for it
-            k_agc_compose<FMT><<<std::min(ntiles, d.fir_ctas * 2), FIR_THREADS, 0, d.stream>>>(raw, n, u.rate, need, ntiles, d.tile_map.p);
-            k_agc_scan<<<1, 1024, 0, d.stream>>>(d.tile_map.p, ntiles, u.gain_in, need, d.seeds.p, &S->agc_exact);
+            k_agc_compose<FMT><<<std::min(ntiles, d.fir_ctas * 2), FIR_THREADS, 0, d.stream>>>(raw, n, u.rate, u.max_gain, need, ~0, ntiles, d.tile_map.p);
+            k_tile_scan<<<1, 1024, 0, d.stream>>>(d.tile_map.p, ntiles, u.gain_in, need, ~0, d.seeds.p, &S->agc_exact);
         }
         fir<<<grid, 32 * FW_WARPS, 0, d.stream>>>(raw, n, u.rate, u.gain_in, R, ctl, taps, u.tail_in, u.tail_out, u.fir_out, u.dump, u.gain_out, &S->flags);
     }
     // clamp pass: the gain reached max_gain somewhere in this batch (silent input), so the unclamped maps above do not describe
     // the reference's loop; redo the stage with the clamped ones. All three launches return at once otherwise.
     ctl.seeded = 1;
-    k_agc_compose3<FMT><<<std::min(ntiles, d.fir_ctas * 2), FIR_THREADS, 0, d.stream>>>(raw, n, u.rate, (double)u.max_gain, &S->flags, ntiles, d.tile_map3.p);
-    k_agc_scan3<<<1, 1024, 0, d.stream>>>(d.tile_map3.p, ntiles, u.gain_in, &S->flags, d.seeds.p);
+    k_agc_compose<FMT><<<std::min(ntiles, d.fir_ctas * 2), FIR_THREADS, 0, d.stream>>>(raw, n, u.rate, u.max_gain, &S->flags, 1, ntiles, d.tile_map3.p);
+    k_tile_scan<<<1, 1024, 0, d.stream>>>(d.tile_map3.p, ntiles, u.gain_in, &S->flags, 1, d.seeds.p, nullptr);
     const auto fir_clamp = u.dump ? k_agc_fir_w<FMT, true, true> : k_agc_fir_w<FMT, false, true>;
     fir_clamp<<<grid, 32 * FW_WARPS, 0, d.stream>>>(raw, n, u.rate, u.gain_in, R, ctl, taps, u.tail_in, u.tail_out, u.fir_out, u.dump, u.gain_out, &S->flags);
     d.launches += 7;
@@ -609,10 +609,20 @@ void Demod::run_dc(const void *src, int fmt, int iq_swap, long n, const float2 *
     const float alpha = 0.0001f, beta = 1.0f - alpha;
     with_fmt(fmt, [&](auto F) {
         k_dc_tile<F><<<nt, FIR_THREADS, 0, stream>>>(src, n, iq_swap, alpha, beta, dc_map.p);
-        k_dc_scan<<<1, 1024, 0, stream>>>(dc_map.p, nt, acc_in, dc_seeds.p);
+        k_tile_scan<<<1, 1024, 0, stream>>>(dc_map.p, nt, acc_in, nullptr, 0, dc_seeds.p, nullptr);
         k_dc_apply<F><<<nt, FIR_THREADS, 0, stream>>>(src, n, iq_swap, alpha, beta, dc_seeds.p, dst, acc_out);
     });
     launches += 3;
+}
+
+// A loop stage: round(grid, repair_list, repair_count, r) launches the loop kernel and its junction check. Round 0 runs all segments,
+// rounds 1..REPAIR_ROUNDS re-run the flagged ones on 8 CTAs (both kernels return at once when no junction is flagged).
+template <class Round> static void run_loop_stage(Demod &d, int nblk, Round round)
+{
+    round(nblk, nullptr, nullptr, 0);
+    for (int r = 1; r <= REPAIR_ROUNDS; r++)
+        round(8, d.repair.p + 1, d.repair.p, r);
+    d.launches += 2 + 2 * REPAIR_ROUNDS;
 }
 
 // pm_demod: PLLCarrierTrackingBlock over the AGC output (pm_agc -> pm_pll; junction check / repair rounds as for the Costas loop, with
@@ -632,15 +642,11 @@ void Demod::run_pll(const float2 *in, float2 *out, long n, float bw, float max_o
     }
     P.fmax = max_offset; // PLLCarrierTrackingBlock(input, bw, max_offset, -max_offset)
     P.fmin = -max_offset;
-    k_pll<<<nblk, SEG_THREADS, PLL_SMEM_BYTES, stream>>>(in, n, L, Wp, nseg, P, S->pll[cur], d_atan_tab.p, out, crec.p, nullptr, nullptr);
-    k_costas_fix<<<1, 1024, 0, stream>>>(crec.p, nseg, 1, tol_pphase, tol_pfreq, quad.p, S->pll[nxt], &S->pll_unconv, repair.p + 1, repair.p, 0, &S->repairs);
-    for (int round = 1; round <= REPAIR_ROUNDS; round++) { // both kernels return at once when no junction is flagged
-        k_pll<<<8, SEG_THREADS, PLL_SMEM_BYTES, stream>>>(in, n, L, Wp, nseg, P, S->pll[cur], d_atan_tab.p, out, crec.p, repair.p + 1, repair.p);
+    run_loop_stage(*this, nblk, [&](int grid, const int *list, const int *count, int round) {
+        k_pll<<<grid, SEG_THREADS, PLL_SMEM_BYTES, stream>>>(in, n, L, Wp, nseg, P, S->pll[cur], d_atan_tab.p, out, crec.p, list, count);
         k_costas_fix<<<1, 1024, 0, stream>>>(crec.p, nseg, 1, tol_pphase, tol_pfreq, quad.p, S->pll[nxt], &S->pll_unconv, repair.p + 1, repair.p, round,
                                              &S->repairs);
-        launches += 2;
-    }
-    launches += 2;
+    });
 }
 
 void Demod::stage_pll(long n, int cur, int nxt)
@@ -680,19 +686,15 @@ float2 *Demod::stage_costas(long n, int L, int nseg, int cur, int nxt, bool mate
         P.fmin = -cfg.costas_max_offset;
         P.fmax = cfg.costas_max_offset;
         const auto costas = order == 2 ? k_costas<2> : (order == 4 ? k_costas<4> : k_costas<8>);
-        costas<<<nblk, SEG_THREADS, COSTAS_SMEM_BYTES, stream>>>(fir_out, n, L, Wc, Gc, nseg, P, S->costas[cur], cos_out, crec.p, nullptr, nullptr);
-        k_costas_fix<<<1, 1024, 0, stream>>>(crec.p, nseg, order, tol_cphase, tol_cfreq, quad.p, S->costas[nxt], &S->costas_unconv, repair.p + 1, repair.p, 0,
-                                             &S->repairs);
-        for (int round = 1; round <= REPAIR_ROUNDS; round++) { // both kernels return at once when no junction is flagged
-            costas<<<8, SEG_THREADS, COSTAS_SMEM_BYTES, stream>>>(fir_out, n, L, Wc, Gc, nseg, P, S->costas[cur], cos_out, crec.p, repair.p + 1, repair.p);
+        run_loop_stage(*this, nblk, [&](int grid, const int *list, const int *count, int round) {
+            costas<<<grid, SEG_THREADS, COSTAS_SMEM_BYTES, stream>>>(fir_out, n, L, Wc, Gc, nseg, P, S->costas[cur], cos_out, crec.p, list, count);
             k_costas_fix<<<1, 1024, 0, stream>>>(crec.p, nseg, order, tol_cphase, tol_cfreq, quad.p, S->costas[nxt], &S->costas_unconv, repair.p + 1, repair.p,
                                                  round, &S->repairs);
-            launches += 2;
-        }
+        });
         if (!materialise && !cfg.post_costas_dc) {
             // fused: the clock recovery rotates (and, for OQPSK, delays) its input rows itself
             k_mm_prep<<<1, 32, 0, stream>>>(bufB.p, n, L, order, quad.p, S->mm_hist[cur], S->mm_hist[nxt]);
-            launches += 3;
+            launches += 1;
             mm_quad = quad.p;
             mm_rot = order;
             mm_oqpsk = cfg.constellation == B200_OQPSK;
@@ -700,7 +702,7 @@ float2 *Demod::stage_costas(long n, int L, int nseg, int cur, int nxt, bool mate
         }
         mmin = bufA.p; // FIR output is dead now: reuse its buffer (in place compatible: same index mapping)
         k_rotate<<<2048, 256, 0, stream>>>(cos_out, n, L, order, cfg.constellation == B200_OQPSK, quad.p, S->mm_hist[cur], S->mm_hist[nxt], mmin);
-        launches += 3;
+        launches += 1;
         if (cfg.post_costas_dc) {
             // CorrectIQBlock on the loop's output (module_psk_demod.cpp:127-134); the clock recovery's 8-sample history are ITS outputs
             run_dc(mmin + 16, B200_CF32, 0, n, &S->dc_acc2[cur], &S->dc_acc2[nxt], pdc_out.p + 16);
@@ -734,19 +736,15 @@ void Demod::stage_mm(float2 *mmin, long n, int L, int nseg, int cur, int nxt, in
     MP.mu_gain = cfg.clock_gain_mu;
     const int cap = slot_cap_for(L);
     B200_REQUIRE((size_t)nseg * cap <= slots.n, B200_ENOMEM, "internal: symbol slot storage too small");
-    mm<<<nblk, SEG_THREADS, MM_SMEM_BYTES, stream>>>(mmin, n, L, Wm, Gm, nseg, MP, &S->mm[cur], &S->mm[nxt], d_bank.p, slots.p, cap, mrec.p, nullptr, nullptr,
-                                                    mm_quad, mm_rot, mm_oqpsk);
-    k_mm_scan<<<1, 1024, 0, stream>>>(mrec.p, nseg, tol_mm, offs.p, &S->mm_unconv, cap, &S->flags, repair.p + 1, repair.p, 0, &S->repairs);
-    for (int round = 1; round <= REPAIR_ROUNDS; round++) {
-        mm<<<8, SEG_THREADS, MM_SMEM_BYTES, stream>>>(mmin, n, L, Wm, Gm, nseg, MP, &S->mm[cur], &S->mm[nxt], d_bank.p, slots.p, cap, mrec.p, repair.p + 1, repair.p,
-                                                     mm_quad, mm_rot, mm_oqpsk);
+    run_loop_stage(*this, nblk, [&](int grid, const int *list, const int *count, int round) {
+        mm<<<grid, SEG_THREADS, MM_SMEM_BYTES, stream>>>(mmin, n, L, Wm, Gm, nseg, MP, &S->mm[cur], &S->mm[nxt], d_bank.p, slots.p, cap, mrec.p, list, count,
+                                                        mm_quad, mm_rot, mm_oqpsk);
         k_mm_scan<<<1, 1024, 0, stream>>>(mrec.p, nseg, tol_mm, offs.p, &S->mm_unconv, cap, &S->flags, repair.p + 1, repair.p, round, &S->repairs);
-        launches += 2;
-    }
+    });
     k_mm_compact<<<std::min(nseg, 132 * 8), 256, 0, stream>>>(slots.p, cap, mrec.p, offs.p, nseg, pm ? 2 : (bps == 1), all_symbols ? 1 : 0, sym_out.p,
                                                               sdst);
     k_snr_m2m4<<<1, 1024, 0, stream>>>(sym_out.p, offs.p + nseg, 0.001f, S->snr_y[cur], S->snr_y[nxt]); // M2M4SNREstimator(alpha = 0.001)
-    launches += 4;
+    launches += 2;
 }
 
 // SmartResamplerBlock (module_demod_base.cpp:203-204; behind PMToBPSK for pm_demod with resample_after_pll): power-of-two decimator

@@ -13,16 +13,17 @@
 //
 // The reference runs every stage as a serial per-sample loop. Here:
 //   * AGC: g' = g(1-r|x|) + r is an affine map -> per-tile composition (k_agc_compose), a scan over tiles
-//     (k_agc_scan) and an in-tile block scan in fp64, then an 8-sample replay of the reference's float recurrence.
+//     (k_tile_scan) and an in-tile block scan in fp64, then an 8-sample replay of the reference's float recurrence.
 //   * FIR: data parallel, fused with conversion + AGC scale (k_agc_fir_w).
 //   * Costas / M&M: contracting feedback loops -> one thread per stream segment, started W samples early
 //     (warm-up) so it has converged onto the sequential trajectory at its first owned sample; the first segment
 //     starts from the exact carried state. Costas segments converge up to a k*2pi/order rotation, which
-//     k_costas_fix resolves as a prefix sum; k_rotate applies it (exactly) before M&M, whose TED is not
-//     rotation invariant. Junction consistency is checked on the device and reported in the stats.
+//     k_costas_fix resolves as a prefix sum; k_mm applies it (exactly) to each input row it stages, since its TED
+//     is not rotation invariant. Junction consistency is checked on the device and reported in the stats.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <type_traits>
 
 namespace b200
 {
@@ -45,6 +46,7 @@ struct FirTaps { float h[32]; };
 struct Affine { double a, b; };     // g -> a*g + b
 struct Affine3 { double a, b, c; }; // g -> min(a*g + b, c): an AGC step with its max_gain clamp (agc.cpp:34-35); closed under composition
 struct DcAff { double a, br, bi; };  // DC blocker: acc -> a*acc + (br, bi)
+constexpr double AGC_NO_CLAMP = 1e30; // "c" of an Affine3 without a clamp (finite, so that a * c + b stays a number)
 
 template <int FMT> struct RawBytes;
 template <> struct RawBytes<0> { static constexpr int v = 8; };
@@ -290,25 +292,134 @@ __global__ void __launch_bounds__(256) k_decim_fir(const void *__restrict__ raw,
     out[j] = make_float2(re, im);
 }
 
-// ---------------------------------------------------------------- K0': front-end DC blocker ("dc_block")
-// CorrectIQBlock<complex_t>::work (utils/correct_iq.cpp:18-35): acc = acc*beta + x*alpha; y = x - acc, alpha = 1e-4, beta = 1 - alpha.
-// A constant-coefficient linear recurrence: tiles of 2048 samples, each thread runs the reference's float recurrence over its 8
-// samples from 0, the (beta^8, partial) maps are composed in fp64 (k_dc_tile -> k_dc_scan over tiles -> k_dc_apply), and every thread
-// replays its 8 samples from its scanned accumulator. Output cf32 (what the reference hands to the resampler / AGC).
-__device__ __forceinline__ DcAff dc_compose(const DcAff f, const DcAff s) { return DcAff{s.a * f.a, fma(s.a, f.br, s.br), fma(s.a, f.bi, s.bi)}; }
-__device__ __forceinline__ DcAff dc_warp_scan(DcAff v, int lane)
+// ---------------------------------------------------------------- affine recurrences scanned over 2048-sample tiles
+// The DC blocker and the AGC's exact and clamp passes turn a serial recurrence into maps composed in fp64: per thread over its 8 samples,
+// over the tile (tile_reduce), then across the tiles by one CTA (k_tile_scan) from the value carried over from the previous batch. Each
+// map type has an identity, a composition compose(first, second) = second o first, a lane shuffle and its application to a seed.
+__device__ __forceinline__ Affine compose(const Affine &first, const Affine &second)
+{
+    Affine r;
+    r.a = second.a * first.a;
+    r.b = fma(second.a, first.b, second.b);
+    return r;
+}
+// (second o first)(g) = min(a2 min(a1 g + b1, c1) + b2, c2) = min(a2 a1 g + a2 b1 + b2, min(a2 c1 + b2, c2))   for a2 >= 0
+__device__ __forceinline__ Affine3 compose(const Affine3 &first, const Affine3 &second)
+{
+    Affine3 r;
+    r.a = second.a * first.a;
+    r.b = fma(second.a, first.b, second.b);
+    r.c = fmin(fma(second.a, first.c, second.b), second.c);
+    return r;
+}
+__device__ __forceinline__ DcAff compose(const DcAff f, const DcAff s) { return DcAff{s.a * f.a, fma(s.a, f.br, s.br), fma(s.a, f.bi, s.bi)}; }
+
+template <class M> __device__ __forceinline__ M ident();
+template <> __device__ __forceinline__ Affine ident<Affine>() { return Affine{1.0, 0.0}; }
+template <> __device__ __forceinline__ Affine3 ident<Affine3>() { return Affine3{1.0, 0.0, AGC_NO_CLAMP}; }
+template <> __device__ __forceinline__ DcAff ident<DcAff>() { return DcAff{1.0, 0.0, 0.0}; }
+
+__device__ __forceinline__ Affine shfl_up(const Affine &v, int off)
+{
+    return Affine{__shfl_up_sync(0xffffffffu, v.a, off), __shfl_up_sync(0xffffffffu, v.b, off)};
+}
+__device__ __forceinline__ Affine3 shfl_up(const Affine3 &v, int off)
+{
+    return Affine3{__shfl_up_sync(0xffffffffu, v.a, off), __shfl_up_sync(0xffffffffu, v.b, off), __shfl_up_sync(0xffffffffu, v.c, off)};
+}
+__device__ __forceinline__ DcAff shfl_up(const DcAff &v, int off)
+{
+    return DcAff{__shfl_up_sync(0xffffffffu, v.a, off), __shfl_up_sync(0xffffffffu, v.br, off), __shfl_up_sync(0xffffffffu, v.bi, off)};
+}
+
+// the map applied to a seed: an AGC gain, or the DC blocker's complex accumulator; widen = the carried float value as a seed
+__device__ __forceinline__ double apply(const Affine &m, double g) { return fma(m.a, g, m.b); }
+__device__ __forceinline__ double apply(const Affine3 &m, double g) { return fmin(fma(m.a, g, m.b), m.c); }
+__device__ __forceinline__ double2 apply(const DcAff &m, double2 g) { return make_double2(fma(m.a, g.x, m.br), fma(m.a, g.y, m.bi)); }
+__device__ __forceinline__ double widen(float g) { return (double)g; }
+__device__ __forceinline__ double2 widen(float2 g) { return make_double2((double)g.x, (double)g.y); }
+
+// inclusive scan over the lanes: lane i gets v_i o ... o v_0
+template <class M> __device__ __forceinline__ M warp_scan(M v, int lane)
 {
 #pragma unroll
     for (int off = 1; off < 32; off <<= 1) {
-        DcAff p;
-        p.a = __shfl_up_sync(0xffffffffu, v.a, off);
-        p.br = __shfl_up_sync(0xffffffffu, v.br, off);
-        p.bi = __shfl_up_sync(0xffffffffu, v.bi, off);
+        const M p = shfl_up(v, off);
         if (lane >= off)
-            v = dc_compose(p, v);
+            v = compose(p, v);
     }
     return v;
 }
+
+// the composition of the FIR_THREADS threads' maps m (thread order) -> *out, written by thread 0
+template <class M> __device__ __forceinline__ void tile_reduce(M m, M *out)
+{
+    __shared__ M wsum[FIR_THREADS / 32];
+    const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+    m = warp_scan(m, lane);
+    if (lane == 31)
+        wsum[warp] = m;
+    __syncthreads();
+    if (t == 0) {
+        M tot = wsum[0];
+        for (int w = 1; w < FIR_THREADS / 32; w++)
+            tot = compose(tot, wsum[w]);
+        *out = tot;
+    }
+}
+
+// seeds[k] = the value before tile k and seeds[ntiles] = after the batch, scanned from the carried value *in. Returns at once unless
+// (*gate & mask) != 0 (gate = nullptr: always runs); count (may be nullptr) counts the runs.
+template <class M, class S, class In>
+__global__ void __launch_bounds__(1024) k_tile_scan(const M *__restrict__ tile_map, int ntiles, const In *__restrict__ in, const int *__restrict__ gate,
+                                                   int mask, S *__restrict__ seeds, int *__restrict__ count)
+{
+    if (gate && (*gate & mask) == 0)
+        return;
+    if (count && threadIdx.x == 0)
+        *count += 1;
+    __shared__ M wsum[32];
+    __shared__ S run;
+    const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+    if (t == 0)
+        run = widen(*in);
+    __syncthreads();
+    for (int base = 0; base < ntiles; base += 1024) {
+        const int k = base + t;
+        M m = ident<M>();
+        if (k < ntiles)
+            m = tile_map[k];
+        const M inc = warp_scan(m, lane);
+        if (lane == 31)
+            wsum[warp] = inc;
+        __syncthreads();
+        if (warp == 0) {
+            const M w = warp_scan(wsum[lane], lane);
+            wsum[lane] = w;
+        }
+        __syncthreads();
+        M pre = ident<M>(); // composition of everything before this thread's tile in this round
+        if (warp > 0)
+            pre = wsum[warp - 1];
+        const M e = shfl_up(inc, 1);
+        const M excl = lane > 0 ? compose(pre, e) : pre;
+        const S g0 = run;
+        if (k < ntiles)
+            seeds[k] = apply(excl, g0);
+        __syncthreads();
+        if (t == 1023)
+            run = apply(compose(pre, inc), g0);
+        __syncthreads();
+    }
+    if (t == 0)
+        seeds[ntiles] = run;
+}
+
+// ---------------------------------------------------------------- K0': front-end DC blocker ("dc_block")
+// CorrectIQBlock<complex_t>::work (utils/correct_iq.cpp:18-35): acc = acc*beta + x*alpha; y = x - acc, alpha = 1e-4, beta = 1 - alpha.
+// A constant-coefficient linear recurrence: tiles of 2048 samples, each thread runs the reference's float recurrence over its 8
+// samples from 0, the (beta^8, partial) maps are composed in fp64 (k_dc_tile -> k_tile_scan over tiles -> k_dc_apply), and every thread
+// replays its 8 samples from its scanned accumulator. Output cf32 (what the reference hands to the resampler / AGC).
 template <int FMT>
 __device__ __forceinline__ DcAff dc_local(const void *__restrict__ raw, long s0, long N, int iq_swap, float alpha, float beta, float2 (&x)[8])
 {
@@ -330,64 +441,8 @@ __device__ __forceinline__ DcAff dc_local(const void *__restrict__ raw, long s0,
 template <int FMT>
 __global__ void __launch_bounds__(FIR_THREADS) k_dc_tile(const void *__restrict__ raw, long N, int iq_swap, float alpha, float beta, DcAff *__restrict__ tile_map)
 {
-    __shared__ DcAff wsum[FIR_THREADS / 32];
-    const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
     float2 x[8];
-    DcAff m = dc_local<FMT>(raw, (long)blockIdx.x * FIR_TILE + 8 * t, N, iq_swap, alpha, beta, x);
-    m = dc_warp_scan(m, lane);
-    if (lane == 31)
-        wsum[warp] = m;
-    __syncthreads();
-    if (t == 0) {
-        DcAff tot = wsum[0];
-        for (int w = 1; w < FIR_THREADS / 32; w++)
-            tot = dc_compose(tot, wsum[w]);
-        tile_map[blockIdx.x] = tot;
-    }
-}
-// seeds[k] = accumulator before tile k; seeds[ntiles] = after the batch (carried to the next one through acc_io)
-__global__ void __launch_bounds__(1024) k_dc_scan(const DcAff *__restrict__ tile_map, int ntiles, const float2 *__restrict__ acc_in, double2 *__restrict__ seeds)
-{
-    __shared__ DcAff wsum[32];
-    __shared__ double2 run;
-    const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
-    if (t == 0)
-        run = make_double2((double)acc_in->x, (double)acc_in->y);
-    __syncthreads();
-    for (int base = 0; base < ntiles; base += 1024) {
-        const int k = base + t;
-        DcAff m{1.0, 0.0, 0.0};
-        if (k < ntiles)
-            m = tile_map[k];
-        const DcAff inc = dc_warp_scan(m, lane);
-        if (lane == 31)
-            wsum[warp] = inc;
-        __syncthreads();
-        if (warp == 0) {
-            DcAff w = dc_warp_scan(wsum[lane], lane);
-            wsum[lane] = w;
-        }
-        __syncthreads();
-        DcAff pre{1.0, 0.0, 0.0};
-        if (warp > 0)
-            pre = wsum[warp - 1];
-        DcAff e;
-        e.a = __shfl_up_sync(0xffffffffu, inc.a, 1);
-        e.br = __shfl_up_sync(0xffffffffu, inc.br, 1);
-        e.bi = __shfl_up_sync(0xffffffffu, inc.bi, 1);
-        const DcAff excl = lane > 0 ? dc_compose(pre, e) : pre;
-        const double2 g0 = run;
-        if (k < ntiles)
-            seeds[k] = make_double2(fma(excl.a, g0.x, excl.br), fma(excl.a, g0.y, excl.bi));
-        __syncthreads();
-        if (t == 1023) {
-            const DcAff tot = dc_compose(pre, inc);
-            run = make_double2(fma(tot.a, g0.x, tot.br), fma(tot.a, g0.y, tot.bi));
-        }
-        __syncthreads();
-    }
-    if (t == 0)
-        seeds[ntiles] = run;
+    tile_reduce(dc_local<FMT>(raw, (long)blockIdx.x * FIR_TILE + 8 * threadIdx.x, N, iq_swap, alpha, beta, x), &tile_map[blockIdx.x]);
 }
 template <int FMT>
 __global__ void __launch_bounds__(FIR_THREADS) k_dc_apply(const void *__restrict__ raw, long N, int iq_swap, float alpha, float beta,
@@ -398,20 +453,17 @@ __global__ void __launch_bounds__(FIR_THREADS) k_dc_apply(const void *__restrict
     const long s0 = (long)blockIdx.x * FIR_TILE + 8 * t;
     float2 x[8];
     const DcAff m = dc_local<FMT>(raw, s0, N, iq_swap, alpha, beta, x);
-    const DcAff inc = dc_warp_scan(m, lane);
+    const DcAff inc = warp_scan(m, lane);
     if (lane == 31)
         wsum[warp] = inc;
     __syncthreads();
-    DcAff pre{1.0, 0.0, 0.0};
+    DcAff pre = ident<DcAff>();
     for (int w = 0; w < warp; w++)
-        pre = dc_compose(pre, wsum[w]);
-    DcAff e;
-    e.a = __shfl_up_sync(0xffffffffu, inc.a, 1);
-    e.br = __shfl_up_sync(0xffffffffu, inc.br, 1);
-    e.bi = __shfl_up_sync(0xffffffffu, inc.bi, 1);
-    const DcAff excl = lane > 0 ? dc_compose(pre, e) : pre;
-    const double2 g0 = seeds[blockIdx.x];
-    float2 acc = make_float2((float)fma(excl.a, g0.x, excl.br), (float)fma(excl.a, g0.y, excl.bi));
+        pre = compose(pre, wsum[w]);
+    const DcAff e = shfl_up(inc, 1);
+    const DcAff excl = lane > 0 ? compose(pre, e) : pre;
+    const double2 g = apply(excl, seeds[blockIdx.x]);
+    float2 acc = make_float2((float)g.x, (float)g.y);
 #pragma unroll
     for (int i = 0; i < 8; i++)
         if (s0 + i < N) {
@@ -453,37 +505,6 @@ __device__ __forceinline__ EB eb_compose_if(bool take, const EB first, const EB 
     return r;
 }
 
-__device__ __forceinline__ Affine compose(const Affine &first, const Affine &second)
-{
-    Affine r;
-    r.a = second.a * first.a;
-    r.b = fma(second.a, first.b, second.b);
-    return r;
-}
-
-// (second o first)(g) = min(a2 min(a1 g + b1, c1) + b2, c2) = min(a2 a1 g + a2 b1 + b2, min(a2 c1 + b2, c2))   for a2 >= 0
-__device__ __forceinline__ Affine3 compose3(const Affine3 &first, const Affine3 &second)
-{
-    Affine3 r;
-    r.a = second.a * first.a;
-    r.b = fma(second.a, first.b, second.b);
-    r.c = fmin(fma(second.a, first.c, second.b), second.c);
-    return r;
-}
-__device__ __forceinline__ Affine3 warp_scan_inclusive3(Affine3 v, int lane)
-{
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-        Affine3 p;
-        p.a = __shfl_up_sync(0xffffffffu, v.a, off);
-        p.b = __shfl_up_sync(0xffffffffu, v.b, off);
-        p.c = __shfl_up_sync(0xffffffffu, v.c, off);
-        if (lane >= off)
-            v = compose3(p, v);
-    }
-    return v;
-}
-constexpr double AGC_NO_CLAMP = 1e30;     // "c" of a map without a clamp (finite, so that a * c + b stays a number)
 struct EBC { float E, B, C; };            // g -> min(g*(1 - E) + B, C), the float form used inside a tile
 __device__ __forceinline__ EBC ebc_compose(const EBC first, const EBC second)
 {
@@ -492,20 +513,6 @@ __device__ __forceinline__ EBC ebc_compose(const EBC first, const EBC second)
     r.E = fmaf(-first.E, second.E, first.E + second.E);
     r.C = fminf(fmaf(-second.E, first.C, first.C) + second.B, second.C);
     return r;
-}
-
-__device__ __forceinline__ Affine warp_scan_inclusive(Affine v, int lane)
-{
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-        double pa = __shfl_up_sync(0xffffffffu, v.a, off);
-        double pb = __shfl_up_sync(0xffffffffu, v.b, off);
-        if (lane >= off) {
-            Affine p{pa, pb};
-            v = compose(p, v);
-        }
-    }
-    return v;
 }
 
 // smem index (float2 units): 8 samples + 16 B pad per group -> 16-byte aligned, conflict-free 128-bit accesses at a thread
@@ -859,167 +866,34 @@ __global__ void __launch_bounds__(32 * FW_WARPS, 8) k_agc_fir_w(const void *__re
         fw_chunk<FMT, DUMP, CLAMP, false>(st, rr, c, true, taps, tail_out, fir_out, agc_dump, gain_out, flags);
 }
 
-// ---------------------------------------------------------------- exact pass (weak signals): per-tile maps -> scan -> seeds
-template <int FMT>
-__global__ void __launch_bounds__(FIR_THREADS) k_agc_compose(const void *__restrict__ raw, long N, float rate, const int *__restrict__ need, int ntiles,
-                                                             Affine *__restrict__ tile_map)
+// ---------------------------------------------------------------- exact and clamp passes: per-tile maps -> k_tile_scan -> seeds
+// Per-tile composition of the AGC steps g -> (1 - rate|x|) g + rate: as Affine for the exact pass (weak signals), as Affine3 with the
+// max_gain clamp for the clamp pass (the gain hit max_gain in this batch). Returns at once unless (*gate & mask) != 0: need[epoch & 1]
+// for the exact pass, flags bit 0 for the clamp pass.
+template <int FMT, class M>
+__global__ void __launch_bounds__(FIR_THREADS) k_agc_compose(const void *__restrict__ raw, long N, float rate, double max_gain, const int *__restrict__ gate,
+                                                             int mask, int ntiles, M *__restrict__ tile_map)
 {
-    if (*need == 0) // the usual case: a small grid that returns at once
+    if ((*gate & mask) == 0) // the usual case: a small grid that returns at once
         return;
-    const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
-    __shared__ Affine wsum[FIR_THREADS / 32];
+    const int t = threadIdx.x;
     for (int k = blockIdx.x; k < ntiles; k += gridDim.x) {
         const long s0 = (long)k * FIR_TILE + 8 * t;
-        Affine m{1.0, 0.0};
+        M m = ident<M>();
         float2 x[8];
         load8<FMT>(raw, s0, N, x);
 #pragma unroll
         for (int i = 0; i < 8; i++)
             if (s0 + i < N) {
                 const float mag = fast_mag(fmaf(x[i].x, x[i].x, x[i].y * x[i].y));
-                m = compose(m, Affine{1.0 - (double)rate * (double)mag, (double)rate});
+                if constexpr (std::is_same<M, Affine3>::value)
+                    m = compose(m, Affine3{1.0 - (double)rate * (double)mag, (double)rate, max_gain});
+                else
+                    m = compose(m, Affine{1.0 - (double)rate * (double)mag, (double)rate});
             }
-        m = warp_scan_inclusive(m, lane);
-        if (lane == 31)
-            wsum[warp] = m;
-        __syncthreads();
-        if (t == 0) {
-            Affine tot = wsum[0];
-            for (int w = 1; w < FIR_THREADS / 32; w++)
-                tot = compose(tot, wsum[w]);
-            tile_map[k] = tot;
-        }
+        tile_reduce(m, &tile_map[k]);
         __syncthreads();
     }
-}
-
-// clamp-aware versions of the two kernels above (run only when the flag says the gain hit max_gain in this batch)
-template <int FMT>
-__global__ void __launch_bounds__(FIR_THREADS) k_agc_compose3(const void *__restrict__ raw, long N, float rate, double max_gain, const int *__restrict__ flags,
-                                                              int ntiles, Affine3 *__restrict__ tile_map)
-{
-    if ((*flags & 1) == 0)
-        return;
-    const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
-    __shared__ Affine3 wsum[FIR_THREADS / 32];
-    for (int k = blockIdx.x; k < ntiles; k += gridDim.x) {
-        const long s0 = (long)k * FIR_TILE + 8 * t;
-        Affine3 m{1.0, 0.0, AGC_NO_CLAMP};
-        float2 x[8];
-        load8<FMT>(raw, s0, N, x);
-#pragma unroll
-        for (int i = 0; i < 8; i++)
-            if (s0 + i < N) {
-                const float mag = fast_mag(fmaf(x[i].x, x[i].x, x[i].y * x[i].y));
-                m = compose3(m, Affine3{1.0 - (double)rate * (double)mag, (double)rate, max_gain});
-            }
-        m = warp_scan_inclusive3(m, lane);
-        if (lane == 31)
-            wsum[warp] = m;
-        __syncthreads();
-        if (t == 0) {
-            Affine3 tot = wsum[0];
-            for (int w = 1; w < FIR_THREADS / 32; w++)
-                tot = compose3(tot, wsum[w]);
-            tile_map[k] = tot;
-        }
-        __syncthreads();
-    }
-}
-__global__ void __launch_bounds__(1024) k_agc_scan3(const Affine3 *__restrict__ tile_map, int ntiles, const float *__restrict__ gain_in,
-                                                   const int *__restrict__ flags, double *__restrict__ seeds)
-{
-    if ((*flags & 1) == 0)
-        return;
-    __shared__ Affine3 wsum[32];
-    __shared__ double g_run;
-    const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
-    if (t == 0)
-        g_run = (double)*gain_in;
-    __syncthreads();
-    for (int base = 0; base < ntiles; base += 1024) {
-        const int k = base + t;
-        Affine3 m{1.0, 0.0, AGC_NO_CLAMP};
-        if (k < ntiles)
-            m = tile_map[k];
-        const Affine3 inc = warp_scan_inclusive3(m, lane);
-        if (lane == 31)
-            wsum[warp] = inc;
-        __syncthreads();
-        if (warp == 0) {
-            Affine3 w = warp_scan_inclusive3(wsum[lane], lane);
-            wsum[lane] = w;
-        }
-        __syncthreads();
-        Affine3 pre{1.0, 0.0, AGC_NO_CLAMP};
-        if (warp > 0)
-            pre = wsum[warp - 1];
-        Affine3 e;
-        e.a = __shfl_up_sync(0xffffffffu, inc.a, 1);
-        e.b = __shfl_up_sync(0xffffffffu, inc.b, 1);
-        e.c = __shfl_up_sync(0xffffffffu, inc.c, 1);
-        const Affine3 excl = lane > 0 ? compose3(pre, e) : pre;
-        const double g0 = g_run;
-        if (k < ntiles)
-            seeds[k] = fmin(fma(excl.a, g0, excl.b), excl.c);
-        __syncthreads();
-        if (t == 1023) {
-            const Affine3 tot = compose3(pre, inc);
-            g_run = fmin(fma(tot.a, g0, tot.b), tot.c);
-        }
-        __syncthreads();
-    }
-    if (t == 0)
-        seeds[ntiles] = g_run;
-}
-
-__global__ void __launch_bounds__(1024) k_agc_scan(const Affine *__restrict__ tile_map, int ntiles, const float *__restrict__ gain_in,
-                                                  const int *__restrict__ need, double *__restrict__ seeds, int *__restrict__ exact_count)
-{
-    if (*need == 0)
-        return;
-    if (threadIdx.x == 0)
-        *exact_count += 1;
-    __shared__ Affine wsum[32];
-    __shared__ double g_run;
-    const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
-    if (t == 0)
-        g_run = (double)*gain_in;
-    __syncthreads();
-    for (int base = 0; base < ntiles; base += 1024) {
-        int k = base + t;
-        Affine m{1.0, 0.0};
-        if (k < ntiles)
-            m = tile_map[k];
-        Affine inc = warp_scan_inclusive(m, lane);
-        if (lane == 31)
-            wsum[warp] = inc;
-        __syncthreads();
-        if (warp == 0) {
-            Affine w = wsum[lane];
-            w = warp_scan_inclusive(w, lane);
-            wsum[lane] = w;
-        }
-        __syncthreads();
-        Affine pre{1.0, 0.0}; // composition of everything before this thread's tile in this round
-        if (warp > 0)
-            pre = wsum[warp - 1];
-        double ea = __shfl_up_sync(0xffffffffu, inc.a, 1), eb = __shfl_up_sync(0xffffffffu, inc.b, 1);
-        Affine excl = pre;
-        if (lane > 0)
-            excl = compose(pre, Affine{ea, eb});
-        double g0 = g_run;
-        if (k < ntiles)
-            seeds[k] = fma(excl.a, g0, excl.b);
-        __syncthreads();
-        if (t == 1023) {
-            Affine tot = compose(pre, inc);
-            g_run = fma(tot.a, g0, tot.b);
-        }
-        __syncthreads();
-    }
-    if (t == 0)
-        seeds[ntiles] = g_run;
 }
 
 // ---------------------------------------------------------------- test hook: the FIR alone (b200_demod_debug_run_stage)
@@ -1049,12 +923,7 @@ template <bool STRICT> __global__ void __launch_bounds__(256) k_fir_only(const f
     out[i] = make_float2(ar, ai);
 }
 
-// ---------------------------------------------------------------- cp.async helpers (8-byte granules)
-__device__ __forceinline__ void cp_async8(void *smem_dst, const void *gmem_src)
-{
-    unsigned sa = (unsigned)__cvta_generic_to_shared(smem_dst);
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;\n" ::"r"(sa), "l"(gmem_src));
-}
+// ---------------------------------------------------------------- cp.async helpers
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
 template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N)); }
 
@@ -1082,12 +951,10 @@ __device__ __forceinline__ void cp_async16(void *smem_dst, const void *gmem_src)
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(sa), "l"(gmem_src));
 }
 
-// copies row `row` (16 samples from sample index 16*row; may be negative for the history pad) of every lane's thread into
-// dst (swizzled). `base` must be 16-byte aligned at sample 0 and readable from the first requested sample on.
-// pbase < 0: the destination is a per-thread RING addressed by the row number (chunk slot = 8*row mod (pmask+1)), which differs
-// between the threads of a warp; pbase >= 0: one fixed slot group for the whole warp.
-__device__ __forceinline__ void warp_load_rows(float4 *dst, int pbase, int pmask, const float2 *__restrict__ base, int row, bool row_valid, long limit,
-                                               int lane)
+// copies row `row` (16 samples from sample index 16*row; may be negative for the history pad) of every lane's thread into that
+// thread's ring of 32 chunk slots in dst (swizzled): chunk c of row r lands in slot (8r + 64 + c) mod 32. `base` must be 16-byte aligned
+// at sample 0 and readable from the first requested sample on.
+__device__ __forceinline__ void warp_load_rows(float4 *dst, const float2 *__restrict__ base, int row, bool row_valid, long limit, int lane)
 {
 #pragma unroll
     for (int i = 0; i < 8; i++) {
@@ -1095,15 +962,34 @@ __device__ __forceinline__ void warp_load_rows(float4 *dst, int pbase, int pmask
         const int r = __shfl_sync(0xffffffffu, row, T);
         const int ok = __shfl_sync(0xffffffffu, (int)row_valid, T);
         const long n0 = (long)r * 16 + 2 * c;
-        const int pb = pbase < 0 ? (r << 3) + 64 : pbase; // the SOURCE thread's row decides the ring position
+        const int pb = (r << 3) + 64; // the SOURCE thread's row decides the ring position
         if (ok && n0 < limit)
-            cp_async16(&dst[swz16((pb + c) & pmask, T)], base + n0);
+            cp_async16(&dst[swz16((pb + c) & 31, T)], base + n0);
     }
 }
 
-// Repair mode (repair_list != nullptr): thread i re-runs segment repair_list[i] with NO warm-up, starting from the recorded end
-// state of its predecessor, i.e. as the exact sequential continuation of that segment (used for junctions whose warm-up had
-// not converged; k_costas_fix re-checks afterwards).
+// The segment of this thread in the loop kernels: segment blockIdx.x * SEG_THREADS + threadIdx.x, or in repair mode
+// (repair_list != nullptr) segment repair_list[i] for the i-th of the first min(*repair_count, 1024) threads. Repair mode re-runs a
+// segment with NO warm-up, starting from the recorded end state of its predecessor, i.e. as the exact sequential continuation of that
+// segment (used for junctions whose warm-up had not converged; the junction check runs again afterwards). A thread without a segment
+// gets active = false and s = 0.
+__device__ __forceinline__ int loop_segment(int nseg, const int *__restrict__ repair_list, const int *__restrict__ repair_count, bool &active)
+{
+    int s = blockIdx.x * SEG_THREADS + threadIdx.x;
+    active = true;
+    if (repair_list) {
+        if (s >= min(*repair_count, 1024))
+            active = false;
+        else
+            s = repair_list[s];
+    }
+    if (s >= nseg)
+        active = false;
+    if (!active)
+        s = 0;
+    return s;
+}
+
 constexpr int COSTAS_SMEM_BYTES = (SEG_THREADS / 32) * (16 + 8) * 32 * 16; // per warp: 2 input rows + 1 output row of 8 chunks x 32 threads
 // Gear shift: for the first G samples of a warm-up the loop runs first order (frequency held at the carried value) with 4x the phase
 // gain: a warm-up that starts near an unstable lock point (a hang-up: the detector output is ~0 there) escapes four times faster, so
@@ -1205,46 +1091,37 @@ __device__ __forceinline__ float2 costas_step(const float2 x, CostasRegs &r, flo
     return make_float2(vr, vi);
 }
 
-// in/out: N samples. Segment s owns samples [s*L, min((s+1)L, N)); thread warms up from max(0, s*L - W).
-// state_in = {phase, freq} carried from the previous batch (exact start of segment 0 and of any clipped warm-up).
+// One thread per segment of a phase loop (k_costas, k_pll). in/out: N samples. Segment s owns samples [s*L, min((s+1)L, N)); its
+// thread warms up from max(0, s*L - W), from phase 0 and the carried frequency. state_in = {phase, freq} carried from the previous batch
+// (exact start of segment 0 and of any clipped warm-up). rec[s] = the loop state at the segment's first owned sample and at its end.
 // Rows of 16 samples move between HBM and the warp's shared-memory strip cooperatively (see swz16): lanes 8q..8q+7 carry the eight
 // 16-byte chunks of the row of thread 4i+q in their i-th copy; which row that is (its first row, row count, owned range) is
 // exchanged ONCE before the loop, so a copy costs an add, a compare and the address, no shuffles.
-template <int ORDER>
-__global__ void __launch_bounds__(SEG_THREADS) k_costas(const float2 *__restrict__ in, long N, int L, int W, int G, int nseg, CostasParams P,
-                                                         const float *__restrict__ state_in, float2 *__restrict__ out, LoopRec *__restrict__ rec,
-                                                         const int *__restrict__ repair_list, const int *__restrict__ repair_count)
+// The loop policy supplies G, the length of the gear shift at the start of a warm-up (0: none); begin(phase, freq, gear_end): the start
+// state, with samples below gear_end in the gear shift; row(mine, ring, slot, obuf, lane, b, own1): the loop over the staged row of
+// samples b .. b+15 (those below own1; nothing unless mine) into obuf; and phase() / freq(), the state that goes into the record.
+template <class Loop>
+__device__ __forceinline__ void loop_segments(Loop &lp, unsigned char *smem, const float2 *__restrict__ in, long N, int L, int W, int nseg,
+                                              const float *__restrict__ state_in, float2 *__restrict__ out, LoopRec *__restrict__ rec,
+                                              const int *__restrict__ repair_list, const int *__restrict__ repair_count)
 {
-    extern __shared__ __align__(16) unsigned char cs_smem[];
     const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
-    float4 *ring = reinterpret_cast<float4 *>(cs_smem) + warp * (24 * 32); // [16 chunk slots][32] in, then [8][32] out
+    float4 *ring = reinterpret_cast<float4 *>(smem) + warp * (24 * 32); // [16 chunk slots][32] in, then [8][32] out
     float4 *obuf = ring + 16 * 32;
-    int s = blockIdx.x * SEG_THREADS + t;
-    bool active = true;
-    if (repair_list) {
-        if (s >= min(*repair_count, 1024))
-            active = false;
-        else
-            s = repair_list[s];
-    }
-    if (s >= nseg)
-        active = false;
-    if (!active)
-        s = 0;
+    bool active;
+    const int s = loop_segment(nseg, repair_list, repair_count, active);
     const long own0 = (long)s * L;
     const long own1 = active ? min(own0 + L, N) : own0;
-    long start = own0 - W, gear_end = own0 - W + G;
-    CostasRegs r;
-    r.phase = 0.f;
-    r.freq = state_in[1];
+    long start = own0 - W, gear_end = own0 - W + lp.G;
+    float phase = 0.f, freq = state_in[1];
     if (repair_list && active) {
         start = own0;
-        r.phase = rec[s - 1].ph_end;
-        r.freq = rec[s - 1].fr_end;
+        phase = rec[s - 1].ph_end;
+        freq = rec[s - 1].fr_end;
         gear_end = 0;
     } else if (start <= 0) {
         start = 0;
-        r.phase = state_in[0];
+        phase = state_in[0];
         gear_end = 0;
     }
     const int row0 = (int)(start >> 4), row1 = (int)((own1 + 15) >> 4); // rows of 16 samples, [row0, row1)
@@ -1253,10 +1130,10 @@ __global__ void __launch_bounds__(SEG_THREADS) k_costas(const float2 *__restrict
 #pragma unroll
     for (int off = 16; off; off >>= 1)
         maxrows = max(maxrows, __shfl_xor_sync(0xffffffffu, maxrows, off));
+    lp.begin(phase, freq, gear_end);
     LoopRec lr;
-    lr.ph_start = r.phase;
-    lr.fr_start = r.freq;
-    sincos_loop_phase(r.phase, r.sn, r.cs);
+    lr.ph_start = lp.phase();
+    lr.fr_start = lp.freq();
     // what this lane needs to know about the threads whose rows it carries
     const int c = lane & 7;
     int src_row0[8], src_nrows[8], src_orow0[8], src_own1[8];
@@ -1290,9 +1167,53 @@ __global__ void __launch_bounds__(SEG_THREADS) k_costas(const float2 *__restrict
         const long b = (long)(row0 + it) << 4;
         // start / own0 are multiples of 16, so a row is entirely warm-up or entirely owned; only the batch's last row can be partial
         if (mine && b == own0) {
-            lr.ph_start = r.phase;
-            lr.fr_start = r.freq;
+            lr.ph_start = lp.phase();
+            lr.fr_start = lp.freq();
         }
+        lp.row(mine, ring, slot, obuf, lane, b, own1);
+        __syncwarp();
+        // transposed copy-out: lanes 8q..8q+7 store the eight chunks of thread 4i+q's row (owned samples only)
+#pragma unroll
+        for (int i = 0; i < 8; i++) {
+            const int T = 4 * i + (lane >> 3);
+            const int row = src_row0[i] + it;
+            const int n0 = row * 16 + 2 * c;
+            if (it < src_nrows[i] && row >= src_orow0[i] && n0 < src_own1[i]) {
+                const float4 v = obuf[swz16(c, T)];
+                if (n0 + 1 < src_own1[i])
+                    *reinterpret_cast<float4 *>(out + n0) = v;
+                else
+                    out[n0] = make_float2(v.x, v.y);
+            }
+        }
+        __syncwarp();
+    }
+    cp_async_wait<0>();
+    if (active) {
+        lr.ph_end = lp.phase();
+        lr.fr_end = lp.freq();
+        rec[s] = lr;
+    }
+}
+
+// the Costas loop as the policy of loop_segments, with the gear shift over the first G samples of a warm-up
+template <int ORDER> struct CostasLoop
+{
+    CostasParams P;
+    int G;
+    long gear_end;
+    CostasRegs r;
+    __device__ __forceinline__ float phase() const { return r.phase; }
+    __device__ __forceinline__ float freq() const { return r.freq; }
+    __device__ __forceinline__ void begin(float phase, float freq, long gear_until)
+    {
+        r.phase = phase;
+        r.freq = freq;
+        gear_end = gear_until;
+        sincos_loop_phase(r.phase, r.sn, r.cs);
+    }
+    __device__ __forceinline__ void row(bool mine, const float4 *ring, int slot, float4 *obuf, int lane, long b, long own1)
+    {
         const bool gear = b < gear_end;
         const float al = gear ? 4.0f * P.alpha : P.alpha, be = gear ? 0.0f : P.beta;
         if (mine && b + 16 <= own1) {
@@ -1324,29 +1245,17 @@ __global__ void __launch_bounds__(SEG_THREADS) k_costas(const float2 *__restrict
                 obuf[swz16(p, lane)] = make_float4(o0.x, o0.y, o1.x, o1.y);
             }
         }
-        __syncwarp();
-        // transposed copy-out: lanes 8q..8q+7 store the eight chunks of thread 4i+q's row (owned samples only)
-#pragma unroll
-        for (int i = 0; i < 8; i++) {
-            const int T = 4 * i + (lane >> 3);
-            const int row = src_row0[i] + it;
-            const int n0 = row * 16 + 2 * c;
-            if (it < src_nrows[i] && row >= src_orow0[i] && n0 < src_own1[i]) {
-                const float4 v = obuf[swz16(c, T)];
-                if (n0 + 1 < src_own1[i])
-                    *reinterpret_cast<float4 *>(out + n0) = v;
-                else
-                    out[n0] = make_float2(v.x, v.y);
-            }
-        }
-        __syncwarp();
     }
-    cp_async_wait<0>();
-    if (active) {
-        lr.ph_end = r.phase;
-        lr.fr_end = r.freq;
-        rec[s] = lr;
-    }
+};
+
+template <int ORDER>
+__global__ void __launch_bounds__(SEG_THREADS) k_costas(const float2 *__restrict__ in, long N, int L, int W, int G, int nseg, CostasParams P,
+                                                         const float *__restrict__ state_in, float2 *__restrict__ out, LoopRec *__restrict__ rec,
+                                                         const int *__restrict__ repair_list, const int *__restrict__ repair_count)
+{
+    extern __shared__ __align__(16) unsigned char cs_smem[];
+    CostasLoop<ORDER> lp{P, G};
+    loop_segments(lp, cs_smem, in, N, L, W, nseg, state_in, out, rec, repair_list, repair_count);
 }
 
 // ---------------------------------------------------------------- K2b: resolve per-segment rotation (prefix sum mod order)
@@ -1374,7 +1283,6 @@ __global__ void __launch_bounds__(1024) k_costas_fix(const LoopRec *__restrict__
         *repair_count = 0;
     }
     __syncthreads();
-    int bad = 0;
     for (int base = 0; base < nseg; base += 1024) {
         int s = base + t, k = 0;
         if (s > 0 && s < nseg) {
@@ -1383,7 +1291,6 @@ __global__ void __launch_bounds__(1024) k_costas_fix(const LoopRec *__restrict__
             float resid = fabsf(d - q * step);
             k = ((int)q % order + order) % order;
             if (resid > tol_phase || fabsf(rec[s].fr_start - rec[s - 1].fr_end) > tol_freq) {
-                bad++;
                 const int slot = atomicAdd(repair_count, 1);
                 if (slot < 1024)
                     repair_list[slot] = s;
@@ -1418,10 +1325,6 @@ __global__ void __launch_bounds__(1024) k_costas_fix(const LoopRec *__restrict__
             run = tot % order;
         __syncthreads();
     }
-    // reduce bad count
-    for (int off = 16; off; off >>= 1)
-        bad += __shfl_xor_sync(0xffffffffu, bad, off);
-    (void)bad;
     __syncthreads();
     if (t == 0) {
         *unconv = *repair_count; // junctions still failing after this pass
@@ -1519,123 +1422,51 @@ __device__ __forceinline__ float2 pll_step(const float2 x, float &phase, float &
     return o;
 }
 
-// Same staging as k_costas: rows of 16 samples move between HBM and the warp's shared-memory strip cooperatively (swz16).
-// Dynamic shared memory: COSTAS_SMEM_BYTES of strips + the 257-entry table.
+// the carrier PLL as the policy of loop_segments (no gear shift)
+struct PllLoop
+{
+    PllParams P;
+    const float *tab;
+    static constexpr int G = 0; // no gear shift
+    float ph, fr;
+    __device__ __forceinline__ float phase() const { return ph; }
+    __device__ __forceinline__ float freq() const { return fr; }
+    __device__ __forceinline__ void begin(float phase, float freq, long)
+    {
+        ph = phase;
+        fr = freq;
+    }
+    __device__ __forceinline__ void row(bool mine, const float4 *ring, int slot, float4 *obuf, int lane, long b, long own1)
+    {
+        if (!mine)
+            return;
+        const int nvalid = (int)min(16L, own1 - b);
+#pragma unroll 1
+        for (int p = 0; p < 8; p++) {
+            const float4 v = ring[swz16(slot + p, lane)];
+            float2 o0 = make_float2(0.f, 0.f), o1 = o0;
+            if (2 * p < nvalid)
+                o0 = pll_step(make_float2(v.x, v.y), ph, fr, P, tab);
+            if (2 * p + 1 < nvalid)
+                o1 = pll_step(make_float2(v.z, v.w), ph, fr, P, tab);
+            obuf[swz16(p, lane)] = make_float4(o0.x, o0.y, o1.x, o1.y);
+        }
+    }
+};
+
+// Same staging as k_costas (loop_segments). Dynamic shared memory: COSTAS_SMEM_BYTES of strips + the 257-entry table.
 constexpr int PLL_SMEM_BYTES = COSTAS_SMEM_BYTES + 260 * 4;
 __global__ void __launch_bounds__(SEG_THREADS) k_pll(const float2 *__restrict__ in, long N, int L, int W, int nseg, PllParams P,
                                                       const float *__restrict__ state_in, const float *__restrict__ atan_tab, float2 *__restrict__ out,
                                                       LoopRec *__restrict__ rec, const int *__restrict__ repair_list, const int *__restrict__ repair_count)
 {
     extern __shared__ __align__(16) unsigned char pl_smem[];
-    const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
-    float4 *ring = reinterpret_cast<float4 *>(pl_smem) + warp * (24 * 32); // [16 chunk slots][32] in, then [8][32] out
-    float4 *obuf = ring + 16 * 32;
     float *tab = reinterpret_cast<float *>(pl_smem + COSTAS_SMEM_BYTES);
-    for (int i = t; i < 257; i += SEG_THREADS)
+    for (int i = threadIdx.x; i < 257; i += SEG_THREADS)
         tab[i] = atan_tab[i];
     __syncthreads();
-    int s = blockIdx.x * SEG_THREADS + t;
-    bool active = true;
-    if (repair_list) {
-        if (s >= min(*repair_count, 1024))
-            active = false;
-        else
-            s = repair_list[s];
-    }
-    if (s >= nseg)
-        active = false;
-    if (!active)
-        s = 0;
-    const long own0 = (long)s * L;
-    const long own1 = active ? min(own0 + L, N) : own0;
-    long start = own0 - W;
-    float phase = 0.f, freq = state_in[1];
-    if (repair_list && active) {
-        start = own0;
-        phase = rec[s - 1].ph_end;
-        freq = rec[s - 1].fr_end;
-    } else if (start <= 0) {
-        start = 0;
-        phase = state_in[0];
-    }
-    const int row0 = (int)(start >> 4), row1 = (int)((own1 + 15) >> 4);
-    const int nrows = active ? row1 - row0 : 0;
-    int maxrows = nrows;
-#pragma unroll
-    for (int off = 16; off; off >>= 1)
-        maxrows = max(maxrows, __shfl_xor_sync(0xffffffffu, maxrows, off));
-    LoopRec lr;
-    lr.ph_start = phase;
-    lr.fr_start = freq;
-    const int c = lane & 7;
-    int src_row0[8], src_nrows[8], src_orow0[8], src_own1[8];
-#pragma unroll
-    for (int i = 0; i < 8; i++) {
-        const int T = 4 * i + (lane >> 3);
-        src_row0[i] = __shfl_sync(0xffffffffu, row0, T);
-        src_nrows[i] = __shfl_sync(0xffffffffu, nrows, T);
-        src_orow0[i] = __shfl_sync(0xffffffffu, (int)(own0 >> 4), T);
-        src_own1[i] = __shfl_sync(0xffffffffu, (int)own1, T);
-    }
-    const float2 *in_c = in + 2 * c;
-    auto load_row = [&](int it) {
-        const int pb = (it & 1) * 8;
-#pragma unroll
-        for (int i = 0; i < 8; i++) {
-            const int T = 4 * i + (lane >> 3);
-            const int row = src_row0[i] + it;
-            if (it < src_nrows[i] && (long)row * 16 + 2 * c < N)
-                cp_async16(&ring[swz16(pb + c, T)], in_c + (long)row * 16);
-        }
-        cp_async_commit();
-    };
-    load_row(0);
-    for (int it = 0; it < maxrows; it++) {
-        const int slot = (it & 1) * 8;
-        load_row(it + 1);
-        cp_async_wait<1>();
-        __syncwarp();
-        const bool mine = it < nrows;
-        const long b = (long)(row0 + it) << 4;
-        if (mine && b == own0) {
-            lr.ph_start = phase;
-            lr.fr_start = freq;
-        }
-        if (mine) {
-            const int nvalid = (int)min(16L, own1 - b);
-#pragma unroll 1
-            for (int p = 0; p < 8; p++) {
-                const float4 v = ring[swz16(slot + p, lane)];
-                float2 o0 = make_float2(0.f, 0.f), o1 = o0;
-                if (2 * p < nvalid)
-                    o0 = pll_step(make_float2(v.x, v.y), phase, freq, P, tab);
-                if (2 * p + 1 < nvalid)
-                    o1 = pll_step(make_float2(v.z, v.w), phase, freq, P, tab);
-                obuf[swz16(p, lane)] = make_float4(o0.x, o0.y, o1.x, o1.y);
-            }
-        }
-        __syncwarp();
-#pragma unroll
-        for (int i = 0; i < 8; i++) {
-            const int T = 4 * i + (lane >> 3);
-            const int row = src_row0[i] + it;
-            const int n0 = row * 16 + 2 * c;
-            if (it < src_nrows[i] && row >= src_orow0[i] && n0 < src_own1[i]) {
-                const float4 v = obuf[swz16(c, T)];
-                if (n0 + 1 < src_own1[i])
-                    *reinterpret_cast<float4 *>(out + n0) = v;
-                else
-                    out[n0] = make_float2(v.x, v.y);
-            }
-        }
-        __syncwarp();
-    }
-    cp_async_wait<0>();
-    if (active) {
-        lr.ph_end = phase;
-        lr.fr_end = freq;
-        rec[s] = lr;
-    }
+    PllLoop lp{P, tab};
+    loop_segments(lp, pl_smem, in, N, L, W, nseg, state_in, out, rec, repair_list, repair_count);
 }
 
 // The VOLK rotator behind FreqShiftBlock (freq_shift.cpp:16-50) and PMToBPSK (pm_to_bpsk.cpp:10-35): out[n] = in[n] * e^{j n delta}
@@ -1834,18 +1665,8 @@ __global__ void __launch_bounds__(SEG_THREADS) k_mm(const float2 *__restrict__ m
     for (int i = t; i < 128 * 8; i += SEG_THREADS)
         sbank[(i >> 3) * MM_BANK_STRIDE + (i & 7)] = bank[i];
     __syncthreads();
-    int s = blockIdx.x * SEG_THREADS + t;
-    bool active = true;
-    if (repair_list) { // exact sequential continuation of segment s-1 (see k_costas)
-        if (s >= min(*repair_count, 1024))
-            active = false;
-        else
-            s = repair_list[s];
-    }
-    if (s >= nseg)
-        active = false;
-    if (!active)
-        s = 0;
+    bool active;
+    const int s = loop_segment(nseg, repair_list, repair_count, active); // repair mode: exact sequential continuation of segment s-1
     const long own0 = (long)s * L, own1 = active ? min(own0 + L, N) : own0;
     // buffer coordinate u: window = input samples u-7 .. u
     long u;
@@ -1883,7 +1704,7 @@ __global__ void __launch_bounds__(SEG_THREADS) k_mm(const float2 *__restrict__ m
     for (int off = 16; off; off >>= 1)
         maxit = max(maxit, __shfl_xor_sync(0xffffffffu, maxit, off));
     const float2 *base = mmin + 16; // sample 0
-    auto load = [&](int row, bool ok) { warp_load_rows(ring, -1, 31, base, row, ok && row < rend, N, lane); cp_async_commit(); };
+    auto load = [&](int row, bool ok) { warp_load_rows(ring, base, row, ok && row < rend, N, lane); cp_async_commit(); };
     load(r0, active);
     load(r0 + 1, active);
     float carry_im = 0.f; // OQPSK: imaginary part (after rotation) of the sample in front of the next row

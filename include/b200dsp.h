@@ -16,6 +16,7 @@
  *                    plugins/noaa_metop_support/metop/module_metop_ahrpt_decoder.cpp:34-90      (kind METOP)
  *                    src-core/pipeline/modules/ccsds/module_ccsds_conv_concat_decoder.cpp:140-200 (kind CCSDS, r=1/2)
  *                    src-core/pipeline/modules/ccsds/module_ccsds_ldpc_decoder.cpp:134-277       (kind LDPC, ldpc_rate "7/8")
+ *                    src-core/pipeline/modules/ccsds/module_ccsds_turbo_decoder.cpp:137-235      (kind TURBO)
  *   b200_chain_*   both modules joined the way Pipeline::run joins them with a byte FIFO
  *                    src-core/pipeline/pipeline_run.cpp:44-117 — here the int8 soft stream never leaves HBM.
  *   b200_demux_*   the step behind the decoder: CADUs -> CCSDS space packets
@@ -46,7 +47,7 @@ enum { B200_BPSK = 0, B200_QPSK = 1, B200_OQPSK = 2, B200_8PSK = 3, B200_NONE = 
 /* baseband_format (common/dsp/io/baseband_type.h:7-21) */
 enum { B200_CF32 = 0, B200_CS16 = 1, B200_CS8 = 2 };
 /* decoder kind */
-enum { B200_FEC_METOP = 0, B200_FEC_CCSDS = 1, B200_FEC_SIMPLE = 2, B200_FEC_LDPC = 3 };
+enum { B200_FEC_METOP = 0, B200_FEC_CCSDS = 1, B200_FEC_SIMPLE = 2, B200_FEC_LDPC = 3, B200_FEC_TURBO = 4 };
 /* debug stage ids for b200_demod_debug_stage */
 enum { B200_STAGE_AGC = 0, B200_STAGE_FIR = 1, B200_STAGE_COSTAS = 2, B200_STAGE_RESAMP = 3, B200_STAGE_DC = 4, B200_STAGE_MM = 5,
        B200_STAGE_PLL = 6 /* pm_demod: PLLCarrierTrackingBlock output */, B200_STAGE_PM = 7 /* pm_demod: PMToBPSK output */ };
@@ -134,6 +135,13 @@ typedef struct b200_fec_cfg
     int internal_stream;      /* "internal_stream": the 7136 info bits of every codeword go through BPSK_CCSDS_Deframer(internal_cadu_size,
                                  internal_asm) and its frames are the output (cadu_bytes = internal_cadu_size / 8; no RS)               */
     int internal_cadu_size;   /* "internal_cadu_size" bits, a multiple of 8 (frame padding is rejected); asm_sync carries "internal_asm"  */
+    /* kind B200_FEC_TURBO = ccsds_turbo_decoder (module_ccsds_turbo_decoder.cpp:17-135): correlator on the rate's ASM (64, 96, 128 or 192
+       bits) over frames of codeword + ASM soft bytes, derandomiser, CCSDS turbo decoder (log-MAP BCJR in double, deepspace-turbo), CRC-16;
+       the frames whose CRC passes are written as 1A CF FC 1D + turbo_base bytes. All three fields are required. Device memory: about
+       2.7 MB per frame of a decoding batch (at most 1024 frames) at turbo_base 1115, plus about 7 bytes per max_soft byte.              */
+    int turbo_rate;           /* "turbo_rate": 2, 3, 4, 6 = "1/2", "1/3", "1/4", "1/6"                                                     */
+    int turbo_base;           /* "turbo_base": 223, 446, 892 or 1115 (information bytes per frame)                                          */
+    int turbo_iters;          /* "turbo_iters" >= 1 (the reference dereferences NULL with 0)                                               */
 } b200_fec_cfg;
 
 typedef struct b200_demod_stats
@@ -173,6 +181,9 @@ typedef struct b200_fec_stats
     float correlator_corr;    /* "correlator_corr": the correlator's best score                                                       */
     int ldpc_corr;            /* "ldpc_corr": info positions whose decoded bit differs from the sign of the input                     */
     long ldpc_resyncs;        /* frames so far whose ASM was not at the expected place (the frame walk shifted)                       */
+    /* ccsds_turbo_decoder: correlator_lock / correlator_corr above are its "Corr" and lock state; ldpc_resyncs counts its shifted frames */
+    long crc_ok, crc_fail;    /* frames so far whose CRC-16 passed (written) / failed ("CRC Check" PASS / FAIL)                        */
+    long turbo_near_ties;     /* decisions so far whose margin |one - zero| was below 1e-9 (where libm rounding could tip a bit)       */
 } b200_fec_stats;
 
 typedef struct b200_demod b200_demod;
@@ -258,6 +269,23 @@ int b200_fec_debug_ldpc_frames(b200_fec *f, b200_ldpc_frame *out, long cap, long
    stream): [0] correlation, [1] frame walk, [2] gather, [3] decode + CADU repack (+ internal_stream: bit append, deframer, frames),
    [4] the whole push */
 int b200_fec_ldpc_timing(b200_fec *f, float *ms_out, int n);
+/* ccsds_turbo_decoder: one record per frame of the LAST push, in stream order (frames whose CRC fails included) */
+typedef struct b200_turbo_frame
+{
+    long offset;              /* stream offset (soft bytes since create / reset) of the frame's first byte                           */
+    int pos;                  /* the correlator's position in the window read before it (0 = locked)                                */
+    float cor;                /* the correlator's best score ("Corr")                                                               */
+    int swapped;              /* the ASM correlated negatively: the soft bits were negated                                          */
+    int crc_ok;               /* the CRC-16 passed and the frame was written                                                        */
+} b200_turbo_frame;
+int b200_fec_debug_turbo_frames(b200_fec *f, b200_turbo_frame *out, long cap, long *n_out);
+/* ccsds_turbo_decoder: the a-priori arrays (log-domain, input 0 and input 1, in information-bit order) that frame `frame` of the LAST push
+   held after its last iteration, 8 turbo_base values each: turbo_decode's `messages` after the final message_deinterleave. Frames of the
+   push's last decoding batch only (the last 1024 frames). */
+int b200_fec_debug_turbo_llr(b200_fec *f, long frame, double *app0, double *app1, long cap, long *n_out);
+/* ccsds_turbo_decoder only (B200_EINVAL for the other kinds): elapsed device milliseconds of the last push: [0] correlation, [1] frame
+   walk, [2] gather, [3] BCJR iterations, [4] packing, CRC and compaction, [5] the whole push */
+int b200_fec_turbo_timing(b200_fec *f, float *ms_out, int n);
 
 /* ---- fused chain: raw IQ -> CADUs, soft stream stays in HBM ---------------------------------------- */
 b200_chain *b200_chain_create(const b200_demod_cfg *dcfg, const b200_fec_cfg *fcfg);

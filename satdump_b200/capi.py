@@ -24,6 +24,7 @@ SYMBOLS = [
     "b200_demod_pull_symbols", "b200_demod_debug_stage", "b200_demod_debug_convert", "b200_demod_debug_run_stage", "b200_demod_debug_junctions", "b200_demod_reset", "b200_demod_prefetch_iq", "b200_demod_last_timing", "b200_demod_get_stats", "b200_demod_get_taps",
     "b200_fec_create", "b200_fec_destroy", "b200_fec_push_soft", "b200_fec_push_soft_device", "b200_fec_pull_frames",
     "b200_fec_debug_bits", "b200_fec_get_stats", "b200_fec_cadu_bytes", "b200_fec_chunk_size", "b200_fec_debug_ldpc_frames", "b200_fec_ldpc_timing",
+    "b200_fec_debug_turbo_frames", "b200_fec_debug_turbo_llr", "b200_fec_turbo_timing",
     "b200_chain_create", "b200_chain_destroy", "b200_chain_push_iq", "b200_chain_push_iq_device", "b200_chain_prefetch_iq", "b200_chain_pull_frames",
     "b200_chain_frames_device", "b200_chain_get_stats", "b200_chain_last_timing", "b200_chain_reset",
     "b200_chain_set_pipelined", "b200_chain_sync", "b200_chain_span_begin", "b200_chain_span_end",
@@ -51,7 +52,7 @@ class FecCfg(C.Structure):
                 ("rs_usecheck", C.c_int), ("rs_type", C.c_int), ("iq_invert", C.c_int), ("asm_sync", C.c_uint),
                 ("device", C.c_int), ("max_soft", C.c_long), ("qpsk_swap_iq", C.c_int), ("qpsk_swap_diff", C.c_int), ("oqpsk_delay", C.c_int), ("conv_rate", C.c_int),
                 ("ldpc_rate", C.c_int), ("ldpc_block_size", C.c_int), ("ldpc_iterations", C.c_int), ("ldpc2", C.c_int), ("internal_stream", C.c_int),
-                ("internal_cadu_size", C.c_int)]
+                ("internal_cadu_size", C.c_int), ("turbo_rate", C.c_int), ("turbo_base", C.c_int), ("turbo_iters", C.c_int)]
 
 
 class DemuxCfg(C.Structure):
@@ -80,11 +81,16 @@ class FecStats(C.Structure):
                 ("viterbi_state", C.c_int), ("viterbi_ber", C.c_float), ("deframer_state", C.c_int), ("rs_corrected", C.c_long),
                 ("rs_failed", C.c_long), ("replays", C.c_long), ("kernel_launches", C.c_long), ("start_redone", C.c_long), ("tb_serial", C.c_long),
                 ("spec_steps", C.c_int), ("tb_overlap", C.c_int),
-                ("correlator_lock", C.c_int), ("correlator_corr", C.c_float), ("ldpc_corr", C.c_int), ("ldpc_resyncs", C.c_long)]
+                ("correlator_lock", C.c_int), ("correlator_corr", C.c_float), ("ldpc_corr", C.c_int), ("ldpc_resyncs", C.c_long),
+                ("crc_ok", C.c_long), ("crc_fail", C.c_long), ("turbo_near_ties", C.c_long)]
 
 
 class LdpcFrame(C.Structure):
     _fields_ = [("offset", C.c_long), ("pos", C.c_int), ("cor", C.c_float), ("phase", C.c_int), ("swap", C.c_int), ("ldpc_corr", C.c_int)]
+
+
+class TurboFrame(C.Structure):
+    _fields_ = [("offset", C.c_long), ("pos", C.c_int), ("cor", C.c_float), ("swapped", C.c_int), ("crc_ok", C.c_int)]
 
 
 class B200Error(RuntimeError):
@@ -136,6 +142,9 @@ def lib():
         L.b200_fec_chunk_size.argtypes = [vp]
         L.b200_fec_debug_ldpc_frames.argtypes = [vp, C.POINTER(LdpcFrame), cl, C.POINTER(cl)]
         L.b200_fec_ldpc_timing.argtypes = [vp, vp, ci]
+        L.b200_fec_debug_turbo_frames.argtypes = [vp, C.POINTER(TurboFrame), cl, C.POINTER(cl)]
+        L.b200_fec_turbo_timing.argtypes = [vp, vp, ci]
+        L.b200_fec_debug_turbo_llr.argtypes = [vp, cl, vp, vp, cl, C.POINTER(cl)]
         L.b200_chain_create.restype = vp
         L.b200_chain_create.argtypes = [C.POINTER(DemodCfg), C.POINTER(FecCfg)]
         L.b200_chain_destroy.argtypes = [vp]
@@ -251,11 +260,32 @@ def ldpc_cfg(constellation, ldpc_rate="7/8", ldpc_iterations=10, derandomize=Tru
     return cfg
 
 
+TURBO_RATES = {"1/2": 2, "1/3": 3, "1/4": 4, "1/6": 6}
+
+
+def turbo_cfg(turbo_rate=None, turbo_base=None, turbo_iters=None, device=0, max_soft=1 << 24):
+    """ccsds_turbo_decoder (module_ccsds_turbo_decoder.cpp:17-135): all three parameters are required, as the module's constructor asks.
+    The library refuses an unknown rate or base and turbo_iters < 1 by name."""
+    if turbo_rate is None:
+        raise ValueError("Turbo Rate is required!")
+    if turbo_base is None:
+        raise ValueError("Turbo Base is required!")
+    if turbo_iters is None:
+        raise ValueError("Turbo Iters is required!")
+    cfg = FecCfg()
+    cfg.kind, cfg.device, cfg.max_soft = 4, device, max_soft
+    cfg.turbo_rate = TURBO_RATES.get(turbo_rate, -1) if isinstance(turbo_rate, str) else int(turbo_rate)
+    cfg.turbo_base, cfg.turbo_iters = int(turbo_base), int(turbo_iters)
+    return cfg
+
+
 def fec_cfg_for(sig, max_soft, device=0):
     """The decoder configuration that goes with a satdump_b200.synth.SignalCfg (metop_ahrpt_decoder / ccsds_conv_concat_decoder /
     ccsds_simple_psk_decoder parameters of the shipped pipeline JSONs)."""
     if sig.decoder == "metop":
         return metop_cfg(sig.ber_thresold, sig.outsync_after, device=device, max_soft=max_soft)
+    if sig.decoder == "turbo":
+        return turbo_cfg(sig.turbo_rate, sig.turbo_base, sig.turbo_iters, device=device, max_soft=max_soft)
     if sig.decoder == "ldpc":
         return ldpc_cfg(sig.constellation, internal_stream=bool(sig.internal_cadu_size), internal_cadu_size=sig.internal_cadu_size,
                         internal_asm=sig.internal_asm, device=device, max_soft=max_soft)
@@ -269,6 +299,8 @@ def fec_cfg_for(sig, max_soft, device=0):
 def demod_cfg_for(sig, max_batch, device=0, **kw):
     """psk_demod parameters of a satdump_b200.synth.SignalCfg (decoder "none": the Costas-less DVB-S2 front half)."""
     extra = dict(clock_alpha=sig.clock_alpha) if sig.clock_alpha else {}
+    if sig.post_costas_dc:
+        extra["post_costas_dc"] = True
     return demod_cfg(sig.samplerate, sig.symbolrate, sig.constellation if sig.decoder != "none" else "none", sig.rrc_alpha, sig.pll_bw, sig.fmt,
                      device=device, max_batch=max_batch, **extra, **kw)
 
@@ -451,6 +483,32 @@ class Fec:
             out[k] = [r.offset, r.pos, int(np.float32(r.cor).view(np.uint32)), r.phase, r.swap, r.ldpc_corr, int(r.pos == 0)]
         return out
 
+    def turbo_frames(self):
+        """ccsds_turbo_decoder: one record per frame of the last push as int64 [n, 6] = offset, pos, cor (float32 bits), swapped, crc_ok,
+        correlator_locked."""
+        cap = int(self._n) // 1000 + 4
+        recs = (TurboFrame * cap)()
+        n = C.c_long(0)
+        _chk(lib().b200_fec_debug_turbo_frames(self.h, recs, cap, C.byref(n)))
+        out = np.zeros((n.value, 6), np.int64)
+        for k in range(n.value):
+            r = recs[k]
+            out[k] = [r.offset, r.pos, int(np.float32(r.cor).view(np.uint32)), r.swapped, r.crc_ok, int(r.pos == 0)]
+        return out
+
+    def turbo_llr(self, frame, K):
+        """ccsds_turbo_decoder: the a-priori arrays (input 0, input 1) of a frame of the last push after its last iteration."""
+        a0, a1 = np.zeros(K), np.zeros(K)
+        n = C.c_long(0)
+        _chk(lib().b200_fec_debug_turbo_llr(self.h, frame, a0.ctypes.data, a1.ctypes.data, K, C.byref(n)))
+        return a0, a1
+
+    def turbo_timing(self):
+        """ccsds_turbo_decoder: device milliseconds of the last push: correlation, walk, gather, BCJR, pack + CRC + compaction, whole push."""
+        ms = np.zeros(6, np.float32)
+        _chk(lib().b200_fec_turbo_timing(self.h, ms.ctypes.data, 6))
+        return dict(zip(["corr", "walk", "gather", "bcjr", "pack", "push"], ms.tolist()))
+
     def timing(self):
         """ccsds_ldpc_decoder: device milliseconds of the last push: correlation, walk, gather, decode (+ repack), whole push."""
         ms = np.zeros(5, np.float32)
@@ -466,7 +524,7 @@ class Chain:
         self.h = lib().b200_chain_create(C.byref(dcfg), C.byref(fcfg))
         if not self.h:
             raise B200Error(-1 if "device" not in last_error().lower() else -2, last_error())
-        self.cadu_bytes = (fcfg.cadu_size + 7) // 8 if fcfg.kind in (1, 3) else 1024
+        self.cadu_bytes = (fcfg.cadu_size + 7) // 8 if fcfg.kind in (1, 3) else (fcfg.turbo_base + 4 if fcfg.kind == 4 else 1024)
 
     def close(self):
         if getattr(self, "h", None):

@@ -48,12 +48,16 @@ void build_rs_tables(RsTables &T)
 
 Fec::Fec(const b200_fec_cfg &c) : cfg(c)
 {
-    B200_REQUIRE(c.kind == B200_FEC_METOP || c.kind == B200_FEC_CCSDS || c.kind == B200_FEC_SIMPLE || c.kind == B200_FEC_LDPC, B200_EINVAL,
-                 "unknown decoder kind %d", c.kind);
+    B200_REQUIRE(c.kind == B200_FEC_METOP || c.kind == B200_FEC_CCSDS || c.kind == B200_FEC_SIMPLE || c.kind == B200_FEC_LDPC || c.kind == B200_FEC_TURBO,
+                 B200_EINVAL, "unknown decoder kind %d", c.kind);
     B200_REQUIRE(c.max_soft >= 65536, B200_EINVAL, "max_soft must be >= 65536");
     memset(&geom, 0, sizeof(geom));
     if (c.kind == B200_FEC_LDPC) {
         ldpc_init();
+        return;
+    }
+    if (c.kind == B200_FEC_TURBO) {
+        turbo_init();
         return;
     }
     if (c.kind != B200_FEC_METOP) {
@@ -198,6 +202,7 @@ Fec::~Fec()
     if (stream)
         cudaStreamSynchronize(stream);
     ldpc_free();
+    turbo_free();
     for (auto &e : ev)
         cudaEventDestroy(e);
     for (auto &e : evm)
@@ -643,6 +648,10 @@ void Fec::reset()
         ldpc_reset();
         return;
     }
+    if (turbo) {
+        turbo_reset();
+        return;
+    }
     start_stream(64);
     B200_CUDA(cudaStreamSynchronize(stream));
 }
@@ -876,6 +885,10 @@ void Fec::process()
         ldpc_process();
         return;
     }
+    if (turbo) {
+        turbo_process();
+        return;
+    }
     const long nch = soft_have / geom.chunk;
     B200_REQUIRE(nch <= max_chunks, B200_ESTATE, "internal: too many chunks");
     // (lazy, so that b200_fec_debug_bits can still read the previous push's bits until now)
@@ -938,6 +951,8 @@ void Fec::stats(b200_fec_stats *o)
     o->kernel_launches = launches;
     if (ldpc)
         ldpc_stats(o);
+    if (turbo)
+        turbo_stats(o);
 }
 
 } // namespace b200
@@ -1029,6 +1044,29 @@ int b200_fec_ldpc_timing(b200_fec *h, float *ms_out, int n)
         B200_REQUIRE(h && ms_out, B200_EINVAL, "NULL argument");
         B200_REQUIRE(h->f->ldpc, B200_EINVAL, "not an LDPC decoder (kind B200_FEC_LDPC)");
         h->f->ldpc_timing(ms_out, n);
+    });
+}
+int b200_fec_debug_turbo_frames(b200_fec *h, b200_turbo_frame *out, long cap, long *n_out)
+{
+    return guarded([&] {
+        B200_REQUIRE(h && out && n_out, B200_EINVAL, "NULL argument");
+        *n_out = h->f->turbo_frames(out, cap);
+    });
+}
+int b200_fec_debug_turbo_llr(b200_fec *h, long frame, double *app0, double *app1, long cap, long *n_out)
+{
+    return guarded([&] {
+        B200_REQUIRE(h && app0 && app1 && n_out, B200_EINVAL, "NULL argument");
+        DeviceGuard g(h->f->cfg.device);
+        *n_out = h->f->turbo_llr(frame, app0, app1, cap);
+    });
+}
+int b200_fec_turbo_timing(b200_fec *h, float *ms_out, int n)
+{
+    return guarded([&] {
+        B200_REQUIRE(h && ms_out, B200_EINVAL, "NULL argument");
+        B200_REQUIRE(h->f->turbo, B200_EINVAL, "not a turbo decoder (kind B200_FEC_TURBO)");
+        h->f->turbo_timing(ms_out, n);
     });
 }
 }

@@ -134,6 +134,22 @@ int syncwords(int constellation, LdpcSync &sw)
 }
 } // namespace
 
+void ccsds_pn_bits(unsigned char *pn)
+{
+    uint8_t reg = 0xFF;
+    for (int i = 0; i < 255; i++) {
+        pn[i] = reg >> 7;
+        const uint8_t nb = ((reg >> 7) ^ (reg >> 4) ^ (reg >> 2) ^ reg) & 1;
+        reg = (uint8_t)((reg << 1) | nb);
+    }
+}
+
+void frame_walk(const float *score, const unsigned char *best_sync, const float *bval, const int *bidx, long have, int F, int npos,
+                int constellation, LdpcFrameRec *frames, int max_frames, LdpcWalkOut *out, cudaStream_t stream)
+{
+    k_ldpc_walk<<<1, LDPC_WALK_WARPS * 32, 0, stream>>>(score, best_sync, bval, bidx, have, F, npos, constellation, frames, max_frames, out);
+}
+
 // Everything this build does not cover is refused by name before the device is touched.
 void Fec::ldpc_init()
 {
@@ -203,12 +219,7 @@ void Fec::ldpc_init()
     L.level_ptr.alloc(ptr.size());
     L.level_rows.alloc(std::max<size_t>(rows.size(), 1));
     unsigned char pnb[255];
-    uint8_t reg = 0xFF; // the CCSDS sequence (x^8+x^7+x^5+x^3+1 from all ones), one bit per entry as derand_ccsds_soft applies it
-    for (int i = 0; i < 255; i++) {
-        pnb[i] = reg >> 7;
-        const uint8_t nb = ((reg >> 7) ^ (reg >> 4) ^ (reg >> 2) ^ reg) & 1;
-        reg = (uint8_t)((reg << 1) | nb);
-    }
+    ccsds_pn_bits(pnb);
     L.pn.alloc(256);
     B200_CUDA(cudaMemcpyAsync(L.cols.p, cols.data(), cols.size() * sizeof(uint16_t), cudaMemcpyHostToDevice, stream));
     B200_CUDA(cudaMemcpyAsync(L.level_ptr.p, ptr.data(), ptr.size() * sizeof(int), cudaMemcpyHostToDevice, stream));
@@ -273,8 +284,7 @@ void Fec::ldpc_process()
     B200_CUDA(cudaEventRecord(L.ev[0], stream));
     k_ldpc_corr<<<(unsigned)((npos + 255) / 256), 256, 0, stream>>>(softbuf.p, npos, L.sw, L.nsync, L.score.p, L.bsync.p, L.bval.p, L.bidx.p);
     B200_CUDA(cudaEventRecord(L.ev[1], stream));
-    k_ldpc_walk<<<1, LDPC_WALK_WARPS * 32, 0, stream>>>(L.score.p, L.bsync.p, L.bval.p, L.bidx.p, have, L.constellation, L.frames.p,
-                                                          (int)L.max_frames, L.walk.p);
+    frame_walk(L.score.p, L.bsync.p, L.bval.p, L.bidx.p, have, LDPC_F, LDPC_NPOS, L.constellation, L.frames.p, (int)L.max_frames, L.walk.p, stream);
     B200_CUDA(cudaEventRecord(L.ev[2], stream));
     launches += 2;
     B200_CUDA(cudaMemcpyAsync(L.h_walk, L.walk.p, sizeof(LdpcWalkOut), cudaMemcpyDeviceToHost, stream));

@@ -4,6 +4,7 @@
 // (src-core/pipeline/modules/ccsds/module_ccsds_conv_concat_decoder.cpp:140-200).
 #pragma once
 #include "fec.cuh"
+#include "walk.cuh"
 #include "host_common.h"
 #include <vector>
 
@@ -12,6 +13,13 @@ namespace b200
 
 struct DefrEvent { long pos; int state; int pad; };
 struct Ldpc; // ccsds_ldpc_decoder's state (api_ldpc.cu)
+struct Turbo; // ccsds_turbo_decoder's state (api_turbo.cu)
+
+// the CCSDS sequence (x^8+x^7+x^5+x^3+1 from all ones), one bit per entry as derand_ccsds_soft applies it to soft bytes (255 entries)
+void ccsds_pn_bits(unsigned char *pn);
+// k_ldpc_walk (ldpc.cuh) on `stream`: the frame walk of the correlator-driven decoders
+void frame_walk(const float *score, const unsigned char *best_sync, const float *bval, const int *bidx, long have, int F, int npos,
+                int constellation, LdpcFrameRec *frames, int max_frames, LdpcWalkOut *out, cudaStream_t stream);
 
 class Fec
 {
@@ -41,6 +49,11 @@ class Fec
     Ldpc *ldpc = nullptr;
     long ldpc_frames(b200_ldpc_frame *out, long cap); // records of the last push
     void ldpc_timing(float *ms, int n);
+    // ccsds_turbo_decoder (B200_FEC_TURBO): the same soft FIFO and frame walk
+    Turbo *turbo = nullptr;
+    long turbo_frames(b200_turbo_frame *out, long cap); // records of the last push
+    long turbo_llr(long frame, double *app0, double *app1, long cap);
+    void turbo_timing(float *ms, int n);
 
     // device storage
     DevBuf<int8_t> softbuf;
@@ -130,6 +143,11 @@ class Fec
     void ldpc_reset();
     void ldpc_process();
     void ldpc_stats(b200_fec_stats *o);
+    void turbo_init();
+    void turbo_free();
+    void turbo_reset();
+    void turbo_process();
+    void turbo_stats(b200_fec_stats *o);
 };
 
 void build_rs_tables(RsTables &T);

@@ -5,8 +5,7 @@
 //   k_ldpc_gather  rotate_soft / OQPSK re-delay / derand_ccsds_soft of each frame -> the decoder's input with its 18 zero positions
 //   k_ldpc_decode  LDPCDecoderGeneric::decode (ldpc_decoder_generic.cpp:69-194) on a level schedule, then the CADU repack
 #pragma once
-#include <cuda_runtime.h>
-#include <stdint.h>
+#include "walk.cuh"
 
 constexpr int LDPC_ASM = 32;                 // syncword bits (d_ldpc_asm_size)
 constexpr int LDPC_CW = 8160;                // code soft bytes per frame (d_ldpc_codeword_size)
@@ -17,25 +16,7 @@ constexpr int LDPC_CADU = 1024;
 constexpr int LDPC_WALK_WARPS = 32, LDPC_WALK_SPEC = 4 * LDPC_WALK_WARPS; // frames of the current lattice checked per round
 constexpr int LDPC_DEC_THREADS = 1024;
 
-struct LdpcFrameRec { long long off; int pos; float cor; int phase, swap, corr, pad; };
-struct LdpcWalkOut { long long next; int nf, shifted; };
-
 struct LdpcSync { float w[4][LDPC_ASM]; }; // the correlator's syncword tables, built on the host (ldpc_syncwords)
-
-// (value, index) of a maximum, first index on ties: the order in which the correlator's strict '>' keeps its best
-__device__ __forceinline__ void ldpc_best(float &v, int &i, float v2, int i2)
-{
-    if (v2 > v || (v2 == v && i2 < i)) { v = v2; i = i2; }
-}
-__device__ __forceinline__ void ldpc_best_warp(float &v, int &i)
-{
-#pragma unroll
-    for (int o = 16; o; o >>= 1) {
-        const float v2 = __shfl_xor_sync(0xffffffffu, v, o);
-        const int i2 = __shfl_xor_sync(0xffffffffu, i, o);
-        ldpc_best(v, i, v2, i2);
-    }
-}
 
 // Score of every position i < npos: the best over the nsync tables of the fp32 dot product of soft[i .. i+31] / 63 with the table, summed
 // left to right without contraction (the generic VOLK kernels), and the first table that reaches it. Block b's maximum over positions
@@ -77,13 +58,13 @@ __global__ void __launch_bounds__(256) k_ldpc_corr(const int8_t *__restrict__ so
     }
 }
 
-// first maximum of the scores over window [a, a + LDPC_NPOS), by one warp: the partial blocks at both ends position by position, the
+// first maximum of the scores over window [a, a + npos), by one warp: the partial blocks at both ends position by position, the
 // complete blocks through their maxima
 __device__ void ldpc_window_max(const float *__restrict__ score, const float *__restrict__ bval, const int *__restrict__ bidx, long a,
-                                float &v, int &vi)
+                                int npos, float &v, int &vi)
 {
     const int lane = threadIdx.x & 31;
-    const long e = a + LDPC_NPOS;
+    const long e = a + npos;
     const long b0 = (a + 31) >> 5, b1 = e >> 5;
     v = -INFINITY;
     vi = 0x7fffffff;
@@ -95,14 +76,16 @@ __device__ void ldpc_window_max(const float *__restrict__ score, const float *__
     ldpc_best_warp(v, vi);
 }
 
-// The frame walk over the `have` soft bytes of the FIFO, from offset 0. Each round checks up to LDPC_WALK_SPEC frames of the current
-// lattice o + jF at once (one warp per frame): the frames up to and including the first one whose ASM is not at its window's start are
-// exact, since their windows start where the module would read them; the walk then continues on the shifted lattice. Without signal every
-// frame shifts, and each round takes one frame. A frame whose shifted start leaves fewer than F bytes waits for the next push.
-// Offsets are < 2^31 (the FIFO is sized by max_soft).
+// The frame walk over the `have` soft bytes of the FIFO, from offset 0, for frames of F soft bytes whose windows hold npos correlator
+// positions. Each round checks up to LDPC_WALK_SPEC frames of the current lattice o + jF at once (one warp per frame): the frames up to
+// and including the first one whose ASM is not at its window's start are exact, since their windows start where the module would read
+// them; the walk then continues on the shifted lattice. Without signal every frame shifts, and each round takes one frame. A frame whose
+// shifted start leaves fewer than F bytes waits for the next push. Offsets are < 2^31 (the FIFO is sized by max_soft).
+// constellation WALK_SWAP_ONLY (the turbo correlator): the table index found is the frame's `swap`, its phase is 0.
 __global__ void __launch_bounds__(1024) k_ldpc_walk(const float *__restrict__ score, const unsigned char *__restrict__ best_sync,
-                                                     const float *__restrict__ bval, const int *__restrict__ bidx, long have, int constellation,
-                                                     LdpcFrameRec *__restrict__ frames, int max_frames, LdpcWalkOut *__restrict__ out)
+                                                     const float *__restrict__ bval, const int *__restrict__ bidx, long have, int F, int npos,
+                                                     int constellation, LdpcFrameRec *__restrict__ frames, int max_frames,
+                                                     LdpcWalkOut *__restrict__ out)
 {
     __shared__ float s_v[LDPC_WALK_SPEC];
     __shared__ int s_i[LDPC_WALK_SPEC];
@@ -114,12 +97,12 @@ __global__ void __launch_bounds__(1024) k_ldpc_walk(const float *__restrict__ sc
     __syncthreads();
     while (!s_done) {
         const long o = s_o;
-        const long avail = have >= o + LDPC_F ? (have - o - LDPC_F) / LDPC_F + 1 : 0;
+        const long avail = have >= o + F ? (have - o - F) / F + 1 : 0;
         const int n = (int)min(min(avail, (long)LDPC_WALK_SPEC), (long)(max_frames - s_nf));
         for (int j = warp; j < n; j += LDPC_WALK_WARPS) {
             float v;
             int vi;
-            ldpc_window_max(score, bval, bidx, o + (long)j * LDPC_F, v, vi);
+            ldpc_window_max(score, bval, bidx, o + (long)j * F, npos, v, vi);
             if (lane == 0) { s_v[j] = v; s_i[j] = vi; s_bs[j] = v > 0.0f ? best_sync[vi] : 0; }
         }
         __syncthreads();
@@ -130,10 +113,11 @@ __global__ void __launch_bounds__(1024) k_ldpc_walk(const float *__restrict__ sc
             for (; j < n; j++) {
                 const float v = s_v[j];
                 const int pos = v > 0.0f ? (int)(s_i[j] - oo) : 0;
-                if (pos != 0 && oo + pos + LDPC_F > have) { stop = true; break; }
+                if (pos != 0 && oo + pos + F > have) { stop = true; break; }
                 const int bs = s_bs[j];
                 int phase, swap = 0; // generic_correlator.cpp:233-262
-                if (constellation == 0) phase = bs ? 2 : 0;
+                if (constellation == WALK_SWAP_ONLY) { phase = 0; swap = bs; }
+                else if (constellation == 0) phase = bs ? 2 : 0;
                 else if (constellation == 1) phase = bs;
                 else { phase = bs == 0 ? 1 : (bs == 1 ? 3 : (bs == 2 ? 0 : 2)); swap = bs >> 1; }
                 LdpcFrameRec r;
@@ -145,7 +129,7 @@ __global__ void __launch_bounds__(1024) k_ldpc_walk(const float *__restrict__ sc
                 r.corr = 0;
                 r.pad = 0;
                 frames[nf++] = r;
-                oo += pos + LDPC_F;
+                oo += pos + F;
                 if (pos != 0) { s_shifted++; j++; break; }
             }
             if (n == 0 || nf >= max_frames) stop = true;

@@ -10,7 +10,7 @@ using namespace b200host;
 int main(int argc, char **argv)
 {
     if (argc < 5) {
-        fprintf(stderr, "usage: %s <metop_ahrpt|jpss_hrd|npp_hrd|simple_bpsk|simple_qpsk|pm_bpsk|ldpc_qpsk|landsat> baseband <input> <output_hint> [--fused] [--key value ...]\n", argv[0]);
+        fprintf(stderr, "usage: %s <metop_ahrpt|jpss_hrd|npp_hrd|simple_bpsk|simple_qpsk|pm_bpsk|ldpc_qpsk|landsat|turbo_pm|turbo_bpsk> baseband <input> <output_hint> [--fused] [--key value ...]\n", argv[0]);
         return 2;
     }
     const std::string pipe = argv[1], level = argv[2], in = argv[3], out = argv[4];
@@ -51,6 +51,17 @@ int main(int argc, char **argv)
             fp.set("internal_asm", "352EF853");
         }
         dec = "ccsds_ldpc_decoder";
+    } else if (pipe == "turbo_pm") { // pm_demod -> ccsds_turbo_decoder, rate 1/2, base 1115: the shape of the Juice, TGO, ORX, Hera, Escapade
+        // and Chandrayaan-3 pipelines (residual-carrier PM), with Juice's parameters (resources/pipelines/Juice.json)
+        dp = Params{{"b200_demod_module", "pm_demod"}, {"symbolrate", "526316"}, {"rrc_alpha", "0.35"}, {"pll_bw", "0.002"}, {"pll_max_offset", "3.14"},
+                    {"costas_bw", "0.001"}};
+        fp = Params{{"turbo_rate", "1/2"}, {"turbo_base", "1115"}, {"turbo_iters", "5"}};
+        dec = "ccsds_turbo_decoder";
+    } else if (pipe == "turbo_bpsk") { // psk_demod BPSK -> ccsds_turbo_decoder, rate 1/6, base 1115: the shape of the Psyche and STEREO
+        // pipelines, with Psyche's parameters (resources/pipelines/Psyche.json)
+        dp = Params{{"constellation", "bpsk"}, {"symbolrate", "368000"}, {"rrc_alpha", "0.35"}, {"pll_bw", "0.002"}, {"post_costas_dc", "true"}};
+        fp = Params{{"turbo_rate", "1/6"}, {"turbo_base", "1115"}, {"turbo_iters", "1"}};
+        dec = "ccsds_turbo_decoder";
     } else {
         fprintf(stderr, "unknown pipeline %s\n", pipe.c_str());
         return 2;

@@ -256,6 +256,28 @@ b200_demod_cfg pm_demod_cfg_from_params(const Params &p, bool &is_bpsk)
 b200_fec_cfg fec_cfg_from_params(const std::string &id, const Params &p)
 {
     b200_fec_cfg c{};
+    if (id == "ccsds_turbo_decoder") { // module_ccsds_turbo_decoder.cpp:17-36,118-119; the library checks the values (turbo_iters >= 1)
+        c.kind = B200_FEC_TURBO;
+        c.device = (int)p.num("b200_device", 0);
+        if (!p.has("turbo_rate"))
+            throw ModuleError("Turbo Rate is required!");
+        if (!p.has("turbo_base"))
+            throw ModuleError("Turbo Base is required!");
+        if (!p.has("turbo_iters"))
+            throw ModuleError("Turbo Iters is required!");
+        c.turbo_base = (int)p.num("turbo_base");
+        c.turbo_iters = (int)p.num("turbo_iters");
+        if (!(c.turbo_base == 223 || c.turbo_base == 446 || c.turbo_base == 892 || c.turbo_base == 1115))
+            throw ModuleError("Turbo Base must be 223, 446, 892 or 1115!");
+        const std::string rate = p.str("turbo_rate");
+        if (rate == "1/2") c.turbo_rate = 2;
+        else if (rate == "1/3") c.turbo_rate = 3;
+        else if (rate == "1/4") c.turbo_rate = 4;
+        else if (rate == "1/6") c.turbo_rate = 6;
+        else throw ModuleError("Invalid Turbo Rate!");
+        c.cadu_size = (c.turbo_base + 4) * 8; // what one output frame holds (ASM + base bytes), written to .cadu (:147)
+        return c;
+    }
     if (id == "ccsds_ldpc_decoder") { // module_ccsds_ldpc_decoder.cpp:19-124
         c.kind = B200_FEC_LDPC;
         c.device = (int)p.num("b200_device", 0);
@@ -556,6 +578,12 @@ void FecStage::process()
                 fwrite(out.data(), 1, (size_t)nb, fout);
             else if (output_fifo->write(out.data(), (int)nb) < 0)
                 break;
+        }
+        if (cfg.kind == B200_FEC_TURBO) { // "CRC Check": the CRC of the last frame decoded
+            std::vector<b200_turbo_frame> recs(got / 1024 + 4);
+            long nrec = 0;
+            if (b200_fec_debug_turbo_frames(h, recs.data(), (long)recs.size(), &nrec) == B200_OK && nrec > 0)
+                crc_lock = recs[nrec - 1].crc_ok;
         }
         b200_fec_stats st;
         if (b200_fec_get_stats(h, &st) == B200_OK) {

@@ -123,9 +123,11 @@ class FecStage : public StageBase
     // getModuleStats() keys: deframer_lock, viterbi_ber, viterbi_lock, rs_avg (module_metop_ahrpt_decoder.cpp:92-104)
     std::atomic<int> viterbi_lock{0}, deframer_state{2};
     std::atomic<float> viterbi_ber{10.f};
-    // ccsds_ldpc_decoder: correlator_lock, correlator_corr, ldpc_corr (module_ccsds_ldpc_decoder.cpp:279-295); deframer_state above
+    // ccsds_ldpc_decoder: correlator_lock, correlator_corr, ldpc_corr (module_ccsds_ldpc_decoder.cpp:279-295); deframer_state above.
+    // ccsds_turbo_decoder: correlator_lock, correlator_corr and crc_lock, what its window shows (module_ccsds_turbo_decoder.cpp:259-290)
     std::atomic<int> correlator_lock{0}, ldpc_corr{0};
     std::atomic<float> correlator_corr{0.f};
+    std::atomic<int> crc_lock{0};
     std::atomic<long> frames_written{0};
     b200_fec_cfg cfg{};
     long batch_soft = 1 << 24;

@@ -208,9 +208,16 @@ class SignalCfg:
     # bits carry inner CADUs of this many bits that start with internal_asm
     internal_cadu_size: int = 0
     internal_asm: int = 0x1ACFFC1D
+    # ccsds_turbo_decoder (decoder "turbo"): "turbo_rate" 2, 3, 4, 6 = 1/2 .. 1/6, "turbo_base", "turbo_iters"; psk_demod's "post_costas_dc"
+    turbo_rate: int = 2
+    turbo_base: int = 1115
+    turbo_iters: int = 5
+    post_costas_dc: bool = False
 
     @property
     def cadu_bytes(self):
+        if self.decoder == "turbo":
+            return self.turbo_base + 4
         if self.decoder == "ldpc":
             return self.internal_cadu_size // 8 if self.internal_cadu_size else 1024
         return 4 + 255 * self.interleave
@@ -286,6 +293,15 @@ CONFIGS = {
     # above OQPSK's MAX_SPS 2.4, so the front-end resampler runs (6 -> 4.8 MS/s)
     "ldpc_landsat": SignalCfg(name="ldpc_landsat", samplerate=6e6, symbolrate=2000000, constellation="oqpsk", conv="ldpc", rrc_alpha=0.5, fmt="cs16",
                               decoder="ldpc", esn0_db=12.0, pll_bw=0.002, internal_cadu_size=8272, internal_asm=0x352EF853),
+    # pm_demod -> ccsds_turbo_decoder, Juice-like (Juice.json): residual-carrier PM, BPSK on a subcarrier at the symbol rate, turbo rate 1/2
+    # with base 1115 and 5 iterations; 526316 baud at 3 MS/s (5.7 samples per symbol, no resampler)
+    "turbo_pm": SignalCfg(name="turbo_pm", samplerate=3e6, symbolrate=526316, constellation="bpsk", conv="turbo", rrc_alpha=0.35, fmt="cs16",
+                          decoder="turbo", esn0_db=14.0, pll_bw=0.001, pm_pll_bw=0.002, carrier_rad=2e-2, pm_index=1.0, turbo_rate=2,
+                          turbo_base=1115, turbo_iters=5),
+    # psk_demod BPSK -> ccsds_turbo_decoder, Psyche-like (Psyche.json): rate 1/6, base 1115, 1 iteration, post_costas_dc; 368 kbaud at
+    # 1 MS/s (2.7 samples per symbol)
+    "turbo_bpsk": SignalCfg(name="turbo_bpsk", samplerate=1e6, symbolrate=368000, constellation="bpsk", conv="turbo", rrc_alpha=0.35, fmt="cs16",
+                            decoder="turbo", esn0_db=6.0, pll_bw=0.002, post_costas_dc=True, turbo_rate=6, turbo_base=1115, turbo_iters=1),
 }
 
 
@@ -314,6 +330,9 @@ def qpsk_diff_encode(dibits, swap=True):
 
 
 def make_bitstream(cfg: SignalCfg, nframes, seed):
+    if cfg.decoder == "turbo":  # nframes turbo frames
+        tx, clear = turbo_frames(nframes, cfg.turbo_rate, cfg.turbo_base, seed)
+        return tx.reshape(-1), clear
     if cfg.decoder == "ldpc":  # nframes LDPC frames
         if cfg.internal_cadu_size:
             info, clear = ldpc_inner_frames(nframes, cfg.internal_cadu_size, cfg.internal_asm, seed)
@@ -428,6 +447,9 @@ def modulate(cfg: SignalCfg, coded, seed, nsamples=None, device="cpu"):
 
 def frames_for_samples(cfg: SignalCfg, nsamples):
     bps = 1 if cfg.constellation == "bpsk" else 2
+    if cfg.decoder == "turbo":  # turbo frames of ASM + codeword bits
+        nbits = turbo_codeword_bits(cfg.turbo_rate, cfg.turbo_base) + TURBO_ASM_BITS[cfg.turbo_rate]
+        return int(nsamples * bps / (cfg.samplerate / cfg.symbolrate) / nbits) + 2
     if cfg.decoder == "ldpc":  # LDPC frames of 8192 bits
         return int(nsamples * bps / (cfg.samplerate / cfg.symbolrate) / 8192) + 2
     rate = {"1/2": 0.5, "3/4": 0.75, "none": 1.0, "p2/3": 2 / 3, "p3/4": 0.75, "p5/6": 5 / 6, "p7/8": 7 / 8}[cfg.conv]
@@ -673,3 +695,95 @@ def ldpc_inner_frames(nframes, cadu_size, asm, seed):
     inner = np.concatenate([np.tile(asm_bits, (k, 1)), rng.integers(0, 2, (k, cadu_size - 32), dtype=np.uint8)], axis=1)
     bits = np.concatenate([inner.reshape(-1), rng.integers(0, 2, total - k * cadu_size, dtype=np.uint8)])
     return bits.reshape(nframes, LDPC_INFO), np.packbits(inner, axis=1)
+
+
+# ---- CCSDS turbo code (CCSDS 131.0-B section 6), as ccsds_turbo_decoder receives it ---------------------------------------------------
+TURBO_ASM = {2: 0x034776C7272895B0, 3: 0x25D5C0CE8990F6C9461BF79C, 4: 0x034776C7272895B0FCB88938D8D76A4F,
+             6: 0x25D5C0CE8990F6C9461BF79CDA2A3F31766F0936B9E40863}   # attached sync marker per rate 1/2, 1/3, 1/4, 1/6
+TURBO_ASM_BITS = {2: 64, 3: 96, 4: 128, 6: 192}
+TURBO_BASES = (223, 446, 892, 1115)
+# feed-forward polynomials of the upper and lower component codes (taps 0..4; the first one is the systematic output), feedback 0011
+TURBO_CODES = {2: (("10011", "11011"), ("11011",)), 3: (("10011", "11011"), ("11011",)), 4: (("10011", "10101", "11111"), ("11011",)),
+               6: (("10011", "11011", "10101", "11111"), ("11011", "11111"))}
+
+
+def turbo_interleaver(base):
+    """The CCSDS turbo interleaver pi for k = 8 base bits (CCSDS 131.0-B 6.3): the lower encoder reads info[pi[j]] at step j."""
+    p = (31, 37, 43, 47, 53, 59, 61, 67)
+    k1, k2 = 8, base
+    s = np.arange(8 * base)
+    m = s % 2
+    i = s // (2 * k2)
+    j = s // 2 - i * k2
+    t = (19 * i + 1) % (k1 // 2)
+    q = t % 8
+    c = (np.array(p)[q] * j + 21 * m) % k2
+    return 2 * (t + c * (k1 // 2) + 1) - m - 1
+
+
+def turbo_codeword_bits(rate, base):
+    n = 8 * base + 4
+    return 2 * n if rate == 2 else rate * n
+
+
+def _rsc_encode(bits, taps):
+    """Recursive systematic component encoder with feedback 1 + D^3 + D^4 ("0011" on registers 1..4) over bits [nframes, K], terminated
+    by 4 tail steps that feed the feedback back in. Returns uint8 [nframes, K + 4, len(taps)]."""
+    nf, K = bits.shape
+    reg = np.zeros((nf, 4), np.uint8)   # registers 1..4
+    fwd = np.array([[int(ch) for ch in t] for t in taps], np.uint8)
+    out = np.zeros((nf, K + 4, len(taps)), np.uint8)
+    for k in range(K + 4):
+        fb = reg[:, 2] ^ reg[:, 3]
+        u = bits[:, k] if k < K else fb
+        first = u ^ fb
+        for c in range(len(taps)):
+            o = fwd[c, 0] & first
+            for r in range(4):
+                o = o ^ (fwd[c, r + 1] & reg[:, r])
+            out[:, k, c] = o
+        reg = np.concatenate([first[:, None], reg[:, :3]], axis=1)
+    return out
+
+
+def turbo_encode(info_bytes, rate):
+    """uint8 [nframes, base] -> the turbo codewords as sent, bits uint8 [nframes, codeword bits]: per trellis step the upper code's outputs
+    then the lower code's (on the interleaved bits); rate 1/2 keeps the systematic bit and alternately the upper and the lower parity."""
+    info_bytes = np.atleast_2d(np.asarray(info_bytes, np.uint8))
+    nf, base = info_bytes.shape
+    bits = np.unpackbits(info_bytes, axis=1)
+    up_taps, lo_taps = TURBO_CODES[rate]
+    up = _rsc_encode(bits, up_taps)
+    lo = _rsc_encode(bits[:, turbo_interleaver(base)], lo_taps)
+    full = np.concatenate([up, lo], axis=2).reshape(nf, -1)
+    if rate != 2:
+        return full
+    k = np.arange(full.shape[1])
+    keep = (k % 3 == 0) | np.where((k // 3) % 2 == 1, k % 3 == 2, k % 3 == 1)
+    return full[:, keep]
+
+
+def crc16_ccitt(data):
+    """CRC-16, polynomial 0x1021, initial value 0xFFFF, no reflection, no final xor, over each row of uint8 [n, len]."""
+    data = np.atleast_2d(np.asarray(data, np.uint8))
+    crc = np.full(data.shape[0], 0xFFFF, np.uint32)
+    for col in range(data.shape[1]):
+        crc ^= data[:, col].astype(np.uint32) << 8
+        for _ in range(8):
+            crc = np.where(crc & 0x8000, (crc << 1) ^ 0x1021, crc << 1) & 0xFFFF
+    return crc
+
+
+def turbo_frames(nframes, rate, base, seed=0):
+    """(tx bits uint8 [n, ASM + codeword bits] = the rate's ASM + the PN-randomised codeword, the CADUs the decoder writes for them
+    [n, 4 + base] = 1A CF FC 1D + the information bytes, whose last two are the CRC-16 of the others)."""
+    rng = np.random.default_rng(seed)
+    data = rng.integers(0, 256, (nframes, base - 2), dtype=np.uint8)
+    crc = crc16_ccitt(data)
+    info = np.concatenate([data, (crc >> 8).astype(np.uint8)[:, None], (crc & 0xFF).astype(np.uint8)[:, None]], axis=1)
+    cw = turbo_encode(info, rate)
+    nasm = TURBO_ASM_BITS[rate]
+    asm = np.unpackbits(np.frombuffer(TURBO_ASM[rate].to_bytes(nasm // 8, "big"), np.uint8))
+    tx = np.concatenate([np.tile(asm, (nframes, 1)), cw ^ ldpc_pn_bits(cw.shape[1])[None, :]], axis=1)
+    cadu = np.concatenate([np.tile(np.frombuffer(ASM, np.uint8), (nframes, 1)), info], axis=1)
+    return tx, cadu

@@ -160,6 +160,8 @@ typedef struct b200_demod_stats
     float pll_freq;           /* pm_demod: carrier PLL frequency, rad/sample (PLLCarrierTrackingBlock::getFreq; module stats key "freq" =
                                  rad_to_hz(pll_freq, final_samplerate), module_pm_demod.cpp:138,186) */
     long pll_unconverged;     /* pm_demod: carrier PLL junctions still inconsistent after the repair rounds of the last push (expected 0) */
+    int repair_merge_hist[8]; /* the repairs by where they ended: [0] ran the whole segment; [i] met the segment's stored run at its
+                                 checkpoint j (512 samples apart), 2^(i-2) < j <= 2^(i-1), and stopped there; [7]: any later one */
 } b200_demod_stats;
 
 typedef struct b200_fec_stats
@@ -231,6 +233,8 @@ int b200_demod_debug_run_stage(b200_demod *d, int stage, const float *host_in, l
 int b200_demod_debug_junctions(b200_demod *d, double *costas_out, double *mm_out, long cap_segments, long *nseg_out, long *seg_len);
 /* test hook: only the sample conversion (BasebandReader::read_samples, baseband_interface.h:170-190) of `nsamples` host samples */
 int b200_demod_debug_convert(b200_demod *d, const void *host_iq, long nsamples, float *host_out);
+/* test hook: enable = 0 gives the repairs a tolerance of 0 for meeting the stored run, so every repair runs its whole segment */
+int b200_demod_debug_repair_merge(b200_demod *d, int enable);
 int b200_demod_get_stats(b200_demod *d, b200_demod_stats *out);
 /* forget the stream (loop state, resampler counters) but keep every allocation: the next push starts a new stream */
 int b200_demod_reset(b200_demod *d);

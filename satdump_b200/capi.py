@@ -15,13 +15,14 @@ LIB_PATH = os.path.join(_HERE, "csrc", "libb200dsp.so")
 CONST = {"bpsk": 0, "qpsk": 1, "oqpsk": 2, "8psk": 3, "none": 4, "bpsk_90": 5}
 FMT = {"cf32": 0, "cs16": 1, "cs8": 2}
 FMT_BYTES = {0: 8, 1: 4, 2: 2}
+CKPT = 512  # samples between the repair checkpoints of the loop kernels (demod.cuh)
 E_NAMES = {0: "OK", -1: "EINVAL", -2: "ENODEV", -3: "ECUDA", -4: "ENOMEM", -5: "ESTATE", -6: "EUNSUPPORTED"}
 
 # every symbol include/b200dsp.h declares (tests check the built library exports all of them)
 SYMBOLS = [
     "b200_last_error", "b200_device_count", "b200_demod_final_samplerate", "b200_demod_resample_decision", "b200_demod_resampler_bank",
     "b200_demod_create", "b200_demod_destroy", "b200_demod_push_iq", "b200_demod_push_iq_device", "b200_demod_pull_soft",
-    "b200_demod_pull_symbols", "b200_demod_debug_stage", "b200_demod_debug_convert", "b200_demod_debug_run_stage", "b200_demod_debug_junctions", "b200_demod_reset", "b200_demod_prefetch_iq", "b200_demod_last_timing", "b200_demod_get_stats", "b200_demod_get_taps",
+    "b200_demod_pull_symbols", "b200_demod_debug_stage", "b200_demod_debug_convert", "b200_demod_debug_run_stage", "b200_demod_debug_junctions", "b200_demod_debug_repair_merge", "b200_demod_reset", "b200_demod_prefetch_iq", "b200_demod_last_timing", "b200_demod_get_stats", "b200_demod_get_taps",
     "b200_fec_create", "b200_fec_destroy", "b200_fec_push_soft", "b200_fec_push_soft_device", "b200_fec_pull_frames",
     "b200_fec_debug_bits", "b200_fec_get_stats", "b200_fec_cadu_bytes", "b200_fec_chunk_size", "b200_fec_debug_ldpc_frames", "b200_fec_ldpc_timing",
     "b200_fec_debug_turbo_frames", "b200_fec_debug_turbo_llr", "b200_fec_turbo_timing",
@@ -73,7 +74,7 @@ class DemodStats(C.Structure):
                 ("costas_freq", C.c_float), ("mm_mu", C.c_float), ("mm_omega", C.c_float), ("costas_unconverged", C.c_long),
                 ("mm_unconverged", C.c_long), ("agc_clamped", C.c_int), ("repairs", C.c_int), ("kernel_launches", C.c_long),
                 ("agc_exact_passes", C.c_long), ("last_front_samples", C.c_long), ("snr", C.c_float), ("peak_snr", C.c_float),
-                ("pll_freq", C.c_float), ("pll_unconverged", C.c_long)]
+                ("pll_freq", C.c_float), ("pll_unconverged", C.c_long), ("repair_merge_hist", C.c_int * 8)]
 
 
 class FecStats(C.Structure):
@@ -126,6 +127,7 @@ def lib():
         L.b200_demod_debug_run_stage.argtypes = [vp, ci, vp, cl, ci, vp, cl, C.POINTER(cl)]
         L.b200_demod_debug_junctions.argtypes = [vp, vp, vp, cl, C.POINTER(cl), C.POINTER(cl)]
         L.b200_demod_get_stats.argtypes = [vp, C.POINTER(DemodStats)]
+        L.b200_demod_debug_repair_merge.argtypes = [vp, ci]
         L.b200_demod_reset.argtypes = [vp]
         L.b200_demod_prefetch_iq.argtypes = [vp, vp, cl]
         L.b200_demod_last_timing.argtypes = [vp, vp, ci]
@@ -313,7 +315,7 @@ def _nsamples(raw, fmt):
 
 
 def _struct_dict(s):
-    return {k: getattr(s, k) for k, _ in s._fields_}
+    return {k: list(v) if isinstance(v, C.Array) else v for k, v in ((k, getattr(s, k)) for k, _ in s._fields_)}
 
 
 class Demod:
@@ -356,6 +358,11 @@ class Demod:
 
     def reset(self):
         _chk(lib().b200_demod_reset(self.h))
+        return self
+
+    def repair_merge(self, enable):
+        """Test hook: False makes every repair run its whole segment (tolerance 0 for meeting the stored run)."""
+        _chk(lib().b200_demod_debug_repair_merge(self.h, 1 if enable else 0))
         return self
 
     def timing(self):

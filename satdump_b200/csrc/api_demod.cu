@@ -364,9 +364,11 @@ Demod::Demod(const b200_demod_cfg &c) : cfg(c)
         tol_cfreq = 4e-6f;
     }
     tol_mm = 0.01f; // samples (1.3 interpolator arms)
+    // a timing error moves omega by gain_omega and mu by gain_mu per unit of the detector's output: the same disagreement, in omega
+    tol_momega = tol_mm * c.clock_gain_omega / c.clock_gain_mu;
     int dev_sms = 132;
     cudaDeviceGetAttribute(&dev_sms, cudaDevAttrMultiProcessorCount, c.device);
-    seg_cap_threads = dev_sms * 3 * SEG_THREADS; // the segment count aims at 3 resident CTAs of the loop kernels per SM
+    seg_cap_threads = dev_sms * 2 * SEG_THREADS; // the segment count aims at 2 resident CTAs of the loop kernels per SM
     {
         // in a pipelined chain the demodulator of batch i runs next to the decoder of batch i-1 and is the longer of the two: its
         // kernels take freed SM slots first
@@ -409,6 +411,9 @@ Demod::Demod(const b200_demod_cfg &c) : cfg(c)
     const long nseg_max = (max_work + lmin - 1) / lmin + 1;
     crec.alloc(nseg_max);
     mrec.alloc(nseg_max);
+    // nseg * ckpt_per_seg(L) < (n + L) / CKPT; a SEQUENTIAL debug run has one segment of n samples
+    cck.alloc((max_work + 16384) / CKPT + 1);
+    mck.alloc((max_work + 16384) / CKPT + 1);
     quad.alloc(nseg_max);
     offs.alloc(nseg_max + 1);
     repair.alloc(1025);
@@ -642,8 +647,10 @@ void Demod::run_pll(const float2 *in, float2 *out, long n, float bw, float max_o
     }
     P.fmax = max_offset; // PLLCarrierTrackingBlock(input, bw, max_offset, -max_offset)
     P.fmin = -max_offset;
+    const float mt = repair_merge ? 1.0f / MERGE_TIGHTER : 0.0f;
     run_loop_stage(*this, nblk, [&](int grid, const int *list, const int *count, int round) {
-        k_pll<<<grid, SEG_THREADS, PLL_SMEM_BYTES, stream>>>(in, n, L, Wp, nseg, P, S->pll[cur], d_atan_tab.p, out, crec.p, list, count);
+        k_pll<<<grid, SEG_THREADS, PLL_SMEM_BYTES, stream>>>(in, n, L, Wp, nseg, P, S->pll[cur], d_atan_tab.p, out, crec.p, list, count, cck.p, mt * tol_pphase,
+                                                             mt * tol_pfreq, S->merge_hist);
         k_costas_fix<<<1, 1024, 0, stream>>>(crec.p, nseg, 1, tol_pphase, tol_pfreq, quad.p, S->pll[nxt], &S->pll_unconv, repair.p + 1, repair.p, round,
                                              &S->repairs);
     });
@@ -686,8 +693,10 @@ float2 *Demod::stage_costas(long n, int L, int nseg, int cur, int nxt, bool mate
         P.fmin = -cfg.costas_max_offset;
         P.fmax = cfg.costas_max_offset;
         const auto costas = order == 2 ? k_costas<2> : (order == 4 ? k_costas<4> : k_costas<8>);
+        const float mt = repair_merge ? 1.0f / MERGE_TIGHTER : 0.0f;
         run_loop_stage(*this, nblk, [&](int grid, const int *list, const int *count, int round) {
-            costas<<<grid, SEG_THREADS, COSTAS_SMEM_BYTES, stream>>>(fir_out, n, L, Wc, Gc, nseg, P, S->costas[cur], cos_out, crec.p, list, count);
+            costas<<<grid, SEG_THREADS, COSTAS_SMEM_BYTES, stream>>>(fir_out, n, L, Wc, Gc, nseg, P, S->costas[cur], cos_out, crec.p, list, count, cck.p,
+                                                                     mt * tol_cphase, mt * tol_cfreq, S->merge_hist);
             k_costas_fix<<<1, 1024, 0, stream>>>(crec.p, nseg, order, tol_cphase, tol_cfreq, quad.p, S->costas[nxt], &S->costas_unconv, repair.p + 1, repair.p,
                                                  round, &S->repairs);
         });
@@ -735,10 +744,11 @@ void Demod::stage_mm(float2 *mmin, long n, int L, int nseg, int cur, int nxt, in
     MP.omega_gain = cfg.clock_gain_omega;
     MP.mu_gain = cfg.clock_gain_mu;
     const int cap = slot_cap_for(L);
+    const float mt = repair_merge ? 1.0f / MERGE_TIGHTER : 0.0f;
     B200_REQUIRE((size_t)nseg * cap <= slots.n, B200_ENOMEM, "internal: symbol slot storage too small");
     run_loop_stage(*this, nblk, [&](int grid, const int *list, const int *count, int round) {
         mm<<<grid, SEG_THREADS, MM_SMEM_BYTES, stream>>>(mmin, n, L, Wm, Gm, nseg, MP, &S->mm[cur], &S->mm[nxt], d_bank.p, slots.p, cap, mrec.p, list, count,
-                                                        mm_quad, mm_rot, mm_oqpsk);
+                                                        mm_quad, mm_rot, mm_oqpsk, mck.p, mt * tol_mm, mt * tol_momega, S->merge_hist);
         k_mm_scan<<<1, 1024, 0, stream>>>(mrec.p, nseg, tol_mm, offs.p, &S->mm_unconv, cap, &S->flags, repair.p + 1, repair.p, round, &S->repairs);
     });
     k_mm_compact<<<std::min(nseg, 132 * 8), 256, 0, stream>>>(slots.p, cap, mrec.p, offs.p, nseg, pm ? 2 : (bps == 1), all_symbols ? 1 : 0, sym_out.p,
@@ -1031,6 +1041,8 @@ void Demod::stats(b200_demod_stats *o)
     o->mm_unconverged = h_state->mm_unconv;
     o->agc_clamped = (int)std::min<long>(agc_clamped_batches, 0x7fffffff); // batches in which the gain hit max_gain so far
     o->repairs = h_state->repairs;
+    for (int i = 0; i < MERGE_BUCKETS; i++)
+        o->repair_merge_hist[i] = h_state->merge_hist[i];
     o->kernel_launches = launches;
     o->agc_exact_passes = h_state->agc_exact;
     o->last_front_samples = last_front;
@@ -1250,6 +1262,13 @@ int b200_demod_debug_junctions(b200_demod *h, double *costas_out, double *mm_out
         }
         *nseg_out = ns;
         *seg_len = d.last_L;
+    });
+}
+int b200_demod_debug_repair_merge(b200_demod *h, int enable)
+{
+    return guarded([&] {
+        B200_REQUIRE(h, B200_EINVAL, "NULL argument");
+        h->d->repair_merge = enable != 0;
     });
 }
 int b200_demod_reset(b200_demod *h)

@@ -935,8 +935,24 @@ struct CostasParams
     float alpha, beta, fmin, fmax;
 };
 struct LoopRec { float ph_start, fr_start, ph_end, fr_end; };
+// Repair checkpoints. The main pass of a loop kernel stores the loop state of every segment at its owned samples own0 + j * CKPT
+// (j >= 1). A repair (the exact continuation of the predecessor) compares its own state with the stored one there: both loops are
+// contracting, so the two runs approach each other, and once they agree within the junction tolerance everything the stored run
+// produced from that sample on (outputs, end record) is as good a continuation as any accepted junction: the repair stops there
+// instead of running the whole segment. A checkpoint that does not agree is overwritten, so the checkpoints always describe the
+// outputs in memory; a repair that never agrees runs to the segment's end.
+constexpr int CKPT = 512; // samples; a power of two and a multiple of the 16-sample row
+struct LoopCkpt { float phase, freq; };
+struct MMCkpt { int u, count; float mu, omega; }; // in front of the first symbol at or behind the checkpoint; count = slots filled so far
+inline __host__ __device__ int ckpt_per_seg(int L) { return (L - 1) / CKPT; }
+constexpr int MERGE_BUCKETS = 8; // histogram of repairs: [0] ran to the segment's end, [i] joined at checkpoint j, 2^(i-2) < j <= 2^(i-1)
 
 #ifdef B200_DEFINE_KERNELS
+__device__ __forceinline__ void count_repair(int *__restrict__ merge_hist, int joined_at)
+{
+    atomicAdd(&merge_hist[joined_at ? min(MERGE_BUCKETS - 1, 33 - __clz(joined_at - 1)) : 0], 1);
+}
+
 // Warp-cooperative staging shared by the two loop kernels. Every thread walks ITS OWN stretch of the stream, so a per-thread
 // load touches 32 different cache lines per instruction (measured: the L1 wavefront rate, not the math, bounded the first version).
 // Instead the warp moves whole 128-byte rows: in instruction i, lanes 8q..8q+7 copy the eight 16-byte chunks of the row of thread
@@ -971,8 +987,8 @@ __device__ __forceinline__ void warp_load_rows(float4 *dst, const float2 *__rest
 // The segment of this thread in the loop kernels: segment blockIdx.x * SEG_THREADS + threadIdx.x, or in repair mode
 // (repair_list != nullptr) segment repair_list[i] for the i-th of the first min(*repair_count, 1024) threads. Repair mode re-runs a
 // segment with NO warm-up, starting from the recorded end state of its predecessor, i.e. as the exact sequential continuation of that
-// segment (used for junctions whose warm-up had not converged; the junction check runs again afterwards). A thread without a segment
-// gets active = false and s = 0.
+// segment (used for junctions whose warm-up had not converged; the junction check runs again afterwards), up to the checkpoint at
+// which it meets the segment's stored run (see CKPT). A thread without a segment gets active = false and s = 0.
 __device__ __forceinline__ int loop_segment(int nseg, const int *__restrict__ repair_list, const int *__restrict__ repair_count, bool &active)
 {
     int s = blockIdx.x * SEG_THREADS + threadIdx.x;
@@ -1103,7 +1119,8 @@ __device__ __forceinline__ float2 costas_step(const float2 x, CostasRegs &r, flo
 template <class Loop>
 __device__ __forceinline__ void loop_segments(Loop &lp, unsigned char *smem, const float2 *__restrict__ in, long N, int L, int W, int nseg,
                                               const float *__restrict__ state_in, float2 *__restrict__ out, LoopRec *__restrict__ rec,
-                                              const int *__restrict__ repair_list, const int *__restrict__ repair_count)
+                                              const int *__restrict__ repair_list, const int *__restrict__ repair_count,
+                                              LoopCkpt *__restrict__ ckpt, float tol_phase, float tol_freq, int *__restrict__ merge_hist)
 {
     const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
     float4 *ring = reinterpret_cast<float4 *>(smem) + warp * (24 * 32); // [16 chunk slots][32] in, then [8][32] out
@@ -1112,11 +1129,17 @@ __device__ __forceinline__ void loop_segments(Loop &lp, unsigned char *smem, con
     const int s = loop_segment(nseg, repair_list, repair_count, active);
     const long own0 = (long)s * L;
     const long own1 = active ? min(own0 + L, N) : own0;
+    LoopCkpt *my_ck = ckpt + (long)s * ckpt_per_seg(L) - 1; // my_ck[j]: the state at sample own0 + j * CKPT, j >= 1
+    const float lock_step = 6.283185307179586f / (float)lp.order();
+    int joined_at = 0; // repair mode: the checkpoint at which this run met the stored one
     long start = own0 - W, gear_end = own0 - W + lp.G;
     float phase = 0.f, freq = state_in[1];
     if (repair_list && active) {
+        // The predecessor's end state, moved by whole lock-point steps into the frame the stored run of this segment sits in (the loop
+        // is the same loop in every frame, and k_costas_fix resolves the frame from ph_start): a stored tail it joins needs no rotation.
         start = own0;
-        phase = rec[s - 1].ph_end;
+        const int k = (int)rintf((rec[s].ph_start - rec[s - 1].ph_end) / lock_step) % lp.order();
+        phase = rec[s - 1].ph_end + (float)k * lock_step;
         freq = rec[s - 1].fr_end;
         gear_end = 0;
     } else if (start <= 0) {
@@ -1125,7 +1148,7 @@ __device__ __forceinline__ void loop_segments(Loop &lp, unsigned char *smem, con
         gear_end = 0;
     }
     const int row0 = (int)(start >> 4), row1 = (int)((own1 + 15) >> 4); // rows of 16 samples, [row0, row1)
-    const int nrows = active ? row1 - row0 : 0;
+    int nrows = active ? row1 - row0 : 0;
     int maxrows = nrows;
 #pragma unroll
     for (int off = 16; off; off >>= 1)
@@ -1159,6 +1182,28 @@ __device__ __forceinline__ void loop_segments(Loop &lp, unsigned char *smem, con
     };
     load_row(0);
     for (int it = 0; it < maxrows; it++) {
+        if (repair_list && it > 0 && (it & (CKPT / 16 - 1)) == 0) {
+            // every repair starts at its own0, so the whole warp is at a checkpoint: a thread whose state agrees with the stored
+            // one (same frame, junction tolerances) owns no further rows, and the lanes that carry its rows learn that
+            if (it < nrows) {
+                LoopCkpt &ck = my_ck[it / (CKPT / 16)];
+                const float d = lp.phase() - ck.phase, q = rintf(d / lock_step);
+                if ((int)q % lp.order() == 0 && fabsf(d - q * lock_step) < tol_phase && fabsf(lp.freq() - ck.freq) < tol_freq) {
+                    joined_at = it / (CKPT / 16);
+                    nrows = it;
+                } else
+                    ck = LoopCkpt{lp.phase(), lp.freq()};
+            }
+            maxrows = nrows;
+#pragma unroll
+            for (int off = 16; off; off >>= 1)
+                maxrows = max(maxrows, __shfl_xor_sync(0xffffffffu, maxrows, off));
+#pragma unroll
+            for (int i = 0; i < 8; i++)
+                src_nrows[i] = __shfl_sync(0xffffffffu, nrows, 4 * i + (lane >> 3));
+            if (it >= maxrows)
+                break;
+        }
         const int slot = (it & 1) * 8;
         load_row(it + 1);
         cp_async_wait<1>();
@@ -1170,6 +1215,8 @@ __device__ __forceinline__ void loop_segments(Loop &lp, unsigned char *smem, con
             lr.ph_start = lp.phase();
             lr.fr_start = lp.freq();
         }
+        if (!repair_list && mine && b > own0 && ((int)(b - own0) & (CKPT - 1)) == 0)
+            my_ck[(int)(b - own0) / CKPT] = LoopCkpt{lp.phase(), lp.freq()};
         lp.row(mine, ring, slot, obuf, lane, b, own1);
         __syncwarp();
         // transposed copy-out: lanes 8q..8q+7 store the eight chunks of thread 4i+q's row (owned samples only)
@@ -1190,9 +1237,16 @@ __device__ __forceinline__ void loop_segments(Loop &lp, unsigned char *smem, con
     }
     cp_async_wait<0>();
     if (active) {
-        lr.ph_end = lp.phase();
-        lr.fr_end = lp.freq();
+        if (joined_at) { // the stored run's end state stands, so the next junction is what it was
+            lr.ph_end = rec[s].ph_end;
+            lr.fr_end = rec[s].fr_end;
+        } else {
+            lr.ph_end = lp.phase();
+            lr.fr_end = lp.freq();
+        }
         rec[s] = lr;
+        if (repair_list)
+            count_repair(merge_hist, joined_at);
     }
 }
 
@@ -1205,6 +1259,7 @@ template <int ORDER> struct CostasLoop
     CostasRegs r;
     __device__ __forceinline__ float phase() const { return r.phase; }
     __device__ __forceinline__ float freq() const { return r.freq; }
+    __device__ __forceinline__ int order() const { return ORDER; } // lock points per turn
     __device__ __forceinline__ void begin(float phase, float freq, long gear_until)
     {
         r.phase = phase;
@@ -1251,11 +1306,12 @@ template <int ORDER> struct CostasLoop
 template <int ORDER>
 __global__ void __launch_bounds__(SEG_THREADS) k_costas(const float2 *__restrict__ in, long N, int L, int W, int G, int nseg, CostasParams P,
                                                          const float *__restrict__ state_in, float2 *__restrict__ out, LoopRec *__restrict__ rec,
-                                                         const int *__restrict__ repair_list, const int *__restrict__ repair_count)
+                                                         const int *__restrict__ repair_list, const int *__restrict__ repair_count,
+                                                         LoopCkpt *__restrict__ ckpt, float tol_phase, float tol_freq, int *__restrict__ merge_hist)
 {
     extern __shared__ __align__(16) unsigned char cs_smem[];
     CostasLoop<ORDER> lp{P, G};
-    loop_segments(lp, cs_smem, in, N, L, W, nseg, state_in, out, rec, repair_list, repair_count);
+    loop_segments(lp, cs_smem, in, N, L, W, nseg, state_in, out, rec, repair_list, repair_count, ckpt, tol_phase, tol_freq, merge_hist);
 }
 
 // ---------------------------------------------------------------- K2b: resolve per-segment rotation (prefix sum mod order)
@@ -1431,6 +1487,7 @@ struct PllLoop
     float ph, fr;
     __device__ __forceinline__ float phase() const { return ph; }
     __device__ __forceinline__ float freq() const { return fr; }
+    __device__ __forceinline__ int order() const { return 1; } // the lock point is unique
     __device__ __forceinline__ void begin(float phase, float freq, long)
     {
         ph = phase;
@@ -1458,7 +1515,8 @@ struct PllLoop
 constexpr int PLL_SMEM_BYTES = COSTAS_SMEM_BYTES + 260 * 4;
 __global__ void __launch_bounds__(SEG_THREADS) k_pll(const float2 *__restrict__ in, long N, int L, int W, int nseg, PllParams P,
                                                       const float *__restrict__ state_in, const float *__restrict__ atan_tab, float2 *__restrict__ out,
-                                                      LoopRec *__restrict__ rec, const int *__restrict__ repair_list, const int *__restrict__ repair_count)
+                                                      LoopRec *__restrict__ rec, const int *__restrict__ repair_list, const int *__restrict__ repair_count,
+                                                      LoopCkpt *__restrict__ ckpt, float tol_phase, float tol_freq, int *__restrict__ merge_hist)
 {
     extern __shared__ __align__(16) unsigned char pl_smem[];
     float *tab = reinterpret_cast<float *>(pl_smem + COSTAS_SMEM_BYTES);
@@ -1466,7 +1524,7 @@ __global__ void __launch_bounds__(SEG_THREADS) k_pll(const float2 *__restrict__ 
         tab[i] = atan_tab[i];
     __syncthreads();
     PllLoop lp{P, tab};
-    loop_segments(lp, pl_smem, in, N, L, W, nseg, state_in, out, rec, repair_list, repair_count);
+    loop_segments(lp, pl_smem, in, N, L, W, nseg, state_in, out, rec, repair_list, repair_count, ckpt, tol_phase, tol_freq, merge_hist);
 }
 
 // The VOLK rotator behind FreqShiftBlock (freq_shift.cpp:16-50) and PMToBPSK (pm_to_bpsk.cpp:10-35): out[n] = in[n] * e^{j n delta}
@@ -1655,7 +1713,8 @@ __global__ void __launch_bounds__(SEG_THREADS) k_mm(const float2 *__restrict__ m
                                                      MMParams P, const MMState *__restrict__ st_in, MMState *__restrict__ st_out,
                                                      const float *__restrict__ bank /*128x8*/, float2 *__restrict__ slots, int cap,
                                                      MMRec *__restrict__ rec, const int *__restrict__ repair_list, const int *__restrict__ repair_count,
-                                                     const uint8_t *__restrict__ quad, int rot_order, int oqpsk)
+                                                     const uint8_t *__restrict__ quad, int rot_order, int oqpsk, MMCkpt *__restrict__ ckpt, float tol_t,
+                                                     float tol_omega, int *__restrict__ merge_hist)
 {
     extern __shared__ __align__(16) unsigned char mm_smem[];
     const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
@@ -1673,9 +1732,21 @@ __global__ void __launch_bounds__(SEG_THREADS) k_mm(const float2 *__restrict__ m
     float mu, omega;
     float2 p0, p1, p2, c0, c1, c2;
     long ustart = own0 - W, gear_end = own0 - W + G; // gear shift as in k_costas: omega held, 4x the mu gain for the first G samples
+    // Repair mode: the symbols go to the slots from `count` = the stored run's skip on (k_mm_scan: its candidate-zone symbols in
+    // front of the junction), where the stored run has its own first kept symbol; the slots below stay skipped (placeholder heads in
+    // front of the junction). A stored tail the repair joins is then already in place behind the repaired symbols.
+    int count = 0;
+    MMRec mr;
+#pragma unroll
+    for (int i = 0; i < 4; i++) { mr.head_u[i] = 0; mr.head_mu[i] = 0.f; }
     if (repair_list && active) {
         gear_end = 0;
         const MMRec pr = rec[s - 1];
+        count = rec[s].skip & 3;
+#pragma unroll
+        for (int i = 0; i < 3; i++)
+            if (i < count)
+                mr.head_u[i] = pr.u_final - 4 * (count - i);
         mu = pr.mu_final; omega = pr.omega_final; p0 = pr.p0; p1 = pr.p1; p2 = pr.p2; c0 = pr.c0; c1 = pr.c1; c2 = pr.c2;
         u = pr.u_final;
     } else if (ustart <= 0) {
@@ -1735,10 +1806,6 @@ __global__ void __launch_bounds__(SEG_THREADS) k_mm(const float2 *__restrict__ m
             ring[idx] = make_float4(a.x, a.y, b.x, b.y);
         }
     };
-    int count = 0;
-    MMRec mr;
-#pragma unroll
-    for (int i = 0; i < 4; i++) { mr.head_u[i] = 0; mr.head_mu[i] = 0.f; }
     const long emit0 = (s == 0 || repair_list) ? min(own0, u) : own0 - MM_ZONE;
     float2 *my = slots + (long)s * cap;
     // the symbol loop runs on 32-bit offsets from the thread's start: ur = u - ubase (a segment plus its warm-up is far below 2^31)
@@ -1747,6 +1814,9 @@ __global__ void __launch_bounds__(SEG_THREADS) k_mm(const float2 *__restrict__ m
     const int emit32 = (int)max(-0x40000000L, min(0x40000000L, emit0 - ubase)), gear32 = (int)max(-0x40000000L, min(0x40000000L, gear_end - ubase));
     const int uring = (int)(ubase & 63) + 64; // ring sample index of sample n is (n + 64) mod 64 taken over chunk slots: only (n >> 1) & 31 and n & 1 matter
     bool done = !active;
+    MMCkpt *my_ck = ckpt + (long)s * ckpt_per_seg(L) - 1; // my_ck[j]: in front of the first symbol with u >= own0 + j * CKPT, j >= 1
+    const int orow0 = (int)(own0 >> 4);
+    int joined_at = 0; // repair mode: the checkpoint at which this run met the stored one
     for (int it = 0; it < maxit; it++) {
         const int rr = r0 + 1 + it;
         load(rr + 1, active);
@@ -1854,12 +1924,36 @@ __global__ void __launch_bounds__(SEG_THREADS) k_mm(const float2 *__restrict__ m
             }
             if (ubase + ur >= own1)
                 done = true;
+            // the row ended on a checkpoint: the main pass stores the state there; a repair stops when it has filled the same slots as
+            // the stored run and sits on the same sampling instant and omega (the stored symbols from here on follow in place)
+            const int rel = rr + 1 - orow0;
+            if (!done && rel > 0 && (rel & (CKPT / 16 - 1)) == 0) {
+                MMCkpt &ck = my_ck[rel / (CKPT / 16)];
+                const int un = (int)(ubase + ur);
+                if (repair_list && ck.count == count && fabsf((float)(un - ck.u) + (mu - ck.mu)) < tol_t && fabsf(omega - ck.omega) < tol_omega) {
+                    joined_at = rel / (CKPT / 16);
+                    done = true;
+                } else
+                    ck = MMCkpt{un, count, mu, omega};
+            }
         }
         __syncwarp(); // the next iteration's copy overwrites the oldest row of the ring
+        if (repair_list && __all_sync(0xffffffffu, done))
+            break;
     }
     cp_async_wait<0>();
     if (!active)
         return;
+    if (repair_list)
+        count_repair(merge_hist, joined_at);
+    if (joined_at) { // the stored run's symbols behind the checkpoint, its count and its end state stand
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+            rec[s].head_u[i] = mr.head_u[i];
+            rec[s].head_mu[i] = mr.head_mu[i];
+        }
+        return;
+    }
     u = ubase + ur;
     mr.u_final = (int)u;
     mr.mu_final = mu;

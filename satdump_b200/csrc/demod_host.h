@@ -25,6 +25,7 @@ struct DemodDevState
     int costas_unconv;  // junctions still unconverged after the repair rounds of the last batch
     int mm_unconv;
     int repairs;        // segments re-run as exact continuations so far (all batches)
+    int merge_hist[MERGE_BUCKETS]; // ... by the checkpoint at which the re-run met the stored run and stopped (count_repair)
     int agc_exact;      // batches that needed the exact AGC pass so far
     float snr_y[2][2];  // M2M4 SNR estimator: running averages of |s|^2, |s|^4 (snr_estimator.h:26)
     // pm_demod (module_pm_demod.cpp:61-88)
@@ -79,6 +80,13 @@ class Demod
     int dbg_costas_unconv = 0, dbg_mm_unconv = 0, dbg_repairs = 0; // of the last debug_run_stage
     // junction tolerances: Costas phase (rad) / frequency (rad/sample) residual, M&M sampling instant (samples)
     float tol_cphase = 2e-3f, tol_cfreq = 1e-4f, tol_mm = 0.05f;
+    float tol_momega = 0.f;    // M&M omega (samples per symbol): only a repair that joins the stored run checks it
+    // A repair stops at a checkpoint where it agrees with the stored run within 1 / MERGE_TIGHTER of the junction tolerances: the end
+    // record it keeps then differs from the exact continuation's by so little that no junction check of the successor comes out
+    // differently (measured on the 6-samples-per-symbol pm_demod signal, where the M&M runs approach each other slowly: with the
+    // junction tolerance itself 5 of 510 repairs of successors no longer happen, with 1/2 and 1/4 one, from 1/8 on none).
+    static constexpr float MERGE_TIGHTER = 16.0f;
+    bool repair_merge = true;  // test hook (b200_demod_debug_repair_merge): false = tolerance 0, every repair runs its whole segment
 
     b200_demod_cfg cfg;
     cudaStream_t stream = nullptr;
@@ -134,6 +142,8 @@ class Demod
     int agc_warm_max = 24;
     DevBuf<LoopRec> crec;
     DevBuf<MMRec> mrec;
+    DevBuf<LoopCkpt> cck; // repair checkpoints of the last phase-loop / clock-recovery stage: ckpt_per_seg(L) per segment
+    DevBuf<MMCkpt> mck;
     DevBuf<uint8_t> quad;
     DevBuf<int> repair; // [0] count, [1..1024] junction list (shared by the Costas and M&M repair rounds)
     DevBuf<long> offs;

@@ -5,7 +5,7 @@
 Runs a warm-up step, times three synchronous steps with CUDA events, then profiles one more step on its own with torch.profiler (CUDA
 activities only) and prints per-kernel device times of the loop stages: k_costas and k_mm split into their main launch and the
 repair launches (the 8-CTA grids), the fix-up / scan / compaction kernels, plus the demodulator's `repairs` and unconverged-junction
-counters for that step, the loop kernels' main-pass grids (segments / 128) and the card's name, power limit and SM clock.
+counters for that step (and where its repairs stopped: the checkpoint at which each met the stored run), the loop kernels' main-pass grids (segments / 128) and the card's name, power limit and SM clock.
 """
 import collections
 import json
@@ -66,6 +66,7 @@ def main():
         step()
         torch.cuda.synchronize()
     dstats = pipe.stats()["demod"]  # reset() clears the counters: these are the profiled step's own
+    merge_hist = pipe.ch.stats()[0]["repair_merge_hist"]
     with tempfile.TemporaryDirectory() as d:
         path = os.path.join(d, "trace.json")
         prof.export_chrome_trace(path)
@@ -92,6 +93,8 @@ def main():
     print(f"config {wname}, 2^{lg} samples, card {card()}")
     print(f"synchronous step: {' '.join(f'{x:.2f}' for x in step_ms)} ms (CUDA events), stage_ms {json.dumps(timing)}")
     print(f"demodulator counters of the profiled step: {dstats}; main-pass grids (CTAs of {SEG_THREADS} segments): {grids}")
+    buckets = ["whole segment", "1", "2", "3-4", "5-8", "9-16", "17-32", ">32"]
+    print(f"repairs by the {capi.CKPT}-sample checkpoint at which they met the stored run and stopped: {dict(zip(buckets, merge_hist))}")
     print(f"{'kernel':<18}{'launches':>9}{'ms':>10}")
     for k, (ms, cnt) in acc.items():
         if cnt:

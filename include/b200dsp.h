@@ -235,6 +235,11 @@ int b200_demod_debug_junctions(b200_demod *d, double *costas_out, double *mm_out
 int b200_demod_debug_convert(b200_demod *d, const void *host_iq, long nsamples, float *host_out);
 /* test hook: enable = 0 gives the repairs a tolerance of 0 for meeting the stored run, so every repair runs its whole segment */
 int b200_demod_debug_repair_merge(b200_demod *d, int enable);
+/* Cycle counters of the loop kernels' main passes, only in a library built with -DB200_LOOP_CYCLES (tools/profile_loops.py --cycles):
+ * out[0..3] = clock64() cycles summed over the warps of k_costas (or k_pll) in its phases row wait, loop, copy-out, tail, out[4] = those
+ * warps; out[5..9] the same for k_mm (row wait, input fix-up, symbol loop, symbol copy-out; warps), all since the previous call, which
+ * they clear. cap >= 10. A production library returns B200_EUNSUPPORTED. */
+int b200_demod_debug_loop_cycles(unsigned long long *out, int cap);
 int b200_demod_get_stats(b200_demod *d, b200_demod_stats *out);
 /* forget the stream (loop state, resampler counters) but keep every allocation: the next push starts a new stream */
 int b200_demod_reset(b200_demod *d);

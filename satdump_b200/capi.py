@@ -22,7 +22,7 @@ E_NAMES = {0: "OK", -1: "EINVAL", -2: "ENODEV", -3: "ECUDA", -4: "ENOMEM", -5: "
 SYMBOLS = [
     "b200_last_error", "b200_device_count", "b200_demod_final_samplerate", "b200_demod_resample_decision", "b200_demod_resampler_bank",
     "b200_demod_create", "b200_demod_destroy", "b200_demod_push_iq", "b200_demod_push_iq_device", "b200_demod_pull_soft",
-    "b200_demod_pull_symbols", "b200_demod_debug_stage", "b200_demod_debug_convert", "b200_demod_debug_run_stage", "b200_demod_debug_junctions", "b200_demod_debug_repair_merge", "b200_demod_reset", "b200_demod_prefetch_iq", "b200_demod_last_timing", "b200_demod_get_stats", "b200_demod_get_taps",
+    "b200_demod_pull_symbols", "b200_demod_debug_stage", "b200_demod_debug_convert", "b200_demod_debug_run_stage", "b200_demod_debug_junctions", "b200_demod_debug_repair_merge", "b200_demod_debug_loop_cycles", "b200_demod_reset", "b200_demod_prefetch_iq", "b200_demod_last_timing", "b200_demod_get_stats", "b200_demod_get_taps",
     "b200_fec_create", "b200_fec_destroy", "b200_fec_push_soft", "b200_fec_push_soft_device", "b200_fec_pull_frames",
     "b200_fec_debug_bits", "b200_fec_get_stats", "b200_fec_cadu_bytes", "b200_fec_chunk_size", "b200_fec_debug_ldpc_frames", "b200_fec_ldpc_timing",
     "b200_fec_debug_turbo_frames", "b200_fec_debug_turbo_llr", "b200_fec_turbo_timing",
@@ -181,6 +181,16 @@ def last_error():
 def _chk(rc):
     if rc != 0:
         raise B200Error(rc, last_error())
+
+
+def loop_cycles():
+    """Cycle counters of the loop kernels' main passes since the previous call (a library built with -DB200_LOOP_CYCLES only):
+    {"k_costas": [wait, loop, copy-out, tail, warps], "k_mm": [wait, fix-up, symbols, copy-out, warps]}, cycles summed over warps."""
+    out = (C.c_ulonglong * 10)()
+    f = lib().b200_demod_debug_loop_cycles  # (looked up here: tools/profile_loops.py --lib also loads builds that predate it)
+    f.argtypes = [C.c_void_p, C.c_int]
+    _chk(f(out, 10))
+    return {"k_costas": list(out[0:5]), "k_mm": list(out[5:10])}
 
 
 def demod_cfg(samplerate, symbolrate, constellation, rrc_alpha, pll_bw=0.003, fmt="cs16", rrc_taps=31, agc_rate=1e-2, clock_alpha=None,

@@ -1271,6 +1271,20 @@ int b200_demod_debug_repair_merge(b200_demod *h, int enable)
         h->d->repair_merge = enable != 0;
     });
 }
+int b200_demod_debug_loop_cycles(unsigned long long *out, int cap)
+{
+    return guarded([&] {
+        B200_REQUIRE(out && cap >= LC_SLOTS, B200_EINVAL, "need room for %d counters", (int)LC_SLOTS);
+#ifdef B200_LOOP_CYCLES
+        B200_CUDA(cudaDeviceSynchronize());
+        B200_CUDA(cudaMemcpyFromSymbol(out, g_loop_cycles, sizeof(unsigned long long) * LC_SLOTS));
+        const unsigned long long zero[LC_SLOTS] = {};
+        B200_CUDA(cudaMemcpyToSymbol(g_loop_cycles, zero, sizeof(zero)));
+#else
+        B200_REQUIRE(false, B200_EUNSUPPORTED, "this library was built without -DB200_LOOP_CYCLES");
+#endif
+    });
+}
 int b200_demod_reset(b200_demod *h)
 {
     return guarded([&] {

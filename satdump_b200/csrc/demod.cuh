@@ -39,7 +39,9 @@ constexpr int RS_SPAN = 2 * RS_THREADS + RS_MAX_TAPS + 8; // decimation < 2: at 
 constexpr int SEG_THREADS = 128;     // threads (= stream segments) per CTA in the loop kernels
 constexpr int MM_HIST = 16;       // inputs of the previous batch kept in the front pad (M&M reaches 7 back, Gardner up to 11)
 constexpr int MM_BANK_STRIDE = 12; // floats per arm row in smem: 16-byte aligned rows (two 128-bit loads per arm), 8 bank groups
-constexpr int MM_SMEM_BYTES = 64 * SEG_THREADS * 8 + 128 * MM_BANK_STRIDE * 4;
+constexpr int MM_STAGE = 16;     // symbols per thread staged in smem between two coalesced copy-outs (one per 16-sample row)
+// per CTA: the 64-sample rings, the bank, then per warp the staged symbols [MM_STAGE][32] and one int2 per thread for the copy-out
+constexpr int MM_SMEM_BYTES = 64 * SEG_THREADS * 8 + 128 * MM_BANK_STRIDE * 4 + SEG_THREADS * (MM_STAGE + 1) * 8;
 
 struct FirTaps { float h[32]; };
 
@@ -927,6 +929,48 @@ template <bool STRICT> __global__ void __launch_bounds__(256) k_fir_only(const f
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
 template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N)); }
 
+// ---------------------------------------------------------------- opt-in cycle counters of the loop kernels' main passes
+// Built with -DB200_LOOP_CYCLES (tools/profile_loops.py --cycles), lane 0 of every warp of a main pass adds the clock64() cycles of
+// each phase of its row loop to g_loop_cycles (b200_demod_debug_loop_cycles reads and clears them); mark(k) books the time since the
+// previous mark to phase k. Without the flag every member is empty and the kernels are the production ones.
+#endif // B200_DEFINE_KERNELS
+enum { LC_COSTAS = 0, LC_MM = 5, LC_PHASES = 4, LC_SLOTS = 10 }; // per kernel: LC_PHASES phase totals, then the number of warps
+#ifdef B200_DEFINE_KERNELS
+#ifdef B200_LOOP_CYCLES
+__device__ unsigned long long g_loop_cycles[LC_SLOTS];
+struct LoopCycles
+{
+    long long c[LC_PHASES], t;
+    static __device__ __forceinline__ long long now()
+    {
+        long long v;
+        asm volatile("mov.u64 %0, %%clock64;" : "=l"(v));
+        return v;
+    }
+    __device__ __forceinline__ LoopCycles() : c{0, 0, 0, 0}, t(now()) {}
+    __device__ __forceinline__ void mark(int k)
+    {
+        const long long n = now();
+        c[k] += n - t;
+        t = n;
+    }
+    __device__ __forceinline__ void publish(int base, bool main_pass)
+    {
+        if (!main_pass || (threadIdx.x & 31))
+            return;
+        for (int k = 0; k < LC_PHASES; k++)
+            atomicAdd(&g_loop_cycles[base + k], (unsigned long long)c[k]);
+        atomicAdd(&g_loop_cycles[base + LC_PHASES], 1ull);
+    }
+};
+#else
+struct LoopCycles
+{
+    __device__ __forceinline__ void mark(int) {}
+    __device__ __forceinline__ void publish(int, bool) {}
+};
+#endif
+
 // ---------------------------------------------------------------- K2: Costas loop, one thread per segment
 #endif // B200_DEFINE_KERNELS
 struct CostasParams
@@ -1125,6 +1169,7 @@ __device__ __forceinline__ void loop_segments(Loop &lp, unsigned char *smem, con
     const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
     float4 *ring = reinterpret_cast<float4 *>(smem) + warp * (24 * 32); // [16 chunk slots][32] in, then [8][32] out
     float4 *obuf = ring + 16 * 32;
+    LoopCycles cyc;
     bool active;
     const int s = loop_segment(nseg, repair_list, repair_count, active);
     const long own0 = (long)s * L;
@@ -1208,6 +1253,7 @@ __device__ __forceinline__ void loop_segments(Loop &lp, unsigned char *smem, con
         load_row(it + 1);
         cp_async_wait<1>();
         __syncwarp();
+        cyc.mark(0);
         const bool mine = it < nrows;
         const long b = (long)(row0 + it) << 4;
         // start / own0 are multiples of 16, so a row is entirely warm-up or entirely owned; only the batch's last row can be partial
@@ -1219,6 +1265,7 @@ __device__ __forceinline__ void loop_segments(Loop &lp, unsigned char *smem, con
             my_ck[(int)(b - own0) / CKPT] = LoopCkpt{lp.phase(), lp.freq()};
         lp.row(mine, ring, slot, obuf, lane, b, own1);
         __syncwarp();
+        cyc.mark(1);
         // transposed copy-out: lanes 8q..8q+7 store the eight chunks of thread 4i+q's row (owned samples only)
 #pragma unroll
         for (int i = 0; i < 8; i++) {
@@ -1234,8 +1281,11 @@ __device__ __forceinline__ void loop_segments(Loop &lp, unsigned char *smem, con
             }
         }
         __syncwarp();
+        cyc.mark(2);
     }
     cp_async_wait<0>();
+    cyc.mark(3);
+    cyc.publish(LC_COSTAS, !repair_list);
     if (active) {
         if (joined_at) { // the stored run's end state stands, so the next junction is what it was
             lr.ph_end = rec[s].ph_end;
@@ -1721,6 +1771,12 @@ __global__ void __launch_bounds__(SEG_THREADS) k_mm(const float2 *__restrict__ m
     // per warp: ring of 64 samples = 32 chunk slots x 32 threads x 16 B (swizzled, see warp_load_rows); then the interpolator bank
     float4 *ring = reinterpret_cast<float4 *>(mm_smem) + warp * (32 * 32);
     float *sbank = reinterpret_cast<float *>(mm_smem + 64 * SEG_THREADS * sizeof(float2)); // [128][MM_BANK_STRIDE]
+    // the symbols a thread emits in one row iteration: its j-th at stage[j * 32 + (lane ^ j)], so that the lanes storing their j-th
+    // symbols and the copy-out's half-warps (lanes 8q..8q+7 read symbols 0..7 of thread i + 8q) are free of bank conflicts;
+    // pub[lane] = (slot of the first, how many) for the copy-out
+    float2 *stage = reinterpret_cast<float2 *>(sbank + 128 * MM_BANK_STRIDE) + warp * 32 * (MM_STAGE + 1);
+    int2 *pub = reinterpret_cast<int2 *>(stage + 32 * MM_STAGE);
+    LoopCycles cyc;
     for (int i = t; i < 128 * 8; i += SEG_THREADS)
         sbank[(i >> 3) * MM_BANK_STRIDE + (i & 7)] = bank[i];
     __syncthreads();
@@ -1817,14 +1873,22 @@ __global__ void __launch_bounds__(SEG_THREADS) k_mm(const float2 *__restrict__ m
     MMCkpt *my_ck = ckpt + (long)s * ckpt_per_seg(L) - 1; // my_ck[j]: in front of the first symbol with u >= own0 + j * CKPT, j >= 1
     const int orow0 = (int)(own0 >> 4);
     int joined_at = 0; // repair mode: the checkpoint at which this run met the stored one
+    // the copy-out's view of the threads whose symbols this lane writes (lanes 8q..8q+7 carry thread i + 8q in step i)
+    long src_slots[8];
+#pragma unroll
+    for (int i = 0; i < 8; i++)
+        src_slots[i] = (long)__shfl_sync(0xffffffffu, s, i + 8 * (lane >> 3)) * cap;
+    int nst = 0, cfirst = 0; // symbols staged in this row iteration, slot of the first
     for (int it = 0; it < maxit; it++) {
         const int rr = r0 + 1 + it;
         load(rr + 1, active);
         cp_async_wait<1>(); // rows <= rr complete
         __syncwarp();
+        cyc.mark(0);
         if (it == 0)
             fixrow(r0);
         fixrow(rr);
+        cyc.mark(1);
         if (!done) {
             const long lim = min((long)(rr + 1) << 4, own1);
             const int lim32 = (int)(lim - ubase);
@@ -1901,7 +1965,12 @@ __global__ void __launch_bounds__(SEG_THREADS) k_mm(const float2 *__restrict__ m
                 }
                 pe = fminf(1.0f, fmaxf(-1.0f, pe));
                 if (emit) {
-                    if (count < cap)
+                    if (nst < MM_STAGE) { // (only a loop taking steps below one sample could fill the stage within a row)
+                        if (nst == 0)
+                            cfirst = count;
+                        stage[nst * 32 + (lane ^ nst)] = p0;
+                        nst++;
+                    } else if (count < cap)
                         my[count] = p0;
                     count++;
                 }
@@ -1937,11 +2006,34 @@ __global__ void __launch_bounds__(SEG_THREADS) k_mm(const float2 *__restrict__ m
                     ck = MMCkpt{un, count, mu, omega};
             }
         }
-        __syncwarp(); // the next iteration's copy overwrites the oldest row of the ring
+        cyc.mark(2);
+        // copy-out of this iteration's symbols: each thread's are consecutive slots, so a store instruction writes four short runs
+        // instead of 32 scattered symbols
+        pub[lane] = make_int2(cfirst, nst);
+        __syncwarp();
+        {
+            const int c = lane & 7;
+            const bool more = __any_sync(0xffffffffu, nst > 8);
+#pragma unroll
+            for (int i = 0; i < 8; i++) {
+                const int T = i + 8 * (lane >> 3);
+                const int2 pb = pub[T];
+#pragma unroll
+                for (int h = 0; h < 2; h++) {
+                    const int j = c + 8 * h;
+                    if ((h == 0 || more) && j < pb.y && pb.x + j < cap)
+                        slots[src_slots[i] + pb.x + j] = stage[j * 32 + (T ^ j)];
+                }
+            }
+        }
+        nst = 0;
+        cyc.mark(3);
+        __syncwarp(); // the next iteration's copy overwrites the oldest row of the ring, its symbols the stage
         if (repair_list && __all_sync(0xffffffffu, done))
             break;
     }
     cp_async_wait<0>();
+    cyc.publish(LC_MM, !repair_list);
     if (!active)
         return;
     if (repair_list)

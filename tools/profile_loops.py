@@ -6,9 +6,17 @@ Runs a warm-up step, times three synchronous steps with CUDA events, then profil
 activities only) and prints per-kernel device times of the loop stages: k_costas and k_mm split into their main launch and the
 repair launches (the 8-CTA grids), the fix-up / scan / compaction kernels, plus the demodulator's `repairs` and unconverged-junction
 counters for that step (and where its repairs stopped: the checkpoint at which each met the stored run), the loop kernels' main-pass grids (segments / 128) and the card's name, power limit and SM clock.
+For each main pass it also prints the bytes it moves (nseg x (L + W) input samples, its outputs) over its time, and its time as SM cycles
+per sample (k_costas) or per symbol (k_mm) of one warp, at the SM clock read after the run.
+
+  --lib PATH   time another build of libb200dsp.so (e.g. the parent commit's) instead of satdump_b200/csrc's: alternate two builds in
+               one session to compare them
+  --cycles     build the library with -DB200_LOOP_CYCLES into a temporary directory (unless --lib names one built so) and print where
+               the main passes' cycles go: per warp, the row wait, the loop itself and the output path (clock64() totals of lane 0)
 """
 import collections
 import json
+import math
 import os
 import re
 import subprocess
@@ -33,13 +41,40 @@ def card():
         return {}
 
 
+def round_up16(x):
+    return (int(math.ceil(x)) + 15) & ~15
+
+
+def loop_geometry(cfg, n, nblk):
+    """Segment count, L and the Costas / M&M warm-ups of a main pass of nblk CTAs, as the demodulator sets them (api_demod.cu) for a
+    signal without a resampler, with the default clock_gain_mu."""
+    nseg = nblk * SEG_THREADS
+    L = round_up16(n / nseg)
+    sps = cfg.samplerate / cfg.symbolrate
+    wc = round_up16((72.0 if cfg.constellation == "8psk" else 24.0) / cfg.pll_bw)
+    ref_sps = 2.5 if cfg.constellation == "bpsk" else 2.5714
+    wm = round_up16((240.0 if cfg.constellation == "bpsk" else 87.5) * max(1.0, sps * sps / (ref_sps * ref_sps)) / 8.7e-3)
+    return nseg, L, wc, wm, sps
+
+
 def main():
     import torch
     from torch.profiler import ProfilerActivity, profile
 
-    wname = sys.argv[1] if len(sys.argv) > 1 else "c3"
-    lg = int(sys.argv[2]) if len(sys.argv) > 2 else 29
-    esn0 = float(sys.argv[3]) if len(sys.argv) > 3 else None
+    args = [a for a in sys.argv[1:] if not a.startswith("--")]
+    flags = sys.argv[1:]
+    if "--lib" in flags:
+        capi.LIB_PATH = os.path.abspath(flags[flags.index("--lib") + 1])
+        args.remove(flags[flags.index("--lib") + 1])
+    cycles = "--cycles" in flags
+    if cycles and "--lib" not in flags:
+        out = os.path.join(tempfile.gettempdir(), "b200_loop_cycles")
+        subprocess.run(["make", "-s", "-j8", "-C", os.path.join(os.path.dirname(bench.__file__), "satdump_b200", "csrc"), "cycles",
+                        f"CYCLES_DIR={out}"], check=True, stdout=subprocess.DEVNULL)
+        capi.LIB_PATH = os.path.join(out, "libb200dsp.so")
+    wname = args[0] if len(args) > 0 else "c3"
+    lg = int(args[1]) if len(args) > 1 else 29
+    esn0 = float(args[2]) if len(args) > 2 else None
     w = bench.WORKLOADS[wname]
     assert w["kind"] == "chain", "the loop stages are profiled through a chain workload"
     cfg, raw, _ = bench.make_workload(w, lg, 0, "cuda", esn0)
@@ -62,6 +97,8 @@ def main():
         torch.cuda.synchronize()
         step_ms.append(t0.elapsed_time(t1))
     timing = pipe.timing()
+    if cycles:
+        capi.loop_cycles()  # clear what the warm-up and the timed steps counted
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         step()
         torch.cuda.synchronize()
@@ -95,10 +132,33 @@ def main():
     print(f"demodulator counters of the profiled step: {dstats}; main-pass grids (CTAs of {SEG_THREADS} segments): {grids}")
     buckets = ["whole segment", "1", "2", "3-4", "5-8", "9-16", "17-32", ">32"]
     print(f"repairs by the {capi.CKPT}-sample checkpoint at which they met the stored run and stopped: {dict(zip(buckets, merge_hist))}")
+    print(f"library {capi.LIB_PATH}")
     print(f"{'kernel':<18}{'launches':>9}{'ms':>10}")
     for k, (ms, cnt) in acc.items():
         if cnt:
             print(f"{k:<18}{cnt:>9}{ms:>10.3f}")
+    lc = capi.loop_cycles() if cycles else None
+    clock = card().get("clocks.sm", "")
+    hz = float(clock.split()[0]) * 1e6 if clock[:1].isdigit() else None
+    for k, unit in (("k_costas", "sample"), ("k_mm", "symbol")):
+        if k not in grids or not acc[k][1]:
+            continue
+        nseg, L, wc, wm, sps = loop_geometry(cfg, n, grids[k])
+        ms = acc[k][0]
+        if k == "k_costas":
+            steps, nbytes = L + wc, nseg * (L + wc) * 8 + n * 8  # per thread: samples; in: segments with warm-ups, out: the stream
+        else:
+            steps, nbytes = (L + wm) / sps, nseg * (L + wm) * 8 + int(n / sps) * 8  # in: segments with warm-ups, out: owned symbols
+        per = f"{ms * 1e-3 * hz / steps:.0f} SM cycles per {unit} of one warp at {clock}" if hz else "SM clock not read"
+        print(f"{k} main pass: nseg {nseg}, L {L}, W {wc if k == 'k_costas' else wm}: {nbytes / 1e9:.2f} GB in {ms:.3f} ms = "
+              f"{nbytes / ms / 1e9:.2f} TB/s; {per}")
+        if lc:
+            c = lc[k]
+            names = ("row wait", "Costas loop", "copy-out", "tail") if k == "k_costas" else ("row wait", "input fix-up", "symbol loop", "symbol copy-out")
+            warps = max(1, c[4])
+            tot = sum(c[:4])
+            print(f"  clock64() per warp ({warps} warps, per {unit}: / {steps:.0f}): " + ", ".join(
+                f"{nm} {v / warps:.0f} ({100 * v / max(1, tot):.1f} %, {v / warps / steps:.0f}/{unit})" for nm, v in zip(names, c[:4])))
 
 
 if __name__ == "__main__":

@@ -17,6 +17,7 @@
  *                    src-core/pipeline/modules/ccsds/module_ccsds_conv_concat_decoder.cpp:140-200 (kind CCSDS, r=1/2)
  *                    src-core/pipeline/modules/ccsds/module_ccsds_ldpc_decoder.cpp:134-277       (kind LDPC, ldpc_rate "7/8")
  *                    src-core/pipeline/modules/ccsds/module_ccsds_turbo_decoder.cpp:137-235      (kind TURBO)
+ *                    plugins/noaa_metop_support/metop/module_metop_dump_decoder.cpp:27-83        (kind METOP_DUMP)
  *   b200_chain_*   both modules joined the way Pipeline::run joins them with a byte FIFO
  *                    src-core/pipeline/pipeline_run.cpp:44-117 — here the int8 soft stream never leaves HBM.
  *   b200_demux_*   the step behind the decoder: CADUs -> CCSDS space packets
@@ -47,7 +48,7 @@ enum { B200_BPSK = 0, B200_QPSK = 1, B200_OQPSK = 2, B200_8PSK = 3, B200_NONE = 
 /* baseband_format (common/dsp/io/baseband_type.h:7-21) */
 enum { B200_CF32 = 0, B200_CS16 = 1, B200_CS8 = 2 };
 /* decoder kind */
-enum { B200_FEC_METOP = 0, B200_FEC_CCSDS = 1, B200_FEC_SIMPLE = 2, B200_FEC_LDPC = 3, B200_FEC_TURBO = 4 };
+enum { B200_FEC_METOP = 0, B200_FEC_CCSDS = 1, B200_FEC_SIMPLE = 2, B200_FEC_LDPC = 3, B200_FEC_TURBO = 4, B200_FEC_METOP_DUMP = 5 };
 /* debug stage ids for b200_demod_debug_stage */
 enum { B200_STAGE_AGC = 0, B200_STAGE_FIR = 1, B200_STAGE_COSTAS = 2, B200_STAGE_RESAMP = 3, B200_STAGE_DC = 4, B200_STAGE_MM = 5,
        B200_STAGE_PLL = 6 /* pm_demod: PLLCarrierTrackingBlock output */, B200_STAGE_PM = 7 /* pm_demod: PMToBPSK output */ };
@@ -142,6 +143,10 @@ typedef struct b200_fec_cfg
     int turbo_rate;           /* "turbo_rate": 2, 3, 4, 6 = "1/2", "1/3", "1/4", "1/6"                                                     */
     int turbo_base;           /* "turbo_base": 223, 446, 892 or 1115 (information bytes per frame)                                          */
     int turbo_iters;          /* "turbo_iters" >= 1 (the reference dereferences NULL with 0)                                               */
+    /* kind B200_FEC_METOP_DUMP = metop_dump_decoder (no parameters): Correlator32 on the QPSK ASM 0x1ACFFC1D (8 syncwords: 4 phases x IQ
+       swap, hard bits) over 8192-soft-byte frames, phase fix, hard decisions, inversion, derandomiser, RS(255,223) I=4 dual basis; every
+       frame is written as 1A CF FC 1D + 1020 bytes, whatever RS returned. Only device and max_soft are read. Device memory: about 3 bytes
+       per max_soft byte (FIFO, hard bits, correlator scores) plus 2 KiB of CADUs per 8192 soft bytes.                                 */
 } b200_fec_cfg;
 
 typedef struct b200_demod_stats
@@ -183,7 +188,9 @@ typedef struct b200_fec_stats
     float correlator_corr;    /* "correlator_corr": the correlator's best score                                                       */
     int ldpc_corr;            /* "ldpc_corr": info positions whose decoded bit differs from the sign of the input                     */
     long ldpc_resyncs;        /* frames so far whose ASM was not at the expected place (the frame walk shifted)                       */
-    /* ccsds_turbo_decoder: correlator_lock / correlator_corr above are its "Corr" and lock state; ldpc_resyncs counts its shifted frames */
+    /* ccsds_turbo_decoder: correlator_lock / correlator_corr above are its "Corr" and lock state; ldpc_resyncs counts its shifted frames.
+       metop_dump_decoder: correlator_lock is "lock_state" (SYNCED iff the last frame's pos was 0), correlator_corr its correlation (0..32),
+       ldpc_resyncs the frames whose pos was not 0, rs_corrected / rs_failed above its RS results */
     long crc_ok, crc_fail;    /* frames so far whose CRC-16 passed (written) / failed ("CRC Check" PASS / FAIL)                        */
     long turbo_near_ties;     /* decisions so far whose margin |one - zero| was below 1e-9 (where libm rounding could tip a bit)       */
 } b200_fec_stats;
@@ -295,6 +302,17 @@ int b200_fec_debug_turbo_llr(b200_fec *f, long frame, double *app0, double *app1
 /* ccsds_turbo_decoder only (B200_EINVAL for the other kinds): elapsed device milliseconds of the last push: [0] correlation, [1] frame
    walk, [2] gather, [3] BCJR iterations, [4] packing, CRC and compaction, [5] the whole push */
 int b200_fec_turbo_timing(b200_fec *f, float *ms_out, int n);
+/* metop_dump_decoder: one record per frame of the LAST push, in stream order */
+typedef struct b200_dump_frame
+{
+    long offset;              /* stream offset (soft bytes since create / reset) of the frame's first byte (after the shift)          */
+    int pos;                  /* the correlator's position in the window read before it (0 = locked; >= 8192: a window-tail winner,
+                                 which the module does not shift)                                                                   */
+    int corr;                 /* the correlator's value (0..32)                                                                    */
+    int phase, swap;          /* the phase ambiguity fixed (0..3 = 0, 90, 180, 270 degrees) and the IQ swap                        */
+    int rs[4];                /* decode_interlaved's errors[] of the four codewords: -1 = not decodable, else bytes corrected       */
+} b200_dump_frame;
+int b200_fec_debug_dump_frames(b200_fec *f, b200_dump_frame *out, long cap, long *n_out);
 
 /* ---- fused chain: raw IQ -> CADUs, soft stream stays in HBM ---------------------------------------- */
 b200_chain *b200_chain_create(const b200_demod_cfg *dcfg, const b200_fec_cfg *fcfg);

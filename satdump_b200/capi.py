@@ -25,7 +25,7 @@ SYMBOLS = [
     "b200_demod_pull_symbols", "b200_demod_debug_stage", "b200_demod_debug_convert", "b200_demod_debug_run_stage", "b200_demod_debug_junctions", "b200_demod_debug_repair_merge", "b200_demod_debug_loop_cycles", "b200_demod_reset", "b200_demod_prefetch_iq", "b200_demod_last_timing", "b200_demod_get_stats", "b200_demod_get_taps",
     "b200_fec_create", "b200_fec_destroy", "b200_fec_push_soft", "b200_fec_push_soft_device", "b200_fec_pull_frames",
     "b200_fec_debug_bits", "b200_fec_get_stats", "b200_fec_cadu_bytes", "b200_fec_chunk_size", "b200_fec_debug_ldpc_frames", "b200_fec_ldpc_timing",
-    "b200_fec_debug_turbo_frames", "b200_fec_debug_turbo_llr", "b200_fec_turbo_timing",
+    "b200_fec_debug_turbo_frames", "b200_fec_debug_turbo_llr", "b200_fec_turbo_timing", "b200_fec_debug_dump_frames",
     "b200_chain_create", "b200_chain_destroy", "b200_chain_push_iq", "b200_chain_push_iq_device", "b200_chain_prefetch_iq", "b200_chain_pull_frames",
     "b200_chain_frames_device", "b200_chain_get_stats", "b200_chain_last_timing", "b200_chain_reset",
     "b200_chain_set_pipelined", "b200_chain_sync", "b200_chain_span_begin", "b200_chain_span_end",
@@ -94,6 +94,10 @@ class TurboFrame(C.Structure):
     _fields_ = [("offset", C.c_long), ("pos", C.c_int), ("cor", C.c_float), ("swapped", C.c_int), ("crc_ok", C.c_int)]
 
 
+class DumpFrame(C.Structure):
+    _fields_ = [("offset", C.c_long), ("pos", C.c_int), ("corr", C.c_int), ("phase", C.c_int), ("swap", C.c_int), ("rs", C.c_int * 4)]
+
+
 class B200Error(RuntimeError):
     def __init__(self, code, msg):
         super().__init__(f"{E_NAMES.get(code, code)}: {msg}")
@@ -147,6 +151,7 @@ def lib():
         L.b200_fec_debug_turbo_frames.argtypes = [vp, C.POINTER(TurboFrame), cl, C.POINTER(cl)]
         L.b200_fec_turbo_timing.argtypes = [vp, vp, ci]
         L.b200_fec_debug_turbo_llr.argtypes = [vp, cl, vp, vp, cl, C.POINTER(cl)]
+        L.b200_fec_debug_dump_frames.argtypes = [vp, C.POINTER(DumpFrame), cl, C.POINTER(cl)]
         L.b200_chain_create.restype = vp
         L.b200_chain_create.argtypes = [C.POINTER(DemodCfg), C.POINTER(FecCfg)]
         L.b200_chain_destroy.argtypes = [vp]
@@ -291,11 +296,20 @@ def turbo_cfg(turbo_rate=None, turbo_base=None, turbo_iters=None, device=0, max_
     return cfg
 
 
+def dump_cfg(device=0, max_soft=1 << 24):
+    """metop_dump_decoder (module_metop_dump_decoder.cpp): the module takes no parameters."""
+    cfg = FecCfg()
+    cfg.kind, cfg.constellation, cfg.cadu_size, cfg.device, cfg.max_soft = 5, CONST["qpsk"], 8192, device, max_soft
+    return cfg
+
+
 def fec_cfg_for(sig, max_soft, device=0):
     """The decoder configuration that goes with a satdump_b200.synth.SignalCfg (metop_ahrpt_decoder / ccsds_conv_concat_decoder /
     ccsds_simple_psk_decoder parameters of the shipped pipeline JSONs)."""
     if sig.decoder == "metop":
         return metop_cfg(sig.ber_thresold, sig.outsync_after, device=device, max_soft=max_soft)
+    if sig.decoder == "dump":
+        return dump_cfg(device=device, max_soft=max_soft)
     if sig.decoder == "turbo":
         return turbo_cfg(sig.turbo_rate, sig.turbo_base, sig.turbo_iters, device=device, max_soft=max_soft)
     if sig.decoder == "ldpc":
@@ -511,6 +525,19 @@ class Fec:
         for k in range(n.value):
             r = recs[k]
             out[k] = [r.offset, r.pos, int(np.float32(r.cor).view(np.uint32)), r.swapped, r.crc_ok, int(r.pos == 0)]
+        return out
+
+    def dump_frames(self):
+        """metop_dump_decoder: one record per frame of the last push as int64 [n, 9] = offset, pos, corr, phase, swap, rs[0..3]
+        (oracle.dump.REC)."""
+        cap = int(self._n) // 8192 + 4
+        recs = (DumpFrame * cap)()
+        n = C.c_long(0)
+        _chk(lib().b200_fec_debug_dump_frames(self.h, recs, cap, C.byref(n)))
+        out = np.zeros((n.value, 9), np.int64)
+        for k in range(n.value):
+            r = recs[k]
+            out[k] = [r.offset, r.pos, r.corr, r.phase, r.swap, *r.rs]
         return out
 
     def turbo_llr(self, frame, K):

@@ -48,7 +48,8 @@ void build_rs_tables(RsTables &T)
 
 Fec::Fec(const b200_fec_cfg &c) : cfg(c)
 {
-    B200_REQUIRE(c.kind == B200_FEC_METOP || c.kind == B200_FEC_CCSDS || c.kind == B200_FEC_SIMPLE || c.kind == B200_FEC_LDPC || c.kind == B200_FEC_TURBO,
+    B200_REQUIRE(c.kind == B200_FEC_METOP || c.kind == B200_FEC_CCSDS || c.kind == B200_FEC_SIMPLE || c.kind == B200_FEC_LDPC || c.kind == B200_FEC_TURBO ||
+                     c.kind == B200_FEC_METOP_DUMP,
                  B200_EINVAL, "unknown decoder kind %d", c.kind);
     B200_REQUIRE(c.max_soft >= 65536, B200_EINVAL, "max_soft must be >= 65536");
     memset(&geom, 0, sizeof(geom));
@@ -58,6 +59,10 @@ Fec::Fec(const b200_fec_cfg &c) : cfg(c)
     }
     if (c.kind == B200_FEC_TURBO) {
         turbo_init();
+        return;
+    }
+    if (c.kind == B200_FEC_METOP_DUMP) {
+        dump_init();
         return;
     }
     if (c.kind != B200_FEC_METOP) {
@@ -203,6 +208,7 @@ Fec::~Fec()
         cudaStreamSynchronize(stream);
     ldpc_free();
     turbo_free();
+    dump_free();
     for (auto &e : ev)
         cudaEventDestroy(e);
     for (auto &e : evm)
@@ -652,6 +658,10 @@ void Fec::reset()
         turbo_reset();
         return;
     }
+    if (dump) {
+        dump_reset();
+        return;
+    }
     start_stream(64);
     B200_CUDA(cudaStreamSynchronize(stream));
 }
@@ -889,6 +899,10 @@ void Fec::process()
         turbo_process();
         return;
     }
+    if (dump) {
+        dump_process();
+        return;
+    }
     const long nch = soft_have / geom.chunk;
     B200_REQUIRE(nch <= max_chunks, B200_ESTATE, "internal: too many chunks");
     // (lazy, so that b200_fec_debug_bits can still read the previous push's bits until now)
@@ -953,6 +967,8 @@ void Fec::stats(b200_fec_stats *o)
         ldpc_stats(o);
     if (turbo)
         turbo_stats(o);
+    if (dump)
+        dump_stats(o);
 }
 
 } // namespace b200
@@ -1059,6 +1075,13 @@ int b200_fec_debug_turbo_llr(b200_fec *h, long frame, double *app0, double *app1
         B200_REQUIRE(h && app0 && app1 && n_out, B200_EINVAL, "NULL argument");
         DeviceGuard g(h->f->cfg.device);
         *n_out = h->f->turbo_llr(frame, app0, app1, cap);
+    });
+}
+int b200_fec_debug_dump_frames(b200_fec *h, b200_dump_frame *out, long cap, long *n_out)
+{
+    return guarded([&] {
+        B200_REQUIRE(h && out && n_out, B200_EINVAL, "NULL argument");
+        *n_out = h->f->dump_frames(out, cap);
     });
 }
 int b200_fec_turbo_timing(b200_fec *h, float *ms_out, int n)

@@ -1225,7 +1225,7 @@ struct FrameCfg
     uint32_t sync;
 };
 
-#ifdef B200_DEFINE_KERNELS
+// (the Reed-Solomon device code up to k_frames is also used by the MetOp dump decoder's frame kernel, dump.cuh)
 __device__ __forceinline__ uint8_t gf_mul(const RsTables &T, uint8_t a, uint8_t b) { return (!a || !b) ? 0 : T.exp[T.log[a] + T.log[b]]; }
 __device__ __forceinline__ uint8_t gf_div(const RsTables &T, uint8_t a, uint8_t b) { return (!a || !b) ? 0 : T.exp[255 + T.log[a] - T.log[b]]; }
 __device__ __forceinline__ uint8_t gf_pow(const RsTables &T, uint8_t a, int p) { return T.exp[((int)T.log[a] * p) % 255]; }
@@ -1241,7 +1241,7 @@ __device__ __forceinline__ uint8_t log_mul(uint8_t a, uint8_t b) { unsigned r = 
 //   Forney (:165-196) + the location search (:198-222): lane q handles root q. The reference finds the location by scanning j = 0..255
 //     for j^11 == 1/root; that is j = (1/root)^(11^-1 mod 255), i.e. log j = 116 * log(1/root) mod 255 - except that its scan meets
 //     j = 0 first, whose "power" reads exp[0] = 1: for 1/root == 1 the location is log[0] = 0 (checked against the scan for every value).
-__device__ bool rs_correct_warp(const RsTables &T, uint8_t *r, const uint8_t *syn, int nroots, int fcr, uint8_t *lam, uint8_t *prev, uint8_t *lamlog,
+__device__ inline bool rs_correct_warp(const RsTables &T, uint8_t *r, const uint8_t *syn, int nroots, int fcr, uint8_t *lam, uint8_t *prev, uint8_t *lamlog,
                                 uint8_t *roots, uint8_t *om, uint8_t *der, int lane)
 {
     unsigned order = 0;
@@ -1326,10 +1326,60 @@ __device__ bool rs_correct_warp(const RsTables &T, uint8_t *r, const uint8_t *sy
     return true;
 }
 
-// One CTA per frame; warp w decodes interleave w (up to 8 warps). Writes the frame (cadu_bytes) and rs_err[frame*rs_i + w].
-#endif // B200_DEFINE_KERNELS
 constexpr int RS_MAX_I = 8;
+
+// decode_interlaved for interleave `warp` of the frame in shared memory, by one warp (`work`: its 704 bytes of scratch): deinterleave,
+// dual basis -> conventional, syndromes, then rs_correct_warp. Writes the corrected message bytes back into the frame; returns -1 when
+// the codeword does not decode, else the number of message bytes changed.
+__device__ __forceinline__ int rs_decode_interleave(const RsTables &T, uint8_t *frame, const FrameCfg &fc, uint8_t *work, int warp, int lane)
+{
+    uint8_t *r = work, *syn = r + 256, *lam = syn + 64, *prev = lam + 66, *lamlog = prev + 66, *roots = lamlog + 66, *om = roots + 64,
+            *der = om + 32;
+    // deinterleave + dual->conventional + reverse: r[i] = cw[254-i]  (reedsolomon.cpp:145-149,73-77; decode.c:322-324)
+    for (int i = lane; i < 255; i += 32) {
+        uint8_t v = frame[4 + (254 - i) * fc.rs_i + warp];
+        r[i] = fc.rs_dual ? T.from_dual[v] : v;
+    }
+    __syncwarp();
+    // syndromes, lane j -> syndrome j (decode.c:12-28)
+    uint8_t s = 0;
+    if (lane < fc.rs_nroots) {
+        const uint8_t rootlog = T.log[T.exp[(11 * (lane + fc.rs_fcr)) % 255]];
+        uint8_t pw = T.log[1];
+#pragma unroll 5
+        for (int i = 0; i < 255; i++) {
+            const uint8_t v = r[i];
+            if (v) s ^= T.exp[T.log[v] + pw];
+            pw = log_mul(pw, rootlog);
+        }
+        syn[lane] = s;
+    }
+    const unsigned nz = __ballot_sync(0xffffffffu, s != 0);
+    __syncwarp();
+    int err = 0;
+    if (nz) {
+        const int ok = rs_correct_warp(T, r, syn, fc.rs_nroots, fc.rs_fcr, lam, prev, lamlog, roots, om, der, lane) ? 1 : 0;
+        if (!ok) err = -1;
+        else {
+            // copy back the message bytes only; parity stays as received (reedsolomon.cpp:96-104)
+            const int k = 255 - fc.rs_nroots;
+            int changed = 0;
+            for (int i = lane; i < k; i += 32) {
+                const uint8_t nv = r[254 - i];
+                const int idx = 4 + i * fc.rs_i + warp;
+                const uint8_t ov = fc.rs_dual ? T.from_dual[frame[idx]] : frame[idx];
+                if (nv != ov) changed++;
+                frame[idx] = fc.rs_dual ? T.to_dual[nv] : nv;
+            }
+            for (int off = 16; off; off >>= 1) changed += __shfl_xor_sync(0xffffffffu, changed, off);
+            err = changed;
+        }
+    }
+    return err;
+}
+
 #ifdef B200_DEFINE_KERNELS
+// One CTA per frame; warp w decodes interleave w (up to 8 warps). Writes the frame (cadu_bytes) and rs_err[frame*rs_i + w].
 __global__ void __launch_bounds__(256) k_frames(const uint32_t *__restrict__ fifo, const FrameRec *__restrict__ frames, int nframes, FrameCfg fc,
                                                  const RsTables *__restrict__ gtab, uint8_t *__restrict__ out, int *__restrict__ rs_err)
 {
@@ -1362,48 +1412,7 @@ __global__ void __launch_bounds__(256) k_frames(const uint32_t *__restrict__ fif
         (void)pay_bytes;
         __syncthreads();
         if (warp < fc.rs_i) {
-            uint8_t *r = work + warp * 704, *syn = r + 256, *lam = syn + 64, *prev = lam + 66, *lamlog = prev + 66, *roots = lamlog + 66, *om = roots + 64,
-                    *der = om + 32;
-            // deinterleave + dual->conventional + reverse: r[i] = cw[254-i]  (reedsolomon.cpp:145-149,73-77; decode.c:322-324)
-            for (int i = lane; i < 255; i += 32) {
-                uint8_t v = frame[4 + (254 - i) * fc.rs_i + warp];
-                r[i] = fc.rs_dual ? T.from_dual[v] : v;
-            }
-            __syncwarp();
-            // syndromes, lane j -> syndrome j (decode.c:12-28)
-            uint8_t s = 0;
-            if (lane < fc.rs_nroots) {
-                const uint8_t rootlog = T.log[T.exp[(11 * (lane + fc.rs_fcr)) % 255]];
-                uint8_t pw = T.log[1];
-#pragma unroll 5
-                for (int i = 0; i < 255; i++) {
-                    const uint8_t v = r[i];
-                    if (v) s ^= T.exp[T.log[v] + pw];
-                    pw = log_mul(pw, rootlog);
-                }
-                syn[lane] = s;
-            }
-            const unsigned nz = __ballot_sync(0xffffffffu, s != 0);
-            __syncwarp();
-            int err = 0;
-            if (nz) {
-                const int ok = rs_correct_warp(T, r, syn, fc.rs_nroots, fc.rs_fcr, lam, prev, lamlog, roots, om, der, lane) ? 1 : 0;
-                if (!ok) err = -1;
-                else {
-                    // copy back the message bytes only; parity stays as received (reedsolomon.cpp:96-104)
-                    const int k = 255 - fc.rs_nroots;
-                    int changed = 0;
-                    for (int i = lane; i < k; i += 32) {
-                        const uint8_t nv = r[254 - i];
-                        const int idx = 4 + i * fc.rs_i + warp;
-                        const uint8_t ov = fc.rs_dual ? T.from_dual[frame[idx]] : frame[idx];
-                        if (nv != ov) changed++;
-                        frame[idx] = fc.rs_dual ? T.to_dual[nv] : nv;
-                    }
-                    for (int off = 16; off; off >>= 1) changed += __shfl_xor_sync(0xffffffffu, changed, off);
-                    err = changed;
-                }
-            }
+            const int err = rs_decode_interleave(T, frame, fc, work + warp * 704, warp, lane);
             if (lane == 0) rs_err[(long)f * fc.rs_i + warp] = err;
         }
         __syncthreads();

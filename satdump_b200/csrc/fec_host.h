@@ -14,6 +14,7 @@ namespace b200
 struct DefrEvent { long pos; int state; int pad; };
 struct Ldpc; // ccsds_ldpc_decoder's state (api_ldpc.cu)
 struct Turbo; // ccsds_turbo_decoder's state (api_turbo.cu)
+struct Dump; // metop_dump_decoder's state (api_dump.cu)
 
 // the CCSDS sequence (x^8+x^7+x^5+x^3+1 from all ones), one bit per entry as derand_ccsds_soft applies it to soft bytes (255 entries)
 void ccsds_pn_bits(unsigned char *pn);
@@ -54,6 +55,9 @@ class Fec
     long turbo_frames(b200_turbo_frame *out, long cap); // records of the last push
     long turbo_llr(long frame, double *app0, double *app1, long cap);
     void turbo_timing(float *ms, int n);
+    // metop_dump_decoder (B200_FEC_METOP_DUMP): the same soft FIFO, its own correlator and frame walk, RS through k_frames' decoder
+    Dump *dump = nullptr;
+    long dump_frames(b200_dump_frame *out, long cap); // records of the last push
 
     // device storage
     DevBuf<int8_t> softbuf;
@@ -148,6 +152,11 @@ class Fec
     void turbo_reset();
     void turbo_process();
     void turbo_stats(b200_fec_stats *o);
+    void dump_init();
+    void dump_free();
+    void dump_reset();
+    void dump_process();
+    void dump_stats(b200_fec_stats *o);
 };
 
 void build_rs_tables(RsTables &T);

@@ -58,24 +58,6 @@ __global__ void __launch_bounds__(256) k_ldpc_corr(const int8_t *__restrict__ so
     }
 }
 
-// first maximum of the scores over window [a, a + npos), by one warp: the partial blocks at both ends position by position, the
-// complete blocks through their maxima
-__device__ void ldpc_window_max(const float *__restrict__ score, const float *__restrict__ bval, const int *__restrict__ bidx, long a,
-                                int npos, float &v, int &vi)
-{
-    const int lane = threadIdx.x & 31;
-    const long e = a + npos;
-    const long b0 = (a + 31) >> 5, b1 = e >> 5;
-    v = -INFINITY;
-    vi = 0x7fffffff;
-    const long h = a + lane;
-    if (h < (b0 << 5) && h < e) ldpc_best(v, vi, score[h], (int)h);
-    for (long b = b0 + lane; b < b1; b += 32) ldpc_best(v, vi, bval[b], bidx[b]);
-    const long t = (b1 << 5) + lane;
-    if (b1 >= b0 && t < e) ldpc_best(v, vi, score[t], (int)t);
-    ldpc_best_warp(v, vi);
-}
-
 // The frame walk over the `have` soft bytes of the FIFO, from offset 0, for frames of F soft bytes whose windows hold npos correlator
 // positions. Each round checks up to LDPC_WALK_SPEC frames of the current lattice o + jF at once (one warp per frame): the frames up to
 // and including the first one whose ASM is not at its window's start are exact, since their windows start where the module would read
@@ -144,23 +126,6 @@ __global__ void __launch_bounds__(1024) k_ldpc_walk(const float *__restrict__ sc
         out->nf = s_nf;
         out->shifted = s_shifted;
     }
-}
-
-// soft byte k (0 .. F-1) of a frame after rotate_soft(phase, swap) (rotation.cpp:4-63)
-__device__ __forceinline__ int ldpc_rot(const int8_t *__restrict__ f, int k, int phase, int swap)
-{
-    int vi = f[k & ~1], vq = f[k | 1];
-    if (vi == -128) vi = -127;
-    if (vq == -128) vq = -127;
-    if (swap) { const int t = vi; vi = vq; vq = t; }
-    int oi, oq;
-    switch (phase) {
-    case 1: oi = vq; oq = -vi; break;
-    case 2: oi = -vi; oq = -vq; break;
-    case 3: oi = -vq; oq = vi; break;
-    default: oi = vi; oq = vq; break;
-    }
-    return (k & 1) ? oq : oi;
 }
 
 // One CTA per frame: the decoder's input vn[0 .. 8175] = 18 zeros, then code soft bytes 0 .. 8157 of the frame after the phase fix

@@ -256,6 +256,13 @@ b200_demod_cfg pm_demod_cfg_from_params(const Params &p, bool &is_bpsk)
 b200_fec_cfg fec_cfg_from_params(const std::string &id, const Params &p)
 {
     b200_fec_cfg c{};
+    if (id == "metop_dump_decoder") { // module_metop_dump_decoder.cpp:18-23: no parameters
+        c.kind = B200_FEC_METOP_DUMP;
+        c.device = (int)p.num("b200_device", 0);
+        c.constellation = B200_QPSK;
+        c.cadu_size = 8192;
+        return c;
+    }
     if (id == "ccsds_turbo_decoder") { // module_ccsds_turbo_decoder.cpp:17-36,118-119; the library checks the values (turbo_iters >= 1)
         c.kind = B200_FEC_TURBO;
         c.device = (int)p.num("b200_device", 0);
@@ -663,8 +670,10 @@ void FusedStage::process()
         {
             b200_demod_stats dst;
             b200_fec_stats fst;
-            if (b200_chain_get_stats(h, &dst, &fst) == B200_OK)
+            if (b200_chain_get_stats(h, &dst, &fst) == B200_OK) {
                 warn_unconverged(dst);
+                correlator_lock = fst.correlator_lock;
+            }
         }
         drain();
         size_t used = (size_t)ns * bpsamp;

@@ -125,6 +125,7 @@ class FecStage : public StageBase
     std::atomic<float> viterbi_ber{10.f};
     // ccsds_ldpc_decoder: correlator_lock, correlator_corr, ldpc_corr (module_ccsds_ldpc_decoder.cpp:279-295); deframer_state above.
     // ccsds_turbo_decoder: correlator_lock, correlator_corr and crc_lock, what its window shows (module_ccsds_turbo_decoder.cpp:259-290)
+    // metop_dump_decoder: "lock_state" = correlator_lock (module_metop_dump_decoder.cpp:84-90)
     std::atomic<int> correlator_lock{0}, ldpc_corr{0};
     std::atomic<float> correlator_corr{0.f};
     std::atomic<int> crc_lock{0};
@@ -146,6 +147,7 @@ class FusedStage : public StageBase
     void process() override;
     std::string getID() const override { return "b200_psk_" + dec_id; }
     std::atomic<long> frames_written{0};
+    std::atomic<int> correlator_lock{0}; // the decoder's correlator lock ("lock_state" of metop_dump_decoder / ccsds_ldpc_decoder)
     std::atomic<double> progress{0};
     long batch_samples = 1 << 26;
   private:

@@ -302,6 +302,10 @@ CONFIGS = {
     # 1 MS/s (2.7 samples per symbol)
     "turbo_bpsk": SignalCfg(name="turbo_bpsk", samplerate=1e6, symbolrate=368000, constellation="bpsk", conv="turbo", rrc_alpha=0.35, fmt="cs16",
                             decoder="turbo", esn0_db=6.0, pll_bw=0.002, post_costas_dc=True, turbo_rate=6, turbo_base=1115, turbo_iters=1),
+    # psk_demod QPSK -> metop_dump_decoder, the MetOp X-band dump (MetOp.json "metop_dump"): 35 Msym/s at 45 MS/s (1.286 samples per
+    # symbol), pll_bw 0.03, no convolutional code, randomised CADUs with RS(255,223) I=4 dual basis; cs16 (cs8: dataclasses.replace)
+    "metop_dump": SignalCfg(name="metop_dump", samplerate=45e6, symbolrate=35000000, constellation="qpsk", conv="none", interleave=4,
+                            rrc_alpha=0.5, pll_bw=0.03, fmt="cs16", decoder="dump", esn0_db=16.0),
 }
 
 
@@ -332,6 +336,9 @@ def qpsk_diff_encode(dibits, swap=True):
 def make_bitstream(cfg: SignalCfg, nframes, seed):
     if cfg.decoder == "turbo":  # nframes turbo frames
         tx, clear = turbo_frames(nframes, cfg.turbo_rate, cfg.turbo_base, seed)
+        return tx.reshape(-1), clear
+    if cfg.decoder == "dump":  # nframes CADUs, sent as they are
+        tx, clear = dump_frames(nframes, seed)
         return tx.reshape(-1), clear
     if cfg.decoder == "ldpc":  # nframes LDPC frames
         if cfg.internal_cadu_size:
@@ -450,7 +457,7 @@ def frames_for_samples(cfg: SignalCfg, nsamples):
     if cfg.decoder == "turbo":  # turbo frames of ASM + codeword bits
         nbits = turbo_codeword_bits(cfg.turbo_rate, cfg.turbo_base) + TURBO_ASM_BITS[cfg.turbo_rate]
         return int(nsamples * bps / (cfg.samplerate / cfg.symbolrate) / nbits) + 2
-    if cfg.decoder == "ldpc":  # LDPC frames of 8192 bits
+    if cfg.decoder in ("ldpc", "dump"):  # LDPC frames / MetOp dump CADUs of 8192 bits
         return int(nsamples * bps / (cfg.samplerate / cfg.symbolrate) / 8192) + 2
     rate = {"1/2": 0.5, "3/4": 0.75, "none": 1.0, "p2/3": 2 / 3, "p3/4": 0.75, "p5/6": 5 / 6, "p7/8": 7 / 8}[cfg.conv]
     bits_per_sample = bps * rate / (cfg.samplerate / cfg.symbolrate)
@@ -695,6 +702,33 @@ def ldpc_inner_frames(nframes, cadu_size, asm, seed):
     inner = np.concatenate([np.tile(asm_bits, (k, 1)), rng.integers(0, 2, (k, cadu_size - 32), dtype=np.uint8)], axis=1)
     bits = np.concatenate([inner.reshape(-1), rng.integers(0, 2, total - k * cadu_size, dtype=np.uint8)])
     return bits.reshape(nframes, LDPC_INFO), np.packbits(inner, axis=1)
+
+
+# ---- MetOp X-band dump (metop_dump_decoder) ---------------------------------------------------------------------------------------------
+def dump_frames(nframes, seed=0):
+    """(tx bits uint8 [n, 8192] of randomised CADUs with RS(255,223) I=4 dual basis, the CADUs metop_dump_decoder writes for them
+    [n, 1024]: the ASM and the derandomised codewords)."""
+    payload = np.random.default_rng(seed).integers(0, 256, size=(nframes, 4 * 223), dtype=np.uint8)
+    tx, clear = build_cadus(payload, 4)
+    return np.unpackbits(tx, axis=1), clear
+
+
+def dump_soft(tx_bits, phase=0, swap=False, amp=60.0, sigma=0.0, seed=0):
+    """int8 soft stream of the bit stream (I, Q = consecutive bits) that metop_dump_decoder decodes with phase `phase` (0..3 = 0 .. 270
+    degrees) and `swap`: the symbols the correlator's syncword 4 + phase (swap: phase) matches. The decoder inverts its hard decisions, so
+    bit 1 is -amp after rotate_soft(phase, swap); here the inverse of that rotation is applied: rotation by -phase, then the IQ swap."""
+    b = np.asarray(tx_bits, np.uint8).reshape(-1).astype(np.float64)
+    s = (1 - 2 * b) * amp
+    I, Q = s[0::2], s[1::2]
+    for _ in range((4 - phase) % 4):  # rotate_soft's PHASE_90 step: (I, Q) -> (Q, -I)
+        I, Q = Q, -I
+    if swap:
+        I, Q = Q, I
+    out = np.empty(2 * I.size)
+    out[0::2], out[1::2] = I, Q
+    if sigma:
+        out = out + np.random.default_rng(seed).normal(0, sigma, out.size)
+    return np.clip(np.round(out), -127, 127).astype(np.int8)
 
 
 # ---- CCSDS turbo code (CCSDS 131.0-B section 6), as ccsds_turbo_decoder receives it ---------------------------------------------------

@@ -276,9 +276,10 @@ static int decode_pass(Fec &f, const int8_t *src, long c, int nrange, long out_b
 }
 
 // Optimistic parallel decode of n consecutive decoder windows (chunks c .. c+n-1 of `src`, f.geom.chunk bytes apart) into chunk_bits[out_base ..]:
-// start-state speculation, one decode pass, and the redo rounds for chunks whose speculated start state was wrong. Leaves the per-chunk
-// records in f.h_rec[0 .. n).
-static void decode_range(Fec &f, const int8_t *src, long c, int n, long out_base)
+// start-state speculation, one decode pass, and up to `max_rounds` redo rounds for chunks whose speculated start state was wrong. Leaves
+// the per-chunk records in f.h_rec[0 .. n). Each round makes the first inconsistent chunk consistent (its predecessor is not redone), so
+// n rounds always settle the range.
+static void decode_range(Fec &f, const int8_t *src, long c, int n, long out_base, int max_rounds)
 {
     B200_CUDA(cudaMemcpyAsync(f.start_state.p, &f.main_next_start, sizeof(int), cudaMemcpyHostToDevice, f.stream));
     if (n > 1) {
@@ -292,7 +293,7 @@ static void decode_range(Fec &f, const int8_t *src, long c, int n, long out_base
     // Start states that were speculated wrong (k_vit_spec: common at low SNR, where 768 steps do not always pin the state): those
     // chunks alone are decoded again from the state their predecessor really left. A chunk's end state almost never depends on its
     // start state, so one round normally settles it; a round that changes a successor's start state is followed by another.
-    for (int round = 0; round < 6; round++) {
+    for (int round = 0; round < max_rounds; round++) {
         f.h_redo.clear();
         for (int i = 1; i < n; i++)
             if (f.h_rec[i].start_used != f.h_rec[i - 1].next_start) {
@@ -369,7 +370,7 @@ static void viterbi_segment(Fec &f, long c0, long nch, std::vector<OutChunk> &ou
             f.enc_state = f.idle_st.enc_state;
         }
         const int n = (int)(nch - c);
-        decode_range(f, f.softbuf.p, c, n, out_base);
+        decode_range(f, f.softbuf.p, c, n, out_base, 6); // (what is still inconsistent after six rounds is decoded again below)
         int accepted = 0;
         for (int i = 0; i < n; i++) {
             if (i > 0 && f.h_rec[i].start_used != f.h_rec[i - 1].next_start) {
@@ -466,7 +467,9 @@ static void punc_segment(Fec &f, long c0, long ncalls, std::vector<OutChunk> &ou
         f.geom.tail_real = f.tail_real.p;
         f.geom.ber_bits = VIT_TESTLEN;      // cc_encoder_ber.work(output, ...) encodes TEST_BITS_LENGTH bits (viterbi_punc.cpp:124)
         f.geom.ber_syms = f.test_bit_len;   // get_ber(vit_buffer, ..., test_bit_len, 5) (:125)
-        decode_range(f, reinterpret_cast<const int8_t *>(f.vitbuf.p), 0, nw, out_base);
+        // the lock machine below accepts windows call by call and has no way back to a window decoded from a wrong start state, so the
+        // redo rounds run until every window's start state is its predecessor's next start
+        decode_range(f, reinterpret_cast<const int8_t *>(f.vitbuf.p), 0, nw, out_base, nw);
         // replay the lock machine call by call
         int jacc = n, wacc = nw;
         for (int j = 1, wi = 0; j <= n; j++) {

@@ -1380,8 +1380,10 @@ static int rs_decode_block(const uint8_t *enc, int nroots, int fcr, uint8_t *msg
     return 0;
 }
 
-/* ReedSolomon::decode — common/codings/reedsolomon/reedsolomon.cpp:63-116 (fill_bytes <= 0 only: no shortening) */
-static int rs_decode_cw(uint8_t *data, int dual, int rs_type)
+/* ReedSolomon::decode — common/codings/reedsolomon/reedsolomon.cpp:63-116 (fill_bytes <= 0 only: no shortening). *odata0: the first
+ * byte of the decoder's message buffer, which the decoder overwrites with the corrected first message byte (conventional basis) when
+ * the word decodes and leaves alone when it does not (decode.c:337-339,361,375) */
+static int rs_decode_cw(uint8_t *data, int dual, int rs_type, uint8_t *odata0)
 {
     gf_init();
     int nroots = rs_type == 1 ? 16 : 32, fcr = rs_type == 1 ? 120 : 112, k = 255 - nroots;
@@ -1392,19 +1394,25 @@ static int rs_decode_cw(uint8_t *data, int dual, int rs_type)
         err = 0;
         for (int i = 0; i < k; i++) if (data[i] != msg[i]) err++;
         memcpy(data, msg, k); /* only the message bytes are replaced; parity stays as received */
+        *odata0 = msg[0];
     }
     if (dual) for (int i = 0; i < 255; i++) data[i] = to_dual[data[i]];
     return err;
 }
-/* ReedSolomon::decode_interlaved — reedsolomon.cpp:53-61,145-155 */
+/* ReedSolomon::decode_interlaved — reedsolomon.cpp:53-61,145-155. The (de)interleave loops run 255 - fill_bytes rows: with fill_bytes
+ * -1 (the decoder modules' default) that is 256, one row past the codewords. The extra byte of codeword b, data[255 * interleave + b],
+ * lands one past the 255-byte deinterleave buffer, in the first byte of the message buffer that follows it (reedsolomon.h:24-25), and is
+ * written back from there after the decode: the corrected first message byte when the word decodes, the byte as read when it does not.
+ * Callers keep `interleave` bytes of room behind the codewords. */
 void orc_rs_decode_interleaved(uint8_t *data, int dual, int interleave, int rs_type, int fill_bytes, int *errors)
 {
-    (void)fill_bytes;
     uint8_t cw[255];
     for (int b = 0; b < interleave; b++) {
         for (int i = 0; i < 255; i++) cw[i] = data[i * interleave + b];
-        errors[b] = rs_decode_cw(cw, dual, rs_type);
+        uint8_t odata0 = fill_bytes == -1 ? data[255 * interleave + b] : 0;
+        errors[b] = rs_decode_cw(cw, dual, rs_type, &odata0);
         for (int i = 0; i < 255; i++) data[i * interleave + b] = cw[i];
+        if (fill_bytes == -1) data[255 * interleave + b] = odata0;
     }
 }
 

@@ -376,10 +376,15 @@ def rs_encode_interleaved(data, dual=True, interleave=4, rs_type=0):
 
 
 def rs_decode_interleaved(data, dual=True, interleave=4, rs_type=0, fill_bytes=-1):
-    d = np.ascontiguousarray(data, np.uint8).copy()
+    # with fill_bytes -1 ReedSolomon's (de)interleave loops run 256 rows (255 - fill_bytes): the decoder reads and writes one byte per
+    # codeword past the 255 * interleave bytes, so the buffer gets that many spare bytes. They are dropped here: what comes back in them
+    # (the corrected first message byte of each word that decodes, the byte as it was for one that does not) is tested through Fec with
+    # CADUs longer than 4 + 255 * interleave
+    d = np.zeros(np.asarray(data).size + interleave, np.uint8)
+    d[:np.asarray(data).size] = np.ascontiguousarray(data, np.uint8).reshape(-1)
     err = np.zeros(interleave, np.int32)
     lib().ref_rs_decode_interleaved(_p(d), int(dual), interleave, rs_type, fill_bytes, _p(err))
-    return d, err
+    return d[:d.size - interleave].reshape(np.shape(data)), err
 
 
 def derand(data):

@@ -71,6 +71,8 @@ Fec::Fec(const b200_fec_cfg &c) : cfg(c)
         B200_REQUIRE(c.rs_i >= 0 && c.rs_i <= RS_MAX_I, B200_EINVAL, "rs_i out of range (0..%d)", RS_MAX_I);
         B200_REQUIRE(c.rs_i == 0 || c.cadu_size / 8 >= 4 + 255 * c.rs_i, B200_EINVAL, "cadu_size too small for rs_i interleaved codewords");
         B200_REQUIRE(c.rs_fill_bytes <= 0, B200_EINVAL, "rs_fill_bytes (shortened codes) is not built");
+        B200_REQUIRE(c.rs_fill_bytes >= -1, B200_EINVAL, "rs_fill_bytes must be -1 (none) or >= 0 (got %d)", c.rs_fill_bytes);
+        B200_REQUIRE(!c.derandomize || c.derand_start >= 0, B200_EINVAL, "derand_start must be >= 0 (got %d)", c.derand_start);
         if (cfg.asm_sync == 0)
             cfg.asm_sync = 0x1ACFFC1D;
     }
@@ -547,6 +549,7 @@ void Fec::deframe_and_rs(long new_bits)
         fc.rs_nroots = cfg.rs_type == 1 ? 16 : 32;
         fc.rs_fcr = cfg.rs_type == 1 ? 120 : 112;
         fc.sync = cfg.asm_sync;
+        fc.rs_row256 = cfg.rs_fill_bytes == -1;
         const bool filter = cfg.rs_usecheck && cfg.rs_i > 0;
         uint8_t *dst = filter ? frames_tmp.p : frames_out.p + out_frames * cadu_bytes;
         k_frames<<<std::min(nf, 132 * 8), 256, fr_smem, stream>>>(fifo.p, frames.p, nf, fc, tables.p, dst, rs_err.p);

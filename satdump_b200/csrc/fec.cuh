@@ -1223,6 +1223,7 @@ struct FrameCfg
     int derandomize, derand_after_rs, derand_start;
     int rs_i, rs_dual, rs_nroots, rs_fcr;
     uint32_t sync;
+    int rs_row256; // rs_fill_bytes -1: the reference's (de)interleave runs one row past the codewords (see rs_decode_interleave)
 };
 
 // (the Reed-Solomon device code up to k_frames is also used by the MetOp dump decoder's frame kernel, dump.cuh)
@@ -1375,6 +1376,13 @@ __device__ __forceinline__ int rs_decode_interleave(const RsTables &T, uint8_t *
             err = changed;
         }
     }
+    // With rs_fill_bytes -1 the reference's (de)interleave loops run 256 rows (reedsolomon.cpp:145-155): byte 4 + 255*I + warp is read
+    // into the slot one past its 255-byte codeword buffer, which is the first byte of its message buffer (reedsolomon.h:24-25), and is
+    // written back from there: the corrected first message byte (conventional basis) when the word decodes, unchanged when it does not.
+    // Here that byte is a spare byte of a CADU longer than 4 + 255*I; no other warp reads it. (When the CADU ends with the codewords the
+    // reference writes the next frame of its module call instead; that is not restated.)
+    const int spare = 4 + 255 * fc.rs_i + warp;
+    if (fc.rs_row256 && err >= 0 && spare < fc.cadu_bytes && lane == 0) frame[spare] = r[254];
     return err;
 }
 
@@ -1393,12 +1401,15 @@ __global__ void __launch_bounds__(256) k_frames(const uint32_t *__restrict__ fif
     for (int f = blockIdx.x; f < nframes; f += gridDim.x) {
         __syncthreads();
         const FrameRec fr = frames[f];
-        // reset_frame + write_bit: ASM forced clean, payload bits XOR inversion (bpsk_ccsds_deframer.cpp:109-122)
+        // reset_frame + write_bit: ASM forced clean, payload bits XOR inversion (bpsk_ccsds_deframer.cpp:109-122). The derandomiser runs
+        // from derand_start over the whole CADU, so with derand_start < 4 it also covers the (clean) ASM bytes
         const int pay_bytes = fc.cadu_bytes - 4;
         for (int i = t; i < fc.cadu_bytes; i += blockDim.x) {
             uint8_t b;
-            if (i < 4) b = (uint8_t)(fc.sync >> (24 - 8 * i));
-            else {
+            if (i < 4) {
+                b = (uint8_t)(fc.sync >> (24 - 8 * i));
+                if (fc.derandomize && !fc.derand_after_rs && i >= fc.derand_start) b ^= T.pn[(i - fc.derand_start) % 255];
+            } else {
                 const long bit0 = fr.pay_bit + 8L * (i - 4);
                 uint32_t wv = fifo_window(fifo, bit0);
                 b = (uint8_t)(wv >> 24);

@@ -108,11 +108,12 @@ def ccsds_pn(n):
     return np.resize(pn, n)
 
 
-def build_cadus(payload, interleave, dual=True, randomize=True):
-    """payload: (nframes, interleave*223) -> (nframes, 4 + interleave*255) CADUs and the clear (pre-randomiser) frames."""
-    nf = payload.shape[0]
-    msg = payload.reshape(nf, 223, interleave).transpose(0, 2, 1).reshape(nf * interleave, 223)
-    cw = rs_encode(msg, dual).reshape(nf, interleave, 255).transpose(0, 2, 1).reshape(nf, 255 * interleave)
+def build_cadus(payload, interleave, dual=True, randomize=True, nroots=32):
+    """payload: (nframes, interleave*(255-nroots)) -> (nframes, 4 + interleave*255) CADUs and the clear (pre-randomiser) frames.
+    nroots 32 = RS(255,223), 16 = RS(255,239)."""
+    nf, k = payload.shape[0], 255 - nroots
+    msg = payload.reshape(nf, k, interleave).transpose(0, 2, 1).reshape(nf * interleave, k)
+    cw = rs_encode(msg, dual, nroots).reshape(nf, interleave, 255).transpose(0, 2, 1).reshape(nf, 255 * interleave)
     clear = np.concatenate([np.tile(np.frombuffer(ASM, np.uint8), (nf, 1)), cw], axis=1)
     tx = clear.copy()
     if randomize:

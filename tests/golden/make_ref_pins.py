@@ -1,6 +1,6 @@
 """Regenerates tests/golden/ref_pins.json: digests of every reference array the CPU tests compare with (tests/refpin.py: the
-C restatement in tests/test_oracle.py, the synthetic transmitter's encoders, the demultiplexer model). Needs oracle/_ref; the cases
-run as tests, so they also check what they compare.
+C restatement in tests/test_oracle.py, the synthetic transmitter's encoders, the demultiplexer model, the frame stage models). Needs
+oracle/_ref; the cases run as tests, so they also check what they compare.
 
     python tests/golden/make_ref_pins.py
 """
@@ -10,7 +10,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
-TESTS = ["test_oracle.py", "test_synth.py", "test_demux_model.py"]
+TESTS = ["test_oracle.py", "test_synth.py", "test_demux_model.py", "test_rs_model.py"]
 
 
 def main():

@@ -53,6 +53,10 @@ def test_parameter_validation_mirrors_reference_modules(built):
         capi.Fec(capi.ccsds_cfg("8psk", 8192, 0.3, 20, 4))
     with pytest.raises(capi.B200Error):
         capi.Fec(capi.ccsds_cfg("qpsk", 8192, 0.3, 20, 5))  # 5 interleaved codewords do not fit 1024 bytes
+    for cfg in (capi.simple_cfg("bpsk", 8192, 4, derand_start=-1), capi.ccsds_cfg("qpsk", 8192, 0.3, 20, 4, derand_start=-4, derand_after_rs=True)):
+        with pytest.raises(capi.B200Error) as e:  # the derandomiser would start before the CADU
+            capi.Fec(cfg)
+        assert e.value.code == -1 and "derand_start" in str(e.value)
 
 
 def test_no_cpu_fallback(built):

@@ -168,12 +168,14 @@ def test_simple_psk_decoder_bit_exact(built, mode):
 
 
 def test_simple_psk_decoder_options(built):
-    """rs_i = 0 (no RS), RS(255,239), derandomize off / after RS, rs_usecheck, a non-default ASM, cadu_size 10232 with I=5."""
+    """rs_i = 0 (no RS), RS(255,239), derandomize off / after RS, rs_usecheck, a non-default ASM, cadu_size 10232 with I=5, and the
+    derandomiser from byte 0 (before RS: it covers the ASM too) and from byte 10 (after RS)."""
     from satdump_b200 import capi
     O = oracle()
     rng = np.random.default_rng(9)
     for kw in [dict(rs_i=0, derandomize=False), dict(rs_i=4, rs_type=1), dict(rs_i=4, derand_after_rs=True), dict(rs_i=4, rs_usecheck=True),
-               dict(rs_i=4, asm_sync=0xFAF3200D), dict(rs_i=5, cadu_size=10232)]:
+               dict(rs_i=4, asm_sync=0xFAF3200D), dict(rs_i=5, cadu_size=10232), dict(rs_i=4, derand_start=0),
+               dict(rs_i=4, derand_start=10, derand_after_rs=True)]:
         cadu_size = kw.pop("cadu_size", 8192)
         I = max(1, kw["rs_i"])
         pay = rng.integers(0, 256, size=(12, I * (239 if kw.get("rs_type") else 223)), dtype=np.uint8)

@@ -194,12 +194,14 @@ def test_primitives_vs_reference(built):
 
 
 def test_simple_psk_decoder_options_port_equals_reference(built):
-    """rs_i = 0, RS(255,239), derandomiser off / after RS, rs_usecheck, another ASM, 10232-bit CADUs with I = 5 — restatement vs reference."""
+    """rs_i = 0, RS(255,239), derandomiser off / after RS, rs_usecheck, another ASM, 10232-bit CADUs with I = 5, the derandomiser from byte 0
+    (over the ASM) and from byte 10 after RS — restatement vs reference."""
     from oracle import port
     pin = Pin("simple_psk_options")
     rng = np.random.default_rng(9)
     for kw in [dict(rs_i=0, derandomize=False), dict(rs_i=4, rs_type=1), dict(rs_i=4, derand_after_rs=True), dict(rs_i=4, rs_usecheck=True),
-               dict(rs_i=4, asm_sync=0xFAF3200D), dict(rs_i=5, cadu_size=10232), dict(rs_i=1, cadu_size=2072)]:
+               dict(rs_i=4, asm_sync=0xFAF3200D), dict(rs_i=5, cadu_size=10232), dict(rs_i=1, cadu_size=2072), dict(rs_i=4, derand_start=0),
+               dict(rs_i=4, derand_start=10, derand_after_rs=True)]:
         kw = dict(kw)
         cadu_size = kw.pop("cadu_size", 8192)
         body = rng.integers(0, 256, size=(12, cadu_size // 8 - 4), dtype=np.uint8)

@@ -476,8 +476,8 @@ Demod::Demod(const b200_demod_cfg &c) : cfg(c)
     }
     st.alloc(1);
     B200_CUDA(cudaMemcpyAsync(d_bank.p, bank.data(), 128 * 8 * sizeof(float), cudaMemcpyHostToDevice, stream));
-    B200_CUDA(cudaMallocHost((void **)&h_total, sizeof(long)));
-    B200_CUDA(cudaMallocHost((void **)&h_state, sizeof(DemodDevState)));
+    h_total.alloc(1);
+    h_state.alloc(1);
     init_state();
     bufA.zero(stream);
     bufB.zero(stream);
@@ -505,10 +505,6 @@ Demod::~Demod()
     for (auto &p : pf)
         if (p.done)
             cudaEventDestroy(p.done);
-    if (h_total)
-        cudaFreeHost(h_total);
-    if (h_state)
-        cudaFreeHost(h_state);
     if (stream)
         cudaStreamDestroy(stream);
 }
@@ -516,14 +512,14 @@ Demod::~Demod()
 // initial loop state, uploaded on the stream: AGC gain 1 (module_demod_base.cpp:207), Costas 0/0, M&M mu / omega (clock_recovery_mm.cpp:11)
 void Demod::init_state()
 {
-    memset(h_state, 0, sizeof(DemodDevState));
-    h_state->gain[0] = h_state->gain[1] = 1.0f;
-    h_state->gain2[0] = h_state->gain2[1] = 1.0f;
+    memset(h_state.p, 0, sizeof(DemodDevState));
+    h_state.p->gain[0] = h_state.p->gain[1] = 1.0f;
+    h_state.p->gain2[0] = h_state.p->gain2[1] = 1.0f;
     for (int i = 0; i < 2; i++) {
-        h_state->mm[i].mu = cfg.clock_mu;
-        h_state->mm[i].omega = sps;
+        h_state.p->mm[i].mu = cfg.clock_mu;
+        h_state.p->mm[i].omega = sps;
     }
-    B200_CUDA(cudaMemcpyAsync(st.p, h_state, sizeof(DemodDevState), cudaMemcpyHostToDevice, stream));
+    B200_CUDA(cudaMemcpyAsync(st.p, h_state.p, sizeof(DemodDevState), cudaMemcpyHostToDevice, stream));
 }
 
 void Demod::reset()
@@ -879,8 +875,8 @@ long Demod::process(const void *d_raw, long n, int8_t *soft_dst)
     // a caller-supplied soft destination (the fused chain) consumes the soft stream only: its demodulator's symbols are never pulled
     stage_mm(mmin, n, L, nseg, cur, nxt, soft_dst ? soft_dst : soft.p, false, soft_dst == nullptr);
     B200_CUDA(cudaEventRecord(ev[3], stream));
-    B200_CUDA(cudaMemcpyAsync(h_total, offs.p + nseg, sizeof(long), cudaMemcpyDeviceToHost, stream));
-    B200_CUDA(cudaMemcpyAsync(h_state, st.p, sizeof(DemodDevState), cudaMemcpyDeviceToHost, stream));
+    B200_CUDA(cudaMemcpyAsync(h_total.p, offs.p + nseg, sizeof(long), cudaMemcpyDeviceToHost, stream));
+    B200_CUDA(cudaMemcpyAsync(h_state.p, st.p, sizeof(DemodDevState), cudaMemcpyDeviceToHost, stream));
     B200_CUDA(cudaStreamSynchronize(stream));
     B200_CUDA(cudaGetLastError());
     cudaEventElapsedTime(&t_agcfir, ev[0], ev[1]);
@@ -888,12 +884,12 @@ long Demod::process(const void *d_raw, long n, int8_t *soft_dst)
     cudaEventElapsedTime(&t_mm, ev[2], ev[3]);
     parity = nxt;
     last_n = n;
-    last_syms = *h_total;
+    last_syms = *h_total.p;
     total_in += n_in;
     total_syms += last_syms;
     {
         // M2M4SNREstimator::snr (snr_estimator.cpp:41-47), float arithmetic as there
-        const float y1 = h_state->snr_y[nxt][0], y2 = h_state->snr_y[nxt][1];
+        const float y1 = h_state.p->snr_y[nxt][0], y2 = h_state.p->snr_y[nxt][1];
         const float y1_2 = y1 * y1;
         const float sig = (float)sqrt(2 * y1_2 - y2), noise = (float)(y1 - sqrt(2 * y1_2 - y2));
         snr_now = std::max<float>(0, (float)(10.0 * log10(sig / noise)));
@@ -902,9 +898,9 @@ long Demod::process(const void *d_raw, long n, int8_t *soft_dst)
         if (snr_now > snr_peak)
             snr_peak = snr_now;
     }
-    if (h_state->flags & 1)
+    if (h_state.p->flags & 1)
         agc_clamped_batches++; // the clamp pass produced this batch's front stage (silent input): information, not an error
-    if (h_state->flags & 2)
+    if (h_state.p->flags & 2)
         throw ApiError(B200_EUNSUPPORTED, "M&M produced more symbols per segment than the omega limit allows (slot overflow)");
     return last_syms;
 }
@@ -962,19 +958,19 @@ long Demod::debug_run_stage(int stage, const float *h_in, long n, int mode, floa
         last_L = L;
         last_nseg = nseg;
         stage_mm(mmin, n, L, nseg, 0, 1, soft.p, strict, true);
-        B200_CUDA(cudaMemcpyAsync(h_total, offs.p + nseg, sizeof(long), cudaMemcpyDeviceToHost, stream));
+        B200_CUDA(cudaMemcpyAsync(h_total.p, offs.p + nseg, sizeof(long), cudaMemcpyDeviceToHost, stream));
         B200_CUDA(cudaStreamSynchronize(stream));
-        count = *h_total;
+        count = *h_total.p;
         src = sym_out.p;
     }
     B200_REQUIRE(count <= cap, B200_ESTATE, "output buffer too small: need %ld complex values", count);
     B200_CUDA(cudaMemcpyAsync(h_out, src, count * sizeof(float2), cudaMemcpyDeviceToHost, stream));
-    B200_CUDA(cudaMemcpyAsync(h_state, S, sizeof(DemodDevState), cudaMemcpyDeviceToHost, stream));
+    B200_CUDA(cudaMemcpyAsync(h_state.p, S, sizeof(DemodDevState), cudaMemcpyDeviceToHost, stream));
     B200_CUDA(cudaStreamSynchronize(stream));
     B200_CUDA(cudaGetLastError());
-    dbg_costas_unconv = (stage == B200_STAGE_PLL || stage == B200_STAGE_PM) ? h_state->pll_unconv : h_state->costas_unconv;
-    dbg_mm_unconv = h_state->mm_unconv;
-    dbg_repairs = h_state->repairs;
+    dbg_costas_unconv = (stage == B200_STAGE_PLL || stage == B200_STAGE_PM) ? h_state.p->pll_unconv : h_state.p->costas_unconv;
+    dbg_mm_unconv = h_state.p->mm_unconv;
+    dbg_repairs = h_state.p->repairs;
     last_syms = stage == B200_STAGE_MM ? count : 0;
     reset();
     return count;
@@ -1032,24 +1028,24 @@ void Demod::stats(b200_demod_stats *o)
     memset(o, 0, sizeof(*o));
     o->samples_in = total_in;
     o->symbols_out = total_syms;
-    o->agc_gain = h_state->gain[parity];
-    o->costas_phase = h_state->costas[parity][0];
-    o->costas_freq = h_state->costas[parity][1];
-    o->mm_mu = h_state->mm[parity].mu;
-    o->mm_omega = h_state->mm[parity].omega;
-    o->costas_unconverged = h_state->costas_unconv;
-    o->mm_unconverged = h_state->mm_unconv;
+    o->agc_gain = h_state.p->gain[parity];
+    o->costas_phase = h_state.p->costas[parity][0];
+    o->costas_freq = h_state.p->costas[parity][1];
+    o->mm_mu = h_state.p->mm[parity].mu;
+    o->mm_omega = h_state.p->mm[parity].omega;
+    o->costas_unconverged = h_state.p->costas_unconv;
+    o->mm_unconverged = h_state.p->mm_unconv;
     o->agc_clamped = (int)std::min<long>(agc_clamped_batches, 0x7fffffff); // batches in which the gain hit max_gain so far
-    o->repairs = h_state->repairs;
+    o->repairs = h_state.p->repairs;
     for (int i = 0; i < MERGE_BUCKETS; i++)
-        o->repair_merge_hist[i] = h_state->merge_hist[i];
+        o->repair_merge_hist[i] = h_state.p->merge_hist[i];
     o->kernel_launches = launches;
-    o->agc_exact_passes = h_state->agc_exact;
+    o->agc_exact_passes = h_state.p->agc_exact;
     o->last_front_samples = last_front;
     o->snr = snr_now;
     o->peak_snr = snr_peak;
-    o->pll_freq = (pm || cfg.has_carrier) ? h_state->pll[parity][1] : 0.f;
-    o->pll_unconverged = (pm || cfg.has_carrier) ? h_state->pll_unconv : 0;
+    o->pll_freq = (pm || cfg.has_carrier) ? h_state.p->pll[parity][1] : 0.f;
+    o->pll_unconverged = (pm || cfg.has_carrier) ? h_state.p->pll_unconv : 0;
 }
 
 } // namespace b200

@@ -26,9 +26,9 @@ struct Demux
     DevBuf<PktRec> recs;
     DevBuf<DmxOut> orec;
     DevBuf<DmxCarry> st[2];
-    long *h_counts = nullptr; // pinned: packets, bytes
-    int *h_flags = nullptr;
-    unsigned long long *h_redo = nullptr;
+    PinnedBuf<long> h_counts; // packets, bytes
+    PinnedBuf<int> h_flags;
+    PinnedBuf<unsigned long long> h_redo;
     long redone_channels = 0; // channels walked again by one warp because a guess at a window boundary was wrong (so far)
     long last_packets = 0, last_bytes = 0, total_packets = 0, total_frames = 0, launches = 0;
 
@@ -70,9 +70,9 @@ struct Demux
             st[i].alloc(64);
             st[i].zero(stream);
         }
-        B200_CUDA(cudaMallocHost((void **)&h_counts, 2 * sizeof(long)));
-        B200_CUDA(cudaMallocHost((void **)&h_flags, sizeof(int)));
-        B200_CUDA(cudaMallocHost((void **)&h_redo, sizeof(unsigned long long)));
+        h_counts.alloc(2);
+        h_flags.alloc(1);
+        h_redo.alloc(1);
         B200_CUDA(cudaStreamSynchronize(stream));
     }
     ~Demux()
@@ -82,12 +82,6 @@ struct Demux
             cudaStreamSynchronize(stream);
             cudaStreamDestroy(stream);
         }
-        if (h_counts)
-            cudaFreeHost(h_counts);
-        if (h_flags)
-            cudaFreeHost(h_flags);
-        if (h_redo)
-            cudaFreeHost(h_redo);
     }
     void reset()
     {
@@ -116,31 +110,31 @@ struct Demux
         k_dmx_scan<<<1, 1024, 0, stream>>>(cnt.p, n, nullptr, base.p);
         k_dmx_frames<true><<<fb, 256, 0, stream>>>(d_frames, n, frame0, G, cfg.vcid_mask, nullptr, base.p, fxa.p, fxb.p, recs.p, cap_recs, flags.p);
         k_dmx_place<<<fb, 256, 0, stream>>>(wp.p, sums.p, fxa.p, fxb.p, n, base.p, recs.p, cap_recs, flags.p);
-        B200_CUDA(cudaMemcpyAsync(h_redo, redo_mask.p, sizeof(unsigned long long), cudaMemcpyDeviceToHost, stream));
-        B200_CUDA(cudaMemcpyAsync(&h_counts[0], base.p + n, sizeof(long), cudaMemcpyDeviceToHost, stream));
-        B200_CUDA(cudaMemcpyAsync(h_flags, flags.p, sizeof(int), cudaMemcpyDeviceToHost, stream));
+        B200_CUDA(cudaMemcpyAsync(h_redo.p, redo_mask.p, sizeof(unsigned long long), cudaMemcpyDeviceToHost, stream));
+        B200_CUDA(cudaMemcpyAsync(&h_counts.p[0], base.p + n, sizeof(long), cudaMemcpyDeviceToHost, stream));
+        B200_CUDA(cudaMemcpyAsync(h_flags.p, flags.p, sizeof(int), cudaMemcpyDeviceToHost, stream));
         B200_CUDA(cudaStreamSynchronize(stream));
-        B200_REQUIRE(!(*h_flags & 1) && h_counts[0] <= cap_recs, B200_ESTATE, "packet table too small: %ld packets in this batch, room for %ld (max_packets)",
-                     h_counts[0], cap_recs);
-        const long P = h_counts[0];
+        B200_REQUIRE(!(*h_flags.p & 1) && h_counts.p[0] <= cap_recs, B200_ESTATE, "packet table too small: %ld packets in this batch, room for %ld (max_packets)",
+                     h_counts.p[0], cap_recs);
+        const long P = h_counts.p[0];
         k_dmx_sizes<<<(unsigned)std::min<long>(1024, (P + 255) / 256 + 1), 256, 0, stream>>>(recs.p, base.p + n, sizes.p);
         k_dmx_scan<<<1, 1024, 0, stream>>>(sizes.p, P, nullptr, offs.p);
         k_dmx_copy<<<(unsigned)std::min<long>(132 * 16, (P + 7) / 8 + 1), 256, 0, stream>>>(recs.p, base.p + n, offs.p, segs.p, d_frames, G, carry[cur].p, carry_cap, out.p,
                                                                                              cap_bytes, orec.p, flags.p);
         k_dmx_carry<<<64, 256, 0, stream>>>(tailseg.p, segs.p, d_frames, G, carry[cur].p, carry[nxt].p, carry_cap, flags.p);
-        B200_CUDA(cudaMemcpyAsync(&h_counts[1], offs.p + P, sizeof(long), cudaMemcpyDeviceToHost, stream));
-        B200_CUDA(cudaMemcpyAsync(h_flags, flags.p, sizeof(int), cudaMemcpyDeviceToHost, stream));
+        B200_CUDA(cudaMemcpyAsync(&h_counts.p[1], offs.p + P, sizeof(long), cudaMemcpyDeviceToHost, stream));
+        B200_CUDA(cudaMemcpyAsync(h_flags.p, flags.p, sizeof(int), cudaMemcpyDeviceToHost, stream));
         B200_CUDA(cudaStreamSynchronize(stream));
         B200_CUDA(cudaGetLastError());
         launches += 12;
-        if (*h_redo)
-            redone_channels += __builtin_popcountll(*h_redo);
-        B200_REQUIRE(!(*h_flags & 2), B200_ESTATE, "internal: packet byte buffer too small");
-        B200_REQUIRE(!(*h_flags & 4), B200_EUNSUPPORTED, "a packet under construction grew beyond %d bytes (inconsistent frames)", carry_cap);
+        if (*h_redo.p)
+            redone_channels += __builtin_popcountll(*h_redo.p);
+        B200_REQUIRE(!(*h_flags.p & 2), B200_ESTATE, "internal: packet byte buffer too small");
+        B200_REQUIRE(!(*h_flags.p & 4), B200_EUNSUPPORTED, "a packet under construction grew beyond %d bytes (inconsistent frames)", carry_cap);
         parity = nxt;
         frame0 += n;
         last_packets = P;
-        last_bytes = h_counts[1];
+        last_bytes = h_counts.p[1];
         total_packets += P;
         total_frames += n;
     }

@@ -7,6 +7,15 @@
 namespace b200
 {
 
+// one step of the CCSDS randomiser (LFSR h(x) = x^8+x^7+x^5+x^3+1): the bit it outputs
+static int pn_step(uint8_t &reg)
+{
+    const int out = reg >> 7;
+    const uint8_t nb = ((reg >> 7) ^ (reg >> 4) ^ (reg >> 2) ^ reg) & 1;
+    reg = (uint8_t)((reg << 1) | nb);
+    return out;
+}
+
 // GF(256) tables exactly as libcorrect builds them (libs/correct/reed-solomon/field.h:26-62: log[1] ends up 255, log[0] = 0),
 // CCSDS dual-basis maps (GF(2)-linear, generated from the images of the unit vectors) and the CCSDS randomiser bytes
 // (LFSR h(x) = x^8+x^7+x^5+x^3+1 from all ones).
@@ -37,13 +46,17 @@ void build_rs_tables(RsTables &T)
     uint8_t reg = 0xFF;
     for (int i = 0; i < 255; i++) {
         uint8_t byte = 0;
-        for (int k = 0; k < 8; k++) {
-            byte = (uint8_t)((byte << 1) | (reg >> 7));
-            uint8_t nb = ((reg >> 7) ^ (reg >> 4) ^ (reg >> 2) ^ reg) & 1;
-            reg = (uint8_t)((reg << 1) | nb);
-        }
+        for (int k = 0; k < 8; k++)
+            byte = (uint8_t)((byte << 1) | pn_step(reg));
         T.pn[i] = byte;
     }
+}
+
+void ccsds_pn_bits(unsigned char *pn)
+{
+    uint8_t reg = 0xFF;
+    for (int i = 0; i < 255; i++)
+        pn[i] = (unsigned char)pn_step(reg);
 }
 
 Fec::Fec(const b200_fec_cfg &c) : cfg(c)
@@ -53,18 +66,14 @@ Fec::Fec(const b200_fec_cfg &c) : cfg(c)
                  B200_EINVAL, "unknown decoder kind %d", c.kind);
     B200_REQUIRE(c.max_soft >= 65536, B200_EINVAL, "max_soft must be >= 65536");
     memset(&geom, 0, sizeof(geom));
-    if (c.kind == B200_FEC_LDPC) {
-        ldpc_init();
+    if (c.kind == B200_FEC_LDPC)
+        framed = ldpc_decoder(*this);
+    else if (c.kind == B200_FEC_TURBO)
+        framed = turbo_decoder(*this);
+    else if (c.kind == B200_FEC_METOP_DUMP)
+        framed = dump_decoder(*this);
+    if (framed)
         return;
-    }
-    if (c.kind == B200_FEC_TURBO) {
-        turbo_init();
-        return;
-    }
-    if (c.kind == B200_FEC_METOP_DUMP) {
-        dump_init();
-        return;
-    }
     if (c.kind != B200_FEC_METOP) {
         B200_REQUIRE(c.cadu_size >= 64 && c.cadu_size <= 65536, B200_EINVAL, "cadu_size out of range");
         B200_REQUIRE(c.cadu_size % 8 == 0, B200_EINVAL, "cadu_size must be a multiple of 8 (frame padding is not built)");
@@ -151,7 +160,7 @@ Fec::Fec(const b200_fec_cfg &c) : cfg(c)
         bdep.alloc(4 * VIT_TESTLEN);
         tail_real.alloc(max_chunks + 2);
         punc_out.alloc(1);
-        B200_CUDA(cudaMallocHost((void **)&h_punc, sizeof(PuncIdleOut)));
+        h_punc.alloc(1);
     }
     softbuf.alloc((size_t)c.max_soft + 2 * geom.chunk);
     const bool simple = cfg.kind == B200_FEC_SIMPLE;
@@ -169,7 +178,7 @@ Fec::Fec(const b200_fec_cfg &c) : cfg(c)
     tb_list.alloc((size_t)max_chunks + 2); // chunks whose parallel chainback blocks disagreed at an edge (any number: low SNR makes them common)
     idle_out.alloc(1);
     idle2_out.alloc(1);
-    B200_CUDA(cudaMallocHost((void **)&h_idle2, sizeof(VitIdle2Out)));
+    h_idle2.alloc(1);
     B200_CUDA(cudaFuncSetAttribute(k_vit_idle2, cudaFuncAttributeMaxDynamicSharedMemorySize, 8 * VIT_IDLE_WARP_BYTES));
     dstate.alloc(2);
     devents.alloc(4096);
@@ -187,12 +196,12 @@ Fec::Fec(const b200_fec_cfg &c) : cfg(c)
     frame_dst.alloc((size_t)max_frames_push + 4);
     counters.alloc(8);
     tables.alloc(1);
-    B200_CUDA(cudaMallocHost((void **)&h_rec, sizeof(VitRec) * (max_chunks + 1)));
-    B200_CUDA(cudaMallocHost((void **)&h_idle, sizeof(VitIdleOut)));
-    B200_CUDA(cudaMallocHost((void **)&h_counters, sizeof(int) * 8));
-    B200_CUDA(cudaMallocHost((void **)&h_dstate, sizeof(DefrState) * 2));
-    B200_CUDA(cudaMallocHost((void **)&h_events, sizeof(DefrEvent) * 4096));
-    B200_CUDA(cudaMallocHost((void **)&h_rs_err, sizeof(int) * (max_frames_push + 4) * std::max(1, cfg.rs_i)));
+    h_rec.alloc(max_chunks + 1);
+    h_idle.alloc(1);
+    h_counters.alloc(8);
+    h_dstate.alloc(2);
+    h_events.alloc(4096);
+    h_rs_err.alloc((size_t)(max_frames_push + 4) * std::max(1, cfg.rs_i));
     RsTables T;
     build_rs_tables(T);
     B200_CUDA(cudaMemcpyAsync(tables.p, &T, sizeof(T), cudaMemcpyHostToDevice, stream));
@@ -208,18 +217,13 @@ Fec::~Fec()
     DeviceGuard g(cfg.device);
     if (stream)
         cudaStreamSynchronize(stream);
-    ldpc_free();
-    turbo_free();
-    dump_free();
+    framed.reset();
     for (auto &e : ev)
         cudaEventDestroy(e);
     for (auto &e : evm)
         cudaEventDestroy(e);
     for (auto &e : evf)
         cudaEventDestroy(e);
-    for (void *p : {(void *)h_idle2, (void *)h_rec, (void *)h_idle, (void *)h_counters, (void *)h_dstate, (void *)h_events, (void *)h_rs_err, (void *)h_punc})
-        if (p)
-            cudaFreeHost(p);
     if (stream)
         cudaStreamDestroy(stream);
 }
@@ -266,7 +270,7 @@ static int decode_pass(Fec &f, const int8_t *src, long c, int nrange, long out_b
     k_vit_tb_serial<<<(n + 127) / 128, 128, 0, f.stream>>>(f.tb_list.p, nrange, f.geom, f.dec.p, f.chunk_bits.p, out_base, f.rec.p); // (threads beyond the list return at once)
     k_vit_ber<<<(nber + WPB - 1) / WPB, 32 * WPB, 0, f.stream>>>(src, c, nber, f.geom, f.hyp, f.chunk_bits.p, out_base, f.enc_state, f.rec.p, ber_list);
     f.launches += 5;
-    B200_CUDA(cudaMemcpyAsync(f.h_rec, f.rec.p, sizeof(VitRec) * nrange, cudaMemcpyDeviceToHost, f.stream));
+    B200_CUDA(cudaMemcpyAsync(f.h_rec.p, f.rec.p, sizeof(VitRec) * nrange, cudaMemcpyDeviceToHost, f.stream));
     int tb_redone = 0;
     B200_CUDA(cudaMemcpyAsync(&tb_redone, f.tb_list.p, sizeof(int), cudaMemcpyDeviceToHost, f.stream));
     B200_CUDA(cudaStreamSynchronize(f.stream));
@@ -298,9 +302,9 @@ static void decode_range(Fec &f, const int8_t *src, long c, int n, long out_base
     for (int round = 0; round < max_rounds; round++) {
         f.h_redo.clear();
         for (int i = 1; i < n; i++)
-            if (f.h_rec[i].start_used != f.h_rec[i - 1].next_start) {
+            if (f.h_rec.p[i].start_used != f.h_rec.p[i - 1].next_start) {
                 f.h_redo.push_back(i);
-                f.h_start[i] = f.h_rec[i - 1].next_start;
+                f.h_start[i] = f.h_rec.p[i - 1].next_start;
             }
         if (round == 0 && n > 64) // wrong guesses: the survivors of the speculation window had not all merged (low SNR)
             adapt_window(f.spec_steps, f.spec_clean, (double)f.h_redo.size() / (double)n, f.geom.rate34 ? VIT_SPEC_STEPS_34 : VIT_SPEC_STEPS_12,
@@ -343,31 +347,31 @@ static void viterbi_segment(Fec &f, long c0, long nch, std::vector<OutChunk> &ou
                 k_vit_idle2<<<1, 32 * nh, nh * VIT_IDLE_WARP_BYTES, f.stream>>>(f.softbuf.p, c, (int)(nch - c), f.geom, f.nswap, f.nphases, f.ph0, f.ph1,
                                                                                f.cfg.ber_thresold, f.idle_st, f.idle2_out.p);
                 f.launches++;
-                B200_CUDA(cudaMemcpyAsync(f.h_idle2, f.idle2_out.p, sizeof(VitIdle2Out), cudaMemcpyDeviceToHost, f.stream));
+                B200_CUDA(cudaMemcpyAsync(f.h_idle2.p, f.idle2_out.p, sizeof(VitIdle2Out), cudaMemcpyDeviceToHost, f.stream));
                 B200_CUDA(cudaStreamSynchronize(f.stream));
-                *f.h_idle = f.h_idle2->o;
-                if (f.h_idle2->fallback_chunk >= 0) {
-                    const long c2 = c + f.h_idle2->fallback_chunk;
+                *f.h_idle.p = f.h_idle2.p->o;
+                if (f.h_idle2.p->fallback_chunk >= 0) {
+                    const long c2 = c + f.h_idle2.p->fallback_chunk;
                     k_vit_idle<<<1, 32, 0, f.stream>>>(f.softbuf.p, c2, (int)(nch - c2), f.geom, f.nswap, f.nphases, f.ph0, f.ph1, f.cfg.ber_thresold,
-                                                      f.h_idle2->o.st, f.idle_dec.p, f.idle_out.p);
+                                                      f.h_idle2.p->o.st, f.idle_dec.p, f.idle_out.p);
                     f.launches++;
-                    B200_CUDA(cudaMemcpyAsync(f.h_idle, f.idle_out.p, sizeof(VitIdleOut), cudaMemcpyDeviceToHost, f.stream));
+                    B200_CUDA(cudaMemcpyAsync(f.h_idle.p, f.idle_out.p, sizeof(VitIdleOut), cudaMemcpyDeviceToHost, f.stream));
                     B200_CUDA(cudaStreamSynchronize(f.stream));
-                    if (f.h_idle->lock_chunk >= 0)
-                        f.h_idle->lock_chunk += (int)(c2 - c);
+                    if (f.h_idle.p->lock_chunk >= 0)
+                        f.h_idle.p->lock_chunk += (int)(c2 - c);
                 }
             }
-            f.idle_st = f.h_idle->st;
+            f.idle_st = f.h_idle.p->st;
             f.enc_state = f.idle_st.enc_state;
             float bb = 10.f;
             for (int i = 0; i < 16; i++)
-                bb = std::min(bb, f.h_idle->bers[i]);
+                bb = std::min(bb, f.h_idle.p->bers[i]);
             f.last_ber = bb;
-            if (f.h_idle->lock_chunk < 0)
+            if (f.h_idle.p->lock_chunk < 0)
                 break;
-            c += f.h_idle->lock_chunk;
+            c += f.h_idle.p->lock_chunk;
             f.vit_state = 1;
-            f.hyp = VitHyp{f.h_idle->swap, f.h_idle->phase, f.h_idle->shift};
+            f.hyp = VitHyp{f.h_idle.p->swap, f.h_idle.p->phase, f.h_idle.p->shift};
             f.invalid = 0;
             f.enc_state = f.idle_st.enc_state;
         }
@@ -375,12 +379,12 @@ static void viterbi_segment(Fec &f, long c0, long nch, std::vector<OutChunk> &ou
         decode_range(f, f.softbuf.p, c, n, out_base, 6); // (what is still inconsistent after six rounds is decoded again below)
         int accepted = 0;
         for (int i = 0; i < n; i++) {
-            if (i > 0 && f.h_rec[i].start_used != f.h_rec[i - 1].next_start) {
+            if (i > 0 && f.h_rec.p[i].start_used != f.h_rec.p[i - 1].next_start) {
                 f.replays++; // still inconsistent after the redo rounds above: decode again from here with the true state
                 break;
             }
             accepted = i + 1;
-            const float ber = ((float)f.h_rec[i].ber_errors / (float)f.h_rec[i].ber_total) * kber;
+            const float ber = ((float)f.h_rec.p[i].ber_errors / (float)f.h_rec.p[i].ber_total) * kber;
             f.last_ber = ber;
             bool lost = false;
             if (ber > f.cfg.ber_thresold) { // viterbi_3_4.cpp:160-169
@@ -391,12 +395,12 @@ static void viterbi_segment(Fec &f, long c0, long nch, std::vector<OutChunk> &ou
                 }
             } else
                 f.invalid = 0;
-            outs.push_back(OutChunk{c + i, f.h_rec[i].next_start, f.h_rec[i].enc_tail, f.invalid, f.vit_state, f.idle_st});
+            outs.push_back(OutChunk{c + i, f.h_rec.p[i].next_start, f.h_rec.p[i].enc_tail, f.invalid, f.vit_state, f.idle_st});
             if (lost)
                 break;
         }
-        f.main_next_start = f.h_rec[accepted - 1].next_start;
-        f.enc_state = f.h_rec[accepted - 1].enc_tail;
+        f.main_next_start = f.h_rec.p[accepted - 1].next_start;
+        f.enc_state = f.h_rec.p[accepted - 1].enc_tail;
         out_base += accepted;
         c += accepted;
     }
@@ -423,9 +427,9 @@ static void punc_segment(Fec &f, long c0, long ncalls, std::vector<OutChunk> &ou
             k_punc_idle<<<1, 32, 0, f.stream>>>(f.softbuf.p, c, (int)(ncalls - c), size, P, f.nswap, f.nphases, f.ph0, f.ph1, f.cfg.ber_thresold, st, f.bdep.p,
                                                 f.idle_dec.p, f.punc_out.p);
             f.launches++;
-            B200_CUDA(cudaMemcpyAsync(f.h_punc, f.punc_out.p, sizeof(PuncIdleOut), cudaMemcpyDeviceToHost, f.stream));
+            B200_CUDA(cudaMemcpyAsync(f.h_punc.p, f.punc_out.p, sizeof(PuncIdleOut), cudaMemcpyDeviceToHost, f.stream));
             B200_CUDA(cudaStreamSynchronize(f.stream));
-            const PuncIdleOut &o = *f.h_punc;
+            const PuncIdleOut &o = *f.h_punc.p;
             f.pdec_start = o.st.dec_start;
             f.enc_state = o.st.enc_state;
             f.test_bit_len = o.test_bit_len;
@@ -479,7 +483,7 @@ static void punc_segment(Fec &f, long c0, long ncalls, std::vector<OutChunk> &ou
             while (wi < nw && f.h_wcall[wi] == j)
                 last = wi++;
             if (last >= 0)
-                f.last_ber = ((float)f.h_rec[last].ber_errors / (float)f.h_rec[last].ber_total) * 5.0f;
+                f.last_ber = ((float)f.h_rec.p[last].ber_errors / (float)f.h_rec.p[last].ber_total) * 5.0f;
             if (f.last_ber > f.cfg.ber_thresold) { // viterbi_punc.cpp:133-141
                 f.invalid++;
                 if (f.invalid > f.cfg.outsync_after) {
@@ -492,10 +496,10 @@ static void punc_segment(Fec &f, long c0, long ncalls, std::vector<OutChunk> &ou
                 f.invalid = 0;
         }
         for (int i = 0; i < wacc; i++)
-            outs.push_back(OutChunk{c + f.h_wcall[i] - 1, f.h_rec[i].next_start, f.h_rec[i].enc_tail, f.invalid, f.vit_state, f.idle_st});
+            outs.push_back(OutChunk{c + f.h_wcall[i] - 1, f.h_rec.p[i].next_start, f.h_rec.p[i].enc_tail, f.invalid, f.vit_state, f.idle_st});
         if (wacc > 0) {
-            f.main_next_start = f.h_rec[wacc - 1].next_start;
-            f.enc_state = f.h_rec[wacc - 1].enc_tail;
+            f.main_next_start = f.h_rec.p[wacc - 1].next_start;
+            f.enc_state = f.h_rec.p[wacc - 1].enc_tail;
         }
         // what stays in the sliding buffer: the symbols behind the decoded windows up to the last accepted call's total, plus the one
         // that call held back (its value is DepuncXX::buf from now on)
@@ -528,14 +532,14 @@ void Fec::deframe_and_rs(long new_bits)
     k_deframe<<<1, 32, 0, stream>>>(fifo.p, nbits, cfg.cadu_size, st_synced, cfg.asm_sync, dstate.p, frames.p, (int)max_frames_push,
                                    reinterpret_cast<DefrEventDev *>(devents.p), 4096, counters.p);
     launches++;
-    B200_CUDA(cudaMemcpyAsync(h_counters, counters.p, sizeof(int) * 2, cudaMemcpyDeviceToHost, stream));
-    B200_CUDA(cudaMemcpyAsync(h_dstate, dstate.p, sizeof(DefrState), cudaMemcpyDeviceToHost, stream));
-    B200_CUDA(cudaMemcpyAsync(h_events, devents.p, sizeof(DefrEvent) * 4096, cudaMemcpyDeviceToHost, stream));
+    B200_CUDA(cudaMemcpyAsync(h_counters.p, counters.p, sizeof(int) * 2, cudaMemcpyDeviceToHost, stream));
+    B200_CUDA(cudaMemcpyAsync(h_dstate.p, dstate.p, sizeof(DefrState), cudaMemcpyDeviceToHost, stream));
+    B200_CUDA(cudaMemcpyAsync(h_events.p, devents.p, sizeof(DefrEvent) * 4096, cudaMemcpyDeviceToHost, stream));
     B200_CUDA(cudaStreamSynchronize(stream));
-    const int nf = h_counters[0];
+    const int nf = h_counters.p[0];
     last_nf = nf;
     B200_REQUIRE(nf <= max_frames_push, B200_ESTATE, "internal: frame list overflow");
-    B200_REQUIRE(h_counters[1] <= 4096, B200_EUNSUPPORTED, "deframer changed state more than 4096 times in one push (noise input?): push smaller batches");
+    B200_REQUIRE(h_counters.p[1] <= 4096, B200_EUNSUPPORTED, "deframer changed state more than 4096 times in one push (noise input?): push smaller batches");
     if (nf > 0) {
         B200_REQUIRE((size_t)(out_frames + nf) * cadu_bytes <= frames_out.n, B200_ESTATE, "frame output buffer full: call pull_frames");
         FrameCfg fc;
@@ -559,18 +563,18 @@ void Fec::deframe_and_rs(long new_bits)
             k_frames_filter<<<1, 1024, 0, stream>>>(rs_err.p, nf, cfg.rs_i, frame_dst.p, counters.p + 2);
             k_frames_gather<<<std::min(nf, 132 * 16), 256, 0, stream>>>(frames_tmp.p, frame_dst.p, nf, cadu_bytes, frames_out.p + out_frames * cadu_bytes);
             launches += 2;
-            B200_CUDA(cudaMemcpyAsync(h_counters + 2, counters.p + 2, sizeof(int), cudaMemcpyDeviceToHost, stream));
+            B200_CUDA(cudaMemcpyAsync(h_counters.p + 2, counters.p + 2, sizeof(int), cudaMemcpyDeviceToHost, stream));
         }
         if (cfg.rs_i > 0)
-            B200_CUDA(cudaMemcpyAsync(h_rs_err, rs_err.p, sizeof(int) * nf * cfg.rs_i, cudaMemcpyDeviceToHost, stream));
+            B200_CUDA(cudaMemcpyAsync(h_rs_err.p, rs_err.p, sizeof(int) * nf * cfg.rs_i, cudaMemcpyDeviceToHost, stream));
         B200_CUDA(cudaStreamSynchronize(stream));
         if (filter)
-            kept = h_counters[2];
+            kept = h_counters.p[2];
         for (long i = 0; i < (long)nf * cfg.rs_i; i++) {
-            if (h_rs_err[i] < 0)
+            if (h_rs_err.p[i] < 0)
                 rs_failed++;
             else
-                rs_corrected += h_rs_err[i];
+                rs_corrected += h_rs_err.p[i];
         }
         out_frames += kept;
         total_frames += kept;
@@ -583,7 +587,7 @@ void Fec::deframe_and_rs(long new_bits)
         t_frames += ms;
     }
     fifo_bits = nbits;
-    defr_state_now = h_dstate->state;
+    defr_state_now = h_dstate.p->state;
 }
 
 // The state a new stream starts from: the lock machines, the punctured decoder's sliding buffer and the deframers (the FIFO starts
@@ -606,21 +610,108 @@ void Fec::start_stream(size_t fifo_bytes)
     out_frames = 0;
     last_bits0 = last_nbits = 0;
     B200_CUDA(cudaMemsetAsync(fifo.p, 0, fifo_bytes, stream));
-    h_dstate[0].state = 2;
-    h_dstate[0].inversion = h_dstate[0].good = h_dstate[0].bad = 0;
-    h_dstate[0].pos = 32;
-    h_dstate[0].frame_pay = -1;
-    B200_CUDA(cudaMemcpyAsync(dstate.p, h_dstate, sizeof(DefrState), cudaMemcpyHostToDevice, stream));
+    h_dstate.p[0].state = 2;
+    h_dstate.p[0].inversion = h_dstate.p[0].good = h_dstate.p[0].bad = 0;
+    h_dstate.p[0].pos = 32;
+    h_dstate.p[0].frame_pay = -1;
+    B200_CUDA(cudaMemcpyAsync(dstate.p, h_dstate.p, sizeof(DefrState), cudaMemcpyHostToDevice, stream));
     if (cfg.kind == B200_FEC_SIMPLE) {
-        h_dstate2 = h_dstate[0];
+        h_dstate2 = h_dstate.p[0];
         fifo_bits2 = 32;
         defr_state2 = 2;
         slice_par = 0;
         total_chunks = 0; // the hard-decision stage knows the stream's very first chunk by this count
         B200_CUDA(cudaMemsetAsync(fifo2.p, 0, fifo_bytes, stream));
         slice_carry.zero(stream);
-        B200_CUDA(cudaMemcpyAsync(dstate2.p, h_dstate, sizeof(DefrState), cudaMemcpyHostToDevice, stream));
+        B200_CUDA(cudaMemcpyAsync(dstate2.p, h_dstate.p, sizeof(DefrState), cudaMemcpyHostToDevice, stream));
     }
+}
+
+// The set-up of the decoder object that every Framed decoder shares: the stream and events, the soft FIFO of max_soft + 2F bytes, the
+// scratch of keep_soft_tail and the CADU output for `frames_per_push` frames a push (0: the deframer stage sizes it, deframer_storage).
+void Fec::framed_storage(int F, long frames_per_push)
+{
+    B200_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
+    for (cudaEvent_t *e : {&ev[0], &ev[1], &evm[0], &evm[1], &evf[0], &evf[1]}) // (the destructor destroys all six)
+        B200_CUDA(cudaEventCreate(e));
+    softbuf.alloc((size_t)cfg.max_soft + 2L * F);
+    dec.alloc((size_t)(2 * F) / sizeof(uint2) + 16);
+    if (frames_per_push > 0) {
+        max_frames_push = frames_per_push;
+        frames_out.alloc((size_t)(2 * frames_per_push + 4) * cadu_bytes);
+    }
+}
+
+void Framed::alloc(long positions, long frames_cap)
+{
+    score.alloc((size_t)positions);
+    bsync.alloc((size_t)positions);
+    bval.alloc((size_t)positions / 32 + 2);
+    bidx.alloc((size_t)positions / 32 + 2);
+    max_frames = frames_cap;
+    frames.alloc((size_t)max_frames);
+    walk.alloc(1);
+    h_walk.alloc(1);
+    h_frames.alloc((size_t)max_frames);
+}
+
+void Framed::reset(Fec &f)
+{
+    f.soft_have = 0;
+    f.out_frames = 0;
+    tail_seen = -1;
+    base_off = 0;
+    last_nf = 0;
+    lock = 0;
+    cor = 0.f;
+}
+
+void Framed::stats(b200_fec_stats *o)
+{
+    o->correlator_lock = lock;
+    o->correlator_corr = cor;
+    o->ldpc_resyncs = resyncs;
+}
+
+// A push's records, timings and debug bits start empty, unless it brought no new bytes (then it changes nothing).
+bool Framed::begin(Fec &f, int F)
+{
+    if (f.soft_have == tail_seen)
+        return false;
+    last_nf = 0;
+    for (float &t : t_ms)
+        t = 0;
+    f.last_bits0 = f.last_nbits = 0;
+    f.t_frames = 0;
+    if (f.soft_have < F) {
+        tail_seen = f.soft_have;
+        return false;
+    }
+    return true;
+}
+
+int Framed::walked(cudaStream_t stream)
+{
+    B200_CUDA(cudaMemcpyAsync(h_walk.p, walk.p, sizeof(WalkOut), cudaMemcpyDeviceToHost, stream));
+    B200_CUDA(cudaStreamSynchronize(stream));
+    return h_walk.p->nf;
+}
+
+// after keep_soft_tail: `soft_have` is what the FIFO keeps
+void Framed::finish(int nf, long soft_have)
+{
+    for (int k = 0; k < nf; k++) {
+        WalkFrame &r = h_frames.p[k];
+        r.off += base_off;
+        resyncs += r.pos != 0;
+    }
+    if (nf > 0) {
+        lock = h_frames.p[nf - 1].pos == 0;
+        cor = h_frames.p[nf - 1].cor;
+    }
+    last_nf = nf;
+    base_off += h_walk.p->next;
+    tail_seen = soft_have;
 }
 
 // The deframer and frame stage behind another decoder (ccsds_ldpc_decoder's internal_stream): storage for `max_new_bits` new bits per
@@ -638,10 +729,10 @@ void Fec::deframer_storage(long max_new_bits)
     frame_dst.alloc((size_t)max_frames_push + 4);
     counters.alloc(8);
     tables.alloc(1);
-    B200_CUDA(cudaMallocHost((void **)&h_counters, sizeof(int) * 8));
-    B200_CUDA(cudaMallocHost((void **)&h_dstate, sizeof(DefrState) * 2));
-    B200_CUDA(cudaMallocHost((void **)&h_events, sizeof(DefrEvent) * 4096));
-    B200_CUDA(cudaMallocHost((void **)&h_rs_err, sizeof(int) * (max_frames_push + 4)));
+    h_counters.alloc(8);
+    h_dstate.alloc(2);
+    h_events.alloc(4096);
+    h_rs_err.alloc(max_frames_push + 4);
     RsTables T;
     build_rs_tables(T);
     B200_CUDA(cudaMemcpyAsync(tables.p, &T, sizeof(T), cudaMemcpyHostToDevice, stream));
@@ -656,16 +747,8 @@ void Fec::reset()
 {
     DeviceGuard g(cfg.device);
     B200_CUDA(cudaStreamSynchronize(stream));
-    if (ldpc) {
-        ldpc_reset();
-        return;
-    }
-    if (turbo) {
-        turbo_reset();
-        return;
-    }
-    if (dump) {
-        dump_reset();
+    if (framed) {
+        framed->reset(*this);
         return;
     }
     start_stream(64);
@@ -678,7 +761,7 @@ void Fec::swap_unit()
     std::swap(fifo.n, fifo2.n);
     std::swap(dstate.p, dstate2.p);
     std::swap(fifo_bits, fifo_bits2);
-    std::swap(h_dstate[0], h_dstate2);
+    std::swap(h_dstate.p[0], h_dstate2);
     std::swap(defr_state_now, defr_state2);
 }
 
@@ -686,7 +769,7 @@ void Fec::swap_unit()
 // pinned deframer mirror when one was queued (swap_unit() overwrites the mirror next).
 void Fec::compact_fifo(bool sync)
 {
-    DefrState S = *h_dstate;
+    DefrState S = *h_dstate.p;
     long keep = S.frame_pay >= 0 ? S.frame_pay : S.pos - 31;
     keep = std::max<long>(0, std::min<long>(keep, fifo_bits));
     const long keep_al = keep & ~31L;
@@ -698,8 +781,8 @@ void Fec::compact_fifo(bool sync)
         if (S.frame_pay >= 0)
             S.frame_pay -= keep_al;
         fifo_bits -= keep_al;
-        *h_dstate = S;
-        B200_CUDA(cudaMemcpyAsync(dstate.p, h_dstate, sizeof(DefrState), cudaMemcpyHostToDevice, stream));
+        *h_dstate.p = S;
+        B200_CUDA(cudaMemcpyAsync(dstate.p, h_dstate.p, sizeof(DefrState), cudaMemcpyHostToDevice, stream));
         if (sync)
             B200_CUDA(cudaStreamSynchronize(stream));
     }
@@ -709,12 +792,12 @@ void Fec::compact_fifo(bool sync)
 Fec::Mark Fec::mark()
 {
     B200_CUDA(cudaMemcpyAsync(dstate.p + 1, dstate.p, sizeof(DefrState), cudaMemcpyDeviceToDevice, stream));
-    return Mark{h_dstate[0], fifo_bits, out_frames, total_frames, rs_corrected, rs_failed, defr_state_now};
+    return Mark{h_dstate.p[0], fifo_bits, out_frames, total_frames, rs_corrected, rs_failed, defr_state_now};
 }
 void Fec::rewind(const Mark &m)
 {
     B200_CUDA(cudaMemcpyAsync(dstate.p, dstate.p + 1, sizeof(DefrState), cudaMemcpyDeviceToDevice, stream));
-    h_dstate[0] = m.h_dstate;
+    h_dstate.p[0] = m.h_dstate;
     fifo_bits = m.fifo_bits;
     out_frames = m.out_frames;
     total_frames = m.total_frames;
@@ -840,7 +923,7 @@ void Fec::decode_conv(long nch)
             long redo_from = -1;
             if (cfg.kind == B200_FEC_METOP) {
                 // module_metop_ahrpt_decoder.cpp:59-72: ten consecutive decoder calls that end with the deframer in NOSYNC reset the Viterbi
-                const int ne = h_counters[1];
+                const int ne = h_counters.p[1];
                 int ei = 0, st = 0;
                 {   // state before this segment = snapshot
                     DefrState snap;
@@ -850,8 +933,8 @@ void Fec::decode_conv(long nch)
                 }
                 for (long k = 0; k < nout; k++) {
                     const long end = m0.fifo_bits + (k + 1) * (long)geom.F; // exclusive
-                    while (ei < ne && h_events[ei].pos < end)
-                        st = h_events[ei++].state;
+                    while (ei < ne && h_events.p[ei].pos < end)
+                        st = h_events.p[ei++].state;
                     if (st == 2) {
                         if (++nosync_runs >= 10) {
                             nosync_runs = 0;
@@ -897,16 +980,8 @@ void Fec::decode_conv(long nch)
 void Fec::process()
 {
     DeviceGuard g(cfg.device);
-    if (ldpc) {
-        ldpc_process();
-        return;
-    }
-    if (turbo) {
-        turbo_process();
-        return;
-    }
-    if (dump) {
-        dump_process();
+    if (framed) {
+        framed->process(*this);
         return;
     }
     const long nch = soft_have / geom.chunk;
@@ -969,12 +1044,8 @@ void Fec::stats(b200_fec_stats *o)
     o->spec_steps = spec_steps;
     o->tb_overlap = tb_overlap;
     o->kernel_launches = launches;
-    if (ldpc)
-        ldpc_stats(o);
-    if (turbo)
-        turbo_stats(o);
-    if (dump)
-        dump_stats(o);
+    if (framed)
+        framed->stats(o);
 }
 
 } // namespace b200
@@ -1064,7 +1135,6 @@ int b200_fec_ldpc_timing(b200_fec *h, float *ms_out, int n)
 {
     return guarded([&] {
         B200_REQUIRE(h && ms_out, B200_EINVAL, "NULL argument");
-        B200_REQUIRE(h->f->ldpc, B200_EINVAL, "not an LDPC decoder (kind B200_FEC_LDPC)");
         h->f->ldpc_timing(ms_out, n);
     });
 }
@@ -1094,7 +1164,6 @@ int b200_fec_turbo_timing(b200_fec *h, float *ms_out, int n)
 {
     return guarded([&] {
         B200_REQUIRE(h && ms_out, B200_EINVAL, "NULL argument");
-        B200_REQUIRE(h->f->turbo, B200_EINVAL, "not a turbo decoder (kind B200_FEC_TURBO)");
         h->f->turbo_timing(ms_out, n);
     });
 }

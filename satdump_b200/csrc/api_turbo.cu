@@ -12,31 +12,27 @@ namespace b200
 
 constexpr int TURBO_BATCH = 1024; // frames decoded at once: their BCJR metrics take 2 (K + 4) x 16 doubles each (2.3 MB at base 1115)
 
-struct Turbo
+struct Turbo : Framed
 {
     TurboGeom G{};
     TurboCode upper{}, lower{};
     int base = 0, iters = 0, batch = 0;
     double two_nv = 0, ln_half = 0;
-    long tail_seen = -1; // FIFO bytes left by the last pass (a second process() without new bytes changes nothing)
-    long max_frames = 0;
-    DevBuf<float> score, bval, table, recv;
-    DevBuf<int> bidx, perm;
-    DevBuf<unsigned char> bsync, pn, bits;
+    DevBuf<float> table, recv;
+    DevBuf<int> perm;
+    DevBuf<unsigned char> pn, bits;
     DevBuf<double> msg, bwd, fwd;
-    DevBuf<LdpcFrameRec> frames;
-    DevBuf<LdpcWalkOut> walk;
     DevBuf<uint8_t> cadu_tmp;
     DevBuf<unsigned long long> ties;
-    LdpcWalkOut *h_walk = nullptr;
-    LdpcFrameRec *h_frames = nullptr;
-    unsigned long long *h_ties = nullptr;
-    long last_nf = 0, last_b0 = 0; // frames of the last push; the first one of its last decoding batch
-    long base_off = 0, resyncs = 0, crc_ok = 0, crc_fail = 0, near_ties = 0;
-    int lock = 0;
-    float cor = 0.f;
-    cudaEvent_t ev[7]{};
-    float t_ms[6]{}; // last push: correlation, walk, gather, BCJR, pack + CRC + compaction, the whole push
+    PinnedBuf<unsigned long long> h_ties;
+    long last_b0 = 0; // the first frame of the last push's last decoding batch
+    long crc_ok = 0, crc_fail = 0, near_ties = 0;
+    Events<7> ev; // t_ms: correlation, walk, gather, BCJR, pack + CRC + compaction, the whole push
+
+    explicit Turbo(Fec &f);
+    void process(Fec &f) override;
+    void reset(Fec &f) override;
+    void stats(b200_fec_stats *o) override;
 };
 
 namespace
@@ -131,9 +127,9 @@ void launch_corr(const int8_t *soft, long npos, Turbo &T, cudaStream_t st)
 } // namespace
 
 // The module's parameter checks (:20-36, :118-119), and the iteration count, refused by name before the device is touched
-void Fec::turbo_init()
+Turbo::Turbo(Fec &f)
 {
-    const b200_fec_cfg &c = cfg;
+    const b200_fec_cfg &c = f.cfg;
     B200_REQUIRE(c.turbo_rate != 0, B200_EINVAL, "Turbo Rate is required!");
     B200_REQUIRE(c.turbo_base != 0, B200_EINVAL, "Turbo Base is required!");
     B200_REQUIRE(c.turbo_base == 223 || c.turbo_base == 446 || c.turbo_base == 892 || c.turbo_base == 1115, B200_EINVAL,
@@ -144,11 +140,8 @@ void Fec::turbo_init()
                  "turbo_iters %d: at least 1 iteration is needed (with 0 the reference decodes nothing and dereferences NULL)", c.turbo_iters);
     B200_REQUIRE(c.turbo_iters <= 10000, B200_EINVAL, "turbo_iters out of range (1..10000)");
     B200_REQUIRE(c.max_soft <= (1L << 30), B200_EINVAL, "max_soft must be <= 2^30 for the turbo decoder");
-    turbo = new Turbo();
-    Turbo &T = *turbo;
-    TurboGeom &G = T.G;
-    T.base = c.turbo_base;
-    T.iters = c.turbo_iters;
+    base = c.turbo_base;
+    iters = c.turbo_iters;
     G.K = 8 * c.turbo_base;
     G.N = G.K + TURBO_MEM;
     G.asm_bits = c.turbo_rate == 2 ? 64 : (c.turbo_rate == 3 ? 96 : (c.turbo_rate == 4 ? 128 : 192));
@@ -159,226 +152,168 @@ void Fec::turbo_init()
     G.F = G.cw + G.asm_bits;
     G.recv_stride = (long)(G.cu + G.cl) * G.N;
     if (c.turbo_rate == 6) {
-        T.upper = make_code({"10011", "11011", "10101", "11111"});
-        T.lower = make_code({"11011", "11111"});
+        upper = make_code({"10011", "11011", "10101", "11111"});
+        lower = make_code({"11011", "11111"});
     } else {
-        T.upper = c.turbo_rate == 4 ? make_code({"10011", "10101", "11111"}) : make_code({"10011", "11011"});
-        T.lower = make_code({"11011"});
+        upper = c.turbo_rate == 4 ? make_code({"10011", "10101", "11111"}) : make_code({"10011", "11011"});
+        lower = make_code({"11011"});
     }
     const float sigma = 0.707f; // CCSDSTurbo::d_sigma; turbo_decode gets d_sigma * d_sigma, a float product widened to double
     const float var = sigma * sigma;
-    T.two_nv = 2 * (double)var;
-    T.ln_half = std::log(0.5);
-    geom.chunk = G.F;
-    cadu_bytes = c.turbo_base + 4;
-    cfg.cadu_size = cadu_bytes * 8;
+    two_nv = 2 * (double)var;
+    ln_half = std::log(0.5);
+    f.geom.chunk = G.F;
+    f.cadu_bytes = c.turbo_base + 4;
+    f.cfg.cadu_size = f.cadu_bytes * 8;
     check_device(c.device);
     DeviceGuard g(c.device);
-    B200_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
-    for (cudaEvent_t *e : {&ev[0], &ev[1], &evm[0], &evm[1], &evf[0], &evf[1]}) // (the destructor destroys all six)
-        B200_CUDA(cudaEventCreate(e));
-    for (auto &e : T.ev)
-        B200_CUDA(cudaEventCreate(&e));
     const long fifo = c.max_soft + 2L * G.F;
-    softbuf.alloc((size_t)fifo);
-    dec.alloc((size_t)(2 * G.F) / sizeof(uint2) + 16); // scratch of keep_soft_tail
-    T.score.alloc((size_t)fifo);
-    T.bsync.alloc((size_t)fifo);
-    T.bval.alloc((size_t)fifo / 32 + 2);
-    T.bidx.alloc((size_t)fifo / 32 + 2);
-    T.max_frames = fifo / G.F + 2;
-    T.batch = (int)std::min<long>(T.max_frames, TURBO_BATCH);
-    T.frames.alloc((size_t)T.max_frames);
-    T.walk.alloc(1);
-    T.recv.alloc((size_t)T.batch * G.recv_stride);
-    T.msg.alloc((size_t)T.batch * 2 * G.K);
-    T.bwd.alloc((size_t)T.batch * G.N * TURBO_STATES);
-    T.fwd.alloc((size_t)T.batch * G.N * TURBO_STATES);
-    T.bits.alloc((size_t)T.batch * G.K);
-    T.cadu_tmp.alloc((size_t)T.max_frames * cadu_bytes);
-    T.ties.alloc(1);
-    max_frames_push = T.max_frames;
-    frames_out.alloc((size_t)(2 * T.max_frames + 4) * cadu_bytes);
+    alloc(fifo, fifo / G.F + 2);
+    f.framed_storage(G.F, max_frames);
+    ev.create();
+    batch = (int)std::min<long>(max_frames, TURBO_BATCH);
+    recv.alloc((size_t)batch * G.recv_stride);
+    msg.alloc((size_t)batch * 2 * G.K);
+    bwd.alloc((size_t)batch * G.N * TURBO_STATES);
+    fwd.alloc((size_t)batch * G.N * TURBO_STATES);
+    bits.alloc((size_t)batch * G.K);
+    cadu_tmp.alloc((size_t)max_frames * f.cadu_bytes);
+    ties.alloc(1);
+    h_ties.alloc(1);
     const std::vector<int> pi = interleaver(c.turbo_base);
-    T.perm.alloc(pi.size());
+    perm.alloc(pi.size());
     const char *hex = asm_hex(c.turbo_rate);
-    std::vector<float> table(G.asm_bits);
+    std::vector<float> table_h(G.asm_bits);
     for (int i = 0; i < G.asm_bits; i++) {
         const char h = hex[i / 4];
         const int nib = h <= '9' ? h - '0' : h - 'A' + 10;
-        table[i] = (nib >> (3 - i % 4)) & 1 ? 1.0f : -1.0f;
+        table_h[i] = (nib >> (3 - i % 4)) & 1 ? 1.0f : -1.0f;
     }
-    T.table.alloc(table.size());
+    table.alloc(table_h.size());
     unsigned char pnb[255];
     ccsds_pn_bits(pnb);
-    T.pn.alloc(256);
-    B200_CUDA(cudaMemcpyAsync(T.perm.p, pi.data(), pi.size() * sizeof(int), cudaMemcpyHostToDevice, stream));
-    B200_CUDA(cudaMemcpyAsync(T.table.p, table.data(), table.size() * sizeof(float), cudaMemcpyHostToDevice, stream));
-    B200_CUDA(cudaMemcpyAsync(T.pn.p, pnb, 255, cudaMemcpyHostToDevice, stream));
-    T.ties.zero(stream);
-    B200_CUDA(cudaFuncSetAttribute(k_turbo_pack, cudaFuncAttributeMaxDynamicSharedMemorySize, T.base));
-    B200_CUDA(cudaMallocHost((void **)&T.h_walk, sizeof(LdpcWalkOut)));
-    B200_CUDA(cudaMallocHost((void **)&T.h_frames, sizeof(LdpcFrameRec) * T.max_frames));
-    B200_CUDA(cudaMallocHost((void **)&T.h_ties, sizeof(unsigned long long)));
-    B200_CUDA(cudaStreamSynchronize(stream)); // (the host vectors above die here)
+    pn.alloc(256);
+    B200_CUDA(cudaMemcpyAsync(perm.p, pi.data(), pi.size() * sizeof(int), cudaMemcpyHostToDevice, f.stream));
+    B200_CUDA(cudaMemcpyAsync(table.p, table_h.data(), table_h.size() * sizeof(float), cudaMemcpyHostToDevice, f.stream));
+    B200_CUDA(cudaMemcpyAsync(pn.p, pnb, 255, cudaMemcpyHostToDevice, f.stream));
+    ties.zero(f.stream);
+    B200_CUDA(cudaFuncSetAttribute(k_turbo_pack, cudaFuncAttributeMaxDynamicSharedMemorySize, base));
+    B200_CUDA(cudaStreamSynchronize(f.stream)); // (the host vectors above die here)
 }
 
-void Fec::turbo_free()
-{
-    if (!turbo)
-        return;
-    for (auto &e : turbo->ev)
-        if (e)
-            cudaEventDestroy(e);
-    for (void *p : {(void *)turbo->h_walk, (void *)turbo->h_frames, (void *)turbo->h_ties})
-        if (p)
-            cudaFreeHost(p);
-    delete turbo;
-    turbo = nullptr;
-}
+std::unique_ptr<Framed> turbo_decoder(Fec &f) { return std::make_unique<Turbo>(f); }
 
-void Fec::turbo_reset()
+void Turbo::reset(Fec &f)
 {
-    soft_have = 0;
-    out_frames = 0;
-    Turbo &T = *turbo;
-    T.tail_seen = -1;
-    T.base_off = 0;
-    T.last_nf = 0;
-    T.lock = 0;
-    T.cor = 0.f;
-    T.near_ties = 0;
-    T.ties.zero(stream);
-    B200_CUDA(cudaStreamSynchronize(stream));
+    Framed::reset(f);
+    near_ties = 0;
+    ties.zero(f.stream);
+    B200_CUDA(cudaStreamSynchronize(f.stream));
 }
 
 // The module loop over every frame the FIFO completes: correlation at every position and the frame walk, then, batch by batch, gather,
-// turbo_iters x (upper BCJR, lower BCJR) and the CRC; the frames that pass are compacted into frames_out. The bytes behind the walk's
-// next window stay in the FIFO; a call that finds no new bytes behind them has nothing to do.
-void Fec::turbo_process()
+// turbo_iters x (upper BCJR, lower BCJR) and the CRC; the frames that pass are compacted into frames_out.
+void Turbo::process(Fec &f)
 {
-    Turbo &T = *turbo;
-    const TurboGeom &G = T.G;
-    if (soft_have == T.tail_seen)
+    if (!begin(f, G.F))
         return;
-    T.last_nf = 0;
-    for (float &t : T.t_ms)
-        t = 0;
-    if (soft_have < G.F) {
-        T.tail_seen = soft_have;
-        return;
-    }
-    const long have = soft_have, npos = have - (G.asm_bits - 1);
-    B200_CUDA(cudaEventRecord(T.ev[0], stream));
+    cudaStream_t stream = f.stream;
+    const long have = f.soft_have, npos = have - (G.asm_bits - 1);
+    B200_CUDA(cudaEventRecord(ev[0], stream));
     switch (G.asm_bits) {
-    case 64: launch_corr<64>(softbuf.p, npos, T, stream); break;
-    case 96: launch_corr<96>(softbuf.p, npos, T, stream); break;
-    case 128: launch_corr<128>(softbuf.p, npos, T, stream); break;
-    default: launch_corr<192>(softbuf.p, npos, T, stream); break;
+    case 64: launch_corr<64>(f.softbuf.p, npos, *this, stream); break;
+    case 96: launch_corr<96>(f.softbuf.p, npos, *this, stream); break;
+    case 128: launch_corr<128>(f.softbuf.p, npos, *this, stream); break;
+    default: launch_corr<192>(f.softbuf.p, npos, *this, stream); break;
     }
-    B200_CUDA(cudaEventRecord(T.ev[1], stream));
-    frame_walk(T.score.p, T.bsync.p, T.bval.p, T.bidx.p, have, G.F, G.F - G.asm_bits, WALK_SWAP_ONLY, T.frames.p, (int)T.max_frames, T.walk.p,
-               stream);
-    B200_CUDA(cudaEventRecord(T.ev[2], stream));
-    launches += 2;
-    B200_CUDA(cudaMemcpyAsync(T.h_walk, T.walk.p, sizeof(LdpcWalkOut), cudaMemcpyDeviceToHost, stream));
-    B200_CUDA(cudaStreamSynchronize(stream));
-    const int nf = T.h_walk->nf;
+    B200_CUDA(cudaEventRecord(ev[1], stream));
+    const CorrWindow win{score.p, bsync.p, bval.p, bidx.p, G.F - G.asm_bits, WALK_SWAP_ONLY};
+    k_frame_walk<<<1, WALK_WARPS * 32, 0, stream>>>(win, have, G.F, frames.p, (int)max_frames, walk.p);
+    B200_CUDA(cudaEventRecord(ev[2], stream));
+    f.launches += 2;
+    const int nf = walked(stream);
+    const int cadu_bytes = f.cadu_bytes;
     float t_gather = 0, t_bcjr = 0;
     if (nf > 0) {
-        B200_REQUIRE((size_t)(out_frames + nf) * cadu_bytes <= frames_out.n, B200_ESTATE, "%ld frames not pulled yet: pull the frames between pushes",
-                     out_frames);
-        for (int b0 = 0; b0 < nf; b0 += T.batch) {
-            const int nb = std::min(T.batch, nf - b0);
-            T.last_b0 = b0;
-            B200_CUDA(cudaEventRecord(T.ev[3], stream));
-            k_turbo_gather<<<nb, 256, 0, stream>>>(softbuf.p, T.frames.p + b0, G, T.pn.p, T.recv.p, T.msg.p, T.ln_half);
-            B200_CUDA(cudaEventRecord(T.ev[4], stream));
-            for (int it = 0; it < T.iters; it++) {
-                half_iteration(T, nb, false, nullptr, stream);
-                half_iteration(T, nb, true, it == T.iters - 1 ? T.bits.p : nullptr, stream);
+        B200_REQUIRE((size_t)(f.out_frames + nf) * cadu_bytes <= f.frames_out.n, B200_ESTATE,
+                     "%ld frames not pulled yet: pull the frames between pushes", f.out_frames);
+        for (int b0 = 0; b0 < nf; b0 += batch) {
+            const int nb = std::min(batch, nf - b0);
+            last_b0 = b0;
+            B200_CUDA(cudaEventRecord(ev[3], stream));
+            k_turbo_gather<<<nb, 256, 0, stream>>>(f.softbuf.p, frames.p + b0, G, pn.p, recv.p, msg.p, ln_half);
+            B200_CUDA(cudaEventRecord(ev[4], stream));
+            for (int it = 0; it < iters; it++) {
+                half_iteration(*this, nb, false, nullptr, stream);
+                half_iteration(*this, nb, true, it == iters - 1 ? bits.p : nullptr, stream);
             }
-            B200_CUDA(cudaEventRecord(T.ev[5], stream));
-            k_turbo_pack<<<nb, 256, T.base, stream>>>(T.bits.p, T.base, T.frames.p + b0, T.cadu_tmp.p + (size_t)b0 * cadu_bytes);
-            launches += 2 + 4L * T.iters;
-            B200_CUDA(cudaEventSynchronize(T.ev[5]));
+            B200_CUDA(cudaEventRecord(ev[5], stream));
+            k_turbo_pack<<<nb, 256, base, stream>>>(bits.p, base, frames.p + b0, cadu_tmp.p + (size_t)b0 * cadu_bytes);
+            f.launches += 2 + 4L * iters;
+            B200_CUDA(cudaEventSynchronize(ev[5]));
             float a = 0, b = 0;
-            cudaEventElapsedTime(&a, T.ev[3], T.ev[4]);
-            cudaEventElapsedTime(&b, T.ev[4], T.ev[5]);
+            cudaEventElapsedTime(&a, ev[3], ev[4]);
+            cudaEventElapsedTime(&b, ev[4], ev[5]);
             t_gather += a;
             t_bcjr += b;
         }
-        k_turbo_compact<<<nf, 256, 0, stream>>>(T.cadu_tmp.p, T.frames.p, cadu_bytes, frames_out.p + out_frames * cadu_bytes);
-        launches++;
-        B200_CUDA(cudaMemcpyAsync(T.h_frames, T.frames.p, sizeof(LdpcFrameRec) * nf, cudaMemcpyDeviceToHost, stream));
-        B200_CUDA(cudaMemcpyAsync(T.h_ties, T.ties.p, sizeof(unsigned long long), cudaMemcpyDeviceToHost, stream));
+        k_turbo_compact<<<nf, 256, 0, stream>>>(cadu_tmp.p, frames.p, cadu_bytes, f.frames_out.p + f.out_frames * cadu_bytes);
+        f.launches++;
+        B200_CUDA(cudaMemcpyAsync(h_frames.p, frames.p, sizeof(WalkFrame) * nf, cudaMemcpyDeviceToHost, stream));
+        B200_CUDA(cudaMemcpyAsync(h_ties.p, ties.p, sizeof(unsigned long long), cudaMemcpyDeviceToHost, stream));
     }
-    B200_CUDA(cudaEventRecord(T.ev[6], stream));
-    keep_soft_tail(T.h_walk->next);
+    B200_CUDA(cudaEventRecord(ev[6], stream));
+    f.keep_soft_tail(h_walk.p->next);
     B200_CUDA(cudaStreamSynchronize(stream));
     B200_CUDA(cudaGetLastError());
-    cudaEventElapsedTime(&T.t_ms[0], T.ev[0], T.ev[1]);
-    cudaEventElapsedTime(&T.t_ms[1], T.ev[1], T.ev[2]);
-    T.t_ms[2] = t_gather;
-    T.t_ms[3] = t_bcjr;
+    cudaEventElapsedTime(&t_ms[0], ev[0], ev[1]);
+    cudaEventElapsedTime(&t_ms[1], ev[1], ev[2]);
+    t_ms[2] = t_gather;
+    t_ms[3] = t_bcjr;
     if (nf > 0) {
-        float tail = 0, whole = 0;
-        cudaEventElapsedTime(&tail, T.ev[5], T.ev[6]);
-        cudaEventElapsedTime(&whole, T.ev[0], T.ev[6]);
-        T.t_ms[4] = whole - T.t_ms[0] - T.t_ms[1] - t_gather - t_bcjr; // the pack launches of all batches, compaction and copies
-        T.t_ms[5] = whole;
+        float whole = 0;
+        cudaEventElapsedTime(&whole, ev[0], ev[6]);
+        t_ms[4] = whole - t_ms[0] - t_ms[1] - t_gather - t_bcjr; // the pack launches of all batches, compaction and copies
+        t_ms[5] = whole;
     } else
-        T.t_ms[5] = T.t_ms[0] + T.t_ms[1];
-    t_vit = T.t_ms[5];
+        t_ms[5] = t_ms[0] + t_ms[1];
+    f.t_vit = t_ms[5];
+    finish(nf, f.soft_have);
     int ok = 0;
-    for (int k = 0; k < nf; k++) {
-        LdpcFrameRec &r = T.h_frames[k];
-        r.off += T.base_off;
-        T.resyncs += r.pos != 0;
-        ok += r.corr != 0;
-    }
-    if (nf > 0) {
-        const LdpcFrameRec &r = T.h_frames[nf - 1];
-        T.lock = r.pos == 0;
-        T.cor = r.cor;
-        T.near_ties = (long)*T.h_ties;
-    }
-    T.crc_ok += ok;
-    T.crc_fail += nf - ok;
-    T.last_nf = nf;
-    T.base_off += T.h_walk->next;
-    T.tail_seen = soft_have;
-    out_frames += ok;
-    total_frames += ok;
-    total_chunks += nf;
-    total_bits += (long)ok * T.base * 8;
+    for (int k = 0; k < nf; k++)
+        ok += h_frames.p[k].corr != 0;
+    if (nf > 0)
+        near_ties = (long)*h_ties.p;
+    crc_ok += ok;
+    crc_fail += nf - ok;
+    f.out_frames += ok;
+    f.total_frames += ok;
+    f.total_chunks += nf;
+    f.total_bits += (long)ok * base * 8;
 }
 
-void Fec::turbo_stats(b200_fec_stats *o)
+void Turbo::stats(b200_fec_stats *o)
 {
-    o->correlator_lock = turbo->lock;
-    o->correlator_corr = turbo->cor;
-    o->ldpc_resyncs = turbo->resyncs;
-    o->crc_ok = turbo->crc_ok;
-    o->crc_fail = turbo->crc_fail;
-    o->turbo_near_ties = turbo->near_ties;
+    Framed::stats(o);
+    o->crc_ok = crc_ok;
+    o->crc_fail = crc_fail;
+    o->turbo_near_ties = near_ties;
 }
 
 long Fec::turbo_frames(b200_turbo_frame *out, long cap)
 {
-    B200_REQUIRE(turbo, B200_EINVAL, "not a turbo decoder");
-    B200_REQUIRE(turbo->last_nf <= cap, B200_ESTATE, "output buffer too small: need %ld records", turbo->last_nf);
-    for (long k = 0; k < turbo->last_nf; k++) {
-        const LdpcFrameRec &r = turbo->h_frames[k];
+    const Turbo &T = framed_as<Turbo>("not a turbo decoder");
+    B200_REQUIRE(T.last_nf <= cap, B200_ESTATE, "output buffer too small: need %ld records", T.last_nf);
+    for (long k = 0; k < T.last_nf; k++) {
+        const WalkFrame &r = T.h_frames.p[k];
         out[k] = b200_turbo_frame{(long)r.off, r.pos, r.cor, r.swap, r.corr};
     }
-    return turbo->last_nf;
+    return T.last_nf;
 }
 
 long Fec::turbo_llr(long frame, double *app0, double *app1, long cap)
 {
-    B200_REQUIRE(turbo, B200_EINVAL, "not a turbo decoder");
-    Turbo &T = *turbo;
+    const Turbo &T = framed_as<Turbo>("not a turbo decoder");
     const int K = T.G.K;
     B200_REQUIRE(frame >= T.last_b0 && frame < T.last_nf, B200_ESTATE, "frame %ld is not in the last decoding batch [%ld, %ld) of the last push",
                  frame, T.last_b0, T.last_nf);
@@ -392,8 +327,9 @@ long Fec::turbo_llr(long frame, double *app0, double *app1, long cap)
 
 void Fec::turbo_timing(float *ms, int n)
 {
+    const Turbo &T = framed_as<Turbo>("not a turbo decoder (kind B200_FEC_TURBO)");
     for (int k = 0; k < n && k < 6; k++)
-        ms[k] = turbo->t_ms[k];
+        ms[k] = T.t_ms[k];
 }
 
 } // namespace b200

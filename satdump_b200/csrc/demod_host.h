@@ -149,8 +149,8 @@ class Demod
     DevBuf<long> offs;
     DevBuf<float> d_bank;
     DevBuf<DemodDevState> st;
-    long *h_total = nullptr; // pinned
-    DemodDevState *h_state = nullptr; // pinned snapshot for stats
+    PinnedBuf<long> h_total;
+    PinnedBuf<DemodDevState> h_state; // snapshot for stats
     cudaEvent_t ev[4];
     int Wc, Wm, Gc = 0, Gm = 0, seg_cap_threads; // warm-up lengths, gear-shift parts of them
     // pm_demod / freq_shift

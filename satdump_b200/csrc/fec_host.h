@@ -6,21 +6,49 @@
 #include "fec.cuh"
 #include "walk.cuh"
 #include "host_common.h"
+#include <memory>
 #include <vector>
 
 namespace b200
 {
 
 struct DefrEvent { long pos; int state; int pad; };
-struct Ldpc; // ccsds_ldpc_decoder's state (api_ldpc.cu)
-struct Turbo; // ccsds_turbo_decoder's state (api_turbo.cu)
-struct Dump; // metop_dump_decoder's state (api_dump.cu)
+class Fec;
 
-// the CCSDS sequence (x^8+x^7+x^5+x^3+1 from all ones), one bit per entry as derand_ccsds_soft applies it to soft bytes (255 entries)
-void ccsds_pn_bits(unsigned char *pn);
-// k_ldpc_walk (ldpc.cuh) on `stream`: the frame walk of the correlator-driven decoders
-void frame_walk(const float *score, const unsigned char *best_sync, const float *bval, const int *bidx, long have, int F, int npos,
-                int constellation, LdpcFrameRec *frames, int max_frames, LdpcWalkOut *out, cudaStream_t stream);
+// The stream state of a correlator-driven decoder (ccsds_ldpc_decoder, ccsds_turbo_decoder, metop_dump_decoder): a correlator scores
+// every position of the soft FIFO, k_frame_walk (walk.cuh) goes o -> o + pos + F over its windows, the frames are decoded, and the
+// FIFO keeps the bytes behind the walk's next window. Each decoder derives from it (Ldpc, Turbo, Dump in api_ldpc.cu, api_turbo.cu,
+// api_dump.cu); its process() reads begin -> correlate -> walk -> walked -> decode -> keep_soft_tail -> timings -> finish.
+struct Framed
+{
+    DevBuf<float> score, bval;        // the correlator's score at every position, the maxima of 32-position blocks
+    DevBuf<int> bidx;                 // ... and their positions
+    DevBuf<unsigned char> bsync;      // the correlator's table index at every position
+    DevBuf<WalkFrame> frames;         // the walk's records
+    DevBuf<WalkOut> walk;
+    PinnedBuf<WalkOut> h_walk;
+    PinnedBuf<WalkFrame> h_frames;    // records of the last push (offsets made absolute)
+    long max_frames = 0;
+    long tail_seen = -1;              // FIFO bytes left by the last pass (a second process() without new bytes changes nothing)
+    long base_off = 0;                // stream offset of the FIFO's first byte
+    long last_nf = 0, resyncs = 0;
+    int lock = 0;
+    float cor = 0.f;
+    float t_ms[6]{};                  // device ms of the last push's stages, as the decoder's timing getter lists them
+
+    virtual ~Framed() = default;
+    virtual void process(Fec &f) = 0;
+    virtual void reset(Fec &f);       // a new stream: the FIFO, the walk's position and the lock (the counters carry over)
+    virtual void stats(b200_fec_stats *o); // correlator_lock, correlator_corr and ldpc_resyncs
+
+    void alloc(long positions, long frames_cap); // the correlator's outputs for `positions` scores, the walk's records
+    bool begin(Fec &f, int F);        // false when there is nothing to do: no new bytes, or fewer than F in the FIFO
+    int walked(cudaStream_t stream);  // waits for the walk; its frame count
+    void finish(int nf, long soft_have); // records made absolute, resyncs, lock and cor of the last frame, the next pass's start
+};
+std::unique_ptr<Framed> ldpc_decoder(Fec &f);
+std::unique_ptr<Framed> turbo_decoder(Fec &f);
+std::unique_ptr<Framed> dump_decoder(Fec &f);
 
 class Fec
 {
@@ -46,17 +74,20 @@ class Fec
     cudaEvent_t evm[2], evf[2];
     long last_main_chunks = 0;
     void reset();
-    // ccsds_ldpc_decoder (B200_FEC_LDPC): set up by the constructor instead of the Viterbi / deframer storage
-    Ldpc *ldpc = nullptr;
+    // the correlator-driven decoders (B200_FEC_LDPC, B200_FEC_TURBO, B200_FEC_METOP_DUMP): set up by the constructor instead of the
+    // Viterbi / deframer storage (ccsds_ldpc_decoder's internal_stream adds the deframer stage)
+    std::unique_ptr<Framed> framed;
+    template <class D> D &framed_as(const char *what) // the decoder as a D, or B200_EINVAL with `what`
+    {
+        D *d = dynamic_cast<D *>(framed.get());
+        B200_REQUIRE(d, B200_EINVAL, "%s", what);
+        return *d;
+    }
     long ldpc_frames(b200_ldpc_frame *out, long cap); // records of the last push
     void ldpc_timing(float *ms, int n);
-    // ccsds_turbo_decoder (B200_FEC_TURBO): the same soft FIFO and frame walk
-    Turbo *turbo = nullptr;
     long turbo_frames(b200_turbo_frame *out, long cap); // records of the last push
     long turbo_llr(long frame, double *app0, double *app1, long cap);
     void turbo_timing(float *ms, int n);
-    // metop_dump_decoder (B200_FEC_METOP_DUMP): the same soft FIFO, its own correlator and frame walk, RS through k_frames' decoder
-    Dump *dump = nullptr;
     long dump_frames(b200_dump_frame *out, long cap); // records of the last push
 
     // device storage
@@ -78,7 +109,7 @@ class Fec
     DevBuf<unsigned char> vitbuf, vitbuf_tmp, bdep;
     DevBuf<int> tail_real;
     DevBuf<PuncIdleOut> punc_out;
-    PuncIdleOut *h_punc = nullptr;
+    PinnedBuf<PuncIdleOut> h_punc;
     std::vector<int> h_tail, h_wcall;
     long in_buffer = 0;       // symbols waiting in vitbuf (ViterbiSlidingBuffer::in_buffer)
     int changing_shift = 0;   // DepuncXX::changing_shift
@@ -92,7 +123,7 @@ class Fec
     long tb_serial_total = 0, start_redone = 0; // chunks chained back serially / decoded again from a corrected start state
     DevBuf<VitIdleOut> idle_out;
     DevBuf<VitIdle2Out> idle2_out;
-    VitIdle2Out *h_idle2 = nullptr;
+    PinnedBuf<VitIdle2Out> h_idle2;
     DevBuf<DefrState> dstate;
     DevBuf<DefrEvent> devents;
     DevBuf<FrameRec> frames;
@@ -111,12 +142,12 @@ class Fec
     void swap_unit();
     void compact_fifo(bool sync);
     // pinned host mirrors
-    VitRec *h_rec = nullptr;
-    VitIdleOut *h_idle = nullptr;
-    int *h_counters = nullptr;
-    DefrState *h_dstate = nullptr;
-    DefrEvent *h_events = nullptr;
-    int *h_rs_err = nullptr;
+    PinnedBuf<VitRec> h_rec;
+    PinnedBuf<VitIdleOut> h_idle;
+    PinnedBuf<int> h_counters;
+    PinnedBuf<DefrState> h_dstate;
+    PinnedBuf<DefrEvent> h_events;
+    PinnedBuf<int> h_rs_err;
 
     // stream state
     long soft_have = 0, max_chunks = 0, fifo_bits = 32, max_frames_push = 0;
@@ -131,6 +162,9 @@ class Fec
     long total_soft = 0, total_chunks = 0, total_bits = 0, total_frames = 0, rs_corrected = 0, rs_failed = 0, replays = 0, launches = 0;
 
   private:
+    friend struct Ldpc;
+    friend struct Turbo;
+    friend struct Dump;
     // the main deframer and the frame counters at a point a pass may have to roll back to
     struct Mark { DefrState h_dstate; long fifo_bits, out_frames, total_frames, rs_corrected, rs_failed; int defr_state_now; };
     Mark mark();
@@ -141,24 +175,12 @@ class Fec
     int last_raw_bit(long q, int nbits);
     void keep_soft_tail(long used);
     void deframe_and_rs(long new_bits);
-    void ldpc_init();
+    void framed_storage(int F, long frames_per_push); // what every Framed decoder needs of the decoder object (api_fec.cu)
     void deframer_storage(long max_new_bits); // bit FIFO, deframer and frame stage of LDPC's internal_stream (api_fec.cu)
-    void ldpc_free();
-    void ldpc_reset();
-    void ldpc_process();
-    void ldpc_stats(b200_fec_stats *o);
-    void turbo_init();
-    void turbo_free();
-    void turbo_reset();
-    void turbo_process();
-    void turbo_stats(b200_fec_stats *o);
-    void dump_init();
-    void dump_free();
-    void dump_reset();
-    void dump_process();
-    void dump_stats(b200_fec_stats *o);
 };
 
 void build_rs_tables(RsTables &T);
+// the CCSDS sequence (x^8+x^7+x^5+x^3+1 from all ones), one bit per entry as derand_ccsds_soft applies it to soft bytes (255 entries)
+void ccsds_pn_bits(unsigned char *pn);
 
 } // namespace b200

@@ -69,6 +69,51 @@ template <typename T> struct DevBuf
     DevBuf &operator=(const DevBuf &) = delete;
 };
 
+// DevBuf's counterpart in pinned host memory (the mirrors the device results are copied back into)
+template <typename T> struct PinnedBuf
+{
+    T *p = nullptr;
+    size_t n = 0;
+    void alloc(size_t count)
+    {
+        free();
+        B200_CUDA(cudaMallocHost((void **)&p, count * sizeof(T)));
+        n = count;
+    }
+    void free()
+    {
+        if (p)
+            cudaFreeHost(p);
+        p = nullptr;
+        n = 0;
+    }
+    ~PinnedBuf() { free(); }
+    PinnedBuf() = default;
+    PinnedBuf(const PinnedBuf &) = delete;
+    PinnedBuf &operator=(const PinnedBuf &) = delete;
+};
+
+// N CUDA events, created by create() and destroyed with the holder
+template <int N> struct Events
+{
+    cudaEvent_t e[N]{};
+    void create()
+    {
+        for (auto &x : e)
+            B200_CUDA(cudaEventCreate(&x));
+    }
+    cudaEvent_t operator[](int i) const { return e[i]; }
+    ~Events()
+    {
+        for (auto &x : e)
+            if (x)
+                cudaEventDestroy(x);
+    }
+    Events() = default;
+    Events(const Events &) = delete;
+    Events &operator=(const Events &) = delete;
+};
+
 // selects the device for the calling thread for the lifetime of the guard
 struct DeviceGuard
 {

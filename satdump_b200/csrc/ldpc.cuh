@@ -1,7 +1,7 @@
 // Kernels of ccsds_ldpc_decoder for the CCSDS C2 (8176, 7154) code (module_ccsds_ldpc_decoder.cpp:134-277, ldpc_rate "7/8").
-// Included by api_ldpc.cu only.
+// Included by api_ldpc.cu only. The frame walk (o_{k+1} = o_k + pos_k + F, pos_k = the window's first maximum if > 0, else 0) is
+// k_frame_walk<CorrWindow> of walk.cuh.
 //   k_ldpc_corr    CorrelatorGeneric::correlate's score (generic_correlator.cpp:176-231) at every soft position + the maxima of 32-position blocks
-//   k_ldpc_walk    the module's frame walk: o_{k+1} = o_k + pos_k + F, pos_k = the window's first maximum if > 0, else 0
 //   k_ldpc_gather  rotate_soft / OQPSK re-delay / derand_ccsds_soft of each frame -> the decoder's input with its 18 zero positions
 //   k_ldpc_decode  LDPCDecoderGeneric::decode (ldpc_decoder_generic.cpp:69-194) on a level schedule, then the CADU repack
 #pragma once
@@ -13,7 +13,6 @@ constexpr int LDPC_F = LDPC_CW + LDPC_ASM;   // 8192 soft bytes per frame (d_ldp
 constexpr int LDPC_NPOS = LDPC_F - LDPC_ASM; // positions the correlator tries per window
 constexpr int LDPC_VN = 8176, LDPC_ROWS = 1022, LDPC_DEG = 32, LDPC_SHORT = 18, LDPC_INFO_VN = LDPC_VN - LDPC_ROWS;
 constexpr int LDPC_CADU = 1024;
-constexpr int LDPC_WALK_WARPS = 32, LDPC_WALK_SPEC = 4 * LDPC_WALK_WARPS; // frames of the current lattice checked per round
 constexpr int LDPC_DEC_THREADS = 1024;
 
 struct LdpcSync { float w[4][LDPC_ASM]; }; // the correlator's syncword tables, built on the host (ldpc_syncwords)
@@ -50,7 +49,7 @@ __global__ void __launch_bounds__(256) k_ldpc_corr(const int8_t *__restrict__ so
     }
     float v = i < npos ? best : -INFINITY;
     int vi = (int)i;
-    ldpc_best_warp(v, vi);
+    first_max_warp(v, vi);
     const long b = i >> 5;
     if ((threadIdx.x & 31) == 0 && (b + 1) * 32 <= npos) {
         bval[b] = v;
@@ -58,83 +57,13 @@ __global__ void __launch_bounds__(256) k_ldpc_corr(const int8_t *__restrict__ so
     }
 }
 
-// The frame walk over the `have` soft bytes of the FIFO, from offset 0, for frames of F soft bytes whose windows hold npos correlator
-// positions. Each round checks up to LDPC_WALK_SPEC frames of the current lattice o + jF at once (one warp per frame): the frames up to
-// and including the first one whose ASM is not at its window's start are exact, since their windows start where the module would read
-// them; the walk then continues on the shifted lattice. Without signal every frame shifts, and each round takes one frame. A frame whose
-// shifted start leaves fewer than F bytes waits for the next push. Offsets are < 2^31 (the FIFO is sized by max_soft).
-// constellation WALK_SWAP_ONLY (the turbo correlator): the table index found is the frame's `swap`, its phase is 0.
-__global__ void __launch_bounds__(1024) k_ldpc_walk(const float *__restrict__ score, const unsigned char *__restrict__ best_sync,
-                                                     const float *__restrict__ bval, const int *__restrict__ bidx, long have, int F, int npos,
-                                                     int constellation, LdpcFrameRec *__restrict__ frames, int max_frames,
-                                                     LdpcWalkOut *__restrict__ out)
-{
-    __shared__ float s_v[LDPC_WALK_SPEC];
-    __shared__ int s_i[LDPC_WALK_SPEC];
-    __shared__ unsigned char s_bs[LDPC_WALK_SPEC];
-    __shared__ long s_o;
-    __shared__ int s_nf, s_shifted, s_done;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (threadIdx.x == 0) { s_o = 0; s_nf = 0; s_shifted = 0; s_done = 0; }
-    __syncthreads();
-    while (!s_done) {
-        const long o = s_o;
-        const long avail = have >= o + F ? (have - o - F) / F + 1 : 0;
-        const int n = (int)min(min(avail, (long)LDPC_WALK_SPEC), (long)(max_frames - s_nf));
-        for (int j = warp; j < n; j += LDPC_WALK_WARPS) {
-            float v;
-            int vi;
-            ldpc_window_max(score, bval, bidx, o + (long)j * F, npos, v, vi);
-            if (lane == 0) { s_v[j] = v; s_i[j] = vi; s_bs[j] = v > 0.0f ? best_sync[vi] : 0; }
-        }
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            long oo = o;
-            int nf = s_nf, j = 0;
-            bool stop = n == 0;
-            for (; j < n; j++) {
-                const float v = s_v[j];
-                const int pos = v > 0.0f ? (int)(s_i[j] - oo) : 0;
-                if (pos != 0 && oo + pos + F > have) { stop = true; break; }
-                const int bs = s_bs[j];
-                int phase, swap = 0; // generic_correlator.cpp:233-262
-                if (constellation == WALK_SWAP_ONLY) { phase = 0; swap = bs; }
-                else if (constellation == 0) phase = bs ? 2 : 0;
-                else if (constellation == 1) phase = bs;
-                else { phase = bs == 0 ? 1 : (bs == 1 ? 3 : (bs == 2 ? 0 : 2)); swap = bs >> 1; }
-                LdpcFrameRec r;
-                r.off = oo + pos;
-                r.pos = pos;
-                r.cor = v > 0.0f ? v : 0.0f;
-                r.phase = phase;
-                r.swap = swap;
-                r.corr = 0;
-                r.pad = 0;
-                frames[nf++] = r;
-                oo += pos + F;
-                if (pos != 0) { s_shifted++; j++; break; }
-            }
-            if (n == 0 || nf >= max_frames) stop = true;
-            s_o = oo;
-            s_nf = nf;
-            s_done = stop;
-        }
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) {
-        out->next = s_o;
-        out->nf = s_nf;
-        out->shifted = s_shifted;
-    }
-}
-
 // One CTA per frame: the decoder's input vn[0 .. 8175] = 18 zeros, then code soft bytes 0 .. 8157 of the frame after the phase fix
 // (OQPSK: rotate_soft without swap, then on swap Q moves one symbol earlier and the frame's last Q is 0, module :159-173) and the
 // derandomiser (~x where the sequence `pn`, one bit per entry, has a one; pn = NULL: "derandomize" off).
-__global__ void __launch_bounds__(256) k_ldpc_gather(const int8_t *__restrict__ soft, const LdpcFrameRec *__restrict__ frames, int oqpsk,
+__global__ void __launch_bounds__(256) k_ldpc_gather(const int8_t *__restrict__ soft, const WalkFrame *__restrict__ frames, int oqpsk,
                                                       const unsigned char *__restrict__ pn, int8_t *__restrict__ vn)
 {
-    const LdpcFrameRec r = frames[blockIdx.x];
+    const WalkFrame r = frames[blockIdx.x];
     const int8_t *f = soft + r.off;
     int8_t *o = vn + (size_t)blockIdx.x * LDPC_VN;
     for (int t = threadIdx.x; t < LDPC_VN; t += blockDim.x) {
@@ -142,10 +71,10 @@ __global__ void __launch_bounds__(256) k_ldpc_gather(const int8_t *__restrict__ 
         const int c = t - LDPC_SHORT, k = LDPC_ASM + c; // code soft byte c = frame byte k
         int v;
         if (oqpsk) {
-            if (r.swap && (k & 1)) v = k + 2 < LDPC_F ? ldpc_rot(f, k + 2, r.phase, 0) : 0;
-            else v = ldpc_rot(f, k, r.phase, 0);
+            if (r.swap && (k & 1)) v = k + 2 < LDPC_F ? rot_soft(f, k + 2, r.phase, 0) : 0;
+            else v = rot_soft(f, k, r.phase, 0);
         } else
-            v = ldpc_rot(f, k, r.phase, r.swap);
+            v = rot_soft(f, k, r.phase, r.swap);
         if (pn && pn[c % 255]) v = ~v;
         o[t] = (int8_t)v;
     }
@@ -160,7 +89,7 @@ struct LdpcRowMsg { uint32_t sign, eq; uint16_t m1, m2; };
 
 __global__ void __launch_bounds__(LDPC_DEC_THREADS) k_ldpc_decode(const int8_t *__restrict__ vn_in, const uint16_t *__restrict__ cols,
                                                                    const int *__restrict__ level_ptr, const uint16_t *__restrict__ level_rows,
-                                                                   int nlevels, LdpcFrameRec *__restrict__ frames, uint8_t *__restrict__ cadu)
+                                                                   int nlevels, WalkFrame *__restrict__ frames, uint8_t *__restrict__ cadu)
 {
     extern __shared__ __align__(16) unsigned char smem[];
     int16_t *v = reinterpret_cast<int16_t *>(smem);

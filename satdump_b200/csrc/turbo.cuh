@@ -1,5 +1,5 @@
 // Kernels of ccsds_turbo_decoder (module_ccsds_turbo_decoder.cpp:137-235, CCSDSTurbo::decode and the deepspace-turbo log-MAP BCJR).
-// Included by api_turbo.cu only. The frame walk is k_ldpc_walk (ldpc.cuh), launched through frame_walk() of api_ldpc.cu.
+// Included by api_turbo.cu only. The frame walk is the LDPC decoder's, k_frame_walk<CorrWindow> of walk.cuh.
 //   k_turbo_corr    the module's correlator: |dot(soft[i .. i+ASM-1] / 127, asm table)| and its sign at every position + block maxima
 //   k_turbo_gather  the frame as the module's buffer holds it (shift quirk), derand_ccsds_soft, / 127, sign fix, depuncturing, and the
 //                   serial-to-parallel split into the upper and lower code streams; the a-priori values start at log(0.5)
@@ -8,8 +8,7 @@
 //   k_turbo_pack    the decided bits as bytes behind the ASM, the CRC-16 check
 //   k_turbo_compact the CADUs whose CRC passes, in stream order
 #pragma once
-#include <cuda_runtime.h>
-#include <stdint.h>
+#include "walk.cuh"
 
 constexpr int TURBO_STATES = 16, TURBO_MEM = 4;  // 4 shift registers (backward connections "0011")
 constexpr int TURBO_REC_THREADS = 128;           // 4 warps: 2 frames per warp, one direction per warp
@@ -96,7 +95,7 @@ __global__ void __launch_bounds__(256) k_turbo_corr(const int8_t *__restrict__ s
     }
     float v = i < npos ? v0 : -INFINITY;
     int vi = (int)i;
-    ldpc_best_warp(v, vi);
+    first_max_warp(v, vi);
     const long b = i >> 5;
     if ((threadIdx.x & 31) == 0 && (b + 1) * 32 <= npos) {
         bval[b] = v;
@@ -119,11 +118,11 @@ struct TurboGeom
 // derand_ccsds_soft over the codeword (~x where the sequence has a one), / 127, the sign flip when swapped, and CCSDSTurbo::decode's
 // depuncturing (zeros at the punctured places) and turbo_decode's serial-to-parallel split: block b of cu + cl values feeds upper[b cu ..]
 // and lower[b cl ..]. The a-priori values of the frame start at log(0.5).
-__global__ void __launch_bounds__(256) k_turbo_gather(const int8_t *__restrict__ soft, const LdpcFrameRec *__restrict__ frames, TurboGeom G,
+__global__ void __launch_bounds__(256) k_turbo_gather(const int8_t *__restrict__ soft, const WalkFrame *__restrict__ frames, TurboGeom G,
                                                        const unsigned char *__restrict__ pn, float *__restrict__ recv, double *__restrict__ msg,
                                                        double ln_half)
 {
-    const LdpcFrameRec r = frames[blockIdx.x];
+    const WalkFrame r = frames[blockIdx.x];
     const int8_t *cur = soft + r.off, *stale = soft + (r.off - r.pos);
     float *up = recv + (size_t)blockIdx.x * G.recv_stride, *lo = up + (size_t)G.cu * G.N;
     auto in = [&](int c) { // codeword value c as the decoder reads it
@@ -270,7 +269,7 @@ __global__ void __launch_bounds__(TURBO_EXT_THREADS) k_turbo_ext(const float *__
 
 // One CTA per frame: the K decided bits as base bytes behind 1A CF FC 1D, and GenericCRC(16, 0x1021, 0xFFFF, 0, false, false) over the
 // first base - 2 of them against the last two (big endian). The result goes to the frame record's `corr` field (1 = the CRC passes).
-__global__ void __launch_bounds__(256) k_turbo_pack(const unsigned char *__restrict__ bits, int base, LdpcFrameRec *__restrict__ frames,
+__global__ void __launch_bounds__(256) k_turbo_pack(const unsigned char *__restrict__ bits, int base, WalkFrame *__restrict__ frames,
                                                      uint8_t *__restrict__ cadu)
 {
     extern __shared__ uint8_t sb[];
@@ -299,7 +298,7 @@ __global__ void __launch_bounds__(256) k_turbo_pack(const unsigned char *__restr
 }
 
 // One CTA per frame: a frame whose CRC passes goes to slot (frames before it that pass) of `out`
-__global__ void __launch_bounds__(256) k_turbo_compact(const uint8_t *__restrict__ cadu, const LdpcFrameRec *__restrict__ frames, int bytes,
+__global__ void __launch_bounds__(256) k_turbo_compact(const uint8_t *__restrict__ cadu, const WalkFrame *__restrict__ frames, int bytes,
                                                         uint8_t *__restrict__ out)
 {
     if (!frames[blockIdx.x].corr)

@@ -18,6 +18,7 @@
  *                    src-core/pipeline/modules/ccsds/module_ccsds_ldpc_decoder.cpp:134-277       (kind LDPC, ldpc_rate "7/8")
  *                    src-core/pipeline/modules/ccsds/module_ccsds_turbo_decoder.cpp:137-235      (kind TURBO)
  *                    plugins/noaa_metop_support/metop/module_metop_dump_decoder.cpp:27-83        (kind METOP_DUMP)
+ *                    plugins/meteor_support/meteor/module_meteor_lrpt_decoder.cpp:101-262        (kind METEOR_LRPT)
  *   b200_chain_*   both modules joined the way Pipeline::run joins them with a byte FIFO
  *                    src-core/pipeline/pipeline_run.cpp:44-117 — here the int8 soft stream never leaves HBM.
  *   b200_demux_*   the step behind the decoder: CADUs -> CCSDS space packets
@@ -48,7 +49,8 @@ enum { B200_BPSK = 0, B200_QPSK = 1, B200_OQPSK = 2, B200_8PSK = 3, B200_NONE = 
 /* baseband_format (common/dsp/io/baseband_type.h:7-21) */
 enum { B200_CF32 = 0, B200_CS16 = 1, B200_CS8 = 2 };
 /* decoder kind */
-enum { B200_FEC_METOP = 0, B200_FEC_CCSDS = 1, B200_FEC_SIMPLE = 2, B200_FEC_LDPC = 3, B200_FEC_TURBO = 4, B200_FEC_METOP_DUMP = 5 };
+enum { B200_FEC_METOP = 0, B200_FEC_CCSDS = 1, B200_FEC_SIMPLE = 2, B200_FEC_LDPC = 3, B200_FEC_TURBO = 4, B200_FEC_METOP_DUMP = 5,
+       B200_FEC_METEOR_LRPT = 6 };
 /* debug stage ids for b200_demod_debug_stage */
 enum { B200_STAGE_AGC = 0, B200_STAGE_FIR = 1, B200_STAGE_COSTAS = 2, B200_STAGE_RESAMP = 3, B200_STAGE_DC = 4, B200_STAGE_MM = 5,
        B200_STAGE_PLL = 6 /* pm_demod: PLLCarrierTrackingBlock output */, B200_STAGE_PM = 7 /* pm_demod: PMToBPSK output */ };
@@ -147,6 +149,22 @@ typedef struct b200_fec_cfg
        swap, hard bits) over 8192-soft-byte frames, phase fix, hard decisions, inversion, derandomiser, RS(255,223) I=4 dual basis; every
        frame is written as 1A CF FC 1D + 1020 bytes, whatever RS returned. Only device and max_soft are read. Device memory: about 3 bytes
        per max_soft byte (FIFO, hard bits, correlator scores) plus 2 KiB of CADUs per 8192 soft bytes.                                 */
+    /* kind B200_FEC_METEOR_LRPT = meteor_lrpt_decoder (module_meteor_lrpt_decoder.cpp:22-49), two modes:
+       m2x_mode 0: Correlator on the 64-bit QPSK ASM (0xfca2b63db00d9794, or 0xfc4ef4fd0cc2df89 with diff_decode; 8 syncwords: 4 phases x
+         IQ swap, hard bits) over 16384-soft-byte frames, phase fix, Viterbi27 (one r=1/2 k=7 CCDecoder of 8192 bits per frame, chained
+         across frames), NRZ-M on the bytes when diff_decode, derandomiser, inversion when byte 9 is 0xFF, RS(255,223) I=4 in the
+         conventional basis; the frames whose four codewords decode are written as 1D CF FC 1D + 1020 bytes. Only diff_decode, device
+         and max_soft are read. Device memory: about 9 bytes per max_soft byte (FIFO, hard bits, correlator scores, the rotated frames,
+         the Viterbi decisions), so max_soft = 2^28 (the limit) takes about 2.3 GiB.
+       m2x_mode 1: the module's Viterbi1_2 (phases 0 and 90 degrees, IQ-swap check) -> NRZ-M bits when diff_decode -> BPSK_CCSDS_Deframer
+         (8192) -> derandomiser -> RS(255,223) I=4 in the conventional basis, writing the frames whose four codewords decode: exactly
+         ccsds_conv_concat_decoder with constellation "oqpsk", cadu_size 8192, nrzm = diff_decode, rs_i 4, rs_dualbasis false and
+         rs_usecheck, and run by that decoder. outsync_after and ber_thresold are required ("viterbi_outsync_after",
+         "viterbi_ber_thresold"). interleaved is refused (B200_EUNSUPPORTED): the reference's reader of that mode never delivers a
+         sample, so there is no behaviour to reproduce. */
+    int diff_decode;          /* "diff_decode" (required by the module)                                                                    */
+    int m2x_mode;             /* "m2x_mode", default false                                                                                 */
+    int interleaved;          /* "interleaved" (m2x_mode only), default false: refused                                                     */
 } b200_fec_cfg;
 
 typedef struct b200_demod_stats
@@ -193,6 +211,11 @@ typedef struct b200_fec_stats
        ldpc_resyncs the frames whose pos was not 0, rs_corrected / rs_failed above its RS results */
     long crc_ok, crc_fail;    /* frames so far whose CRC-16 passed (written) / failed ("CRC Check" PASS / FAIL)                        */
     long turbo_near_ties;     /* decisions so far whose margin |one - zero| was below 1e-9 (where libm rounding could tip a bit)       */
+    /* meteor_lrpt_decoder: "rs_avg" = (errors[0] + errors[1] + errors[2] + errors[3]) / 4 of the last frame decoded (0 before the first).
+       m2x_mode 0: correlator_lock ("correlator_lock", "lock_state"), correlator_corr (0..64), ldpc_resyncs (frames whose pos was not 0),
+       viterbi_ber (Viterbi27's BER of the last frame) and rs_corrected / rs_failed above; m2x_mode 1: the keys of
+       ccsds_conv_concat_decoder above */
+    int rs_avg;
 } b200_fec_stats;
 
 typedef struct b200_demod b200_demod;
@@ -313,6 +336,17 @@ typedef struct b200_dump_frame
     int rs[4];                /* decode_interlaved's errors[] of the four codewords: -1 = not decodable, else bytes corrected       */
 } b200_dump_frame;
 int b200_fec_debug_dump_frames(b200_fec *f, b200_dump_frame *out, long cap, long *n_out);
+/* meteor_lrpt_decoder with m2x_mode 0: one record per frame of the LAST push, in stream order (frames dropped by RS included) */
+typedef struct b200_meteor_frame
+{
+    long offset;              /* stream offset (soft bytes since create / reset) of the frame's first byte (after the shift)          */
+    int pos;                  /* the correlator's position in the window read before it (0 = locked)                                */
+    int corr;                 /* the correlator's value (0..64)                                                                    */
+    int phase, swap;          /* the phase ambiguity fixed (0..3 = 0, 90, 180, 270 degrees) and the IQ swap                        */
+    int rs[4];                /* decode_interlaved's errors[] of the four codewords: -1 = not decodable, else bytes corrected       */
+    float ber;                /* Viterbi27's BER of the frame                                                                      */
+} b200_meteor_frame;
+int b200_fec_debug_meteor_frames(b200_fec *f, b200_meteor_frame *out, long cap, long *n_out);
 
 /* ---- fused chain: raw IQ -> CADUs, soft stream stays in HBM ---------------------------------------- */
 b200_chain *b200_chain_create(const b200_demod_cfg *dcfg, const b200_fec_cfg *fcfg);

@@ -6,7 +6,7 @@
 //
 //   loader()                          the one symbol SatDump dlsym()s (core/plugin.cpp:15-33)
 //   B200DSPSupport::init()            on SatDumpStartedEvent (fired after every plugin registered its modules, init.cpp:163) the
-//                                     entries "psk_demod", "pm_demod", "metop_ahrpt_decoder", "ccsds_conv_concat_decoder", "ccsds_simple_psk_decoder", "ccsds_ldpc_decoder", "ccsds_turbo_decoder" and "metop_dump_decoder" of
+//                                     entries "psk_demod", "pm_demod", "metop_ahrpt_decoder", "ccsds_conv_concat_decoder", "ccsds_simple_psk_decoder", "ccsds_ldpc_decoder", "ccsds_turbo_decoder", "metop_dump_decoder" and "meteor_lrpt_decoder" of
 //                                     satdump::pipeline::modules_registry (module.h:210, looked up first-match by id, module.cpp:129-135)
 //                                     get their factory replaced, so existing pipelines instantiate the CUDA modules.
 //                                     Set B200_DSP_REGISTER_ONLY=1 to register "<id>_b200" ids instead and leave the originals alone.
@@ -233,6 +233,16 @@ namespace b200plugin
                 v["lock_state"] = stage->correlator_lock.load() ? "SYNCED" : "NOSYNC";
                 return v;
             }
+            if (stage->getID() == "meteor_lrpt_decoder" && !stage->cfg.m2x_mode) // METEORLRPTDecoderModule::getModuleStats (:282-287)
+            {
+                v["correlator_lock"] = stage->correlator_lock.load() != 0;
+                v["viterbi_ber"] = stage->viterbi_ber.load();
+                v["rs_avg"] = stage->rs_avg.load();
+                v["lock_state"] = stage->correlator_lock.load() ? "SYNCED" : "NOSYNC";
+                return v;
+            }
+            if (stage->getID() == "meteor_lrpt_decoder") // m2x_mode (:271-278): ccsds_conv_concat_decoder's keys below, and rs_avg
+                v["rs_avg"] = stage->rs_avg.load();
             // keys of MetOpAHRPTDecoderModule::getModuleStats (module_metop_ahrpt_decoder.cpp:92-104)
             v["deframer_lock"] = stage->deframer_state.load() > 6;
             v["viterbi_ber"] = stage->viterbi_ber.load();
@@ -269,7 +279,7 @@ public:
     static void registerHandler(const satdump::pipeline::RegisterModulesEvent &evt)
     {
         for (const char *id : {"psk_demod", "pm_demod", "metop_ahrpt_decoder", "ccsds_conv_concat_decoder", "ccsds_simple_psk_decoder", "ccsds_ldpc_decoder",
-                               "ccsds_turbo_decoder", "metop_dump_decoder"})
+                               "ccsds_turbo_decoder", "metop_dump_decoder", "meteor_lrpt_decoder"})
             evt.modules_registry.push_back({std::string(id) + "_b200", nlohmann::json(), factory(id)});
     }
 
@@ -277,7 +287,8 @@ public:
     {
         for (auto &e : satdump::pipeline::modules_registry)
             if (e.id == "psk_demod" || e.id == "pm_demod" || e.id == "metop_ahrpt_decoder" || e.id == "ccsds_conv_concat_decoder" || e.id == "ccsds_simple_psk_decoder" ||
-                e.id == "ccsds_ldpc_decoder" || e.id == "ccsds_turbo_decoder" || e.id == "metop_dump_decoder")
+                e.id == "ccsds_ldpc_decoder" || e.id == "ccsds_turbo_decoder" || e.id == "metop_dump_decoder" ||
+                e.id == "meteor_lrpt_decoder")
             {
                 e.inst = factory(e.id);
                 logger->info("b200_dsp_support: module " + e.id + " now runs on the B200 path");

@@ -25,7 +25,7 @@ SYMBOLS = [
     "b200_demod_pull_symbols", "b200_demod_debug_stage", "b200_demod_debug_convert", "b200_demod_debug_run_stage", "b200_demod_debug_junctions", "b200_demod_debug_repair_merge", "b200_demod_debug_loop_cycles", "b200_demod_reset", "b200_demod_prefetch_iq", "b200_demod_last_timing", "b200_demod_get_stats", "b200_demod_get_taps",
     "b200_fec_create", "b200_fec_destroy", "b200_fec_push_soft", "b200_fec_push_soft_device", "b200_fec_pull_frames",
     "b200_fec_debug_bits", "b200_fec_get_stats", "b200_fec_cadu_bytes", "b200_fec_chunk_size", "b200_fec_debug_ldpc_frames", "b200_fec_ldpc_timing",
-    "b200_fec_debug_turbo_frames", "b200_fec_debug_turbo_llr", "b200_fec_turbo_timing", "b200_fec_debug_dump_frames",
+    "b200_fec_debug_turbo_frames", "b200_fec_debug_turbo_llr", "b200_fec_turbo_timing", "b200_fec_debug_dump_frames", "b200_fec_debug_meteor_frames",
     "b200_chain_create", "b200_chain_destroy", "b200_chain_push_iq", "b200_chain_push_iq_device", "b200_chain_prefetch_iq", "b200_chain_pull_frames",
     "b200_chain_frames_device", "b200_chain_get_stats", "b200_chain_last_timing", "b200_chain_reset",
     "b200_chain_set_pipelined", "b200_chain_sync", "b200_chain_span_begin", "b200_chain_span_end",
@@ -53,7 +53,8 @@ class FecCfg(C.Structure):
                 ("rs_usecheck", C.c_int), ("rs_type", C.c_int), ("iq_invert", C.c_int), ("asm_sync", C.c_uint),
                 ("device", C.c_int), ("max_soft", C.c_long), ("qpsk_swap_iq", C.c_int), ("qpsk_swap_diff", C.c_int), ("oqpsk_delay", C.c_int), ("conv_rate", C.c_int),
                 ("ldpc_rate", C.c_int), ("ldpc_block_size", C.c_int), ("ldpc_iterations", C.c_int), ("ldpc2", C.c_int), ("internal_stream", C.c_int),
-                ("internal_cadu_size", C.c_int), ("turbo_rate", C.c_int), ("turbo_base", C.c_int), ("turbo_iters", C.c_int)]
+                ("internal_cadu_size", C.c_int), ("turbo_rate", C.c_int), ("turbo_base", C.c_int), ("turbo_iters", C.c_int),
+                ("diff_decode", C.c_int), ("m2x_mode", C.c_int), ("interleaved", C.c_int)]
 
 
 class DemuxCfg(C.Structure):
@@ -83,7 +84,7 @@ class FecStats(C.Structure):
                 ("rs_failed", C.c_long), ("replays", C.c_long), ("kernel_launches", C.c_long), ("start_redone", C.c_long), ("tb_serial", C.c_long),
                 ("spec_steps", C.c_int), ("tb_overlap", C.c_int),
                 ("correlator_lock", C.c_int), ("correlator_corr", C.c_float), ("ldpc_corr", C.c_int), ("ldpc_resyncs", C.c_long),
-                ("crc_ok", C.c_long), ("crc_fail", C.c_long), ("turbo_near_ties", C.c_long)]
+                ("crc_ok", C.c_long), ("crc_fail", C.c_long), ("turbo_near_ties", C.c_long), ("rs_avg", C.c_int)]
 
 
 class LdpcFrame(C.Structure):
@@ -96,6 +97,11 @@ class TurboFrame(C.Structure):
 
 class DumpFrame(C.Structure):
     _fields_ = [("offset", C.c_long), ("pos", C.c_int), ("corr", C.c_int), ("phase", C.c_int), ("swap", C.c_int), ("rs", C.c_int * 4)]
+
+
+class MeteorFrame(C.Structure):
+    _fields_ = [("offset", C.c_long), ("pos", C.c_int), ("corr", C.c_int), ("phase", C.c_int), ("swap", C.c_int), ("rs", C.c_int * 4),
+                ("ber", C.c_float)]
 
 
 class B200Error(RuntimeError):
@@ -152,6 +158,7 @@ def lib():
         L.b200_fec_turbo_timing.argtypes = [vp, vp, ci]
         L.b200_fec_debug_turbo_llr.argtypes = [vp, cl, vp, vp, cl, C.POINTER(cl)]
         L.b200_fec_debug_dump_frames.argtypes = [vp, C.POINTER(DumpFrame), cl, C.POINTER(cl)]
+        L.b200_fec_debug_meteor_frames.argtypes = [vp, C.POINTER(MeteorFrame), cl, C.POINTER(cl)]
         L.b200_chain_create.restype = vp
         L.b200_chain_create.argtypes = [C.POINTER(DemodCfg), C.POINTER(FecCfg)]
         L.b200_chain_destroy.argtypes = [vp]
@@ -303,6 +310,24 @@ def dump_cfg(device=0, max_soft=1 << 24):
     return cfg
 
 
+def meteor_lrpt_cfg(diff_decode=None, m2x_mode=False, viterbi_outsync_after=None, viterbi_ber_thresold=None, interleaved=False, device=0,
+                    max_soft=1 << 24):
+    """meteor_lrpt_decoder (module_meteor_lrpt_decoder.cpp:22-49): diff_decode is required; with m2x_mode, viterbi_outsync_after and
+    viterbi_ber_thresold are required too, as the module's constructor asks. The library refuses interleaved (not built) by name."""
+    if diff_decode is None:
+        raise ValueError("meteor_lrpt_decoder: diff_decode is required")
+    cfg = FecCfg()
+    cfg.kind, cfg.constellation, cfg.cadu_size, cfg.device, cfg.max_soft = 6, CONST["qpsk"], 8192, device, max_soft
+    cfg.diff_decode, cfg.m2x_mode, cfg.interleaved = int(bool(diff_decode)), int(bool(m2x_mode)), int(bool(interleaved))
+    if m2x_mode:
+        if viterbi_outsync_after is None:
+            raise ValueError("meteor_lrpt_decoder: viterbi_outsync_after is required with m2x_mode")
+        if viterbi_ber_thresold is None:
+            raise ValueError("meteor_lrpt_decoder: viterbi_ber_thresold is required with m2x_mode")
+        cfg.outsync_after, cfg.ber_thresold = int(viterbi_outsync_after), float(viterbi_ber_thresold)
+    return cfg
+
+
 def fec_cfg_for(sig, max_soft, device=0):
     """The decoder configuration that goes with a satdump_b200.synth.SignalCfg (metop_ahrpt_decoder / ccsds_conv_concat_decoder /
     ccsds_simple_psk_decoder parameters of the shipped pipeline JSONs)."""
@@ -310,6 +335,8 @@ def fec_cfg_for(sig, max_soft, device=0):
         return metop_cfg(sig.ber_thresold, sig.outsync_after, device=device, max_soft=max_soft)
     if sig.decoder == "dump":
         return dump_cfg(device=device, max_soft=max_soft)
+    if sig.decoder == "meteor":
+        return meteor_lrpt_cfg(sig.nrzm, device=device, max_soft=max_soft)
     if sig.decoder == "turbo":
         return turbo_cfg(sig.turbo_rate, sig.turbo_base, sig.turbo_iters, device=device, max_soft=max_soft)
     if sig.decoder == "ldpc":
@@ -538,6 +565,19 @@ class Fec:
         for k in range(n.value):
             r = recs[k]
             out[k] = [r.offset, r.pos, r.corr, r.phase, r.swap, *r.rs]
+        return out
+
+    def meteor_frames(self):
+        """meteor_lrpt_decoder (m2x_mode false): one record per frame of the last push as int64 [n, 10] = offset, pos, corr, phase, swap,
+        rs[0..3], ber (float32 bits) (oracle.meteor.REC)."""
+        cap = int(self._n) // 16384 + 4
+        recs = (MeteorFrame * cap)()
+        n = C.c_long(0)
+        _chk(lib().b200_fec_debug_meteor_frames(self.h, recs, cap, C.byref(n)))
+        out = np.zeros((n.value, 10), np.int64)
+        for k in range(n.value):
+            r = recs[k]
+            out[k] = [r.offset, r.pos, r.corr, r.phase, r.swap, *r.rs, int(np.float32(r.ber).view(np.uint32))]
         return out
 
     def turbo_llr(self, frame, K):

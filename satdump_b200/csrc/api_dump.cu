@@ -69,7 +69,7 @@ void Dump::process(Fec &f)
     cudaStream_t stream = f.stream;
     const long have = f.soft_have, nwords = (have + 31) / 32 + 2, nq = (have - 32) / 2 + 1;
     B200_CUDA(cudaEventRecord(f.ev[0], stream));
-    k_dump_pack<<<(unsigned)((nwords * 32 + 255) / 256), 256, 0, stream>>>(f.softbuf.p, have, nwords, hw.p);
+    k_hard_pack<0><<<(unsigned)((nwords * 32 + 255) / 256), 256, 0, stream>>>(f.softbuf.p, have, nwords, hw.p);
     k_dump_corr<<<(unsigned)((nq + 255) / 256), 256, 0, stream>>>(hw.p, nq, sw, score.p, bsync.p, bval.p, bidx.p);
     const DumpWindow win{hw.p, score.p, bsync.p, bval.p, bidx.p, sw};
     k_frame_walk<<<1, WALK_WARPS * 32, 0, stream>>>(win, have, DUMP_F, frames.p, (int)max_frames, walk.p);

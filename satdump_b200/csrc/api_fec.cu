@@ -59,10 +59,41 @@ void ccsds_pn_bits(unsigned char *pn)
         pn[i] = (unsigned char)pn_step(reg);
 }
 
-Fec::Fec(const b200_fec_cfg &c) : cfg(c)
+// meteor_lrpt_decoder with m2x_mode (module_meteor_lrpt_decoder.cpp:29-43, 103-197) is ccsds_conv_concat_decoder with constellation
+// "oqpsk" (Viterbi1_2 over 8192-byte calls, phases 0 and 90, the IQ-swap check), NRZ-M bits when diff_decode, BPSK_CCSDS_Deframer(8192),
+// the derandomiser from byte 4 before RS, RS223 I=4 in the conventional basis and only the frames whose four codewords decode written:
+// that configuration, run as kind CCSDS. Every other configuration passes unchanged.
+static b200_fec_cfg meteor_m2x_as_ccsds(const b200_fec_cfg &c)
 {
+    if (c.kind != B200_FEC_METEOR_LRPT || !c.m2x_mode)
+        return c;
+    B200_REQUIRE(!c.interleaved, B200_EUNSUPPORTED,
+                 "meteor_lrpt_decoder: \"interleaved\" is not built: the reference's interleaved reader never delivers a sample (its input "
+                 "function always reports failure), so there is no behaviour to reproduce");
+    b200_fec_cfg r = c;
+    r.kind = B200_FEC_CCSDS;
+    r.constellation = B200_OQPSK;
+    r.cadu_size = 8192;
+    r.conv_rate = 0;
+    r.nrzm = c.diff_decode != 0;
+    r.derandomize = 1;
+    r.derand_after_rs = 0;
+    r.derand_start = 4;
+    r.rs_i = 4;
+    r.rs_dualbasis = 0;
+    r.rs_fill_bytes = -1;
+    r.rs_usecheck = 1;
+    r.rs_type = 0;
+    r.iq_invert = 0;
+    r.asm_sync = 0x1ACFFC1D;
+    return r;
+}
+
+Fec::Fec(const b200_fec_cfg &in) : cfg(meteor_m2x_as_ccsds(in))
+{
+    const b200_fec_cfg c = cfg;
     B200_REQUIRE(c.kind == B200_FEC_METOP || c.kind == B200_FEC_CCSDS || c.kind == B200_FEC_SIMPLE || c.kind == B200_FEC_LDPC || c.kind == B200_FEC_TURBO ||
-                     c.kind == B200_FEC_METOP_DUMP,
+                     c.kind == B200_FEC_METOP_DUMP || c.kind == B200_FEC_METEOR_LRPT,
                  B200_EINVAL, "unknown decoder kind %d", c.kind);
     B200_REQUIRE(c.max_soft >= 65536, B200_EINVAL, "max_soft must be >= 65536");
     memset(&geom, 0, sizeof(geom));
@@ -72,6 +103,8 @@ Fec::Fec(const b200_fec_cfg &c) : cfg(c)
         framed = turbo_decoder(*this);
     else if (c.kind == B200_FEC_METOP_DUMP)
         framed = dump_decoder(*this);
+    else if (c.kind == B200_FEC_METEOR_LRPT)
+        framed = meteor_decoder(*this);
     if (framed)
         return;
     if (c.kind != B200_FEC_METOP) {
@@ -330,6 +363,35 @@ static void decode_range(Fec &f, const int8_t *src, long c, int n, long out_base
     }
 }
 
+void viterbi_chained(Fec &f, const int8_t *src, long n, int *ber_errors)
+{
+    long c = 0;
+    while (c < n) {
+        const int m = (int)(n - c);
+        decode_range(f, src, c, m, c, 6); // (what is still inconsistent after six rounds is decoded again below)
+        int accepted = m;
+        for (int i = 1; i < m; i++)
+            if (f.h_rec.p[i].start_used != f.h_rec.p[i - 1].next_start) {
+                f.replays++;
+                accepted = i;
+                break;
+            }
+        for (int i = 0; i < accepted; i++)
+            ber_errors[c + i] = f.h_rec.p[i].ber_errors;
+        f.main_next_start = f.h_rec.p[accepted - 1].next_start;
+        f.enc_state = f.h_rec.p[accepted - 1].enc_tail;
+        c += accepted;
+    }
+}
+
+void rs_usecheck_compact(Fec &f, const uint8_t *in, int nf, int rs_i, uint8_t *out)
+{
+    k_frames_filter<<<1, 1024, 0, f.stream>>>(f.rs_err.p, nf, rs_i, f.frame_dst.p, f.counters.p + 2);
+    k_frames_gather<<<std::min(nf, 132 * 16), 256, 0, f.stream>>>(in, f.frame_dst.p, nf, f.cadu_bytes, out);
+    f.launches += 2;
+    B200_CUDA(cudaMemcpyAsync(f.h_counters.p + 2, f.counters.p + 2, sizeof(int), cudaMemcpyDeviceToHost, f.stream));
+}
+
 // Viterbi over soft chunks [c0, nch): lock search while IDLE, optimistic parallel decode while SYNCED. Decoded chunks land in
 // chunk_bits[0 .. nout). Returns per-output-chunk bookkeeping in `outs`.
 static void viterbi_segment(Fec &f, long c0, long nch, std::vector<OutChunk> &outs)
@@ -576,6 +638,10 @@ void Fec::deframe_and_rs(long new_bits)
             else
                 rs_corrected += h_rs_err.p[i];
         }
+        if (cfg.rs_i == 4) {
+            const int *e = h_rs_err.p + (long)(nf - 1) * 4;
+            rs_avg = (e[0] + e[1] + e[2] + e[3]) / 4;
+        }
         out_frames += kept;
         total_frames += kept;
     }
@@ -607,6 +673,7 @@ void Fec::start_stream(size_t fifo_bytes)
     idle_st = VitIdleState{-1, 0};
     last_ber = 10.f;
     defr_state_now = 2;
+    rs_avg = 0;
     out_frames = 0;
     last_bits0 = last_nbits = 0;
     B200_CUDA(cudaMemsetAsync(fifo.p, 0, fifo_bytes, stream));
@@ -1044,6 +1111,7 @@ void Fec::stats(b200_fec_stats *o)
     o->spec_steps = spec_steps;
     o->tb_overlap = tb_overlap;
     o->kernel_launches = launches;
+    o->rs_avg = rs_avg;
     if (framed)
         framed->stats(o);
 }
@@ -1158,6 +1226,13 @@ int b200_fec_debug_dump_frames(b200_fec *h, b200_dump_frame *out, long cap, long
     return guarded([&] {
         B200_REQUIRE(h && out && n_out, B200_EINVAL, "NULL argument");
         *n_out = h->f->dump_frames(out, cap);
+    });
+}
+int b200_fec_debug_meteor_frames(b200_fec *h, b200_meteor_frame *out, long cap, long *n_out)
+{
+    return guarded([&] {
+        B200_REQUIRE(h && out && n_out, B200_EINVAL, "NULL argument");
+        *n_out = h->f->meteor_frames(out, cap);
     });
 }
 int b200_fec_turbo_timing(b200_fec *h, float *ms_out, int n)

@@ -1,7 +1,7 @@
 // Kernels of metop_dump_decoder (plugins/noaa_metop_support/metop/module_metop_dump_decoder.cpp:27-83, the MetOp X-band dump): no
 // convolutional code, Correlator32(QPSK, 0x1ACFFC1D) (src-core/common/codings/correlator32.cpp) on 8192-soft-byte windows, RS(255,223) I=4
 // dual basis. Included by api_dump.cu only.
-//   k_dump_pack    the hard bits soft >= 0 of the FIFO, MSB first in 32-bit words (the correlator's hard_buf)
+//   k_hard_pack<0> (walk.cuh) the hard bits soft >= 0 of the FIFO, MSB first in 32-bit words (the correlator's hard_buf)
 //   k_dump_corr    the correlation (32 - Hamming distance) of the 8 syncwords at every even position + the maxima of 32-position blocks
 //   DumpWindow     the module's window for k_frame_walk (walk.cuh): the position-0 early accept, the first maximum, the tail past 8192 bits
 //   k_dump_frames  one CTA per frame: the module's buffer after the shift, rotate_soft, hard decisions, inversion, derandomiser, RS, CADU
@@ -41,15 +41,6 @@ __device__ __forceinline__ uint32_t dump_word(const uint32_t *__restrict__ hw, l
     const long w = b >> 5;
     const int o = (int)(b & 31);
     return o ? (hw[w] << o) | (hw[w + 1] >> (32 - o)) : hw[w];
-}
-
-// word w of the hard-bit FIFO = the signs (soft >= 0, correlator32.cpp:75-89) of soft bytes 32w .. 32w+31; bytes at or past `have` are 0
-__global__ void __launch_bounds__(256) k_dump_pack(const int8_t *__restrict__ soft, long have, long nwords, uint32_t *__restrict__ hw)
-{
-    const long j = (long)blockIdx.x * blockDim.x + threadIdx.x;
-    const unsigned bits = __ballot_sync(0xffffffffu, j < have && soft[j] >= 0);
-    if ((threadIdx.x & 31) == 0 && (j >> 5) < nwords)
-        hw[j >> 5] = __brev(bits);
 }
 
 // Score of every even position 2q, q < nq: the best correlation of the 8 syncwords with the 32 hard bits there and the first syncword that

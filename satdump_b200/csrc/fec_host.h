@@ -15,10 +15,10 @@ namespace b200
 struct DefrEvent { long pos; int state; int pad; };
 class Fec;
 
-// The stream state of a correlator-driven decoder (ccsds_ldpc_decoder, ccsds_turbo_decoder, metop_dump_decoder): a correlator scores
+// The stream state of a correlator-driven decoder (ccsds_ldpc_decoder, ccsds_turbo_decoder, metop_dump_decoder, meteor_lrpt_decoder): a correlator scores
 // every position of the soft FIFO, k_frame_walk (walk.cuh) goes o -> o + pos + F over its windows, the frames are decoded, and the
-// FIFO keeps the bytes behind the walk's next window. Each decoder derives from it (Ldpc, Turbo, Dump in api_ldpc.cu, api_turbo.cu,
-// api_dump.cu); its process() reads begin -> correlate -> walk -> walked -> decode -> keep_soft_tail -> timings -> finish.
+// FIFO keeps the bytes behind the walk's next window. Each decoder derives from it (Ldpc, Turbo, Dump, Meteor in api_ldpc.cu, api_turbo.cu,
+// api_dump.cu, api_meteor.cu); its process() reads begin -> correlate -> walk -> walked -> decode -> keep_soft_tail -> timings -> finish.
 struct Framed
 {
     DevBuf<float> score, bval;        // the correlator's score at every position, the maxima of 32-position blocks
@@ -49,6 +49,7 @@ struct Framed
 std::unique_ptr<Framed> ldpc_decoder(Fec &f);
 std::unique_ptr<Framed> turbo_decoder(Fec &f);
 std::unique_ptr<Framed> dump_decoder(Fec &f);
+std::unique_ptr<Framed> meteor_decoder(Fec &f);
 
 class Fec
 {
@@ -89,6 +90,7 @@ class Fec
     long turbo_llr(long frame, double *app0, double *app1, long cap);
     void turbo_timing(float *ms, int n);
     long dump_frames(b200_dump_frame *out, long cap); // records of the last push
+    long meteor_frames(b200_meteor_frame *out, long cap); // records of the last push
 
     // device storage
     DevBuf<int8_t> softbuf;
@@ -156,6 +158,7 @@ class Fec
     VitIdleState idle_st{-1, 0};
     float last_ber = 10.f;
     int defr_state_now = 2;
+    int rs_avg = 0; // (errors[0] + .. + errors[3]) / 4 of the last frame with rs_i = 4 (meteor_lrpt_decoder's "rs_avg")
     long out_frames = 0; // frames waiting in frames_out
     long last_bits0 = 0, last_nbits = 0; // FIFO range of the bits appended by the last process() (debug)
     // statistics
@@ -165,6 +168,7 @@ class Fec
     friend struct Ldpc;
     friend struct Turbo;
     friend struct Dump;
+    friend struct Meteor;
     // the main deframer and the frame counters at a point a pass may have to roll back to
     struct Mark { DefrState h_dstate; long fifo_bits, out_frames, total_frames, rs_corrected, rs_failed; int defr_state_now; };
     Mark mark();
@@ -178,6 +182,13 @@ class Fec
     void framed_storage(int F, long frames_per_push); // what every Framed decoder needs of the decoder object (api_fec.cu)
     void deframer_storage(long max_new_bits); // bit FIFO, deframer and frame stage of LDPC's internal_stream (api_fec.cu)
 };
+
+// Viterbi27 (meteor_lrpt_decoder): the n chunks at src (geom.chunk bytes apart, already rotated) decoded as consecutive calls of ONE chained
+// CCDecoder and its BER encoder, with no lock machine. Chunk q's bits land in chunk_bits[q], its BER error count in ber_errors[q].
+void viterbi_chained(Fec &f, const int8_t *src, long n, int *ber_errors);
+// rs_usecheck on nf frames of cadu_bytes at `in` whose RS results are in f.rs_err: the frames whose rs_i codewords all decoded, in order,
+// to `out`; their number arrives in f.h_counters.p[2] (valid after the stream synchronises)
+void rs_usecheck_compact(Fec &f, const uint8_t *in, int nf, int rs_i, uint8_t *out);
 
 void build_rs_tables(RsTables &T);
 // the CCSDS sequence (x^8+x^7+x^5+x^3+1 from all ones), one bit per entry as derand_ccsds_soft applies it to soft bytes (255 entries)

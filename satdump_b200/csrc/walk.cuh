@@ -1,6 +1,6 @@
-// What the correlator-driven decoders (ccsds_ldpc_decoder, ccsds_turbo_decoder, metop_dump_decoder) share: the frame walk k_frame_walk
-// with its records, the first-maximum reductions over correlator scores, CorrWindow (the LDPC and turbo window; the dump window is
-// DumpWindow in dump.cuh) and rot_soft. Device code and types only, so that more than one translation unit may include it.
+// What the correlator-driven decoders (ccsds_ldpc_decoder, ccsds_turbo_decoder, metop_dump_decoder, meteor_lrpt_decoder) share: the frame
+// walk k_frame_walk with its records, the first-maximum reductions over correlator scores, CorrWindow (the LDPC and turbo window; the dump
+// window is DumpWindow in dump.cuh, the METEOR one Corr64Window in meteor.cuh), the hard-bit packer k_hard_pack and rot_soft. Device code and types only, so that more than one translation unit may include it.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -40,6 +40,21 @@ __device__ __forceinline__ void window_first_max(const float *__restrict__ score
     if (b1 >= b0 && t < e) first_max(v, vi, score[t], (int)t);
     first_max_warp(v, vi);
 }
+
+namespace b200
+{
+// Word w of a correlator's hard-bit FIFO = the hard decisions soft >= Thr of soft bytes 32w .. 32w+31, MSB first; bytes at or past `have`
+// are 0. Correlator32 decides soft >= 0 (Thr 0, correlator32.cpp:75-89), Correlator soft > 0 (Thr 1, correlator.cpp:75-89). (A template,
+// so that more than one translation unit may launch it.)
+template <int Thr>
+__global__ void __launch_bounds__(256) k_hard_pack(const int8_t *__restrict__ soft, long have, long nwords, uint32_t *__restrict__ hw)
+{
+    const long j = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    const unsigned bits = __ballot_sync(0xffffffffu, j < have && soft[j] >= Thr);
+    if ((threadIdx.x & 31) == 0 && (j >> 5) < nwords)
+        hw[j >> 5] = __brev(bits);
+}
+} // namespace b200
 
 // soft byte k (0 .. F-1) of a frame after rotate_soft(phase, swap) (rotation.cpp:4-63)
 __device__ __forceinline__ int rot_soft(const int8_t *__restrict__ f, int k, int phase, int swap)

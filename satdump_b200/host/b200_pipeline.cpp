@@ -10,7 +10,7 @@ using namespace b200host;
 int main(int argc, char **argv)
 {
     if (argc < 5) {
-        fprintf(stderr, "usage: %s <metop_ahrpt|jpss_hrd|npp_hrd|simple_bpsk|simple_qpsk|pm_bpsk|ldpc_qpsk|landsat|turbo_pm|turbo_bpsk|metop_dump> baseband <input> <output_hint> [--fused] [--key value ...]\n", argv[0]);
+        fprintf(stderr, "usage: %s <metop_ahrpt|jpss_hrd|npp_hrd|simple_bpsk|simple_qpsk|pm_bpsk|ldpc_qpsk|landsat|turbo_pm|turbo_bpsk|metop_dump|meteor_lrpt> baseband <input> <output_hint> [--fused] [--key value ...]\n", argv[0]);
         return 2;
     }
     const std::string pipe = argv[1], level = argv[2], in = argv[3], out = argv[4];
@@ -23,6 +23,10 @@ int main(int argc, char **argv)
     } else if (pipe == "metop_dump") { // resources/pipelines/MetOp.json "metop_dump": 35 Msym/s QPSK recorded at 45 MS/s
         dp = Params{{"constellation", "qpsk"}, {"symbolrate", "35000000"}, {"rrc_alpha", "0.5"}, {"pll_bw", "0.03"}};
         dec = "metop_dump_decoder";
+    } else if (pipe == "meteor_lrpt") { // resources/pipelines/Meteor-M.json "METEOR M2 LRPT 72k": QPSK at 72 ksym/s, 1 MS/s by default
+        dp = Params{{"constellation", "qpsk"}, {"symbolrate", "72000"}, {"rrc_alpha", "0.5"}, {"pll_bw", "0.002"}};
+        fp = Params{{"diff_decode", "false"}};
+        dec = "meteor_lrpt_decoder";
     } else if (pipe == "jpss_hrd" || pipe == "npp_hrd") { // resources/pipelines/JPSS.json
         dp = Params{{"constellation", "oqpsk"}, {"symbolrate", pipe == "jpss_hrd" ? "25000000" : "15000000"}, {"rrc_alpha", "0.5"}, {"pll_bw", "0.002"}};
         fp = Params{{"constellation", "oqpsk"}, {"cadu_size", "10232"}, {"viterbi_ber_thresold", "0.3"}, {"viterbi_outsync_after", "20"},
@@ -83,14 +87,14 @@ int main(int argc, char **argv)
             FusedStage m(dec, in, out, dp, fp);
             m.process();
             printf("wrote %s (%ld frames)\n", m.getOutput().c_str(), m.frames_written.load());
-            if (dec == "metop_dump_decoder")
+            if (dec == "metop_dump_decoder" || dec == "meteor_lrpt_decoder")
                 printf("lock_state %s\n", m.correlator_lock.load() ? "SYNCED" : "NOSYNC");
         } else {
             PskDemodStage m1(in, out, dp, dp.str("b200_demod_module", "psk_demod"));
             FecStage m2(dec, "", out, fp);
             run_two_stage(m1, m2);
             printf("wrote %s (%ld frames)\n", m2.getOutput().c_str(), m2.frames_written.load());
-            if (dec == "metop_dump_decoder")
+            if (dec == "metop_dump_decoder" || dec == "meteor_lrpt_decoder")
                 printf("lock_state %s\n", m2.correlator_lock.load() ? "SYNCED" : "NOSYNC");
         }
     } catch (const std::exception &e) {

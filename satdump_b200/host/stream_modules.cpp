@@ -263,6 +263,26 @@ b200_fec_cfg fec_cfg_from_params(const std::string &id, const Params &p)
         c.cadu_size = 8192;
         return c;
     }
+    if (id == "meteor_lrpt_decoder") { // module_meteor_lrpt_decoder.cpp:22-49; the library refuses "interleaved" by name
+        c.kind = B200_FEC_METEOR_LRPT;
+        c.device = (int)p.num("b200_device", 0);
+        c.constellation = B200_QPSK;
+        c.cadu_size = 8192;
+        if (!p.has("diff_decode"))
+            throw ModuleError("meteor_lrpt_decoder: diff_decode is required");
+        c.diff_decode = p.flag("diff_decode", false);
+        c.m2x_mode = p.flag("m2x_mode", false);
+        if (c.m2x_mode) {
+            if (!p.has("viterbi_outsync_after"))
+                throw ModuleError("meteor_lrpt_decoder: viterbi_outsync_after is required with m2x_mode");
+            if (!p.has("viterbi_ber_thresold"))
+                throw ModuleError("meteor_lrpt_decoder: viterbi_ber_thresold is required with m2x_mode");
+            c.outsync_after = (int)p.num("viterbi_outsync_after");
+            c.ber_thresold = (float)p.num("viterbi_ber_thresold");
+            c.interleaved = p.flag("interleaved", false);
+        }
+        return c;
+    }
     if (id == "ccsds_turbo_decoder") { // module_ccsds_turbo_decoder.cpp:17-36,118-119; the library checks the values (turbo_iters >= 1)
         c.kind = B200_FEC_TURBO;
         c.device = (int)p.num("b200_device", 0);
@@ -601,6 +621,7 @@ void FecStage::process()
             correlator_lock = st.correlator_lock;
             correlator_corr = st.correlator_corr;
             ldpc_corr = st.ldpc_corr;
+            rs_avg = st.rs_avg;
         }
     }
     if (fin)

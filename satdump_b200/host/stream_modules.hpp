@@ -129,6 +129,8 @@ class FecStage : public StageBase
     std::atomic<int> correlator_lock{0}, ldpc_corr{0};
     std::atomic<float> correlator_corr{0.f};
     std::atomic<int> crc_lock{0};
+    // meteor_lrpt_decoder: "rs_avg" of the last frame; m2x_mode 0: correlator_lock, viterbi_ber (module_meteor_lrpt_decoder.cpp:266-289)
+    std::atomic<int> rs_avg{0};
     std::atomic<long> frames_written{0};
     b200_fec_cfg cfg{};
     long batch_soft = 1 << 24;

@@ -307,6 +307,13 @@ CONFIGS = {
     # symbol), pll_bw 0.03, no convolutional code, randomised CADUs with RS(255,223) I=4 dual basis; cs16 (cs8: dataclasses.replace)
     "metop_dump": SignalCfg(name="metop_dump", samplerate=45e6, symbolrate=35000000, constellation="qpsk", conv="none", interleave=4,
                             rrc_alpha=0.5, pll_bw=0.03, fmt="cs16", decoder="dump", esn0_db=16.0),
+    # psk_demod QPSK -> meteor_lrpt_decoder, METEOR M2 LRPT 72k (Meteor-M.json): 72 ksym/s, pll_bw 0.002, diff_decode false; r=1/2 k=7
+    # continuous, randomised CADUs with RS(255,223) I=4 in the conventional basis. At 200 kS/s (2.78 samples per symbol, no resampling) and
+    # at the pipeline's default 1 MS/s (13.9 samples per symbol: through the front-end resampler)
+    "meteor_lrpt": SignalCfg(name="meteor_lrpt", samplerate=200e3, symbolrate=72000, constellation="qpsk", conv="1/2", interleave=4,
+                             rrc_alpha=0.5, pll_bw=0.002, fmt="cs16", decoder="meteor", esn0_db=8.0, carrier_rad=2e-4),
+    "meteor_lrpt_1m": SignalCfg(name="meteor_lrpt_1m", samplerate=1e6, symbolrate=72000, constellation="qpsk", conv="1/2", interleave=4,
+                                rrc_alpha=0.5, pll_bw=0.002, fmt="cs16", decoder="meteor", esn0_db=8.0, carrier_rad=4e-5),
 }
 
 
@@ -341,6 +348,9 @@ def make_bitstream(cfg: SignalCfg, nframes, seed):
     if cfg.decoder == "dump":  # nframes CADUs, sent as they are
         tx, clear = dump_frames(nframes, seed)
         return tx.reshape(-1), clear
+    if cfg.decoder == "meteor":  # nframes LRPT CADUs, convolutionally encoded as one stream
+        coded, written = lrpt_frames(nframes, seed, nrzm=cfg.nrzm)
+        return coded, written
     if cfg.decoder == "ldpc":  # nframes LDPC frames
         if cfg.internal_cadu_size:
             info, clear = ldpc_inner_frames(nframes, cfg.internal_cadu_size, cfg.internal_asm, seed)
@@ -458,6 +468,8 @@ def frames_for_samples(cfg: SignalCfg, nsamples):
     if cfg.decoder == "turbo":  # turbo frames of ASM + codeword bits
         nbits = turbo_codeword_bits(cfg.turbo_rate, cfg.turbo_base) + TURBO_ASM_BITS[cfg.turbo_rate]
         return int(nsamples * bps / (cfg.samplerate / cfg.symbolrate) / nbits) + 2
+    if cfg.decoder == "meteor":  # LRPT CADUs of 8192 bits, 16384 coded bits each
+        return int(nsamples * bps / (cfg.samplerate / cfg.symbolrate) / 16384) + 2
     if cfg.decoder in ("ldpc", "dump"):  # LDPC frames / MetOp dump CADUs of 8192 bits
         return int(nsamples * bps / (cfg.samplerate / cfg.symbolrate) / 8192) + 2
     rate = {"1/2": 0.5, "3/4": 0.75, "none": 1.0, "p2/3": 2 / 3, "p3/4": 0.75, "p5/6": 5 / 6, "p7/8": 7 / 8}[cfg.conv]
@@ -720,6 +732,43 @@ def dump_soft(tx_bits, phase=0, swap=False, amp=60.0, sigma=0.0, seed=0):
     bit 1 is -amp after rotate_soft(phase, swap); here the inverse of that rotation is applied: rotation by -phase, then the IQ swap."""
     b = np.asarray(tx_bits, np.uint8).reshape(-1).astype(np.float64)
     s = (1 - 2 * b) * amp
+    I, Q = s[0::2], s[1::2]
+    for _ in range((4 - phase) % 4):  # rotate_soft's PHASE_90 step: (I, Q) -> (Q, -I)
+        I, Q = Q, -I
+    if swap:
+        I, Q = Q, I
+    out = np.empty(2 * I.size)
+    out[0::2], out[1::2] = I, Q
+    if sigma:
+        out = out + np.random.default_rng(seed).normal(0, sigma, out.size)
+    return np.clip(np.round(out), -127, 127).astype(np.int8)
+
+
+# ---- METEOR-M LRPT (meteor_lrpt_decoder) ------------------------------------------------------------------------------------------------
+def lrpt_frames(nframes, seed=0, nrzm=False, inverted=()):
+    """The LRPT transmitter: random payloads, RS(255,223) I=4 in the conventional basis, the randomiser, NRZ-M when `nrzm`, then r=1/2 k=7
+    over the whole stream (conv_encode). Returns (coded bits uint8 [nframes * 16384]: I = first, Q = second output of each step, the CADUs
+    meteor_lrpt_decoder writes for them [n, 1024]: 1D CF FC 1D + the derandomised codewords). Frames listed in `inverted` are sent with
+    bytes 4 .. 1023 inverted and a payload whose derandomised byte 9 is 0x00: the decoder finds 0xFF there and inverts the frame back."""
+    payload = np.random.default_rng(seed).integers(0, 256, size=(nframes, 4 * 223), dtype=np.uint8)
+    for k in inverted:
+        payload[k, 5] = 0  # CADU byte 9 = byte 5 of the interleaved codewords = message byte 1 of codeword 1 = payload byte 1 * 4 + 1
+    tx, clear = build_cadus(payload, 4, dual=False)
+    for k in inverted:
+        tx[k, 4:] ^= 0xFF
+    bits = np.unpackbits(tx.reshape(-1))
+    if nrzm:
+        bits = nrzm_encode(bits)
+    written = clear.copy()
+    written[:, :4] = (0x1D, 0xCF, 0xFC, 0x1D)
+    return conv_encode(bits), written
+
+
+def lrpt_soft(coded, phase=0, swap=False, amp=60.0, sigma=0.0, seed=0):
+    """int8 soft stream of coded bits (bit 1 = +amp, I and Q = consecutive bits) as a receiver with a phase ambiguity `phase` (0..3 = 0 ..
+    270 degrees) and an IQ swap sees it: the inverse of rotate_soft(phase, swap), i.e. rotation by -phase, then the swap."""
+    b = np.asarray(coded, np.uint8).reshape(-1).astype(np.float64)
+    s = (2 * b - 1) * amp
     I, Q = s[0::2], s[1::2]
     for _ in range((4 - phase) % 4):  # rotate_soft's PHASE_90 step: (I, Q) -> (Q, -I)
         I, Q = Q, -I

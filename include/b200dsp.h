@@ -50,7 +50,7 @@ enum { B200_BPSK = 0, B200_QPSK = 1, B200_OQPSK = 2, B200_8PSK = 3, B200_NONE = 
 enum { B200_CF32 = 0, B200_CS16 = 1, B200_CS8 = 2 };
 /* decoder kind */
 enum { B200_FEC_METOP = 0, B200_FEC_CCSDS = 1, B200_FEC_SIMPLE = 2, B200_FEC_LDPC = 3, B200_FEC_TURBO = 4, B200_FEC_METOP_DUMP = 5,
-       B200_FEC_METEOR_LRPT = 6 };
+       B200_FEC_METEOR_LRPT = 6, B200_FEC_NOAA_HRPT = 7 /* noaa_hrpt_decoder */, B200_FEC_METEOR_HRPT = 8 /* meteor_hrpt_decoder */ };
 /* debug stage ids for b200_demod_debug_stage */
 enum { B200_STAGE_AGC = 0, B200_STAGE_FIR = 1, B200_STAGE_COSTAS = 2, B200_STAGE_RESAMP = 3, B200_STAGE_DC = 4, B200_STAGE_MM = 5,
        B200_STAGE_PLL = 6 /* pm_demod: PLLCarrierTrackingBlock output */, B200_STAGE_PM = 7 /* pm_demod: PMToBPSK output */ };
@@ -165,6 +165,16 @@ typedef struct b200_fec_cfg
     int diff_decode;          /* "diff_decode" (required by the module)                                                                    */
     int m2x_mode;             /* "m2x_mode", default false                                                                                 */
     int interleaved;          /* "interleaved" (m2x_mode only), default false: refused                                                     */
+    /* kind B200_FEC_NOAA_HRPT = noaa_hrpt_decoder (module_noaa_hrpt_decoder.cpp, noaa_deframer.cpp): hard bits soft > 0; the 60-bit
+       minor-frame sync 0x0A116FD719D83C95 (or its complement: inverted) within deframer_thresold bits starts a frame, written as the
+       six sync words 0x284 0x16F 0x35C 0x19D 0x20F 0x095 and 11084 10-bit words (MSB first, XOR the inversion). The output unit is ONE
+       word: cadu_bytes = 2 (little-endian uint16, the .raw16 file), frames_out counts words (the module's frame_count = words / 11090),
+       and a push writes every word whose 10th bit it brought. Only deframer_thresold, device and max_soft are read.
+       kind B200_FEC_METEOR_HRPT = meteor_hrpt_decoder (module_meteor_hrpt_decoder.cpp, meteor/deframer.cpp): hard bits soft > 0 XOR the
+       inversion; the ASM 0x1ACFFC1D machine with states 0 / 2 / 6 / 12 (each its own error threshold); every accepted ASM is followed by
+       a frame written as 1A CF FC 1D + the next 8160 bits, returned when complete (cadu_bytes = 1024). Only device and max_soft are read.
+       Both: device memory about 1.3 bytes per max_soft byte (FIFO, hard bits, sync bitmap) plus the output; max_soft <= 2^30. */
+    int deframer_thresold;    /* "deframer_thresold" of noaa_hrpt_decoder (required by the module): 0 .. 60                              */
 } b200_fec_cfg;
 
 typedef struct b200_demod_stats
@@ -192,7 +202,8 @@ typedef struct b200_fec_stats
     long soft_in, chunks, bits_out, frames_out;
     int viterbi_state;        /* 0 NOSYNC 1 SYNCED  (Viterbi3_4::getState)                       */
     float viterbi_ber;
-    int deframer_state;       /* 2 NOSYNC / 6 SYNCING / 12|18 SYNCED (BPSK_CCSDS_Deframer)       */
+    int deframer_state;       /* 2 NOSYNC / 6 SYNCING / 12|18 SYNCED (BPSK_CCSDS_Deframer); meteor_hrpt_decoder: its own state
+                                 numbers 0 (NOSYNC) / 2, 6 (SYNCING) / 12 (SYNCED, "deframer_lock"); noaa_hrpt_decoder: 0           */
     long rs_corrected, rs_failed;
     long replays;             /* slow-path re-decodes (lock changes, start-state mis-speculation) */
     long kernel_launches;
@@ -347,6 +358,14 @@ typedef struct b200_meteor_frame
     float ber;                /* Viterbi27's BER of the frame                                                                      */
 } b200_meteor_frame;
 int b200_fec_debug_meteor_frames(b200_fec *f, b200_meteor_frame *out, long cap, long *n_out);
+/* noaa_hrpt_decoder / meteor_hrpt_decoder: one record per sync accepted in the LAST push, in stream order (frames still open included) */
+typedef struct b200_hrpt_frame
+{
+    long bit;                 /* stream bit index (soft bytes since create / reset) of the sync's last bit                            */
+    int inverted;             /* the frame is written inverted (the sync's complement matched)                                       */
+    int state;                /* the state that accepted it: METEOR 0 / 2 / 6 / 12; NOAA 0                                            */
+} b200_hrpt_frame;
+int b200_fec_debug_hrpt_frames(b200_fec *f, b200_hrpt_frame *out, long cap, long *n_out);
 
 /* ---- fused chain: raw IQ -> CADUs, soft stream stays in HBM ---------------------------------------- */
 b200_chain *b200_chain_create(const b200_demod_cfg *dcfg, const b200_fec_cfg *fcfg);

@@ -6,7 +6,7 @@
 //
 //   loader()                          the one symbol SatDump dlsym()s (core/plugin.cpp:15-33)
 //   B200DSPSupport::init()            on SatDumpStartedEvent (fired after every plugin registered its modules, init.cpp:163) the
-//                                     entries "psk_demod", "pm_demod", "metop_ahrpt_decoder", "ccsds_conv_concat_decoder", "ccsds_simple_psk_decoder", "ccsds_ldpc_decoder", "ccsds_turbo_decoder", "metop_dump_decoder" and "meteor_lrpt_decoder" of
+//                                     entries "psk_demod", "pm_demod", "metop_ahrpt_decoder", "ccsds_conv_concat_decoder", "ccsds_simple_psk_decoder", "ccsds_ldpc_decoder", "ccsds_turbo_decoder", "metop_dump_decoder", "meteor_lrpt_decoder", "noaa_hrpt_decoder" and "meteor_hrpt_decoder" of
 //                                     satdump::pipeline::modules_registry (module.h:210, looked up first-match by id, module.cpp:129-135)
 //                                     get their factory replaced, so existing pipelines instantiate the CUDA modules.
 //                                     Set B200_DSP_REGISTER_ONLY=1 to register "<id>_b200" ids instead and leave the originals alone.
@@ -233,6 +233,19 @@ namespace b200plugin
                 v["lock_state"] = stage->correlator_lock.load() ? "SYNCED" : "NOSYNC";
                 return v;
             }
+            if (stage->getID() == "noaa_hrpt_decoder") // NOAAHRPTDecoderModule::getModuleStats (module_noaa_hrpt_decoder.cpp:47-52)
+            {
+                v["frame_count"] = stage->frames_written.load() / 11090;
+                return v;
+            }
+            if (stage->getID() == "meteor_hrpt_decoder") // METEORHRPTDecoderModule::getModuleStats (module_meteor_hrpt_decoder.cpp:52-60)
+            {
+                const int ds = stage->deframer_state.load();
+                v["deframer_lock"] = ds == 12;
+                v["deframer_state"] = ds == 0 ? "NOSYNC" : (ds == 2 || ds == 6 ? "SYNCING" : "SYNCED");
+                v["frame_count"] = stage->frames_written.load();
+                return v;
+            }
             if (stage->getID() == "meteor_lrpt_decoder" && !stage->cfg.m2x_mode) // METEORLRPTDecoderModule::getModuleStats (:282-287)
             {
                 v["correlator_lock"] = stage->correlator_lock.load() != 0;
@@ -279,7 +292,7 @@ public:
     static void registerHandler(const satdump::pipeline::RegisterModulesEvent &evt)
     {
         for (const char *id : {"psk_demod", "pm_demod", "metop_ahrpt_decoder", "ccsds_conv_concat_decoder", "ccsds_simple_psk_decoder", "ccsds_ldpc_decoder",
-                               "ccsds_turbo_decoder", "metop_dump_decoder", "meteor_lrpt_decoder"})
+                               "ccsds_turbo_decoder", "metop_dump_decoder", "meteor_lrpt_decoder", "noaa_hrpt_decoder", "meteor_hrpt_decoder"})
             evt.modules_registry.push_back({std::string(id) + "_b200", nlohmann::json(), factory(id)});
     }
 
@@ -288,7 +301,7 @@ public:
         for (auto &e : satdump::pipeline::modules_registry)
             if (e.id == "psk_demod" || e.id == "pm_demod" || e.id == "metop_ahrpt_decoder" || e.id == "ccsds_conv_concat_decoder" || e.id == "ccsds_simple_psk_decoder" ||
                 e.id == "ccsds_ldpc_decoder" || e.id == "ccsds_turbo_decoder" || e.id == "metop_dump_decoder" ||
-                e.id == "meteor_lrpt_decoder")
+                e.id == "meteor_lrpt_decoder" || e.id == "noaa_hrpt_decoder" || e.id == "meteor_hrpt_decoder")
             {
                 e.inst = factory(e.id);
                 logger->info("b200_dsp_support: module " + e.id + " now runs on the B200 path");

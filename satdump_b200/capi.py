@@ -26,6 +26,7 @@ SYMBOLS = [
     "b200_fec_create", "b200_fec_destroy", "b200_fec_push_soft", "b200_fec_push_soft_device", "b200_fec_pull_frames",
     "b200_fec_debug_bits", "b200_fec_get_stats", "b200_fec_cadu_bytes", "b200_fec_chunk_size", "b200_fec_debug_ldpc_frames", "b200_fec_ldpc_timing",
     "b200_fec_debug_turbo_frames", "b200_fec_debug_turbo_llr", "b200_fec_turbo_timing", "b200_fec_debug_dump_frames", "b200_fec_debug_meteor_frames",
+    "b200_fec_debug_hrpt_frames",
     "b200_chain_create", "b200_chain_destroy", "b200_chain_push_iq", "b200_chain_push_iq_device", "b200_chain_prefetch_iq", "b200_chain_pull_frames",
     "b200_chain_frames_device", "b200_chain_get_stats", "b200_chain_last_timing", "b200_chain_reset",
     "b200_chain_set_pipelined", "b200_chain_sync", "b200_chain_span_begin", "b200_chain_span_end",
@@ -54,7 +55,7 @@ class FecCfg(C.Structure):
                 ("device", C.c_int), ("max_soft", C.c_long), ("qpsk_swap_iq", C.c_int), ("qpsk_swap_diff", C.c_int), ("oqpsk_delay", C.c_int), ("conv_rate", C.c_int),
                 ("ldpc_rate", C.c_int), ("ldpc_block_size", C.c_int), ("ldpc_iterations", C.c_int), ("ldpc2", C.c_int), ("internal_stream", C.c_int),
                 ("internal_cadu_size", C.c_int), ("turbo_rate", C.c_int), ("turbo_base", C.c_int), ("turbo_iters", C.c_int),
-                ("diff_decode", C.c_int), ("m2x_mode", C.c_int), ("interleaved", C.c_int)]
+                ("diff_decode", C.c_int), ("m2x_mode", C.c_int), ("interleaved", C.c_int), ("deframer_thresold", C.c_int)]
 
 
 class DemuxCfg(C.Structure):
@@ -102,6 +103,10 @@ class DumpFrame(C.Structure):
 class MeteorFrame(C.Structure):
     _fields_ = [("offset", C.c_long), ("pos", C.c_int), ("corr", C.c_int), ("phase", C.c_int), ("swap", C.c_int), ("rs", C.c_int * 4),
                 ("ber", C.c_float)]
+
+
+class HrptFrame(C.Structure):
+    _fields_ = [("bit", C.c_long), ("inverted", C.c_int), ("state", C.c_int)]
 
 
 class B200Error(RuntimeError):
@@ -159,6 +164,7 @@ def lib():
         L.b200_fec_debug_turbo_llr.argtypes = [vp, cl, vp, vp, cl, C.POINTER(cl)]
         L.b200_fec_debug_dump_frames.argtypes = [vp, C.POINTER(DumpFrame), cl, C.POINTER(cl)]
         L.b200_fec_debug_meteor_frames.argtypes = [vp, C.POINTER(MeteorFrame), cl, C.POINTER(cl)]
+        L.b200_fec_debug_hrpt_frames.argtypes = [vp, C.POINTER(HrptFrame), cl, C.POINTER(cl)]
         L.b200_chain_create.restype = vp
         L.b200_chain_create.argtypes = [C.POINTER(DemodCfg), C.POINTER(FecCfg)]
         L.b200_chain_destroy.argtypes = [vp]
@@ -328,6 +334,24 @@ def meteor_lrpt_cfg(diff_decode=None, m2x_mode=False, viterbi_outsync_after=None
     return cfg
 
 
+def noaa_hrpt_cfg(deframer_thresold=None, device=0, max_soft=1 << 24):
+    """noaa_hrpt_decoder (module_noaa_hrpt_decoder.cpp:14-20): deframer_thresold is required, as the module reads it without a default.
+    The output unit is one 10-bit word (cadu_bytes 2: the .raw16 file's little-endian uint16)."""
+    if deframer_thresold is None:
+        raise ValueError("noaa_hrpt_decoder: deframer_thresold is required")
+    cfg = FecCfg()
+    cfg.kind, cfg.constellation, cfg.cadu_size, cfg.device, cfg.max_soft = 7, CONST["bpsk"], 16, device, max_soft
+    cfg.deframer_thresold = int(deframer_thresold)
+    return cfg
+
+
+def meteor_hrpt_cfg(device=0, max_soft=1 << 24):
+    """meteor_hrpt_decoder (module_meteor_hrpt_decoder.cpp): the module takes no parameters; 1024-byte CADUs."""
+    cfg = FecCfg()
+    cfg.kind, cfg.constellation, cfg.cadu_size, cfg.device, cfg.max_soft = 8, CONST["bpsk"], 8192, device, max_soft
+    return cfg
+
+
 def fec_cfg_for(sig, max_soft, device=0):
     """The decoder configuration that goes with a satdump_b200.synth.SignalCfg (metop_ahrpt_decoder / ccsds_conv_concat_decoder /
     ccsds_simple_psk_decoder parameters of the shipped pipeline JSONs)."""
@@ -337,6 +361,10 @@ def fec_cfg_for(sig, max_soft, device=0):
         return dump_cfg(device=device, max_soft=max_soft)
     if sig.decoder == "meteor":
         return meteor_lrpt_cfg(sig.nrzm, device=device, max_soft=max_soft)
+    if sig.decoder == "noaa_hrpt":
+        return noaa_hrpt_cfg(sig.deframer_thresold, device=device, max_soft=max_soft)
+    if sig.decoder == "meteor_hrpt":
+        return meteor_hrpt_cfg(device=device, max_soft=max_soft)
     if sig.decoder == "turbo":
         return turbo_cfg(sig.turbo_rate, sig.turbo_base, sig.turbo_iters, device=device, max_soft=max_soft)
     if sig.decoder == "ldpc":
@@ -580,6 +608,15 @@ class Fec:
             out[k] = [r.offset, r.pos, r.corr, r.phase, r.swap, *r.rs, int(np.float32(r.ber).view(np.uint32))]
         return out
 
+    def hrpt_frames(self):
+        """noaa_hrpt_decoder / meteor_hrpt_decoder: one record per sync accepted in the last push as int64 [n, 3] = stream bit of the
+        sync's last bit, inverted, accepting state (oracle.hrpt)."""
+        cap = int(self._n) // 8000 + 8
+        recs = (HrptFrame * cap)()
+        n = C.c_long(0)
+        _chk(lib().b200_fec_debug_hrpt_frames(self.h, recs, cap, C.byref(n)))
+        return np.array([[recs[k].bit, recs[k].inverted, recs[k].state] for k in range(n.value)], np.int64).reshape(-1, 3)
+
     def turbo_llr(self, frame, K):
         """ccsds_turbo_decoder: the a-priori arrays (input 0, input 1) of a frame of the last push after its last iteration."""
         a0, a1 = np.zeros(K), np.zeros(K)
@@ -608,7 +645,7 @@ class Chain:
         self.h = lib().b200_chain_create(C.byref(dcfg), C.byref(fcfg))
         if not self.h:
             raise B200Error(-1 if "device" not in last_error().lower() else -2, last_error())
-        self.cadu_bytes = (fcfg.cadu_size + 7) // 8 if fcfg.kind in (1, 3) else (fcfg.turbo_base + 4 if fcfg.kind == 4 else 1024)
+        self.cadu_bytes = (fcfg.cadu_size + 7) // 8 if fcfg.kind in (1, 3, 7) else (fcfg.turbo_base + 4 if fcfg.kind == 4 else 1024)
 
     def close(self):
         if getattr(self, "h", None):

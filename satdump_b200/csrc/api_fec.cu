@@ -93,7 +93,7 @@ Fec::Fec(const b200_fec_cfg &in) : cfg(meteor_m2x_as_ccsds(in))
 {
     const b200_fec_cfg c = cfg;
     B200_REQUIRE(c.kind == B200_FEC_METOP || c.kind == B200_FEC_CCSDS || c.kind == B200_FEC_SIMPLE || c.kind == B200_FEC_LDPC || c.kind == B200_FEC_TURBO ||
-                     c.kind == B200_FEC_METOP_DUMP || c.kind == B200_FEC_METEOR_LRPT,
+                     c.kind == B200_FEC_METOP_DUMP || c.kind == B200_FEC_METEOR_LRPT || c.kind == B200_FEC_NOAA_HRPT || c.kind == B200_FEC_METEOR_HRPT,
                  B200_EINVAL, "unknown decoder kind %d", c.kind);
     B200_REQUIRE(c.max_soft >= 65536, B200_EINVAL, "max_soft must be >= 65536");
     memset(&geom, 0, sizeof(geom));
@@ -105,6 +105,8 @@ Fec::Fec(const b200_fec_cfg &in) : cfg(meteor_m2x_as_ccsds(in))
         framed = dump_decoder(*this);
     else if (c.kind == B200_FEC_METEOR_LRPT)
         framed = meteor_decoder(*this);
+    else if (c.kind == B200_FEC_NOAA_HRPT || c.kind == B200_FEC_METEOR_HRPT)
+        framed = hrpt_decoder(*this);
     if (framed)
         return;
     if (c.kind != B200_FEC_METOP) {
@@ -1233,6 +1235,13 @@ int b200_fec_debug_meteor_frames(b200_fec *h, b200_meteor_frame *out, long cap, 
     return guarded([&] {
         B200_REQUIRE(h && out && n_out, B200_EINVAL, "NULL argument");
         *n_out = h->f->meteor_frames(out, cap);
+    });
+}
+int b200_fec_debug_hrpt_frames(b200_fec *h, b200_hrpt_frame *out, long cap, long *n_out)
+{
+    return guarded([&] {
+        B200_REQUIRE(h && out && n_out, B200_EINVAL, "NULL argument");
+        *n_out = h->f->hrpt_frames(out, cap);
     });
 }
 int b200_fec_turbo_timing(b200_fec *h, float *ms_out, int n)

@@ -50,6 +50,7 @@ std::unique_ptr<Framed> ldpc_decoder(Fec &f);
 std::unique_ptr<Framed> turbo_decoder(Fec &f);
 std::unique_ptr<Framed> dump_decoder(Fec &f);
 std::unique_ptr<Framed> meteor_decoder(Fec &f);
+std::unique_ptr<Framed> hrpt_decoder(Fec &f); // noaa_hrpt_decoder, meteor_hrpt_decoder (api_hrpt.cu)
 
 class Fec
 {
@@ -91,6 +92,7 @@ class Fec
     void turbo_timing(float *ms, int n);
     long dump_frames(b200_dump_frame *out, long cap); // records of the last push
     long meteor_frames(b200_meteor_frame *out, long cap); // records of the last push
+    long hrpt_frames(b200_hrpt_frame *out, long cap); // records of the last push
 
     // device storage
     DevBuf<int8_t> softbuf;
@@ -169,6 +171,7 @@ class Fec
     friend struct Turbo;
     friend struct Dump;
     friend struct Meteor;
+    friend struct Hrpt;
     // the main deframer and the frame counters at a point a pass may have to roll back to
     struct Mark { DefrState h_dstate; long fifo_bits, out_frames, total_frames, rs_corrected, rs_failed; int defr_state_now; };
     Mark mark();

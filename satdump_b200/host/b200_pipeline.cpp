@@ -7,10 +7,20 @@
 #include <cstring>
 using namespace b200host;
 
+// the module stats of the HRPT decoders (module_noaa_hrpt_decoder.cpp:47-52, module_meteor_hrpt_decoder.cpp:52-60); frames: output units
+static void print_hrpt_stats(const std::string &dec, long frames, int state)
+{
+    if (dec == "noaa_hrpt_decoder")
+        printf("frame_count %ld\n", frames / 11090);
+    if (dec == "meteor_hrpt_decoder")
+        printf("deframer_lock %d\ndeframer_state %s\nframe_count %ld\n", state == 12, state == 0 ? "NOSYNC" : (state == 2 || state == 6 ? "SYNCING" : "SYNCED"),
+               frames);
+}
+
 int main(int argc, char **argv)
 {
     if (argc < 5) {
-        fprintf(stderr, "usage: %s <metop_ahrpt|jpss_hrd|npp_hrd|simple_bpsk|simple_qpsk|pm_bpsk|ldpc_qpsk|landsat|turbo_pm|turbo_bpsk|metop_dump|meteor_lrpt> baseband <input> <output_hint> [--fused] [--key value ...]\n", argv[0]);
+        fprintf(stderr, "usage: %s <metop_ahrpt|jpss_hrd|npp_hrd|simple_bpsk|simple_qpsk|pm_bpsk|ldpc_qpsk|landsat|turbo_pm|turbo_bpsk|metop_dump|meteor_lrpt|noaa_hrpt|meteor_hrpt> baseband <input> <output_hint> [--fused] [--key value ...]\n", argv[0]);
         return 2;
     }
     const std::string pipe = argv[1], level = argv[2], in = argv[3], out = argv[4];
@@ -27,6 +37,14 @@ int main(int argc, char **argv)
         dp = Params{{"constellation", "qpsk"}, {"symbolrate", "72000"}, {"rrc_alpha", "0.5"}, {"pll_bw", "0.002"}};
         fp = Params{{"diff_decode", "false"}};
         dec = "meteor_lrpt_decoder";
+    } else if (pipe == "noaa_hrpt" || pipe == "meteor_hrpt") { // resources/pipelines/NOAA.json "noaa_hrpt", Meteor-M.json "meteor_hrpt":
+        // pm_demod at 665 400 sym/s (pll_bw 0.01, rrc_alpha 0.6 | 0.5, clock_omega_relative_limit 0.001), 3 MS/s by default
+        const bool noaa = pipe == "noaa_hrpt";
+        dp = Params{{"b200_demod_module", "pm_demod"}, {"symbolrate", "665400"}, {"pll_bw", "0.01"}, {"rrc_alpha", noaa ? "0.6" : "0.5"},
+                    {"clock_omega_relative_limit", "0.001"}};
+        if (noaa)
+            fp = Params{{"deframer_thresold", "10"}};
+        dec = noaa ? "noaa_hrpt_decoder" : "meteor_hrpt_decoder";
     } else if (pipe == "jpss_hrd" || pipe == "npp_hrd") { // resources/pipelines/JPSS.json
         dp = Params{{"constellation", "oqpsk"}, {"symbolrate", pipe == "jpss_hrd" ? "25000000" : "15000000"}, {"rrc_alpha", "0.5"}, {"pll_bw", "0.002"}};
         fp = Params{{"constellation", "oqpsk"}, {"cadu_size", "10232"}, {"viterbi_ber_thresold", "0.3"}, {"viterbi_outsync_after", "20"},
@@ -89,6 +107,7 @@ int main(int argc, char **argv)
             printf("wrote %s (%ld frames)\n", m.getOutput().c_str(), m.frames_written.load());
             if (dec == "metop_dump_decoder" || dec == "meteor_lrpt_decoder")
                 printf("lock_state %s\n", m.correlator_lock.load() ? "SYNCED" : "NOSYNC");
+            print_hrpt_stats(dec, m.frames_written.load(), m.deframer_state.load());
         } else {
             PskDemodStage m1(in, out, dp, dp.str("b200_demod_module", "psk_demod"));
             FecStage m2(dec, "", out, fp);
@@ -96,6 +115,7 @@ int main(int argc, char **argv)
             printf("wrote %s (%ld frames)\n", m2.getOutput().c_str(), m2.frames_written.load());
             if (dec == "metop_dump_decoder" || dec == "meteor_lrpt_decoder")
                 printf("lock_state %s\n", m2.correlator_lock.load() ? "SYNCED" : "NOSYNC");
+            print_hrpt_stats(dec, m2.frames_written.load(), m2.deframer_state.load());
         }
     } catch (const std::exception &e) {
         fprintf(stderr, "error: %s\n", e.what());

@@ -263,6 +263,25 @@ b200_fec_cfg fec_cfg_from_params(const std::string &id, const Params &p)
         c.cadu_size = 8192;
         return c;
     }
+    if (id == "noaa_hrpt_decoder") { // module_noaa_hrpt_decoder.cpp:14-20: deframer_thresold read with no default; 10-bit words as uint16
+        c.kind = B200_FEC_NOAA_HRPT;
+        c.device = (int)p.num("b200_device", 0);
+        c.constellation = B200_BPSK;
+        c.cadu_size = 16; // one output unit = one word
+        if (!p.has("deframer_thresold"))
+            throw ModuleError("noaa_hrpt_decoder: deframer_thresold is required");
+        c.deframer_thresold = (int)p.num("deframer_thresold");
+        if (c.deframer_thresold < 0 || c.deframer_thresold > 60) // (a 60-bit window is within 60 of anything: the bound of the library)
+            throw ModuleError("noaa_hrpt_decoder: deframer_thresold must be 0..60 (got " + std::to_string(c.deframer_thresold) + ")");
+        return c;
+    }
+    if (id == "meteor_hrpt_decoder") { // module_meteor_hrpt_decoder.cpp:14-20: no parameters; 1024-byte CADUs
+        c.kind = B200_FEC_METEOR_HRPT;
+        c.device = (int)p.num("b200_device", 0);
+        c.constellation = B200_BPSK;
+        c.cadu_size = 8192;
+        return c;
+    }
     if (id == "meteor_lrpt_decoder") { // module_meteor_lrpt_decoder.cpp:22-49; the library refuses "interleaved" by name
         c.kind = B200_FEC_METEOR_LRPT;
         c.device = (int)p.num("b200_device", 0);
@@ -580,7 +599,8 @@ void FecStage::process()
     }
     if (out_type == DataType::FILE) {
         const bool ccsds = params.flag("ccsds", true);
-        output_file = output_hint + (ccsds ? ".cadu" : ".frm"); // filestream_to_filestream.cpp:27-36, ccsds decoder :131
+        output_file = output_hint + (cfg.kind == B200_FEC_NOAA_HRPT ? ".raw16" : (ccsds ? ".cadu" : ".frm")); // filestream_to_filestream.cpp:27-36,
+        // ccsds decoder :131, module_noaa_hrpt_decoder.cpp:20
         fout = fopen(output_file.c_str(), "wb");
     }
     const int chunk = b200_fec_chunk_size(h);
@@ -663,7 +683,7 @@ void FusedStage::process()
     const uint64_t fsz = file_size(input_file);
     if (data_offset)
         fseek(fin, (long)data_offset, SEEK_SET);
-    output_file = output_hint + ".cadu";
+    output_file = output_hint + (fcfg.kind == B200_FEC_NOAA_HRPT ? ".raw16" : ".cadu");
     FILE *fout = fopen(output_file.c_str(), "wb");
     uint64_t done = 0;
     size_t have = 0;
@@ -694,6 +714,7 @@ void FusedStage::process()
             if (b200_chain_get_stats(h, &dst, &fst) == B200_OK) {
                 warn_unconverged(dst);
                 correlator_lock = fst.correlator_lock;
+                deframer_state = fst.deframer_state;
             }
         }
         drain();
@@ -707,6 +728,12 @@ void FusedStage::process()
     }
     check(b200_chain_sync(h), "b200_chain_sync");
     drain();
+    {
+        b200_demod_stats dst;
+        b200_fec_stats fst;
+        if (b200_chain_get_stats(h, &dst, &fst) == B200_OK)
+            deframer_state = fst.deframer_state;
+    }
     fclose(fin);
     fclose(fout);
 }

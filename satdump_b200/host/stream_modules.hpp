@@ -130,6 +130,7 @@ class FecStage : public StageBase
     std::atomic<float> correlator_corr{0.f};
     std::atomic<int> crc_lock{0};
     // meteor_lrpt_decoder: "rs_avg" of the last frame; m2x_mode 0: correlator_lock, viterbi_ber (module_meteor_lrpt_decoder.cpp:266-289)
+    // noaa_hrpt_decoder: "frame_count" = frames_written (words) / 11090; meteor_hrpt_decoder: deframer_state (0 / 2 / 6 / 12), frame_count
     std::atomic<int> rs_avg{0};
     std::atomic<long> frames_written{0};
     b200_fec_cfg cfg{};
@@ -150,6 +151,7 @@ class FusedStage : public StageBase
     std::string getID() const override { return "b200_psk_" + dec_id; }
     std::atomic<long> frames_written{0};
     std::atomic<int> correlator_lock{0}; // the decoder's correlator lock ("lock_state" of metop_dump_decoder / ccsds_ldpc_decoder)
+    std::atomic<int> deframer_state{0};  // meteor_hrpt_decoder: its deframer's state (0 / 2 / 6 / 12)
     std::atomic<double> progress{0};
     long batch_samples = 1 << 26;
   private:

@@ -214,6 +214,8 @@ class SignalCfg:
     turbo_base: int = 1115
     turbo_iters: int = 5
     post_costas_dc: bool = False
+    # noaa_hrpt_decoder's "deframer_thresold" (NOAA.json: 10)
+    deframer_thresold: int = 10
 
     @property
     def cadu_bytes(self):
@@ -314,6 +316,13 @@ CONFIGS = {
                              rrc_alpha=0.5, pll_bw=0.002, fmt="cs16", decoder="meteor", esn0_db=8.0, carrier_rad=2e-4),
     "meteor_lrpt_1m": SignalCfg(name="meteor_lrpt_1m", samplerate=1e6, symbolrate=72000, constellation="qpsk", conv="1/2", interleave=4,
                                 rrc_alpha=0.5, pll_bw=0.002, fmt="cs16", decoder="meteor", esn0_db=8.0, carrier_rad=4e-5),
+    # pm_demod -> noaa_hrpt_decoder / meteor_hrpt_decoder (NOAA.json "noaa_hrpt", Meteor-M.json "meteor_hrpt"): residual-carrier PM at
+    # 665 400 sym/s recorded at 3 MS/s (4.5 samples per symbol, no resampler), carrier PLL bandwidth 0.01, rrc_alpha 0.6 | 0.5. The PM
+    # model's sinusoidal subcarrier at the symbol rate stands in for the split-phase data; the decoders only see the soft bits' signs.
+    "noaa_hrpt": SignalCfg(name="noaa_hrpt", samplerate=3e6, symbolrate=665400, constellation="bpsk", conv="none", rrc_alpha=0.6, fmt="cs16",
+                           decoder="noaa_hrpt", esn0_db=20.0, pll_bw=0.005, pm_pll_bw=0.01, carrier_rad=2e-2, pm_index=1.0, deframer_thresold=10),
+    "meteor_hrpt": SignalCfg(name="meteor_hrpt", samplerate=3e6, symbolrate=665400, constellation="bpsk", conv="none", rrc_alpha=0.5, fmt="cs16",
+                             decoder="meteor_hrpt", esn0_db=20.0, pll_bw=0.005, pm_pll_bw=0.01, carrier_rad=2e-2, pm_index=1.0),
 }
 
 
@@ -351,6 +360,12 @@ def make_bitstream(cfg: SignalCfg, nframes, seed):
     if cfg.decoder == "meteor":  # nframes LRPT CADUs, convolutionally encoded as one stream
         coded, written = lrpt_frames(nframes, seed, nrzm=cfg.nrzm)
         return coded, written
+    if cfg.decoder == "noaa_hrpt":  # nframes NOAA HRPT minor frames (10-bit words, no FEC); clear: the words
+        bits, words = noaa_hrpt_frames(nframes, seed)
+        return bits.reshape(-1), words
+    if cfg.decoder == "meteor_hrpt":  # nframes METEOR HRPT CADUs (no FEC)
+        bits, cadu = meteor_hrpt_frames(nframes, seed)
+        return bits.reshape(-1), cadu
     if cfg.decoder == "ldpc":  # nframes LDPC frames
         if cfg.internal_cadu_size:
             info, clear = ldpc_inner_frames(nframes, cfg.internal_cadu_size, cfg.internal_asm, seed)
@@ -470,6 +485,8 @@ def frames_for_samples(cfg: SignalCfg, nsamples):
         return int(nsamples * bps / (cfg.samplerate / cfg.symbolrate) / nbits) + 2
     if cfg.decoder == "meteor":  # LRPT CADUs of 8192 bits, 16384 coded bits each
         return int(nsamples * bps / (cfg.samplerate / cfg.symbolrate) / 16384) + 2
+    if cfg.decoder in ("noaa_hrpt", "meteor_hrpt"):  # bits on air: 110900 per NOAA minor frame, 8192 per METEOR CADU
+        return int(nsamples / (cfg.samplerate / cfg.symbolrate) / (NOAA_WORDS * 10 if cfg.decoder == "noaa_hrpt" else 8192)) + 2
     if cfg.decoder in ("ldpc", "dump"):  # LDPC frames / MetOp dump CADUs of 8192 bits
         return int(nsamples * bps / (cfg.samplerate / cfg.symbolrate) / 8192) + 2
     rate = {"1/2": 0.5, "3/4": 0.75, "none": 1.0, "p2/3": 2 / 3, "p3/4": 0.75, "p5/6": 5 / 6, "p7/8": 7 / 8}[cfg.conv]
@@ -779,6 +796,46 @@ def lrpt_soft(coded, phase=0, swap=False, amp=60.0, sigma=0.0, seed=0):
     if sigma:
         out = out + np.random.default_rng(seed).normal(0, sigma, out.size)
     return np.clip(np.round(out), -127, 127).astype(np.int8)
+
+
+# ---- NOAA and METEOR HRPT (noaa_hrpt_decoder, meteor_hrpt_decoder): bit streams without FEC -------------------------------------------
+NOAA_SYNC_WORDS = (0x284, 0x16F, 0x35C, 0x19D, 0x20F, 0x095)  # the 60-bit minor-frame sync 0x0A116FD719D83C95 as six 10-bit words
+NOAA_WORDS = 11090
+METEOR_HRPT_ASM = bytes([0x1A, 0xCF, 0xFC, 0x1D])
+
+
+def noaa_hrpt_frames(nframes, seed=0):
+    """(bits uint8 [n, 110900] as sent, MSB first; words uint16 [n, 11090]): NOAA HRPT minor frames of 10-bit words, the six sync words
+    then 11084 random words"""
+    words = np.random.default_rng(seed).integers(0, 1024, size=(nframes, NOAA_WORDS)).astype(np.uint16)
+    words[:, :6] = NOAA_SYNC_WORDS
+    bits = ((words[..., None] >> np.arange(9, -1, -1, dtype=np.uint16)) & 1).astype(np.uint8).reshape(nframes, -1)
+    return bits, words
+
+
+def meteor_hrpt_frames(nframes, seed=0):
+    """(bits uint8 [n, 8192] as sent; CADUs uint8 [n, 1024]): the ASM 1ACFFC1D and 1020 random bytes per frame"""
+    cadu = np.random.default_rng(seed).integers(0, 256, size=(nframes, 1024)).astype(np.uint8)
+    cadu[:, :4] = np.frombuffer(METEOR_HRPT_ASM, np.uint8)
+    return np.unpackbits(cadu, axis=1), cadu
+
+
+def hrpt_soft(bits, inverted=False, amp=60.0, sigma=0.0, seed=0, slips=(), gaps=()):
+    """int8 soft stream of a bit stream as pm_demod writes it (bit 1 -> +amp; inverted: the other polarity). slips: bit indices dropped
+    from the stream (a bit slip); gaps: (bit index, length) stretches of noise inserted there. Indices refer to `bits`."""
+    b = np.asarray(bits, np.uint8).reshape(-1)
+    s = (2.0 * b - 1.0) * amp * (-1.0 if inverted else 1.0)
+    rng = np.random.default_rng(seed)
+    if sigma:
+        s = s + rng.normal(0, sigma, s.size)
+    keep = np.ones(s.size, bool)
+    keep[list(slips)] = False
+    pieces, a = [], 0
+    for at, n in sorted(gaps):
+        pieces += [s[a:at][keep[a:at]], rng.normal(0, 1.5 * amp, n)]
+        a = at
+    pieces.append(s[a:][keep[a:]])
+    return np.clip(np.round(np.concatenate(pieces)), -127, 127).astype(np.int8)
 
 
 # ---- CCSDS turbo code (CCSDS 131.0-B section 6), as ccsds_turbo_decoder receives it ---------------------------------------------------

@@ -227,6 +227,13 @@ static int fmt_bytes(int fmt)
 }
 
 static int round_up16(double v) { return ((int)std::ceil(v / 16.0)) * 16; }
+// k_mm instantiation: STRICT (test hook), GARDNER (clock_recovery 1), FIX (the input still needs its rotation / OQPSK delay)
+static decltype(&k_mm<false, false, false>) mm_kernel(bool strict, bool gardner, bool fix)
+{
+    if (strict)
+        return gardner ? (fix ? k_mm<true, true, true> : k_mm<true, true, false>) : (fix ? k_mm<true, false, true> : k_mm<true, false, false>);
+    return gardner ? (fix ? k_mm<false, true, true> : k_mm<false, true, false>) : (fix ? k_mm<false, false, true> : k_mm<false, false, false>);
+}
 // a run of r consecutive unconverged junctions needs r rounds; idle rounds cost two empty launches
 constexpr int REPAIR_ROUNDS = 8;
 
@@ -481,10 +488,8 @@ Demod::Demod(const b200_demod_cfg &c) : cfg(c)
     init_state();
     bufA.zero(stream);
     bufB.zero(stream);
-    B200_CUDA(cudaFuncSetAttribute(k_mm<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, MM_SMEM_BYTES));
-    B200_CUDA(cudaFuncSetAttribute(k_mm<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, MM_SMEM_BYTES));
-    B200_CUDA(cudaFuncSetAttribute(k_mm<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, MM_SMEM_BYTES));
-    B200_CUDA(cudaFuncSetAttribute(k_mm<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, MM_SMEM_BYTES));
+    for (int v = 0; v < 8; v++)
+        B200_CUDA(cudaFuncSetAttribute(mm_kernel(v & 1, v & 2, v & 4), cudaFuncAttributeMaxDynamicSharedMemorySize, MM_SMEM_BYTES));
     B200_CUDA(cudaFuncSetAttribute(k_costas<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, COSTAS_SMEM_BYTES));
     B200_CUDA(cudaFuncSetAttribute(k_costas<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, COSTAS_SMEM_BYTES));
     B200_CUDA(cudaFuncSetAttribute(k_costas<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, COSTAS_SMEM_BYTES));
@@ -733,7 +738,7 @@ void Demod::stage_mm(float2 *mmin, long n, int L, int nseg, int cur, int nxt, in
 {
     DemodDevState *S = st.p;
     const int nblk = (nseg + SEG_THREADS - 1) / SEG_THREADS;
-    const auto mm = cfg.clock_recovery == 1 ? (strict ? k_mm<true, true> : k_mm<false, true>) : (strict ? k_mm<true, false> : k_mm<false, false>);
+    const auto mm = mm_kernel(strict, cfg.clock_recovery == 1, mm_rot || mm_oqpsk);
     MMParams MP;
     MP.omega_mid = sps;
     MP.omega_limit = cfg.clock_omega_limit * sps;

@@ -1627,6 +1627,14 @@ __device__ __forceinline__ float2 rot_steps(float2 v, int q, int order)
     }
 }
 
+// k quarter turns (multiply by j^k) as rot_steps computes them for orders 2 and 4, without a branch: swap = k & 1, then the real
+// part's sign flips for k = 1, 2 and the imaginary part's for k = 2, 3 (neg_* = 0x80000000 or 0: an exact negation)
+__device__ __forceinline__ float2 rot_quarter(float2 v, bool swap, unsigned neg_re, unsigned neg_im)
+{
+    const float re = swap ? v.y : v.x, im = swap ? v.x : v.y;
+    return make_float2(__uint_as_float(__float_as_uint(re) ^ neg_re), __uint_as_float(__float_as_uint(im) ^ neg_im));
+}
+
 // ---------------------------------------------------------------- K2c: apply rotation (+ OQPSK delay) -> M&M input
 // mmin has a 16-sample front pad: mmin[16 + n]; mmin[0..15] = last MM_HIST inputs of the previous batch (hist_in).
 // `src` is the Costas output (or, with order == 0, the FIR output passed straight through).
@@ -1734,9 +1742,11 @@ struct MMRec { int u_final, count, skip, pad; float mu_final, omega_final; int h
 // GARDNER: dsp::GardnerClockRecoveryBlock<complex_t>::work (clock_recovery_gardner.cpp:33-131, SURVEY row G) instead of the M&M
 // detector: same interpolator bank, omega / mu updates, history and segmentation; the error is zc * (last - sample) with a second
 // interpolation half a symbol back (window u - offzc - 7 .. u - offzc); `p1` after the delay-line shift is last_sample.
-// Fused input fix-up (rot_order != 0 or oqpsk): mmin is then the Costas loop's raw output, and every thread applies the exact
+// FIX: fused input fix-up (rot_order != 0 or oqpsk): mmin is then the Costas loop's raw output, and every thread applies the exact
 // rotation by its row's quad[] entry (and the OQPSK one-sample delay of the imaginary rail, delay_one_imag.cpp:18-25) to each 16-sample
-// row of its ring right after the row has landed, instead of a separate pass over the whole stream (k_rotate).
+// row of its ring right after the row has landed, instead of a separate pass over the whole stream (k_rotate). Its state (quadrant,
+// masks, OQPSK carry) would stay live through the symbol loop, which runs at 128 registers: the instantiation without FIX, for input
+// that needs no fix-up, carries none of it.
 // 8 consecutive samples n0 .. n0+7 of this thread's ring (sample n sits in 16-byte chunk slot (n >> 1) & 31 of the swizzled strip): five
 // 128-bit loads and a select per value on the parity of n0, instead of eight 64-bit loads with their own address arithmetic.
 __device__ __forceinline__ void mm_fetch8(const float4 *__restrict__ ring, int n0, int lane, float2 (&x)[8])
@@ -1758,7 +1768,7 @@ __device__ __forceinline__ void mm_fetch8(const float4 *__restrict__ ring, int n
     }
 }
 
-template <bool STRICT, bool GARDNER>
+template <bool STRICT, bool GARDNER, bool FIX>
 __global__ void __launch_bounds__(SEG_THREADS) k_mm(const float2 *__restrict__ mmin /* 16-sample front pad */, long N, int L, int W, int G, int nseg,
                                                      MMParams P, const MMState *__restrict__ st_in, MMState *__restrict__ st_out,
                                                      const float *__restrict__ bank /*128x8*/, float2 *__restrict__ slots, int cap,
@@ -1835,21 +1845,43 @@ __global__ void __launch_bounds__(SEG_THREADS) k_mm(const float2 *__restrict__ m
     load(r0, active);
     load(r0 + 1, active);
     float carry_im = 0.f; // OQPSK: imaginary part (after rotation) of the sample in front of the next row
+    // quadrant of the segment holding the first sample of the last row fixed, and the first row whose first sample lies in a later
+    // segment: rows are fixed in increasing order, so quad[] is read once per segment the thread's rows enter (normally s-1 and s)
+    // instead of once per row, where the global load waited behind the whole SM's row copies and symbol stores. Rows in front of
+    // sample 0 (the front pad) keep q = 0: they come first, before any load.
+    // For orders 2 and 4 the rotation is q * 4 / order quarter turns, applied as a swap and two sign flips chosen once per quadrant
+    // (rot_quarter): the lanes of a warp hold different segments, and rot_steps' branch on q ran the lanes of each quadrant one
+    // after the other for every sample. Order 8 keeps rot_steps (its odd steps multiply).
+    int q = 0, qrow_next = 0;
+    const bool quarter = rot_order == 2 || rot_order == 4;
+    bool qswap = false;
+    unsigned qneg_re = 0, qneg_im = 0;
     auto fixrow = [&](int row) {
-        if (!active || row >= rend || (!rot_order && !oqpsk))
+        if (!FIX || !active || row >= rend || (!rot_order && !oqpsk))
             return;
-        int q = 0;
-        if (rot_order && row >= 0)
-            q = quad[(16 * row) / L];
+        if (rot_order && row >= qrow_next) {
+            const int sq = (16 * row) / L;
+            q = quad[sq];
+            qrow_next = (int)(((long)(sq + 1) * L + 15) >> 4);
+            const int k = quarter ? q * (4 / rot_order) : 0;
+            qswap = k & 1;
+            qneg_re = ((k + 1) & 2) ? 0x80000000u : 0u;
+            qneg_im = (k & 2) ? 0x80000000u : 0u;
+        }
         if (q == 0 && !oqpsk)
             return;
         const int sb = (row << 3) + 64;
+        float4 v[8]; // the whole row in registers first, so that the eight loads are in flight together
+#pragma unroll
+        for (int c = 0; c < 8; c++)
+            v[c] = ring[swz16((sb + c) & 31, lane)];
 #pragma unroll
         for (int c = 0; c < 8; c++) {
-            const int idx = swz16((sb + c) & 31, lane);
-            float4 v = ring[idx];
-            float2 a = make_float2(v.x, v.y), b = make_float2(v.z, v.w);
-            if (q) {
+            float2 a = make_float2(v[c].x, v[c].y), b = make_float2(v[c].z, v[c].w);
+            if (quarter) {
+                a = rot_quarter(a, qswap, qneg_re, qneg_im);
+                b = rot_quarter(b, qswap, qneg_re, qneg_im);
+            } else if (q) {
                 a = rot_steps(a, q, rot_order);
                 b = rot_steps(b, q, rot_order);
             }
@@ -1859,8 +1891,11 @@ __global__ void __launch_bounds__(SEG_THREADS) k_mm(const float2 *__restrict__ m
                 b.y = ta;
                 carry_im = tb;
             }
-            ring[idx] = make_float4(a.x, a.y, b.x, b.y);
+            v[c] = make_float4(a.x, a.y, b.x, b.y);
         }
+#pragma unroll
+        for (int c = 0; c < 8; c++)
+            ring[swz16((sb + c) & 31, lane)] = v[c];
     };
     const long emit0 = (s == 0 || repair_list) ? min(own0, u) : own0 - MM_ZONE;
     float2 *my = slots + (long)s * cap;

@@ -19,6 +19,7 @@
  *                    src-core/pipeline/modules/ccsds/module_ccsds_turbo_decoder.cpp:137-235      (kind TURBO)
  *                    plugins/noaa_metop_support/metop/module_metop_dump_decoder.cpp:27-83        (kind METOP_DUMP)
  *                    plugins/meteor_support/meteor/module_meteor_lrpt_decoder.cpp:101-262        (kind METEOR_LRPT)
+ *                    plugins/eos_support/aqua/module_aqua_db_decoder.cpp:27-83                    (kind AQUA_DB)
  *   b200_chain_*   both modules joined the way Pipeline::run joins them with a byte FIFO
  *                    src-core/pipeline/pipeline_run.cpp:44-117 — here the int8 soft stream never leaves HBM.
  *   b200_demux_*   the step behind the decoder: CADUs -> CCSDS space packets
@@ -50,7 +51,8 @@ enum { B200_BPSK = 0, B200_QPSK = 1, B200_OQPSK = 2, B200_8PSK = 3, B200_NONE = 
 enum { B200_CF32 = 0, B200_CS16 = 1, B200_CS8 = 2 };
 /* decoder kind */
 enum { B200_FEC_METOP = 0, B200_FEC_CCSDS = 1, B200_FEC_SIMPLE = 2, B200_FEC_LDPC = 3, B200_FEC_TURBO = 4, B200_FEC_METOP_DUMP = 5,
-       B200_FEC_METEOR_LRPT = 6, B200_FEC_NOAA_HRPT = 7 /* noaa_hrpt_decoder */, B200_FEC_METEOR_HRPT = 8 /* meteor_hrpt_decoder */ };
+       B200_FEC_METEOR_LRPT = 6, B200_FEC_NOAA_HRPT = 7 /* noaa_hrpt_decoder */, B200_FEC_METEOR_HRPT = 8 /* meteor_hrpt_decoder */,
+       B200_FEC_AQUA_DB = 9 /* aqua_db_decoder */ };
 /* debug stage ids for b200_demod_debug_stage */
 enum { B200_STAGE_AGC = 0, B200_STAGE_FIR = 1, B200_STAGE_COSTAS = 2, B200_STAGE_RESAMP = 3, B200_STAGE_DC = 4, B200_STAGE_MM = 5,
        B200_STAGE_PLL = 6 /* pm_demod: PLLCarrierTrackingBlock output */, B200_STAGE_PM = 7 /* pm_demod: PMToBPSK output */ };
@@ -174,6 +176,12 @@ typedef struct b200_fec_cfg
        inversion; the ASM 0x1ACFFC1D machine with states 0 / 2 / 6 / 12 (each its own error threshold); every accepted ASM is followed by
        a frame written as 1A CF FC 1D + the next 8160 bits, returned when complete (cadu_bytes = 1024). Only device and max_soft are read.
        Both: device memory about 1.3 bytes per max_soft byte (FIFO, hard bits, sync bitmap) plus the output; max_soft <= 2^30. */
+    /* kind B200_FEC_AQUA_DB = aqua_db_decoder (module_aqua_db_decoder.cpp:27-83, no parameters): per soft pair (I, Q) the QPSK hard symbol
+       2*(Q>0) + (I>0); rail A = Q > 0, rail B = I > 0, each through its own NRZMDiff::decode_bits carried across pushes, interleaved A B A B
+       -> BPSK_CCSDS_Deframer(8192, 0x1ACFFC1D) with its SYNCED state (and SYNCED error threshold) 10 instead of 12 -> derandomiser from
+       byte 4 -> RS(255,223) I=4 dual basis; every frame is written as 1A CF FC 1D + 1020 bytes, whatever RS returned (cadu_bytes 1024).
+       deframer_state reports 2 / 6 / 10. A push that ends inside a symbol keeps its odd byte for the next push. Only device and max_soft
+       are read; max_soft <= 2^30. Device memory: about 1.4 bytes per max_soft byte (soft FIFO, bit FIFO, room for two pushes of CADUs). */
     int deframer_thresold;    /* "deframer_thresold" of noaa_hrpt_decoder (required by the module): 0 .. 60                              */
 } b200_fec_cfg;
 
@@ -202,7 +210,7 @@ typedef struct b200_fec_stats
     long soft_in, chunks, bits_out, frames_out;
     int viterbi_state;        /* 0 NOSYNC 1 SYNCED  (Viterbi3_4::getState)                       */
     float viterbi_ber;
-    int deframer_state;       /* 2 NOSYNC / 6 SYNCING / 12|18 SYNCED (BPSK_CCSDS_Deframer); meteor_hrpt_decoder: its own state
+    int deframer_state;       /* 2 NOSYNC / 6 SYNCING / 12|18 SYNCED (BPSK_CCSDS_Deframer; aqua_db_decoder: 10); meteor_hrpt_decoder: its own state
                                  numbers 0 (NOSYNC) / 2, 6 (SYNCING) / 12 (SYNCED, "deframer_lock"); noaa_hrpt_decoder: 0           */
     long rs_corrected, rs_failed;
     long replays;             /* slow-path re-decodes (lock changes, start-state mis-speculation) */

@@ -352,6 +352,33 @@ def meteor_hrpt_cfg(device=0, max_soft=1 << 24):
     return cfg
 
 
+def terra_db_demod_kwargs(samplerate, symbolrate, fmt="cs16"):
+    """demod_cfg arguments of terra_db_demod (module_terra_db_demod.cpp:21-31): psk_demod's BPSK chain at twice the symbol rate (RRC alpha
+    0.5, Costas bw 0.004 with a 1 MHz frequency limit, M&M gains pow(0.001, 2) / 4 and 0.001, mu 0.5, limit 1e-4; soft = clamp(real * 50)),
+    at the working rate BaseDemodModule::initb picks for the real symbol rate. Raises ValueError, naming samplerate, when that rate gives
+    fewer than 1.1 samples per half-symbol."""
+    work = final_samplerate_of(samplerate, symbolrate, "bpsk")
+    if np.float32(work) / np.float32(2 * int(symbolrate)) < np.float32(1.1):
+        raise ValueError(f"terra_db_demod: samplerate {int(work)} gives fewer than 1.1 samples per half-symbol at symbolrate {int(symbolrate)}")
+    return dict(samplerate=samplerate, symbolrate=2 * int(symbolrate), constellation="bpsk", rrc_alpha=0.5, pll_bw=0.004, fmt=fmt,
+                clock_gain_omega=float(np.float32(pow(0.001, 2) / 4.0)), clock_mu=0.5, clock_gain_mu=0.001, clock_omega_limit=1e-4,
+                costas_max_offset=float(np.float32(2.0 * np.pi * (1e6 / work))),
+                final_samplerate=0.0 if work == float(int(samplerate)) else work)
+
+
+def terra_db_demod_cfg(samplerate, symbolrate, fmt="cs16", device=0, max_batch=1 << 24, **kw):
+    """terra_db_demod's chain as a b200_demod_cfg (terra_db_demod_kwargs)."""
+    return demod_cfg(**terra_db_demod_kwargs(samplerate, symbolrate, fmt), device=device, max_batch=max_batch, **kw)
+
+
+def aqua_db_cfg(device=0, max_soft=1 << 24):
+    """aqua_db_decoder (module_aqua_db_decoder.cpp, Aqua and Aura DB): the module takes no parameters; 1024-byte CADUs, every frame
+    written whatever RS returned."""
+    cfg = FecCfg()
+    cfg.kind, cfg.constellation, cfg.cadu_size, cfg.device, cfg.max_soft = 9, CONST["qpsk"], 8192, device, max_soft
+    return cfg
+
+
 def fec_cfg_for(sig, max_soft, device=0):
     """The decoder configuration that goes with a satdump_b200.synth.SignalCfg (metop_ahrpt_decoder / ccsds_conv_concat_decoder /
     ccsds_simple_psk_decoder parameters of the shipped pipeline JSONs)."""
@@ -365,6 +392,8 @@ def fec_cfg_for(sig, max_soft, device=0):
         return noaa_hrpt_cfg(sig.deframer_thresold, device=device, max_soft=max_soft)
     if sig.decoder == "meteor_hrpt":
         return meteor_hrpt_cfg(device=device, max_soft=max_soft)
+    if sig.decoder == "aqua_db":
+        return aqua_db_cfg(device=device, max_soft=max_soft)
     if sig.decoder == "turbo":
         return turbo_cfg(sig.turbo_rate, sig.turbo_base, sig.turbo_iters, device=device, max_soft=max_soft)
     if sig.decoder == "ldpc":

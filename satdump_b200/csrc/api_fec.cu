@@ -93,7 +93,8 @@ Fec::Fec(const b200_fec_cfg &in) : cfg(meteor_m2x_as_ccsds(in))
 {
     const b200_fec_cfg c = cfg;
     B200_REQUIRE(c.kind == B200_FEC_METOP || c.kind == B200_FEC_CCSDS || c.kind == B200_FEC_SIMPLE || c.kind == B200_FEC_LDPC || c.kind == B200_FEC_TURBO ||
-                     c.kind == B200_FEC_METOP_DUMP || c.kind == B200_FEC_METEOR_LRPT || c.kind == B200_FEC_NOAA_HRPT || c.kind == B200_FEC_METEOR_HRPT,
+                     c.kind == B200_FEC_METOP_DUMP || c.kind == B200_FEC_METEOR_LRPT || c.kind == B200_FEC_NOAA_HRPT || c.kind == B200_FEC_METEOR_HRPT ||
+                     c.kind == B200_FEC_AQUA_DB,
                  B200_EINVAL, "unknown decoder kind %d", c.kind);
     B200_REQUIRE(c.max_soft >= 65536, B200_EINVAL, "max_soft must be >= 65536");
     memset(&geom, 0, sizeof(geom));
@@ -107,6 +108,8 @@ Fec::Fec(const b200_fec_cfg &in) : cfg(meteor_m2x_as_ccsds(in))
         framed = meteor_decoder(*this);
     else if (c.kind == B200_FEC_NOAA_HRPT || c.kind == B200_FEC_METEOR_HRPT)
         framed = hrpt_decoder(*this);
+    else if (c.kind == B200_FEC_AQUA_DB)
+        framed = aqua_decoder(*this);
     if (framed)
         return;
     if (c.kind != B200_FEC_METOP) {
@@ -664,6 +667,7 @@ void Fec::deframe_and_rs(long new_bits)
 void Fec::start_stream(size_t fifo_bytes)
 {
     soft_have = 0;
+    swapped = 0;
     fifo_bits = 32;
     vit_state = 0; invalid = 0; main_next_start = -1; enc_state = 0; nrzm_last = 0; nosync_runs = 0;
     in_buffer = 0; changing_shift = 0; is_first = got_extra = false; buf_value = 128; test_bit_len = 0; pdec_start = -1;
@@ -783,8 +787,9 @@ void Framed::finish(int nf, long soft_have)
     tail_seen = soft_have;
 }
 
-// The deframer and frame stage behind another decoder (ccsds_ldpc_decoder's internal_stream): storage for `max_new_bits` new bits per
-// push, as the constructor allocates it for the convolutional decoders; cfg holds the deframer's cadu_size / asm_sync, rs_i = 0.
+// The deframer and frame stage behind another decoder (ccsds_ldpc_decoder's internal_stream, aqua_db_decoder): storage for `max_new_bits`
+// new bits per push, as the constructor allocates it for the convolutional decoders; cfg holds the deframer's cadu_size / asm_sync and the
+// frame stage's RS settings (rs_usecheck is not built here).
 void Fec::deframer_storage(long max_new_bits)
 {
     fifo.alloc((size_t)((max_new_bits + 2L * cfg.cadu_size + 4096) / 32 + 8));
@@ -794,14 +799,14 @@ void Fec::deframer_storage(long max_new_bits)
     frames.alloc(max_frames_push);
     frames_out.alloc((size_t)(2 * max_frames_push + 4) * cadu_bytes);
     frames_tmp.alloc(1);
-    rs_err.alloc((size_t)max_frames_push + 4);
+    rs_err.alloc((size_t)(max_frames_push + 4) * std::max(1, cfg.rs_i));
     frame_dst.alloc((size_t)max_frames_push + 4);
     counters.alloc(8);
     tables.alloc(1);
     h_counters.alloc(8);
     h_dstate.alloc(2);
     h_events.alloc(4096);
-    h_rs_err.alloc(max_frames_push + 4);
+    h_rs_err.alloc((size_t)(max_frames_push + 4) * std::max(1, cfg.rs_i));
     RsTables T;
     build_rs_tables(T);
     B200_CUDA(cudaMemcpyAsync(tables.p, &T, sizeof(T), cudaMemcpyHostToDevice, stream));
@@ -1046,12 +1051,32 @@ void Fec::decode_conv(long nch)
     }
 }
 
+// rotate_soft(buffer, size, PHASE_0, true) of ccsds_conv_concat_decoder with "bpsk_90" or "iq_invert"
+// (module_ccsds_conv_concat_decoder.cpp:149-150): the two bytes of every soft pair swapped, pairs counted from the stream's start
+static __global__ void k_swap_pairs(int8_t *__restrict__ soft, long npairs)
+{
+    for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < npairs; i += (long)gridDim.x * blockDim.x) {
+        const int8_t t = soft[2 * i];
+        soft[2 * i] = soft[2 * i + 1];
+        soft[2 * i + 1] = t;
+    }
+}
+
 void Fec::process()
 {
     DeviceGuard g(cfg.device);
     if (framed) {
         framed->process(*this);
         return;
+    }
+    if (cfg.kind == B200_FEC_CCSDS && (cfg.constellation == B200_BPSK_90 || cfg.iq_invert)) {
+        // every complete pair not swapped yet (the FIFO starts on a pair boundary: chunks are even)
+        const long npairs = (soft_have & ~1L) / 2 - swapped / 2;
+        if (npairs > 0) {
+            k_swap_pairs<<<(unsigned)std::min<long>((npairs + 255) / 256, 132 * 16), 256, 0, stream>>>(softbuf.p + swapped, npairs);
+            launches++;
+            swapped += 2 * npairs;
+        }
     }
     const long nch = soft_have / geom.chunk;
     B200_REQUIRE(nch <= max_chunks, B200_ESTATE, "internal: too many chunks");
@@ -1075,6 +1100,7 @@ void Fec::process()
         decode_conv(nch);
     total_chunks += nch;
     keep_soft_tail(nch * (long)geom.chunk);
+    swapped = std::max(0L, swapped - nch * (long)geom.chunk);
     B200_CUDA(cudaEventRecord(ev[1], stream));
     B200_CUDA(cudaStreamSynchronize(stream));
     B200_CUDA(cudaGetLastError());

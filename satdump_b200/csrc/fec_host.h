@@ -51,6 +51,7 @@ std::unique_ptr<Framed> turbo_decoder(Fec &f);
 std::unique_ptr<Framed> dump_decoder(Fec &f);
 std::unique_ptr<Framed> meteor_decoder(Fec &f);
 std::unique_ptr<Framed> hrpt_decoder(Fec &f); // noaa_hrpt_decoder, meteor_hrpt_decoder (api_hrpt.cu)
+std::unique_ptr<Framed> aqua_decoder(Fec &f); // aqua_db_decoder (api_aqua.cu): the deframer and frame stage behind its own bit stage
 
 class Fec
 {
@@ -155,6 +156,7 @@ class Fec
 
     // stream state
     long soft_have = 0, max_chunks = 0, fifo_bits = 32, max_frames_push = 0;
+    long swapped = 0; // bpsk_90 / iq_invert: FIFO bytes whose pairs are already swapped
     int vit_state = 0, invalid = 0, main_next_start = -1, enc_state = 0, nrzm_last = 0, nosync_runs = 0;
     VitHyp hyp{0, 0, 0};
     VitIdleState idle_st{-1, 0};
@@ -172,6 +174,7 @@ class Fec
     friend struct Dump;
     friend struct Meteor;
     friend struct Hrpt;
+    friend struct Aqua;
     // the main deframer and the frame counters at a point a pass may have to roll back to
     struct Mark { DefrState h_dstate; long fifo_bits, out_frames, total_frames, rs_corrected, rs_failed; int defr_state_now; };
     Mark mark();

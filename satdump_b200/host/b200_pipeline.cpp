@@ -7,9 +7,12 @@
 #include <cstring>
 using namespace b200host;
 
-// the module stats of the HRPT decoders (module_noaa_hrpt_decoder.cpp:47-52, module_meteor_hrpt_decoder.cpp:52-60); frames: output units
+// the module stats of the HRPT and Aqua DB decoders (module_noaa_hrpt_decoder.cpp:47-52, module_meteor_hrpt_decoder.cpp:52-60,
+// module_aqua_db_decoder.cpp:83-93); frames: output units
 static void print_hrpt_stats(const std::string &dec, long frames, int state)
 {
+    if (dec == "aqua_db_decoder")
+        printf("deframer_state %s\n", state == 2 ? "NOSYNC" : (state == 6 ? "SYNCING" : "SYNCED"));
     if (dec == "noaa_hrpt_decoder")
         printf("frame_count %ld\n", frames / 11090);
     if (dec == "meteor_hrpt_decoder")
@@ -20,7 +23,7 @@ static void print_hrpt_stats(const std::string &dec, long frames, int state)
 int main(int argc, char **argv)
 {
     if (argc < 5) {
-        fprintf(stderr, "usage: %s <metop_ahrpt|jpss_hrd|npp_hrd|simple_bpsk|simple_qpsk|pm_bpsk|ldpc_qpsk|landsat|turbo_pm|turbo_bpsk|metop_dump|meteor_lrpt|noaa_hrpt|meteor_hrpt> baseband <input> <output_hint> [--fused] [--key value ...]\n", argv[0]);
+        fprintf(stderr, "usage: %s <metop_ahrpt|jpss_hrd|npp_hrd|simple_bpsk|simple_qpsk|pm_bpsk|ldpc_qpsk|landsat|turbo_pm|turbo_bpsk|metop_dump|meteor_lrpt|noaa_hrpt|meteor_hrpt|aqua_db|aura_db|terra_db> baseband <input> <output_hint> [--fused] [--key value ...]\n", argv[0]);
         return 2;
     }
     const std::string pipe = argv[1], level = argv[2], in = argv[3], out = argv[4];
@@ -45,6 +48,16 @@ int main(int argc, char **argv)
         if (noaa)
             fp = Params{{"deframer_thresold", "10"}};
         dec = noaa ? "noaa_hrpt_decoder" : "meteor_hrpt_decoder";
+    } else if (pipe == "aqua_db" || pipe == "aura_db") { // resources/pipelines/EOS.json "aqua_db", "aura_db": OQPSK at 7.5 Msym/s, 15 MS/s
+        dp = Params{{"constellation", "oqpsk"}, {"symbolrate", "7500000"}, {"rrc_alpha", "0.5"}, {"pll_bw", "0.006"}, {"clock_gain_omega", "0.8"},
+                    {"clock_mu", "0.9"}, {"clock_gain_mu", "0.037"}, {"clock_omega_relative_limit", "0.0001"}, {"costas_max_offset", "1e6"}};
+        dec = "aqua_db_decoder";
+    } else if (pipe == "terra_db") { // resources/pipelines/EOS.json "terra_db": terra_db_demod at 13.125 Msym/s, 45 MS/s, then
+        // ccsds_conv_concat_decoder (bpsk_90, NRZ-M, RS I=4, the derandomiser after RS from byte 10)
+        dp = Params{{"b200_demod_module", "terra_db_demod"}, {"symbolrate", "13125000"}};
+        fp = Params{{"constellation", "bpsk_90"}, {"cadu_size", "8192"}, {"viterbi_ber_thresold", "0.300"}, {"viterbi_outsync_after", "20"},
+                    {"derandomize", "true"}, {"derand_after_rs", "true"}, {"derand_start", "10"}, {"nrzm", "true"}, {"rs_i", "4"}, {"rs_type", "rs223"}};
+        dec = "ccsds_conv_concat_decoder";
     } else if (pipe == "jpss_hrd" || pipe == "npp_hrd") { // resources/pipelines/JPSS.json
         dp = Params{{"constellation", "oqpsk"}, {"symbolrate", pipe == "jpss_hrd" ? "25000000" : "15000000"}, {"rrc_alpha", "0.5"}, {"pll_bw", "0.002"}};
         fp = Params{{"constellation", "oqpsk"}, {"cadu_size", "10232"}, {"viterbi_ber_thresold", "0.3"}, {"viterbi_outsync_after", "20"},

@@ -108,10 +108,67 @@ static void reject(const Params &p, const char *key, const char *why)
         throw ModuleError(std::string("parameter '") + key + "' is not supported by the B200 path (" + why + "); there is no CPU fallback");
 }
 
+// terra_db_demod (module_terra_db_demod.cpp:21-31,84): BaseDemodModule::initb, then RRC(1, final_samplerate, symbolrate * 2, 0.5, 31),
+// CostasLoopBlock(0.004, order 2, hz_to_rad(1e6, final_samplerate)), MMClockRecoveryBlock(((float)final_samplerate / (float)symbolrate) / 2,
+// pow(0.001, 2) / 4, 0.5, 0.001, 1e-4) and soft = clamp(real * 50): psk_demod's BPSK chain at twice the symbol rate (one soft byte per
+// half-symbol), with the working rate chosen for the real symbol rate in BaseDemodModule's window [1.1, 4.0]
+static b200_demod_cfg terra_db_demod_cfg_from_params(const Params &p, bool &is_bpsk)
+{
+    b200_demod_cfg c{};
+    if (!p.has("samplerate"))
+        throw ModuleError("Samplerate parameter must be present!"); // module_demod_base.cpp:17-20
+    c.samplerate = (double)(long)p.num("samplerate");
+    if (!p.has("symbolrate"))
+        throw ModuleError("Symbolrate parameter must be present!"); // module_demod_base.cpp:26-27
+    const double rs = (double)(long)p.num("symbolrate");
+    c.symbolrate = 2.0 * rs;
+    c.constellation = B200_BPSK;
+    is_bpsk = true;
+    c.rrc_alpha = 0.5f;
+    c.rrc_taps = 31;
+    c.pll_bw = 0.004f;
+    c.agc_rate = (float)p.num("agc_rate", 1e-2);
+    c.clock_gain_omega = (float)(pow(0.001, 2) / 4.0);
+    c.clock_mu = 0.5f;
+    c.clock_gain_mu = 0.001f;
+    c.clock_omega_limit = 0.0001f;
+    const std::string fmt = p.str("baseband_format", "cf32");
+    if (fmt == "cf32" || fmt == "f32") c.format = B200_CF32;
+    else if (fmt == "cs16" || fmt == "s16") c.format = B200_CS16;
+    else if (fmt == "cs8" || fmt == "s8") c.format = B200_CS8;
+    else if (fmt == "ziq") c.format = -1;
+    else throw ModuleError("baseband_format " + fmt + " is not supported by the B200 path (cf32/cs16/cs8, uncompressed ziq)");
+    c.dc_block = p.flag("dc_block", false);
+    c.freq_shift = (double)(long)p.num("freq_shift", 0);
+    c.iq_swap = p.flag("iq_swap", false);
+    reject(p, "enable_doppler", "Doppler correction");
+    reject(p, "dump_intermediate", "intermediate dump");
+    const float min_sps = (float)p.num("min_sps", 0), max_sps = (float)p.num("max_sps", 0);
+    c.final_samplerate = b200_demod_final_samplerate(c.samplerate, rs, B200_BPSK, min_sps, max_sps,
+                                                     p.has("custom_samplerate") ? (double)(long)p.num("custom_samplerate") : 0.0);
+    const double work = c.final_samplerate;
+    if (c.final_samplerate == c.samplerate)
+        c.final_samplerate = 0;
+    else if (!b200_demod_resample_decision(c.samplerate, rs, B200_BPSK, min_sps, max_sps))
+        c.front_resample = 2;
+    if ((float)c.samplerate / (float)rs < 1.0f) // module_demod_base.cpp:96-105
+        throw ModuleError("Your sampling rate is too low! Minimum: " + std::to_string(rs / 1e6) + " Msps");
+    // the loops run at half-symbol rate: a working rate inside [1.1, 4.0] samples per symbol can be below 1.1 per half-symbol
+    const float half_sps = (float)work / (float)c.symbolrate;
+    if (half_sps < 1.1f)
+        throw ModuleError("terra_db_demod: samplerate " + std::to_string((long)work) + " gives " + std::to_string(half_sps) +
+                          " samples per half-symbol at symbolrate " + std::to_string((long)rs) + "; the loops need at least 1.1");
+    c.costas_max_offset = (float)(2.0 * M_PI * (1e6 / work)); // dsp::hz_to_rad(1e6, final_samplerate)
+    c.device = (int)p.num("b200_device", 0);
+    return c;
+}
+
 b200_demod_cfg demod_cfg_from_params(const Params &p, bool &is_bpsk, const std::string &module_id)
 {
     if (module_id == "pm_demod")
         return pm_demod_cfg_from_params(p, is_bpsk);
+    if (module_id == "terra_db_demod")
+        return terra_db_demod_cfg_from_params(p, is_bpsk);
     b200_demod_cfg c{};
     if (!p.has("samplerate"))
         throw ModuleError("Samplerate parameter must be present!"); // module_demod_base.cpp:17-20
@@ -273,6 +330,13 @@ b200_fec_cfg fec_cfg_from_params(const std::string &id, const Params &p)
         c.deframer_thresold = (int)p.num("deframer_thresold");
         if (c.deframer_thresold < 0 || c.deframer_thresold > 60) // (a 60-bit window is within 60 of anything: the bound of the library)
             throw ModuleError("noaa_hrpt_decoder: deframer_thresold must be 0..60 (got " + std::to_string(c.deframer_thresold) + ")");
+        return c;
+    }
+    if (id == "aqua_db_decoder") { // module_aqua_db_decoder.cpp:16-22: no parameters; 1024-byte CADUs (Aqua and Aura DB)
+        c.kind = B200_FEC_AQUA_DB;
+        c.device = (int)p.num("b200_device", 0);
+        c.constellation = B200_QPSK;
+        c.cadu_size = 8192;
         return c;
     }
     if (id == "meteor_hrpt_decoder") { // module_meteor_hrpt_decoder.cpp:14-20: no parameters; 1024-byte CADUs
@@ -484,7 +548,7 @@ static void check(int rc, const char *what)
 PskDemodStage::PskDemodStage(std::string in, std::string hint, Params p, std::string module_id)
     : StageBase(std::move(in), std::move(hint), std::move(p)), id(std::move(module_id))
 {
-    if (id != "psk_demod" && id != "pm_demod")
+    if (id != "psk_demod" && id != "pm_demod" && id != "terra_db_demod")
         throw ModuleError("unknown demodulator module " + id);
     cfg = demod_cfg_from_params(params, is_bpsk, id);
     batch_samples = (long)params.num("b200_batch_samples", (double)batch_samples);

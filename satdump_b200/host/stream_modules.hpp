@@ -89,7 +89,9 @@ class StageBase
 // psk_demod: required samplerate, constellation, rrc_alpha, pll_bw (+ symbolrate); optional as in SURVEY.md App. B.
 // Options whose blocks are not part of this build (has_carrier, doppler, dump_intermediate) raise ModuleError instead of silently doing
 // something else. module_id "pm_demod": PMDemodModule's parameter set (pll_bw = the carrier PLL's, costas_bw, pll_max_offset,
-// resample_after_pll, subcarrier_offset), soft = clamp(real * 100), stats key "freq" = the carrier PLL's frequency.
+// resample_after_pll, subcarrier_offset), soft = clamp(real * 100), stats key "freq" = the carrier PLL's frequency. module_id
+// "terra_db_demod": TerraDBDemodModule's fixed chain (BPSK loops at twice "symbolrate"); a working rate below 1.1 samples per half-symbol
+// is refused by name.
 class PskDemodStage : public StageBase
 {
   public:
@@ -131,6 +133,7 @@ class FecStage : public StageBase
     std::atomic<int> crc_lock{0};
     // meteor_lrpt_decoder: "rs_avg" of the last frame; m2x_mode 0: correlator_lock, viterbi_ber (module_meteor_lrpt_decoder.cpp:266-289)
     // noaa_hrpt_decoder: "frame_count" = frames_written (words) / 11090; meteor_hrpt_decoder: deframer_state (0 / 2 / 6 / 12), frame_count
+    // aqua_db_decoder: deframer_state (2 / 6 / 10) above
     std::atomic<int> rs_avg{0};
     std::atomic<long> frames_written{0};
     b200_fec_cfg cfg{};

@@ -323,6 +323,16 @@ CONFIGS = {
                            decoder="noaa_hrpt", esn0_db=20.0, pll_bw=0.005, pm_pll_bw=0.01, carrier_rad=2e-2, pm_index=1.0, deframer_thresold=10),
     "meteor_hrpt": SignalCfg(name="meteor_hrpt", samplerate=3e6, symbolrate=665400, constellation="bpsk", conv="none", rrc_alpha=0.5, fmt="cs16",
                              decoder="meteor_hrpt", esn0_db=20.0, pll_bw=0.005, pm_pll_bw=0.01, carrier_rad=2e-2, pm_index=1.0),
+    # psk_demod OQPSK -> aqua_db_decoder, EOS Aqua / Aura DB (EOS.json "aqua_db", "aura_db"): 7.5 Msym/s recorded at 15 MS/s (2 samples per
+    # symbol), two NRZ-M rails of randomised CADUs with RS(255,223) I=4 dual basis, no convolutional code. The receiver's clock and Costas
+    # parameters are the pipeline's (tests/eos_cases.aqua_demod_cfg); the signal starts in the phase the Costas loop keeps.
+    "aqua_db": SignalCfg(name="aqua_db", samplerate=15e6, symbolrate=7500000, constellation="oqpsk", conv="none", interleave=4, rrc_alpha=0.5,
+                         pll_bw=0.006, fmt="cs16", decoder="aqua_db", esn0_db=20.0, carrier_rad=1e-4, phase0=0.1),
+    # terra_db_demod -> ccsds_conv_concat_decoder, EOS Terra DB (EOS.json "terra_db"): 13.125 Msym/s recorded at 45 MS/s. The demodulator
+    # runs BPSK loops at twice the symbol rate (1.714 samples per half-symbol), so the signal is BPSK at 26.25 Mbaud carrying the r=1/2 code
+    # (terra_db_frames). The receiver's parameters are the module's (capi.terra_db_demod_kwargs); clock_alpha only stands in for them here.
+    "terra_db": SignalCfg(name="terra_db", samplerate=45e6, symbolrate=26250000, constellation="bpsk", conv="none", interleave=4, rrc_alpha=0.5,
+                          pll_bw=0.004, fmt="cs16", decoder="terra_db", esn0_db=12.0, carrier_rad=1e-4, phase0=0.1, clock_alpha=0.001),
 }
 
 
@@ -366,6 +376,15 @@ def make_bitstream(cfg: SignalCfg, nframes, seed):
     if cfg.decoder == "meteor_hrpt":  # nframes METEOR HRPT CADUs (no FEC)
         bits, cadu = meteor_hrpt_frames(nframes, seed)
         return bits.reshape(-1), cadu
+    if cfg.decoder == "aqua_db":  # nframes CADUs on two NRZ-M rails. psk_demod's OQPSK output pairs each Q symbol with the NEXT I
+        # symbol (the half-symbol-delayed Q is read with the I that follows it), so the I rail goes on air one symbol later
+        bits, clear = aqua_db_frames(nframes, seed)
+        I, Q = aqua_db_rails(bits)
+        coded = np.zeros(2 * I.size, np.uint8)
+        coded[2::2], coded[1::2] = I[:-1], Q
+        return coded, clear
+    if cfg.decoder == "terra_db":  # nframes CADUs, NRZ-M, r=1/2: one BPSK symbol per code symbol
+        return terra_db_frames(nframes, seed)
     if cfg.decoder == "ldpc":  # nframes LDPC frames
         if cfg.internal_cadu_size:
             info, clear = ldpc_inner_frames(nframes, cfg.internal_cadu_size, cfg.internal_asm, seed)
@@ -487,7 +506,9 @@ def frames_for_samples(cfg: SignalCfg, nsamples):
         return int(nsamples * bps / (cfg.samplerate / cfg.symbolrate) / 16384) + 2
     if cfg.decoder in ("noaa_hrpt", "meteor_hrpt"):  # bits on air: 110900 per NOAA minor frame, 8192 per METEOR CADU
         return int(nsamples / (cfg.samplerate / cfg.symbolrate) / (NOAA_WORDS * 10 if cfg.decoder == "noaa_hrpt" else 8192)) + 2
-    if cfg.decoder in ("ldpc", "dump"):  # LDPC frames / MetOp dump CADUs of 8192 bits
+    if cfg.decoder == "terra_db":  # 16384 code symbols per CADU, one per sample period of the half-symbol rate
+        return int(nsamples / (cfg.samplerate / cfg.symbolrate) / 16384) + 2
+    if cfg.decoder in ("ldpc", "dump", "aqua_db"):  # LDPC frames / MetOp dump and Aqua DB CADUs of 8192 bits
         return int(nsamples * bps / (cfg.samplerate / cfg.symbolrate) / 8192) + 2
     rate = {"1/2": 0.5, "3/4": 0.75, "none": 1.0, "p2/3": 2 / 3, "p3/4": 0.75, "p5/6": 5 / 6, "p7/8": 7 / 8}[cfg.conv]
     bits_per_sample = bps * rate / (cfg.samplerate / cfg.symbolrate)
@@ -836,6 +857,47 @@ def hrpt_soft(bits, inverted=False, amp=60.0, sigma=0.0, seed=0, slips=(), gaps=
         a = at
     pieces.append(s[a:][keep[a:]])
     return np.clip(np.round(np.concatenate(pieces)), -127, 127).astype(np.int8)
+
+
+# ---- EOS Aqua / Aura DB (aqua_db_decoder): randomised CADUs on two NRZ-M rails -----------------------------------------------------------
+def aqua_db_frames(nframes, seed=0):
+    """(decoded bits uint8 [n, 8192]: randomised CADUs with RS(255,223) I=4 dual basis, the CADUs aqua_db_decoder writes for them
+    [n, 1024]: the ASM and the derandomised codewords). The decoder's frame format is metop_dump_decoder's."""
+    return dump_frames(nframes, seed)
+
+
+def aqua_db_rails(bits):
+    """The hard symbols on air for the decoded stream A0 B0 A1 B1 ... (even length): each rail NRZ-M encoded on its own (the decoder's two
+    NRZMDiff::decode_bits, each starting from 0, undo it), rail A on Q and rail B on I, as constellation_t::soft_demod's 2*(Q>0) + (I>0)
+    and the module's demod >> 1, demod & 1 read them. Returns (I, Q) uint8."""
+    b = np.asarray(bits, np.uint8).reshape(-1)
+    return np.bitwise_xor.accumulate(b[1::2]), np.bitwise_xor.accumulate(b[0::2])
+
+
+def aqua_db_soft(bits, amp=60.0, sigma=0.0, seed=0, swap_iq=False):
+    """int8 soft pairs (I, Q) that aqua_db_decoder decodes to `bits` (bit 1 -> +amp); swap_iq: the rails on the wrong axes."""
+    I, Q = aqua_db_rails(bits)
+    if swap_iq:
+        I, Q = Q, I
+    out = np.empty(2 * I.size, np.float32)
+    out[0::2], out[1::2] = (2.0 * I - 1.0) * amp, (2.0 * Q - 1.0) * amp
+    if sigma:
+        out += np.random.default_rng(seed).normal(0, sigma, out.size).astype(np.float32)
+    return np.clip(np.round(out), -127, 127).astype(np.int8)
+
+
+def terra_db_frames(nframes, seed=0):
+    """(BPSK symbols on air as bits uint8, the CADUs ccsds_conv_concat_decoder writes for them [n, 1024]) of EOS.json "terra_db"'s decoder
+    (bpsk_90, nrzm, RS(255,223) I=4 dual basis, derand_after_rs from byte 10). The CADUs are sent as RS codewords without randomisation
+    (the receiver derandomises after RS), NRZ-M encoded and convolutionally encoded. The module swaps each soft pair and rotates it by 90
+    degrees, (s0, s1) -> (s0, -s1), so a code pair (a, b) goes on air as (a, not b)."""
+    payload = np.random.default_rng(seed).integers(0, 256, size=(nframes, 4 * 223), dtype=np.uint8)
+    tx, _ = build_cadus(payload, 4, randomize=False)
+    written = tx.copy()
+    written[:, 10:] ^= ccsds_pn(1014)[None, :]
+    coded = conv_encode(nrzm_encode(np.unpackbits(tx.reshape(-1))))
+    coded[1::2] ^= 1
+    return coded, written
 
 
 # ---- CCSDS turbo code (CCSDS 131.0-B section 6), as ccsds_turbo_decoder receives it ---------------------------------------------------

@@ -12,6 +12,7 @@
  *                    src-core/pipeline/modules/demod/module_demod_base.cpp:59-208   (initb: source, AGC)
  *                    plugins/dvb_support/dvbs2/module_dvbs2_demod.cpp:98-102        (AGC->RRC->M&M front half; constellation NONE)
  *                    src-core/pipeline/modules/demod/module_pm_demod.cpp:61-160      (PMDemodModule: cfg.pm_demod = 1)
+ *                    src-core/pipeline/modules/demod/module_fsk_demod.cpp:59-158     (FSKDemodModule: cfg.fsk_demod = 1)
  *   b200_fec_*     the decoder modules
  *                    plugins/noaa_metop_support/metop/module_metop_ahrpt_decoder.cpp:34-90      (kind METOP)
  *                    src-core/pipeline/modules/ccsds/module_ccsds_conv_concat_decoder.cpp:140-200 (kind CCSDS, r=1/2)
@@ -55,7 +56,10 @@ enum { B200_FEC_METOP = 0, B200_FEC_CCSDS = 1, B200_FEC_SIMPLE = 2, B200_FEC_LDP
        B200_FEC_AQUA_DB = 9 /* aqua_db_decoder */ };
 /* debug stage ids for b200_demod_debug_stage */
 enum { B200_STAGE_AGC = 0, B200_STAGE_FIR = 1, B200_STAGE_COSTAS = 2, B200_STAGE_RESAMP = 3, B200_STAGE_DC = 4, B200_STAGE_MM = 5,
-       B200_STAGE_PLL = 6 /* pm_demod: PLLCarrierTrackingBlock output */, B200_STAGE_PM = 7 /* pm_demod: PMToBPSK output */ };
+       B200_STAGE_PLL = 6 /* pm_demod: PLLCarrierTrackingBlock output */, B200_STAGE_PM = 7 /* pm_demod: PMToBPSK output */,
+       /* fsk_demod: one float per sample; B200_STAGE_FIR and B200_STAGE_MM then give one float per sample / symbol too */
+       B200_STAGE_QUAD = 8 /* QuadratureDemodBlock output */, B200_STAGE_DC2 = 9 /* CorrectIQBlock<float> output */,
+       B200_STAGE_AGC2 = 10 /* AGCBlock<float> output */ };
 /* mode bits of b200_demod_debug_run_stage */
 #define B200_DEBUG_STRICT 1     /* the reference's operation order: separate multiply and add, left to right (generic VOLK, no FMA) */
 #define B200_DEBUG_SEQUENTIAL 2 /* one segment: the feedback loop runs as ONE sequential thread from the initial state */
@@ -107,6 +111,12 @@ typedef struct b200_demod_cfg
     int has_carrier;
     float carrier_pll_bw;         /* "carrier_pll_bw" (required by the module in this mode)   */
     float carrier_pll_max_offset; /* "carrier_pll_max_offset", default 3.14                    */
+    /* fsk_demod (module_fsk_demod.cpp:13-84): the base front end and AGC -> QuadratureDemodBlock(1.0) -> CorrectIQBlock<float> ->
+       AGCBlock<float>(0.1, 0.5, 1.0, 65535) -> RRC (FIRBlock<float>) -> MMClockRecoveryBlock<float>; soft = clamp(symbol * 50), one byte
+       per symbol; b200_demod_pull_symbols returns one float per symbol. constellation must be B200_BPSK; pll_bw is not read. Not with
+       pm_demod, has_carrier, post_costas_dc or clock_recovery 1. The module's clock defaults differ from psk_demod's: gain_omega
+       pow(1.7e-2, 2) / 4, gain_mu 1.7e-2 (module_fsk_demod.h:28-31) */
+    int fsk_demod;
 } b200_demod_cfg;
 
 typedef struct b200_fec_cfg
@@ -264,7 +274,7 @@ int b200_demod_push_iq(b200_demod *d, const void *host_iq, long nsamples);
 int b200_demod_push_iq_device(b200_demod *d, const void *dev_iq, long nsamples);
 /* int8 soft symbols of the LAST push (I,Q interleaved; BPSK: I only) — the bytes PSKDemodModule writes to .soft / the FIFO */
 int b200_demod_pull_soft(b200_demod *d, int8_t *host_out, long cap, long *n_out);
-/* float symbols of the LAST push (M&M output, interleaved re,im) */
+/* float symbols of the LAST push (M&M output, interleaved re,im; fsk_demod: one float per symbol) */
 int b200_demod_pull_symbols(b200_demod *d, float *host_out, long cap_symbols, long *n_out);
 /* stage outputs of the LAST push (needs keep_stages): nsamples complex values, interleaved re,im */
 int b200_demod_debug_stage(b200_demod *d, int stage, float *host_out, long cap_samples);
@@ -274,6 +284,9 @@ int b200_demod_debug_stage(b200_demod *d, int stage, float *host_out, long cap_s
  *                      mode 0: the production kernel (k_agc_fir_w with the AGC switched off), one fma per tap
  *   B200_STAGE_COSTAS  in = FIR output; out = what the clock recovery reads (rotation fix-up, OQPSK delay, post_costas_dc applied)
  *   B200_STAGE_MM      in = the clock recovery's input; out = symbols (*n_out of them). STRICT | SEQUENTIAL -> bitwise the oracle's
+ * fsk_demod: B200_STAGE_QUAD (in = complex AGC output), DC2, AGC2, FIR and MM (in = the previous stage's output): one float per sample
+ *   in and out (QUAD: complex in). QUAD and FIR are always the reference's arithmetic; DC2 and AGC2 with SEQUENTIAL run the recurrence as
+ *   one float thread, MM as above.
  * SEQUENTIAL runs the loop as one segment (no warm-up, no stitching). The demodulator is reset before and after. */
 int b200_demod_debug_run_stage(b200_demod *d, int stage, const float *host_in, long nsamples, int mode, float *host_out, long cap_complex, long *n_out);
 /* Junction residuals of the LAST push / debug run: per segment s > 0 the Costas phase (mod 2pi/order) and frequency difference

@@ -6,7 +6,7 @@
 //
 //   loader()                          the one symbol SatDump dlsym()s (core/plugin.cpp:15-33)
 //   B200DSPSupport::init()            on SatDumpStartedEvent (fired after every plugin registered its modules, init.cpp:163) the
-//                                     entries "psk_demod", "pm_demod", "terra_db_demod", "metop_ahrpt_decoder", "ccsds_conv_concat_decoder", "ccsds_simple_psk_decoder", "ccsds_ldpc_decoder", "ccsds_turbo_decoder", "metop_dump_decoder", "meteor_lrpt_decoder", "noaa_hrpt_decoder", "meteor_hrpt_decoder" and "aqua_db_decoder" of
+//                                     entries "psk_demod", "pm_demod", "terra_db_demod", "fsk_demod", "metop_ahrpt_decoder", "ccsds_conv_concat_decoder", "ccsds_simple_psk_decoder", "ccsds_ldpc_decoder", "ccsds_turbo_decoder", "metop_dump_decoder", "meteor_lrpt_decoder", "noaa_hrpt_decoder", "meteor_hrpt_decoder" and "aqua_db_decoder" of
 //                                     satdump::pipeline::modules_registry (module.h:210, looked up first-match by id, module.cpp:129-135)
 //                                     get their factory replaced, so existing pipelines instantiate the CUDA modules.
 //                                     Set B200_DSP_REGISTER_ONLY=1 to register "<id>_b200" ids instead and leave the originals alone.
@@ -186,6 +186,13 @@ namespace b200plugin
         nlohmann::json getModuleStats() override
         {
             nlohmann::json v; // keys of PSKDemodModule::getModuleStats (module_psk_demod.cpp:238-246)
+            if (stage->getID() == "fsk_demod") // FSKDemodModule::getModuleStats (module_fsk_demod.cpp:160-167): no "freq"
+            {
+                v["progress"] = stage->progress.load();
+                v["snr"] = stage->snr.load();
+                v["peak_snr"] = stage->peak_snr.load();
+                return v;
+            }
             if (stage->getID() == "terra_db_demod") // TerraDBDemodModule::getModuleStats (module_terra_db_demod.cpp:138-144)
             {
                 v["snr"] = stage->snr.load();
@@ -296,14 +303,14 @@ public:
     using Factory = std::function<std::shared_ptr<satdump::pipeline::ProcessingModule>(std::string, std::string, nlohmann::json)>;
     static Factory factory(const std::string &id)
     {
-        if (id == "psk_demod" || id == "pm_demod" || id == "terra_db_demod")
+        if (id == "psk_demod" || id == "pm_demod" || id == "terra_db_demod" || id == "fsk_demod")
             return [id](std::string in, std::string hint, nlohmann::json p) { return std::make_shared<b200plugin::PskDemod>(id, in, hint, p); };
         return [id](std::string in, std::string hint, nlohmann::json p) { return std::make_shared<b200plugin::Decoder>(id, in, hint, p); };
     }
 
     static void registerHandler(const satdump::pipeline::RegisterModulesEvent &evt)
     {
-        for (const char *id : {"psk_demod", "pm_demod", "terra_db_demod", "metop_ahrpt_decoder", "ccsds_conv_concat_decoder", "ccsds_simple_psk_decoder", "ccsds_ldpc_decoder",
+        for (const char *id : {"psk_demod", "pm_demod", "terra_db_demod", "fsk_demod", "metop_ahrpt_decoder", "ccsds_conv_concat_decoder", "ccsds_simple_psk_decoder", "ccsds_ldpc_decoder",
                                "ccsds_turbo_decoder", "metop_dump_decoder", "meteor_lrpt_decoder", "noaa_hrpt_decoder", "meteor_hrpt_decoder",
                                "aqua_db_decoder"})
             evt.modules_registry.push_back({std::string(id) + "_b200", nlohmann::json(), factory(id)});
@@ -312,7 +319,7 @@ public:
     static void patchHandler(const satdump::SatDumpStartedEvent &)
     {
         for (auto &e : satdump::pipeline::modules_registry)
-            if (e.id == "psk_demod" || e.id == "pm_demod" || e.id == "terra_db_demod" || e.id == "metop_ahrpt_decoder" || e.id == "ccsds_conv_concat_decoder" || e.id == "ccsds_simple_psk_decoder" ||
+            if (e.id == "psk_demod" || e.id == "pm_demod" || e.id == "terra_db_demod" || e.id == "fsk_demod" || e.id == "metop_ahrpt_decoder" || e.id == "ccsds_conv_concat_decoder" || e.id == "ccsds_simple_psk_decoder" ||
                 e.id == "ccsds_ldpc_decoder" || e.id == "ccsds_turbo_decoder" || e.id == "metop_dump_decoder" ||
                 e.id == "meteor_lrpt_decoder" || e.id == "noaa_hrpt_decoder" || e.id == "meteor_hrpt_decoder" ||
                 e.id == "aqua_db_decoder")

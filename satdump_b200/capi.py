@@ -44,7 +44,7 @@ class DemodCfg(C.Structure):
                 ("front_resample", C.c_int), ("clock_recovery", C.c_int),
                 ("pm_demod", C.c_int), ("pm_pll_bw", C.c_float), ("pm_pll_max_offset", C.c_float), ("pm_resample_after_pll", C.c_int),
                 ("pm_subcarrier_offset", C.c_double), ("freq_shift", C.c_double),
-                ("has_carrier", C.c_int), ("carrier_pll_bw", C.c_float), ("carrier_pll_max_offset", C.c_float)]
+                ("has_carrier", C.c_int), ("carrier_pll_bw", C.c_float), ("carrier_pll_max_offset", C.c_float), ("fsk_demod", C.c_int)]
 
 
 class FecCfg(C.Structure):
@@ -215,7 +215,7 @@ def demod_cfg(samplerate, symbolrate, constellation, rrc_alpha, pll_bw=0.003, fm
               clock_gain_omega=None, clock_mu=0.5, clock_gain_mu=8.7e-3, clock_omega_limit=0.005, costas_max_offset=1.0, device=0,
               max_batch=1 << 24, keep_stages=False, iq_swap=False, final_samplerate=None, min_sps=0.0, max_sps=0.0, dc_block=False, post_costas_dc=False,
               front_resample=0, clock_recovery="mm", pm=False, pm_pll_bw=0.01, pm_pll_max_offset=0.5, resample_after_pll=False, subcarrier_offset=0,
-              freq_shift=0.0, has_carrier=False, carrier_pll_bw=0.001, carrier_pll_max_offset=3.14):
+              freq_shift=0.0, has_carrier=False, carrier_pll_bw=0.001, carrier_pll_max_offset=3.14, fsk_demod=False):
     """Parameter defaults = module_psk_demod.h:31-39, module_demod_base.h:54. final_samplerate=None applies BaseDemodModule::initb's
     rule (resample when samplerate/symbolrate is outside [min_sps, max_sps]); 0 forces "no resampler". pm=True: pm_demod's chain
     (module_pm_demod.cpp; pll_bw is then its "costas_bw", pm_pll_bw its "pll_bw", MAX_SPS = 10)."""
@@ -236,7 +236,39 @@ def demod_cfg(samplerate, symbolrate, constellation, rrc_alpha, pll_bw=0.003, fm
                     clock_mu, clock_gain_mu, clock_omega_limit, costas_max_offset, FMT[fmt], device, max_batch, int(keep_stages), int(iq_swap),
                     float(final_samplerate), int(dc_block), int(post_costas_dc), int(front_resample), {"mm": 0, "gardner": 1}[clock_recovery],
                     int(pm), pm_pll_bw, pm_pll_max_offset, int(resample_after_pll), float(subcarrier_offset), float(freq_shift),
-                    int(has_carrier), carrier_pll_bw, carrier_pll_max_offset)
+                    int(has_carrier), carrier_pll_bw, carrier_pll_max_offset, int(fsk_demod))
+
+
+# FSKDemodModule's clock defaults (module_fsk_demod.h:28-31), as the module's float members hold them
+FSK_CLOCK_GAIN_OMEGA = float(np.float32(pow(1.7e-2, 2) / 4.0))
+FSK_CLOCK_GAIN_MU = float(np.float32(1.7e-2))
+
+
+def fsk_demod_kwargs(samplerate, symbolrate, rrc_alpha, fmt="cs16", clock_alpha=None, clock_gain_omega=None, clock_mu=None, clock_gain_mu=None,
+                     clock_omega_relative_limit=None, rrc_taps=31):
+    """demod_cfg arguments of fsk_demod (module_fsk_demod.cpp:13-57): the module's defaults, "clock_alpha" setting gain_omega = alpha^2 / 4
+    and gain_mu = alpha, then the explicit gains over it, in the constructor's order. The working rate is BaseDemodModule::initb's for the
+    base window [1.1, 4.0] samples per symbol."""
+    if rrc_alpha is None:
+        raise ValueError("RRC Alpha parameter must be present!")
+    gain_omega, gain_mu = FSK_CLOCK_GAIN_OMEGA, FSK_CLOCK_GAIN_MU
+    if clock_alpha is not None:  # the module parses a float and squares it exactly in double before the float member rounds it
+        a = np.float32(clock_alpha)
+        gain_omega, gain_mu = float(np.float32(np.float64(a) ** 2 / 4.0)), float(a)
+    if clock_gain_omega is not None:
+        gain_omega = float(np.float32(clock_gain_omega))
+    if clock_gain_mu is not None:
+        gain_mu = float(np.float32(clock_gain_mu))
+    return dict(samplerate=samplerate, symbolrate=symbolrate, constellation="bpsk", rrc_alpha=rrc_alpha, rrc_taps=rrc_taps, fmt=fmt,
+                clock_gain_omega=gain_omega, clock_gain_mu=gain_mu, clock_mu=0.5 if clock_mu is None else clock_mu,
+                clock_omega_limit=0.005 if clock_omega_relative_limit is None else clock_omega_relative_limit, fsk_demod=True)
+
+
+def fsk_demod_cfg(samplerate, symbolrate, rrc_alpha, fmt="cs16", device=0, max_batch=1 << 24, clock_alpha=None, clock_gain_omega=None, clock_mu=None,
+                  clock_gain_mu=None, clock_omega_relative_limit=None, rrc_taps=31, **kw):
+    """fsk_demod's chain as a b200_demod_cfg (fsk_demod_kwargs); kw: the BaseDemodModule parameters of demod_cfg."""
+    return demod_cfg(**fsk_demod_kwargs(samplerate, symbolrate, rrc_alpha, fmt, clock_alpha, clock_gain_omega, clock_mu, clock_gain_mu,
+                                        clock_omega_relative_limit, rrc_taps), device=device, max_batch=max_batch, **kw)
 
 
 def resampler_bank(samplerate, final_samplerate):
@@ -426,6 +458,9 @@ def _struct_dict(s):
     return {k: list(v) if isinstance(v, C.Array) else v for k, v in ((k, getattr(s, k)) for k, _ in s._fields_)}
 
 
+STAGES = {"agc": 0, "fir": 1, "costas": 2, "resamp": 3, "dc": 4, "mm": 5, "pll": 6, "pm": 7, "quad": 8, "dc2": 9, "agc2": 10}
+
+
 class Demod:
     """Host mirror of PSKDemodModule's DSP chain for one stream (module_psk_demod.cpp:86-236)."""
 
@@ -436,6 +471,7 @@ class Demod:
             raise B200Error(-1 if "device" not in last_error().lower() else -2, last_error())
         self.bps = 1 if cfg.constellation == 0 else 2
         self.pm = bool(cfg.pm_demod)
+        self.fsk = bool(cfg.fsk_demod)
 
     def close(self):
         if getattr(self, "h", None):
@@ -492,8 +528,9 @@ class Demod:
         return out[:n.value].copy()
 
     def symbols(self):
+        """complex64 symbols of the last push; fsk_demod: float32, one per symbol."""
         cap = int(self._n) + 1024
-        out = np.zeros(cap, np.complex64)
+        out = np.zeros(cap, np.float32 if self.fsk else np.complex64)
         n = C.c_long(0)
         _chk(lib().b200_demod_pull_symbols(self.h, out.ctypes.data, cap, C.byref(n)))
         return out[:n.value].copy()
@@ -503,16 +540,19 @@ class Demod:
         n = self._n if which == "dc" else self.stats()["last_front_samples"]
         if self.pm and self.cfg.pm_resample_after_pll and which in ("agc", "pll", "pm"):
             n = self._n  # pm_demod with resample_after_pll: the first AGC, the carrier PLL and PMToBPSK run at the input rate
-        out = np.zeros(n, np.complex64)
-        _chk(lib().b200_demod_debug_stage(self.h, {"agc": 0, "fir": 1, "costas": 2, "resamp": 3, "dc": 4, "pll": 6, "pm": 7}[which], out.ctypes.data, n))
+        real = self.fsk and which in ("quad", "dc2", "agc2", "fir")
+        out = np.zeros(n, np.float32 if real else np.complex64)
+        _chk(lib().b200_demod_debug_stage(self.h, STAGES[which], out.ctypes.data, n))
         return out
 
     def run_stage(self, which, x, strict=False, sequential=False):
-        """Stage-isolated parity hook: ONE stage ("fir" / "costas" / "mm") of a freshly reset demodulator on the cf32 stage input x."""
-        x = np.ascontiguousarray(x, np.complex64)
-        out = np.zeros(x.size + 1024, np.complex64)
+        """Stage-isolated parity hook: ONE stage ("fir" / "costas" / "mm") of a freshly reset demodulator on the cf32 stage input x.
+        fsk_demod: "quad" (complex input), "dc2", "agc2", "fir", "mm" on float32 input, float32 output."""
+        real_in = self.fsk and which != "quad"
+        x = np.ascontiguousarray(x, np.float32 if real_in else np.complex64)
+        out = np.zeros(x.size + 1024, np.float32 if self.fsk else np.complex64)
         n = C.c_long(0)
-        _chk(lib().b200_demod_debug_run_stage(self.h, {"fir": 1, "costas": 2, "mm": 5, "pll": 6, "pm": 7}[which], x.ctypes.data, x.size,
+        _chk(lib().b200_demod_debug_run_stage(self.h, STAGES[which], x.ctypes.data, x.size,
                                               (1 if strict else 0) | (2 if sequential else 0), out.ctypes.data, out.size, C.byref(n)))
         return out[:n.value].copy()
 

@@ -227,9 +227,12 @@ static int fmt_bytes(int fmt)
 }
 
 static int round_up16(double v) { return ((int)std::ceil(v / 16.0)) * 16; }
-// k_mm instantiation: STRICT (test hook), GARDNER (clock_recovery 1), FIX (the input still needs its rotation / OQPSK delay)
-static decltype(&k_mm<false, false, false>) mm_kernel(bool strict, bool gardner, bool fix)
+// k_mm instantiation: STRICT (test hook), GARDNER (clock_recovery 1), FIX (the input still needs its rotation / OQPSK delay), REAL
+// (fsk_demod: MMClockRecoveryBlock<float>'s detector on the real part; no Gardner, no fix-up)
+static decltype(&k_mm<false, false, false>) mm_kernel(bool strict, bool gardner, bool fix, bool real = false)
 {
+    if (real)
+        return strict ? k_mm<true, false, false, true> : k_mm<false, false, false, true>;
     if (strict)
         return gardner ? (fix ? k_mm<true, true, true> : k_mm<true, true, false>) : (fix ? k_mm<true, false, true> : k_mm<true, false, false>);
     return gardner ? (fix ? k_mm<false, true, true> : k_mm<false, true, false>) : (fix ? k_mm<false, false, true> : k_mm<false, false, false>);
@@ -245,7 +248,7 @@ Demod::Demod(const b200_demod_cfg &c) : cfg(c)
     B200_REQUIRE((c.rrc_taps | 1) == FIR_NT, B200_EINVAL, "rrc_taps=%d: only the 31-tap RRC kernel is built", c.rrc_taps);
     B200_REQUIRE(c.max_batch >= 4096, B200_EINVAL, "max_batch must be >= 4096 samples");
     B200_REQUIRE(c.agc_rate > 0 && c.agc_rate < 0.5f, B200_EINVAL, "agc_rate out of range");
-    B200_REQUIRE(c.clock_gain_mu > 0 && c.pll_bw > 0, B200_EINVAL, "loop gains must be positive");
+    B200_REQUIRE(c.clock_gain_mu > 0 && (c.fsk_demod || c.pll_bw > 0), B200_EINVAL, "loop gains must be positive");
     B200_REQUIRE(c.clock_recovery == 0 || c.clock_recovery == 1, B200_EINVAL, "clock_recovery must be 0 (M&M) or 1 (Gardner)");
     const long fs = (long)c.samplerate, rs = (long)c.symbolrate;
     const float final_fs = c.final_samplerate > 0 ? (float)c.final_samplerate : (float)fs; // float final_samplerate (module_demod_base.h:67)
@@ -265,6 +268,14 @@ Demod::Demod(const b200_demod_cfg &c) : cfg(c)
         B200_REQUIRE(!pm, B200_EINVAL, "has_carrier is psk_demod's carrier mode, not pm_demod's");
         B200_REQUIRE(c.constellation == B200_BPSK, B200_EINVAL, "For carrier mode, constellation must be BPSK!");
         B200_REQUIRE(c.carrier_pll_bw > 0 && c.carrier_pll_bw < 0.5f && c.carrier_pll_max_offset > 0, B200_EINVAL, "carrier_pll_bw / carrier_pll_max_offset out of range");
+    }
+    fsk = c.fsk_demod != 0;
+    if (fsk) { // FSKDemodModule (module_fsk_demod.cpp:13-84): no Costas loop, the real M&M; the base working window (module_demod_base.h:71-72)
+        B200_REQUIRE(c.constellation == B200_BPSK, B200_EINVAL, "fsk_demod gives one real symbol per sample pair: constellation must be bpsk");
+        B200_REQUIRE(!pm, B200_EINVAL, "fsk_demod cannot be combined with pm_demod");
+        B200_REQUIRE(!c.has_carrier, B200_EINVAL, "fsk_demod cannot be combined with has_carrier");
+        B200_REQUIRE(!c.post_costas_dc, B200_EINVAL, "fsk_demod cannot be combined with post_costas_dc");
+        B200_REQUIRE(c.clock_recovery == 0, B200_EINVAL, "fsk_demod uses the M&M clock recovery (clock_recovery Gardner is psk_demod's)");
     }
     SpsWindow win = sps_window(c.constellation);
     if (pm) // MAX_SPS = 10 for pm_demod ("we do NOT want to resample unless really necessary", module_pm_demod.cpp:56)
@@ -329,7 +340,7 @@ Demod::Demod(const b200_demod_cfg &c) : cfg(c)
         if (c.freq_shift != 0) // FreqShiftBlock(input, d_samplerate, d_frequency_shift): long parameters (module_demod_base.h:56, .cpp:122-123)
             fs_dturn = turn_step((double)(long)c.freq_shift, (double)fs);
     }
-    order = c.constellation == B200_BPSK ? 2 : (c.constellation == B200_8PSK ? 8 : (c.constellation == B200_NONE ? 0 : 4));
+    order = fsk ? 0 : (c.constellation == B200_BPSK ? 2 : (c.constellation == B200_8PSK ? 8 : (c.constellation == B200_NONE ? 0 : 4)));
     max_batch = c.max_batch;
     max_work = resamp ? std::max<long>(max_batch, (long)((double)max_batch * rs_I / rs_D) + 64) : max_batch; // (a decimator in front only shrinks it)
     if (pm || c.has_carrier) {
@@ -458,6 +469,12 @@ Demod::Demod(const b200_demod_cfg &c) : cfg(c)
         B200_CUDA(cudaStreamSynchronize(stream)); // (tab is a local)
         B200_CUDA(cudaFuncSetAttribute(k_pll, cudaFuncAttributeMaxDynamicSharedMemorySize, PLL_SMEM_BYTES));
     }
+    if (fsk) {
+        pm_agc.alloc(max_work + 64);
+        quad_out.alloc(max_work + 64);
+        dc2_out.alloc(max_work + 64);
+        agc2_out.alloc(max_work + 64 + 32);
+    }
     if (cfg.post_costas_dc) {
         B200_REQUIRE(order != 0 && c.constellation != B200_OQPSK, B200_EINVAL, "post_costas_dc needs a Costas loop and is not built for OQPSK");
         pdc_out.alloc(max_work + 64);
@@ -488,8 +505,8 @@ Demod::Demod(const b200_demod_cfg &c) : cfg(c)
     init_state();
     bufA.zero(stream);
     bufB.zero(stream);
-    for (int v = 0; v < 8; v++)
-        B200_CUDA(cudaFuncSetAttribute(mm_kernel(v & 1, v & 2, v & 4), cudaFuncAttributeMaxDynamicSharedMemorySize, MM_SMEM_BYTES));
+    for (int v = 0; v < 10; v++)
+        B200_CUDA(cudaFuncSetAttribute(mm_kernel(v & 1, v & 2, v & 4, v >= 8), cudaFuncAttributeMaxDynamicSharedMemorySize, MM_SMEM_BYTES));
     B200_CUDA(cudaFuncSetAttribute(k_costas<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, COSTAS_SMEM_BYTES));
     B200_CUDA(cudaFuncSetAttribute(k_costas<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, COSTAS_SMEM_BYTES));
     B200_CUDA(cudaFuncSetAttribute(k_costas<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, COSTAS_SMEM_BYTES));
@@ -520,6 +537,7 @@ void Demod::init_state()
     memset(h_state.p, 0, sizeof(DemodDevState));
     h_state.p->gain[0] = h_state.p->gain[1] = 1.0f;
     h_state.p->gain2[0] = h_state.p->gain2[1] = 1.0f;
+    h_state.p->fgain[0] = h_state.p->fgain[1] = 1.0f; // AGCBlock<float>(.., 0.1, 0.5, 1.0, 65535): gain 1 (module_fsk_demod.cpp:70)
     for (int i = 0; i < 2; i++) {
         h_state.p->mm[i].mu = cfg.clock_mu;
         h_state.p->mm[i].omega = sps;
@@ -738,7 +756,7 @@ void Demod::stage_mm(float2 *mmin, long n, int L, int nseg, int cur, int nxt, in
 {
     DemodDevState *S = st.p;
     const int nblk = (nseg + SEG_THREADS - 1) / SEG_THREADS;
-    const auto mm = mm_kernel(strict, cfg.clock_recovery == 1, mm_rot || mm_oqpsk);
+    const auto mm = mm_kernel(strict, cfg.clock_recovery == 1, mm_rot || mm_oqpsk, fsk);
     MMParams MP;
     MP.omega_mid = sps;
     MP.omega_limit = cfg.clock_omega_limit * sps;
@@ -752,9 +770,10 @@ void Demod::stage_mm(float2 *mmin, long n, int L, int nseg, int cur, int nxt, in
                                                         mm_quad, mm_rot, mm_oqpsk, mck.p, mt * tol_mm, mt * tol_momega, S->merge_hist);
         k_mm_scan<<<1, 1024, 0, stream>>>(mrec.p, nseg, tol_mm, offs.p, &S->mm_unconv, cap, &S->flags, repair.p + 1, repair.p, round, &S->repairs);
     });
-    k_mm_compact<<<std::min(nseg, 132 * 8), 256, 0, stream>>>(slots.p, cap, mrec.p, offs.p, nseg, pm ? 2 : (bps == 1), all_symbols ? 1 : 0, sym_out.p,
-                                                              sdst);
-    k_snr_m2m4<<<1, 1024, 0, stream>>>(sym_out.p, offs.p + nseg, 0.001f, S->snr_y[cur], S->snr_y[nxt]); // M2M4SNREstimator(alpha = 0.001)
+    k_mm_compact<<<std::min(nseg, 132 * 8), 256, 0, stream>>>(slots.p, cap, mrec.p, offs.p, nseg, fsk ? 3 : (pm ? 2 : (bps == 1)), all_symbols ? 1 : 0,
+                                                              sym_out.p, sdst);
+    // M2M4SNREstimator(alpha = 0.001); fsk_demod estimates over its float symbols taken as complex pairs (module_fsk_demod.cpp:127)
+    k_snr_m2m4<<<1, 1024, 0, stream>>>(sym_out.p, offs.p + nseg, fsk ? 1 : 0, 0.001f, S->snr_y[cur], S->snr_y[nxt]);
     launches += 2;
 }
 
@@ -802,6 +821,24 @@ void Demod::front_resample(const void *&d_raw, long &n, int &front_fmt, int &rs_
     }
 }
 
+// fsk_demod behind the complex AGC (pm_agc): QuadratureDemodBlock -> CorrectIQBlock<float> -> AGCBlock<float> (both scanned over tiles from
+// the carried accumulator / gain) -> FIRBlock<float> with its carried history -> the clock recovery's input (y, 0) in bufA + 16
+void Demod::stage_fsk(long n, const FirTaps &taps, int cur, int nxt)
+{
+    DemodDevState *S = st.p;
+    const int nt = (int)((n + FIR_TILE - 1) / FIR_TILE);
+    const float alpha = 0.0001f, beta = 1.0f - alpha; // CorrectIQBlock<float> (correct_iq.h:23, correct_iq.cpp:9)
+    k_quad<<<nt, FIR_THREADS, 0, stream>>>(pm_agc.p, n, &S->qphase[cur], &S->qphase[nxt], alpha, beta, quad_out.p, tile_map.p);
+    k_tile_scan<<<1, 1024, 0, stream>>>(tile_map.p, nt, &S->fdc_acc[cur], nullptr, 0, seeds.p, nullptr);
+    k_fsk_dc<<<nt, FIR_THREADS, 0, stream>>>(quad_out.p, n, alpha, beta, seeds.p, dc2_out.p, &S->fdc_acc[nxt], tile_map3.p);
+    k_tile_scan<<<1, 1024, 0, stream>>>(tile_map3.p, nt, &S->fgain[cur], nullptr, 0, seeds.p, nullptr);
+    k_fsk_agc<<<nt, FIR_THREADS, 0, stream>>>(dc2_out.p, n, seeds.p, agc2_out.p + 32, &S->fgain[nxt]);
+    B200_CUDA(cudaMemcpyAsync(agc2_out.p, S->fir_tail[cur], 32 * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+    k_fir_real<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(agc2_out.p + 32, n, taps, bufA.p + 16);
+    B200_CUDA(cudaMemcpyAsync(S->fir_tail[nxt], agc2_out.p + n, 32 * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+    launches += 6;
+}
+
 long Demod::process(const void *d_raw, long n, int8_t *soft_dst)
 {
     B200_REQUIRE(n >= 64, B200_ESTATE, "a batch needs at least 64 samples (got %ld)", n);
@@ -844,7 +881,12 @@ long Demod::process(const void *d_raw, long n, int8_t *soft_dst)
     for (int i = 0; i < FIR_NT; i++)
         taps.h[i] = rrc[i];
     const bool dump = cfg.keep_stages != 0;
-    if (!pm) {
+    if (fsk) {
+        // the complex AGC runs through the front kernel with its output dumped (the FIR it also computes is not used)
+        const AgcUnit u{cfg.agc_rate, 65536.0f, &S->gain[cur], &S->gain[nxt], S->agc_tail[cur], S->agc_tail[nxt], bufA.p + 16, pm_agc.p};
+        launch_front_fmt(*this, front_fmt, d_raw, n, taps, u);
+        stage_fsk(n, taps, cur, nxt);
+    } else if (!pm) {
         const AgcUnit u{cfg.agc_rate, 65536.0f, &S->gain[cur], &S->gain[nxt], S->agc_tail[cur], S->agc_tail[nxt], bufA.p + 16, dump ? agc_dump.p : nullptr};
         launch_front_fmt(*this, front_fmt, d_raw, n, taps, u);
     } else {
@@ -914,6 +956,8 @@ long Demod::process(const void *d_raw, long n, int8_t *soft_dst)
 long Demod::debug_run_stage(int stage, const float *h_in, long n, int mode, float *h_out, long cap)
 {
     B200_REQUIRE(n >= 64 && n <= max_work, B200_ESTATE, "stage input of %ld samples outside [64, %ld]", n, max_work);
+    if (fsk)
+        return debug_run_stage_fsk(stage, h_in, n, mode, h_out, cap);
     B200_REQUIRE(stage == B200_STAGE_FIR || stage == B200_STAGE_COSTAS || stage == B200_STAGE_MM || stage == B200_STAGE_PLL || stage == B200_STAGE_PM, B200_EINVAL,
                  "stage %d cannot be run alone", stage);
     DeviceGuard g(cfg.device);
@@ -974,6 +1018,70 @@ long Demod::debug_run_stage(int stage, const float *h_in, long n, int mode, floa
     B200_CUDA(cudaStreamSynchronize(stream));
     B200_CUDA(cudaGetLastError());
     dbg_costas_unconv = (stage == B200_STAGE_PLL || stage == B200_STAGE_PM) ? h_state.p->pll_unconv : h_state.p->costas_unconv;
+    dbg_mm_unconv = h_state.p->mm_unconv;
+    dbg_repairs = h_state.p->repairs;
+    last_syms = stage == B200_STAGE_MM ? count : 0;
+    reset();
+    return count;
+}
+
+// debug_run_stage of an fsk_demod: every stage input and output is one float per sample (QUAD: complex input)
+long Demod::debug_run_stage_fsk(int stage, const float *h_in, long n, int mode, float *h_out, long cap)
+{
+    B200_REQUIRE(stage == B200_STAGE_QUAD || stage == B200_STAGE_DC2 || stage == B200_STAGE_AGC2 || stage == B200_STAGE_FIR || stage == B200_STAGE_MM,
+                 B200_EINVAL, "stage %d cannot be run alone in fsk_demod", stage);
+    const bool strict = mode & B200_DEBUG_STRICT, seq = mode & B200_DEBUG_SEQUENTIAL;
+    B200_REQUIRE(seq || (stage != B200_STAGE_DC2 && stage != B200_STAGE_AGC2), B200_EINVAL,
+                 "fsk_demod runs its DC blocker and AGC alone only as SEQUENTIAL (the scanned ones run inside a push with keep_stages)");
+    DeviceGuard g(cfg.device);
+    reset();
+    DemodDevState *S = st.p;
+    const float alpha = 0.0001f, beta = 1.0f - alpha;
+    float *in = agc2_out.p + 32; // real stage inputs, behind a zero history
+    const float *src = nullptr;
+    long count = n;
+    if (stage == B200_STAGE_QUAD) {
+        B200_CUDA(cudaMemcpyAsync(pm_agc.p, h_in, n * sizeof(float2), cudaMemcpyHostToDevice, stream));
+        k_quad<<<(unsigned)((n + FIR_TILE - 1) / FIR_TILE), FIR_THREADS, 0, stream>>>(pm_agc.p, n, &S->qphase[0], &S->qphase[1], alpha, beta, quad_out.p,
+                                                                                     tile_map.p);
+        src = quad_out.p;
+    } else if (stage == B200_STAGE_MM) {
+        // the clock recovery's input (x, 0) with a zero history, as k_fir_real writes it
+        const int L = seq ? (int)((n + 15) / 16 * 16) : choose_L(n);
+        const int nseg = (int)((n + L - 1) / L);
+        mm_quad = nullptr;
+        mm_rot = mm_oqpsk = 0;
+        B200_CUDA(cudaMemsetAsync(bufA.p, 0, (n + 16) * sizeof(float2), stream));
+        B200_CUDA(cudaMemcpy2DAsync(bufA.p + 16, sizeof(float2), h_in, sizeof(float), sizeof(float), n, cudaMemcpyHostToDevice, stream));
+        last_L = L;
+        last_nseg = nseg;
+        stage_mm(bufA.p, n, L, nseg, 0, 1, soft.p, strict, true);
+        B200_CUDA(cudaMemcpyAsync(h_total.p, offs.p + nseg, sizeof(long), cudaMemcpyDeviceToHost, stream));
+        B200_CUDA(cudaStreamSynchronize(stream));
+        count = *h_total.p;
+        src = reinterpret_cast<const float *>(sym_out.p);
+    } else {
+        B200_CUDA(cudaMemsetAsync(agc2_out.p, 0, 32 * sizeof(float), stream));
+        B200_CUDA(cudaMemcpyAsync(in, h_in, n * sizeof(float), cudaMemcpyHostToDevice, stream));
+        if (stage == B200_STAGE_FIR) {
+            FirTaps taps;
+            memset(&taps, 0, sizeof(taps));
+            for (int i = 0; i < FIR_NT; i++)
+                taps.h[i] = rrc[i];
+            k_fir_real<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(in, n, taps, bufA.p + 16);
+            B200_CUDA(cudaMemcpy2DAsync(quad_out.p, sizeof(float), bufA.p + 16, sizeof(float2), sizeof(float), n, cudaMemcpyDeviceToDevice, stream));
+            src = quad_out.p;
+        } else {
+            k_fsk_serial<<<1, 1, 0, stream>>>(stage == B200_STAGE_DC2 ? 0 : 1, in, n, alpha, beta, dc2_out.p);
+            src = dc2_out.p;
+        }
+    }
+    B200_REQUIRE(count <= cap, B200_ESTATE, "output buffer too small: need %ld values", count);
+    B200_CUDA(cudaMemcpyAsync(h_out, src, count * sizeof(float), cudaMemcpyDeviceToHost, stream));
+    B200_CUDA(cudaMemcpyAsync(h_state.p, S, sizeof(DemodDevState), cudaMemcpyDeviceToHost, stream));
+    B200_CUDA(cudaStreamSynchronize(stream));
+    B200_CUDA(cudaGetLastError());
+    dbg_costas_unconv = 0;
     dbg_mm_unconv = h_state.p->mm_unconv;
     dbg_repairs = h_state.p->repairs;
     last_syms = stage == B200_STAGE_MM ? count : 0;
@@ -1122,7 +1230,7 @@ int b200_demod_pull_symbols(b200_demod *h, float *out, long cap_symbols, long *n
         Demod &d = *h->d;
         B200_REQUIRE(d.last_syms <= cap_symbols, B200_ESTATE, "output buffer too small: need %ld symbols", d.last_syms);
         DeviceGuard g(d.cfg.device);
-        B200_CUDA(cudaMemcpyAsync(out, d.sym_out.p, d.last_syms * sizeof(float2), cudaMemcpyDeviceToHost, d.stream));
+        B200_CUDA(cudaMemcpyAsync(out, d.sym_out.p, d.last_syms * (d.fsk ? sizeof(float) : sizeof(float2)), cudaMemcpyDeviceToHost, d.stream));
         B200_CUDA(cudaStreamSynchronize(d.stream));
         *n_out = d.last_syms;
     });
@@ -1187,9 +1295,22 @@ int b200_demod_debug_stage(b200_demod *h, int stage, float *out, long cap_sample
         const bool at_pll = d.pm && (stage == B200_STAGE_AGC || stage == B200_STAGE_PLL || stage == B200_STAGE_PM);
         const long count = stage == B200_STAGE_DC ? d.last_in : (at_pll ? d.last_pm : d.last_n);
         B200_REQUIRE(count <= cap_samples, B200_ESTATE, "output buffer too small");
+        if (d.fsk && stage != B200_STAGE_AGC && stage != B200_STAGE_RESAMP && stage != B200_STAGE_DC) {
+            // fsk_demod's real stages: one float per sample (the FIR output is the .x of the clock recovery's input)
+            DeviceGuard g(d.cfg.device);
+            if (stage == B200_STAGE_FIR)
+                B200_CUDA(cudaMemcpy2DAsync(out, sizeof(float), d.fir_dump.p, sizeof(float2), sizeof(float), count, cudaMemcpyDeviceToHost, d.stream));
+            else {
+                const float *fsrc = stage == B200_STAGE_QUAD ? d.quad_out.p : (stage == B200_STAGE_DC2 ? d.dc2_out.p : (stage == B200_STAGE_AGC2 ? d.agc2_out.p + 32 : nullptr));
+                B200_REQUIRE(fsrc, B200_EINVAL, "unknown stage %d of fsk_demod", stage);
+                B200_CUDA(cudaMemcpyAsync(out, fsrc, count * sizeof(float), cudaMemcpyDeviceToHost, d.stream));
+            }
+            B200_CUDA(cudaStreamSynchronize(d.stream));
+            return;
+        }
         const float2 *src = nullptr;
         if (stage == B200_STAGE_AGC)
-            src = d.pm ? d.pm_agc.p : d.agc_dump.p;
+            src = (d.pm || d.fsk) ? d.pm_agc.p : d.agc_dump.p;
         else if (stage == B200_STAGE_FIR)
             src = d.fir_dump.p;
         else if (stage == B200_STAGE_PLL && (d.pm || d.cfg.has_carrier))

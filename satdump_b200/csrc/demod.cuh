@@ -925,6 +925,169 @@ template <bool STRICT> __global__ void __launch_bounds__(256) k_fir_only(const f
     out[i] = make_float2(ar, ai);
 }
 
+// ---------------------------------------------------------------- fsk_demod: quadrature demodulator, float DC blocker, float AGC, real RRC
+// FSKDemodModule::init (module_fsk_demod.cpp:59-84) behind the complex AGC: QuadratureDemodBlock(agc, 1.0f) -> CorrectIQBlock<float> ->
+// AGCBlock<float>(0.1, 0.5, 1.0, 65535) -> FIRBlock<float>(RRC) -> MMClockRecoveryBlock<float>. All stages work on 2048-sample tiles of
+// 256 threads x 8 samples; the two recurrences are scanned like the complex DC blocker and AGC (k_tile_scan) and every thread then
+// replays the reference's float recurrence over its 8 samples from its scanned seed.
+constexpr float FSK_AGC_RATE = 0.1f, FSK_AGC_REF = 0.5f, FSK_AGC_MAX = 65535.0f;
+
+// QuadratureDemodBlock::process (quadrature_demod.cpp:35-48): p = atan2f(im, re). p here is the correctly rounded float of the arctangent
+// (evaluated in double, then rounded once; DESIGN §9), not CUDA's atan2f (up to 2 ulp).
+__device__ __forceinline__ float quad_phase(float2 v) { return (float)atan2((double)v.y, (double)v.x); }
+// d = p - phase; the wrap compares with the double M_PI and subtracts 2.0f * M_PI in double, rounded back to float; out = d * (1.0 / 1.0f)
+__device__ __forceinline__ float quad_diff(float p, float prev)
+{
+    const double pi = 3.14159265358979323846;
+    float d = __fsub_rn(p, prev);
+    if ((double)d > pi)
+        d = (float)((double)d - 2.0 * pi);
+    else if ((double)d <= -pi)
+        d = (float)((double)d + 2.0 * pi);
+    return d;
+}
+// CorrectIQBlock<float> step: acc = acc * beta + x * alpha (correct_iq.cpp:29); the output is x - acc
+__device__ __forceinline__ float dc_step(float acc, float x, float alpha, float beta) { return __fadd_rn(__fmul_rn(acc, beta), __fmul_rn(x, alpha)); }
+// AGCBlock<float> step (agc.cpp:30-36): out = x * gain; gain += rate * (reference - |out|), clamped at max_gain
+__device__ __forceinline__ float agc_step(float &g, float x)
+{
+    const float out = __fmul_rn(x, g);
+    g = __fadd_rn(g, __fmul_rn(FSK_AGC_RATE, __fsub_rn(FSK_AGC_REF, fabsf(out))));
+    if (g > FSK_AGC_MAX)
+        g = FSK_AGC_MAX;
+    return out;
+}
+// the same step as a map of the gain, for the scan: g -> min((1 - rate |x|) g + rate * reference, max_gain)
+__device__ __forceinline__ Affine3 agc_map(float x)
+{
+    return Affine3{1.0 - (double)FSK_AGC_RATE * fabs((double)x), (double)FSK_AGC_RATE * (double)FSK_AGC_REF, (double)FSK_AGC_MAX};
+}
+
+// exclusive composition of the maps of the threads in front of this one in its tile (the block's threads in order)
+template <class M> __device__ __forceinline__ M tile_exclusive(M m)
+{
+    __shared__ M wsum[FIR_THREADS / 32];
+    const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+    const M inc = warp_scan(m, lane);
+    if (lane == 31)
+        wsum[warp] = inc;
+    __syncthreads();
+    M pre = ident<M>();
+    for (int w = 0; w < warp; w++)
+        pre = compose(pre, wsum[w]);
+    const M e = shfl_up(inc, 1);
+    return lane > 0 ? compose(pre, e) : pre;
+}
+
+// the quadrature demodulator over the complex AGC output, and the DC blocker's per-tile maps (acc -> beta^8.. acc + local run from 0).
+// phase_in: p of the sample in front of the batch (QuadratureDemodBlock::phase, 0 for a new stream); phase_out: p of the batch's last one.
+__global__ void __launch_bounds__(FIR_THREADS) k_quad(const float2 *__restrict__ in, long N, const float *__restrict__ phase_in, float *__restrict__ phase_out,
+                                                      float alpha, float beta, float *__restrict__ out, Affine *__restrict__ tile_map)
+{
+    const long s0 = (long)blockIdx.x * FIR_TILE + 8 * threadIdx.x;
+    float prev = s0 == 0 ? *phase_in : (s0 - 1 < N ? quad_phase(in[s0 - 1]) : 0.f);
+    float acc = 0.f;
+    double a = 1.0;
+#pragma unroll
+    for (int i = 0; i < 8; i++)
+        if (s0 + i < N) {
+            const float p = quad_phase(in[s0 + i]);
+            const float d = quad_diff(p, prev);
+            prev = p;
+            out[s0 + i] = d;
+            acc = dc_step(acc, d, alpha, beta);
+            a *= (double)beta;
+            if (s0 + i == N - 1)
+                *phase_out = p;
+        }
+    tile_reduce(Affine{a, (double)acc}, &tile_map[blockIdx.x]);
+}
+
+// the DC blocker's output from the scanned seeds (acc before every tile), and the float AGC's per-tile maps over it (Affine3: clamp)
+__global__ void __launch_bounds__(FIR_THREADS) k_fsk_dc(const float *__restrict__ in, long N, float alpha, float beta, const double *__restrict__ seeds,
+                                                        float *__restrict__ out, float *__restrict__ acc_out, Affine3 *__restrict__ agc_tile_map)
+{
+    const long s0 = (long)blockIdx.x * FIR_TILE + 8 * threadIdx.x;
+    float x[8];
+    float acc = 0.f;
+    double a = 1.0;
+#pragma unroll
+    for (int i = 0; i < 8; i++) {
+        x[i] = s0 + i < N ? in[s0 + i] : 0.f;
+        if (s0 + i < N) {
+            acc = dc_step(acc, x[i], alpha, beta);
+            a *= (double)beta;
+        }
+    }
+    const Affine excl = tile_exclusive(Affine{a, (double)acc});
+    acc = (float)apply(excl, seeds[blockIdx.x]);
+    Affine3 m = ident<Affine3>();
+#pragma unroll
+    for (int i = 0; i < 8; i++)
+        if (s0 + i < N) {
+            acc = dc_step(acc, x[i], alpha, beta);
+            const float y = __fsub_rn(x[i], acc);
+            out[s0 + i] = y;
+            m = compose(m, agc_map(y));
+            if (s0 + i == N - 1)
+                *acc_out = acc;
+        }
+    __syncthreads(); // (tile_reduce's shared memory is its own; the barrier keeps the two reductions' phases apart)
+    tile_reduce(m, &agc_tile_map[blockIdx.x]);
+}
+
+// the float AGC's output from the scanned seeds (gain before every tile)
+__global__ void __launch_bounds__(FIR_THREADS) k_fsk_agc(const float *__restrict__ in, long N, const double *__restrict__ seeds, float *__restrict__ out,
+                                                         float *__restrict__ gain_out)
+{
+    const long s0 = (long)blockIdx.x * FIR_TILE + 8 * threadIdx.x;
+    float x[8];
+    Affine3 m = ident<Affine3>();
+#pragma unroll
+    for (int i = 0; i < 8; i++) {
+        x[i] = s0 + i < N ? in[s0 + i] : 0.f;
+        if (s0 + i < N)
+            m = compose(m, agc_map(x[i]));
+    }
+    const Affine3 excl = tile_exclusive(m);
+    float g = (float)apply(excl, seeds[blockIdx.x]);
+#pragma unroll
+    for (int i = 0; i < 8; i++)
+        if (s0 + i < N) {
+            out[s0 + i] = agc_step(g, x[i]);
+            if (s0 + i == N - 1)
+                *gain_out = g;
+        }
+}
+
+// STRICT | SEQUENTIAL test hook: stage 0 the DC blocker, 1 the AGC, as ONE thread running the reference's recurrence from its initial state
+__global__ void k_fsk_serial(int stage, const float *__restrict__ in, long N, float alpha, float beta, float *__restrict__ out)
+{
+    float acc = 0.f, g = 1.0f;
+    for (long i = 0; i < N; i++) {
+        if (stage == 0) {
+            acc = dc_step(acc, in[i], alpha, beta);
+            out[i] = __fsub_rn(in[i], acc);
+        } else
+            out[i] = agc_step(g, in[i]);
+    }
+}
+
+// FIRBlock<float> (fir.cpp:57-67 with the generic VOLK dot product): y[i] = sum_j x[i-30+j] * h[30-j], oldest sample first, separate
+// multiply and add, so it is bitwise the reference. in[-32 .. -1] holds the previous batch's last samples (zeros for a new stream).
+// The output is the clock recovery's input (y, 0).
+__global__ void __launch_bounds__(256) k_fir_real(const float *__restrict__ in, long N, const FirTaps taps, float2 *__restrict__ out)
+{
+    const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= N)
+        return;
+    float acc = 0.f;
+#pragma unroll
+    for (int j = 0; j < FIR_NT; j++)
+        acc = __fadd_rn(acc, __fmul_rn(in[i - (FIR_NT - 1) + j], taps.h[FIR_NT - 1 - j]));
+    out[i] = make_float2(acc, 0.f);
+}
+
 // ---------------------------------------------------------------- cp.async helpers
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
 template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N)); }
@@ -1768,7 +1931,7 @@ __device__ __forceinline__ void mm_fetch8(const float4 *__restrict__ ring, int n
     }
 }
 
-template <bool STRICT, bool GARDNER, bool FIX>
+template <bool STRICT, bool GARDNER, bool FIX, bool REAL = false>
 __global__ void __launch_bounds__(SEG_THREADS) k_mm(const float2 *__restrict__ mmin /* 16-sample front pad */, long N, int L, int W, int G, int nseg,
                                                      MMParams P, const MMState *__restrict__ st_in, MMState *__restrict__ st_out,
                                                      const float *__restrict__ bank /*128x8*/, float2 *__restrict__ slots, int cap,
@@ -1991,6 +2154,9 @@ __global__ void __launch_bounds__(SEG_THREADS) k_mm(const float2 *__restrict__ m
                 float pe;
                 if (GARDNER) { // zc * (last - sample), last = the previous output (p1 after the shift above); exact clip (:98-100)
                     pe = STRICT ? __fadd_rn(__fmul_rn(zr, __fsub_rn(p1.x, ar)), __fmul_rn(zi, __fsub_rn(p1.y, ai))) : zr * (p1.x - ar) + zi * (p1.y - ai);
+                } else if (REAL) { // MMClockRecoveryBlock<float> (clock_recovery_mm.cpp:70-82): sgn(last) * sample - sgn(sample) * last, sgn(0) = +1
+                    const float last = p1.x; // last_sample: the previous output (p1 after the shift above)
+                    pe = __fsub_rn(last < 0.0f ? -ar : ar, ar < 0.0f ? -last : last);
                 } else {
                     c0 = make_float2(ar > 0.0f ? 1.0f : 0.0f, ai > 0.0f ? 1.0f : 0.0f);
                     // Re[(p0-p2) conj(c1) - (c0-c2) conj(p1)]  (clock_recovery_mm.cpp:103)
@@ -2210,7 +2376,8 @@ __global__ void __launch_bounds__(256) k_mm_compact(const float2 *__restrict__ s
                                                    const long *__restrict__ offs, int nseg, int bpsk, int all_symbols,
                                                    float2 *__restrict__ sym_out, int8_t *__restrict__ soft_out)
 {
-    const long keep0 = all_symbols ? 0 : offs[nseg] - SNR_WINDOW; // symbols from here on are written to sym_out
+    // symbols from here on are written to sym_out (fsk_demod, bpsk 3: one float each, and its SNR estimate reads them as pairs)
+    const long keep0 = all_symbols ? 0 : offs[nseg] - (bpsk == 3 ? 2 * SNR_WINDOW + 1 : SNR_WINDOW);
     for (int s = blockIdx.x; s < nseg; s += gridDim.x) {
         const int sk = rec[s].skip;
         const int c = min(rec[s].count, cap) - sk;
@@ -2229,9 +2396,15 @@ __global__ void __launch_bounds__(256) k_mm_compact(const float2 *__restrict__ s
                 const int i = i0 + j * blockDim.x;
                 if (i >= c)
                     break;
-                if (o + i >= keep0)
-                    sym_out[o + i] = v[j];
-                if (bpsk) // 1: psk_demod's BPSK, real * 50 (module_psk_demod.cpp:199-205); 2: pm_demod, real * 100 (module_pm_demod.cpp:141-144)
+                if (o + i >= keep0) {
+                    if (bpsk == 3)
+                        reinterpret_cast<float *>(sym_out)[o + i] = v[j].x;
+                    else
+                        sym_out[o + i] = v[j];
+                }
+                // 1: psk_demod's BPSK, real * 50 (module_psk_demod.cpp:199-205); 2: pm_demod, real * 100 (module_pm_demod.cpp:141-144);
+                // 3: fsk_demod, real * 50 (module_fsk_demod.cpp:133-134)
+                if (bpsk)
                     soft_out[o + i] = soft_quant(v[j].x * (bpsk == 2 ? 100.0f : 50.0f));
                 else {
                     char2 q;
@@ -2249,11 +2422,12 @@ __global__ void __launch_bounds__(256) k_mm_compact(const float2 *__restrict__ s
 // |s|^4 over the symbol stream (alpha = 0.001: a memory of ~1000 symbols). Linear with constant coefficients, so the end value of a batch
 // is sum_i beta^(n-1-i) alpha m_i + beta^n y_in; terms older than 2^16 symbols weigh below e^-65 and are left out. One CTA: every thread
 // runs the recurrence over 64 consecutive symbols (fp64), the partial results are combined with their powers of beta.
-__global__ void __launch_bounds__(1024) k_snr_m2m4(const float2 *__restrict__ sym, const long *__restrict__ total, float alpha, const float *__restrict__ yin,
-                                                  float *__restrict__ yout)
+// pairs = 1 (fsk_demod): sym holds *total floats, estimated as *total / 2 complex pairs (module_fsk_demod.cpp:127).
+__global__ void __launch_bounds__(1024) k_snr_m2m4(const float2 *__restrict__ sym, const long *__restrict__ total, int pairs, float alpha,
+                                                  const float *__restrict__ yin, float *__restrict__ yout)
 {
     __shared__ double red[2][32];
-    const long n = *total;
+    const long n = *total >> pairs;
     const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
     const int RUN = SNR_WINDOW / 1024;
     const long M = min(n, (long)SNR_WINDOW), base = n - M;

@@ -35,6 +35,11 @@ struct DemodDevState
     float2 agc1_tail[2][32];   // (the first AGC's kernel also keeps a FIR history; unused in pm mode)
     int pll_unconv;            // carrier PLL junctions still unconverged after the repair rounds of the last batch
     float2 dc_acc3[2];         // psk_demod carrier mode: accumulator of the DC blocker behind the carrier PLL (module_psk_demod.cpp:112)
+    // fsk_demod (module_fsk_demod.cpp:59-84)
+    float qphase[2];           // QuadratureDemodBlock::phase: p of the last sample
+    float fdc_acc[2];          // CorrectIQBlock<float>::acc
+    float fgain[2];            // AGCBlock<float>::gain
+    float fir_tail[2][32];     // the FIRBlock<float> history: the AGC's last 32 outputs
 };
 
 // one AGC (+ RRC) pass of k_agc_fir_w: which carried gain / FIR history it uses and where its outputs go
@@ -76,6 +81,7 @@ class Demod
     int mm_rot = 0, mm_oqpsk = 0;
     void stage_mm(float2 *mmin, long n, int L, int nseg, int cur, int nxt, int8_t *sdst, bool strict, bool all_symbols);
     long debug_run_stage(int stage, const float *h_in, long n, int mode, float *h_out, long cap);
+    long debug_run_stage_fsk(int stage, const float *h_in, long n, int mode, float *h_out, long cap);
     int last_L = 0, last_nseg = 0;          // segmentation of the last batch (b200_demod_debug_junctions)
     int dbg_costas_unconv = 0, dbg_mm_unconv = 0, dbg_repairs = 0; // of the last debug_run_stage
     // junction tolerances: Costas phase (rad) / frequency (rad/sample) residual, M&M sampling instant (samples)
@@ -159,11 +165,16 @@ class Demod
     float tol_pphase = 1e-5f, tol_pfreq = 2e-6f;
     unsigned long long pm_dturn = 0, fs_dturn = 0; // rotator steps of PMToBPSK / FreqShiftBlock: fraction of a turn per sample, 0.64 fixed point
     unsigned long long pm_pos = 0, fs_pos = 0;     // samples those rotators have seen so far
-    DevBuf<float2> pm_agc, pm_pll, pm_out, fs_out;
+    DevBuf<float2> pm_agc, pm_pll, pm_out, fs_out; // (pm_agc: also fsk_demod's complex AGC output)
     DevBuf<float> d_atan_tab;
     long last_pm = 0;                    // samples through the carrier PLL in the last batch
     float snr_now = 0.f, snr_peak = 0.f; // M2M4SNREstimator::snr() after the last push / its maximum so far (module_psk_demod.cpp:190-194)
     long max_batch;
+    // fsk_demod: quadrature demodulator, float DC blocker and AGC outputs (agc2_out with a 32-sample front pad: the FIR's history)
+    bool fsk = false;
+    DevBuf<float> quad_out, dc2_out, agc2_out;
+    // complex AGC output (pm_agc) -> k_quad -> k_fsk_dc -> k_fsk_agc -> k_fir_real -> the clock recovery's input in bufA
+    void stage_fsk(long n, const FirTaps &taps, int cur, int nxt);
     int slot_cap_for(int L) const;
     int choose_L(long n) const;
 };

@@ -23,7 +23,7 @@ static void print_hrpt_stats(const std::string &dec, long frames, int state)
 int main(int argc, char **argv)
 {
     if (argc < 5) {
-        fprintf(stderr, "usage: %s <metop_ahrpt|jpss_hrd|npp_hrd|simple_bpsk|simple_qpsk|pm_bpsk|ldpc_qpsk|landsat|turbo_pm|turbo_bpsk|metop_dump|meteor_lrpt|noaa_hrpt|meteor_hrpt|aqua_db|aura_db|terra_db> baseband <input> <output_hint> [--fused] [--key value ...]\n", argv[0]);
+        fprintf(stderr, "usage: %s <metop_ahrpt|jpss_hrd|npp_hrd|simple_bpsk|simple_qpsk|pm_bpsk|ldpc_qpsk|landsat|turbo_pm|turbo_bpsk|metop_dump|meteor_lrpt|noaa_hrpt|meteor_hrpt|aqua_db|aura_db|terra_db|bluewalker3_wide|bluewalker3_narrow> baseband <input> <output_hint> [--fused] [--key value ...]\n", argv[0]);
         return 2;
     }
     const std::string pipe = argv[1], level = argv[2], in = argv[3], out = argv[4];
@@ -57,6 +57,14 @@ int main(int argc, char **argv)
         dp = Params{{"b200_demod_module", "terra_db_demod"}, {"symbolrate", "13125000"}};
         fp = Params{{"constellation", "bpsk_90"}, {"cadu_size", "8192"}, {"viterbi_ber_thresold", "0.300"}, {"viterbi_outsync_after", "20"},
                     {"derandomize", "true"}, {"derand_after_rs", "true"}, {"derand_start", "10"}, {"nrzm", "true"}, {"rs_i", "4"}, {"rs_type", "rs223"}};
+        dec = "ccsds_conv_concat_decoder";
+    } else if (pipe == "bluewalker3_wide" || pipe == "bluewalker3_narrow") { // resources/pipelines/BlueWalker3.json: fsk_demod at 512 | 128
+        // ksym/s (rrc_alpha 0.35), then ccsds_conv_concat_decoder (bpsk_90, CADUs of 9784 | 2648 bits, derandomised, no RS). The pipeline
+        // names no samplerate: it comes from the command line
+        const bool wide = pipe == "bluewalker3_wide";
+        dp = Params{{"b200_demod_module", "fsk_demod"}, {"symbolrate", wide ? "512000" : "128000"}, {"rrc_alpha", "0.35"}};
+        fp = Params{{"constellation", "bpsk_90"}, {"cadu_size", wide ? "9784" : "2648"}, {"viterbi_ber_thresold", "0.300"}, {"viterbi_outsync_after", "20"},
+                    {"derandomize", "true"}, {"rs_i", "0"}};
         dec = "ccsds_conv_concat_decoder";
     } else if (pipe == "jpss_hrd" || pipe == "npp_hrd") { // resources/pipelines/JPSS.json
         dp = Params{{"constellation", "oqpsk"}, {"symbolrate", pipe == "jpss_hrd" ? "25000000" : "15000000"}, {"rrc_alpha", "0.5"}, {"pll_bw", "0.002"}};

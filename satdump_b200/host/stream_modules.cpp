@@ -163,8 +163,70 @@ static b200_demod_cfg terra_db_demod_cfg_from_params(const Params &p, bool &is_b
     return c;
 }
 
+// fsk_demod (module_fsk_demod.cpp:13-57): required samplerate, symbolrate, rrc_alpha; optional rrc_taps, clock_alpha, clock_gain_omega,
+// clock_mu, clock_gain_mu, clock_omega_relative_limit + BaseDemodModule's options, in the constructor's order. The base working window
+// [1.1, 4.0] samples per symbol (module_demod_base.h:71-72; the module's own override is commented out)
+static b200_demod_cfg fsk_demod_cfg_from_params(const Params &p, bool &is_bpsk)
+{
+    b200_demod_cfg c{};
+    if (!p.has("samplerate"))
+        throw ModuleError("Samplerate parameter must be present!"); // module_demod_base.cpp:17-20
+    c.samplerate = (double)(long)p.num("samplerate");
+    if (!p.has("symbolrate"))
+        throw ModuleError("Symbolrate parameter must be present!");
+    c.symbolrate = (double)(long)p.num("symbolrate");
+    c.constellation = B200_BPSK; // one real symbol, one soft byte each (module_fsk_demod.cpp:133-134)
+    is_bpsk = true;
+    c.fsk_demod = 1;
+    // basic_shaping replaces the RRC by final_sps taps of 0.1 (:75-80); only the 31-tap RRC kernel is built
+    reject(p, "basic_shaping", "basic_shaping: the boxcar filter is not built");
+    if (!p.has("rrc_alpha"))
+        throw ModuleError("RRC Alpha parameter must be present!"); // :21-24
+    c.rrc_alpha = (float)p.num("rrc_alpha");
+    c.rrc_taps = (int)p.num("rrc_taps", 31);
+    c.agc_rate = (float)p.num("agc_rate", 1e-2);
+    c.clock_gain_omega = (float)(pow(1.7e-2, 2) / 4.0); // module_fsk_demod.h:28-31
+    c.clock_mu = 0.5f;
+    c.clock_gain_mu = 1.7e-2f;
+    c.clock_omega_limit = 0.005f;
+    if (p.has("clock_alpha")) { // :29-35: the float alpha squared (exactly, in double), then rounded to the float member
+        const float a = (float)p.num("clock_alpha");
+        c.clock_gain_omega = (float)(pow(a, 2) / 4.0);
+        c.clock_gain_mu = a;
+    }
+    c.clock_gain_omega = (float)p.num("clock_gain_omega", c.clock_gain_omega);
+    c.clock_mu = (float)p.num("clock_mu", c.clock_mu);
+    c.clock_gain_mu = (float)p.num("clock_gain_mu", c.clock_gain_mu);
+    c.clock_omega_limit = (float)p.num("clock_omega_relative_limit", c.clock_omega_limit);
+    const std::string fmt = p.str("baseband_format", "cf32");
+    if (fmt == "cf32" || fmt == "f32") c.format = B200_CF32;
+    else if (fmt == "cs16" || fmt == "s16") c.format = B200_CS16;
+    else if (fmt == "cs8" || fmt == "s8") c.format = B200_CS8;
+    else if (fmt == "ziq") c.format = -1;
+    else throw ModuleError("baseband_format " + fmt + " is not supported by the B200 path (cf32/cs16/cs8, uncompressed ziq)");
+    c.dc_block = p.flag("dc_block", false);
+    c.freq_shift = (double)(long)p.num("freq_shift", 0);
+    c.iq_swap = p.flag("iq_swap", false);
+    reject(p, "enable_doppler", "Doppler correction");
+    reject(p, "dump_intermediate", "intermediate dump");
+    const float min_sps = (float)p.num("min_sps", 0), max_sps = (float)p.num("max_sps", 0);
+    c.final_samplerate = b200_demod_final_samplerate(c.samplerate, c.symbolrate, B200_BPSK, min_sps, max_sps,
+                                                     p.has("custom_samplerate") ? (double)(long)p.num("custom_samplerate") : 0.0);
+    if (c.final_samplerate == c.samplerate)
+        c.final_samplerate = 0;
+    else if (!b200_demod_resample_decision(c.samplerate, c.symbolrate, B200_BPSK, min_sps, max_sps))
+        c.front_resample = 2;
+    if ((float)c.samplerate / (float)c.symbolrate < 1.0f) // module_demod_base.cpp:96-105
+        throw ModuleError("Your sampling rate is too low! Minimum: " +
+                          (c.symbolrate > 1e6 ? std::to_string(c.symbolrate / 1e6) + " Msps" : std::to_string(c.symbolrate / 1e3) + " ksps"));
+    c.device = (int)p.num("b200_device", 0);
+    return c;
+}
+
 b200_demod_cfg demod_cfg_from_params(const Params &p, bool &is_bpsk, const std::string &module_id)
 {
+    if (module_id == "fsk_demod")
+        return fsk_demod_cfg_from_params(p, is_bpsk);
     if (module_id == "pm_demod")
         return pm_demod_cfg_from_params(p, is_bpsk);
     if (module_id == "terra_db_demod")
@@ -548,7 +610,7 @@ static void check(int rc, const char *what)
 PskDemodStage::PskDemodStage(std::string in, std::string hint, Params p, std::string module_id)
     : StageBase(std::move(in), std::move(hint), std::move(p)), id(std::move(module_id))
 {
-    if (id != "psk_demod" && id != "pm_demod" && id != "terra_db_demod")
+    if (id != "psk_demod" && id != "pm_demod" && id != "terra_db_demod" && id != "fsk_demod")
         throw ModuleError("unknown demodulator module " + id);
     cfg = demod_cfg_from_params(params, is_bpsk, id);
     batch_samples = (long)params.num("b200_batch_samples", (double)batch_samples);

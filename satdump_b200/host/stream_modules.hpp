@@ -90,6 +90,7 @@ class StageBase
 // Options whose blocks are not part of this build (has_carrier, doppler, dump_intermediate) raise ModuleError instead of silently doing
 // something else. module_id "pm_demod": PMDemodModule's parameter set (pll_bw = the carrier PLL's, costas_bw, pll_max_offset,
 // resample_after_pll, subcarrier_offset), soft = clamp(real * 100), stats key "freq" = the carrier PLL's frequency. module_id
+// "fsk_demod": FSKDemodModule's parameter set (rrc_alpha required, its own clock defaults; basic_shaping refused by name).
 // "terra_db_demod": TerraDBDemodModule's fixed chain (BPSK loops at twice "symbolrate"); a working rate below 1.1 samples per half-symbol
 // is refused by name.
 class PskDemodStage : public StageBase

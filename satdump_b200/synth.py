@@ -990,3 +990,47 @@ def turbo_frames(nframes, rate, base, seed=0):
     tx = np.concatenate([np.tile(asm, (nframes, 1)), cw ^ ldpc_pn_bits(cw.shape[1])[None, :]], axis=1)
     cadu = np.concatenate([np.tile(np.frombuffer(ASM, np.uint8), (nframes, 1)), info], axis=1)
     return tx, cadu
+
+
+def fsk_signal(nsamples, samplerate, symbolrate, h=0.7, seed=0, bits=None, carrier=0.0, rate_offset=0.0, snr_db=None, zeros=(), fmt="cf32",
+               amp=0.5):
+    """Continuous-phase FSK: the bits (random from seed when None) mapped 0 -> -1, 1 -> +1, held for a symbol each, frequency deviation
+    h * symbolrate / 2, plus a carrier offset (Hz), a sample-rate offset (relative), AWGN at snr_db (None: none) and stretches of zero
+    samples zeros = ((start, length), ...). Returns (iq as cf32 complex64 / cs16 or cs8 interleaved int, the bits)."""
+    rng = np.random.default_rng(seed)
+    sps = samplerate / symbolrate * (1.0 + rate_offset)
+    nsym = int(np.ceil(nsamples / sps)) + 2
+    if bits is None:
+        bits = rng.integers(0, 2, nsym, dtype=np.uint8)
+    bits = np.resize(np.asarray(bits, np.uint8), nsym)
+    k = np.minimum((np.arange(nsamples) / sps).astype(np.int64), nsym - 1)
+    f = (2.0 * bits[k].astype(np.float64) - 1.0) * (h * symbolrate / 2.0) + carrier
+    phase = 2.0 * np.pi * np.cumsum(f) / samplerate
+    x = amp * np.exp(1j * phase)
+    if snr_db is not None:
+        sigma = amp / np.sqrt(2.0) * 10.0 ** (-snr_db / 20.0)
+        x = x + sigma * (rng.standard_normal(nsamples) + 1j * rng.standard_normal(nsamples))
+    for a, n in zeros:
+        x[a:a + n] = 0
+    if fmt == "cf32":
+        return x.astype(np.complex64), bits
+    scale = 32767.0 if fmt == "cs16" else 127.0
+    dt = np.int16 if fmt == "cs16" else np.int8
+    out = np.empty(2 * nsamples, dt)
+    out[0::2] = np.clip(np.round(x.real * scale), -scale, scale)
+    out[1::2] = np.clip(np.round(x.imag * scale), -scale, scale)
+    return out, bits
+
+
+def fsk_frames(nframes, cadu_size, seed=0):
+    """(coded bits on air, the CADUs ccsds_conv_concat_decoder writes for them [n, cadu_size / 8]) of BlueWalker3.json's decoder: bpsk_90,
+    cadu_size bits (ASM + payload, no Reed-Solomon), randomised from byte 4, rate 1/2 convolutional code. As for terra_db_frames, the
+    module swaps each soft pair and rotates it by 90 degrees, so a code pair (a, b) goes on air as (a, not b)."""
+    nb = cadu_size // 8
+    payload = np.random.default_rng(seed).integers(0, 256, size=(nframes, nb - 4), dtype=np.uint8)
+    clear = np.concatenate([np.tile(np.frombuffer(ASM, np.uint8), (nframes, 1)), payload], axis=1)
+    tx = clear.copy()
+    tx[:, 4:] ^= ccsds_pn(nb - 4)[None, :]
+    coded = conv_encode(np.unpackbits(tx.reshape(-1)))
+    coded[1::2] ^= 1
+    return coded, clear

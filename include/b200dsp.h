@@ -213,6 +213,7 @@ typedef struct b200_demod_stats
     long pll_unconverged;     /* pm_demod: carrier PLL junctions still inconsistent after the repair rounds of the last push (expected 0) */
     int repair_merge_hist[8]; /* the repairs by where they ended: [0] ran the whole segment; [i] met the segment's stored run at its
                                  checkpoint j (512 samples apart), 2^(i-2) < j <= 2^(i-1), and stopped there; [7]: any later one */
+    int last_range_tiles;     /* 2048-sample tiles per range of the AGC + RRC kernel in the last push (b200_demod_debug_shape) */
 } b200_demod_stats;
 
 typedef struct b200_fec_stats
@@ -297,6 +298,14 @@ int b200_demod_debug_junctions(b200_demod *d, double *costas_out, double *mm_out
 int b200_demod_debug_convert(b200_demod *d, const void *host_iq, long nsamples, float *host_out);
 /* test hook: enable = 0 gives the repairs a tolerance of 0 for meeting the stored run, so every repair runs its whole segment */
 int b200_demod_debug_repair_merge(b200_demod *d, int enable);
+/* test hook: the shape of this handle's pushes, so that tests reach the geometries of large pushes with small ones.
+ *   range_tiles > 0: the AGC + RRC kernel runs ranges of that many 2048-sample tiles (0: the production rule, at least 4 tiles; the
+ *                    floor only amortises the walk back that proves each range's start gain, any length >= 1 computes the same stream)
+ *   seg_len > 0:     the loop kernels' segment length, a multiple of 16 in [4096, 16384] (0: the production rule); else B200_EINVAL
+ *   keep_front != 0: each push copies the production front kernel's RRC output, so that b200_demod_debug_stage(B200_STAGE_FIR)
+ *                    returns it. A keep_stages handle runs the dumping variant of that kernel instead and refuses this.
+ * The range length of the last push is b200_demod_stats.last_range_tiles, its segment length b200_demod_debug_junctions' seg_len. */
+int b200_demod_debug_shape(b200_demod *d, int range_tiles, int seg_len, int keep_front);
 /* Cycle counters of the loop kernels' main passes, only in a library built with -DB200_LOOP_CYCLES (tools/profile_loops.py --cycles):
  * out[0..3] = clock64() cycles summed over the warps of k_costas (or k_pll) in its phases row wait, loop, copy-out, tail, out[4] = those
  * warps; out[5..9] the same for k_mm (row wait, input fix-up, symbol loop, symbol copy-out; warps), all since the previous call, which

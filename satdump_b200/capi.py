@@ -22,7 +22,7 @@ E_NAMES = {0: "OK", -1: "EINVAL", -2: "ENODEV", -3: "ECUDA", -4: "ENOMEM", -5: "
 SYMBOLS = [
     "b200_last_error", "b200_device_count", "b200_demod_final_samplerate", "b200_demod_resample_decision", "b200_demod_resampler_bank",
     "b200_demod_create", "b200_demod_destroy", "b200_demod_push_iq", "b200_demod_push_iq_device", "b200_demod_pull_soft",
-    "b200_demod_pull_symbols", "b200_demod_debug_stage", "b200_demod_debug_convert", "b200_demod_debug_run_stage", "b200_demod_debug_junctions", "b200_demod_debug_repair_merge", "b200_demod_debug_loop_cycles", "b200_demod_reset", "b200_demod_prefetch_iq", "b200_demod_last_timing", "b200_demod_get_stats", "b200_demod_get_taps",
+    "b200_demod_pull_symbols", "b200_demod_debug_stage", "b200_demod_debug_convert", "b200_demod_debug_run_stage", "b200_demod_debug_junctions", "b200_demod_debug_repair_merge", "b200_demod_debug_shape", "b200_demod_debug_loop_cycles", "b200_demod_reset", "b200_demod_prefetch_iq", "b200_demod_last_timing", "b200_demod_get_stats", "b200_demod_get_taps",
     "b200_fec_create", "b200_fec_destroy", "b200_fec_push_soft", "b200_fec_push_soft_device", "b200_fec_pull_frames",
     "b200_fec_debug_bits", "b200_fec_get_stats", "b200_fec_cadu_bytes", "b200_fec_chunk_size", "b200_fec_debug_ldpc_frames", "b200_fec_ldpc_timing",
     "b200_fec_debug_turbo_frames", "b200_fec_debug_turbo_llr", "b200_fec_turbo_timing", "b200_fec_debug_dump_frames", "b200_fec_debug_meteor_frames",
@@ -76,7 +76,8 @@ class DemodStats(C.Structure):
                 ("costas_freq", C.c_float), ("mm_mu", C.c_float), ("mm_omega", C.c_float), ("costas_unconverged", C.c_long),
                 ("mm_unconverged", C.c_long), ("agc_clamped", C.c_int), ("repairs", C.c_int), ("kernel_launches", C.c_long),
                 ("agc_exact_passes", C.c_long), ("last_front_samples", C.c_long), ("snr", C.c_float), ("peak_snr", C.c_float),
-                ("pll_freq", C.c_float), ("pll_unconverged", C.c_long), ("repair_merge_hist", C.c_int * 8)]
+                ("pll_freq", C.c_float), ("pll_unconverged", C.c_long), ("repair_merge_hist", C.c_int * 8),
+                ("last_range_tiles", C.c_int)]
 
 
 class FecStats(C.Structure):
@@ -143,6 +144,7 @@ def lib():
         L.b200_demod_debug_junctions.argtypes = [vp, vp, vp, cl, C.POINTER(cl), C.POINTER(cl)]
         L.b200_demod_get_stats.argtypes = [vp, C.POINTER(DemodStats)]
         L.b200_demod_debug_repair_merge.argtypes = [vp, ci]
+        L.b200_demod_debug_shape.argtypes = [vp, ci, ci, ci]
         L.b200_demod_reset.argtypes = [vp]
         L.b200_demod_prefetch_iq.argtypes = [vp, vp, cl]
         L.b200_demod_last_timing.argtypes = [vp, vp, ci]
@@ -507,6 +509,13 @@ class Demod:
     def repair_merge(self, enable):
         """Test hook: False makes every repair run its whole segment (tolerance 0 for meeting the stored run)."""
         _chk(lib().b200_demod_debug_repair_merge(self.h, 1 if enable else 0))
+        return self
+
+    def debug_shape(self, range_tiles=0, seg_len=0, keep_front=False):
+        """Test hook: force the AGC + RRC kernel's range length (tiles) and the loop kernels' segment length (0: production rules);
+        keep_front makes stage("fir") return the production front kernel's output. stats()["last_range_tiles"] and junctions()[2]
+        report what the last push ran."""
+        _chk(lib().b200_demod_debug_shape(self.h, int(range_tiles), int(seg_len), 1 if keep_front else 0))
         return self
 
     def timing(self):

@@ -567,6 +567,8 @@ int Demod::choose_L(long n) const
 {
     // one segment per thread; aim at one full wave of resident threads, but keep segments within [4096, 16384] samples: a segment
     // shorter than a few loop time constants (M&M: ~1200 samples) spends its whole life in the tail of its warm-up transient
+    if (dbg_seg_len > 0)
+        return dbg_seg_len;
     long L = (n + seg_cap_threads - 1) / seg_cap_threads;
     L = std::max<long>(4096, std::min<long>(16384, L));
     return (int)((L + 15) / 16 * 16);
@@ -581,8 +583,10 @@ int Demod::slot_cap_for(int L) const
 template <int FMT> static void launch_front(Demod &d, const void *raw, long n, int ntiles, FirTaps taps, const AgcUnit &u)
 {
     DemodDevState *S = d.st.p;
-    // one wave of resident warps, each running a range of R consecutive tiles
-    const int R = std::max(4, (ntiles + d.fir_warps - 1) / d.fir_warps);
+    // one wave of resident warps, each running a range of R consecutive tiles. Any R >= 1 computes the same stream; the floor of 4
+    // amortises the walk back that proves a range's start gain (normally 4-5 tiles of map-only work)
+    const int R = d.dbg_range_tiles > 0 ? d.dbg_range_tiles : std::max(4, (ntiles + d.fir_warps - 1) / d.fir_warps);
+    d.last_R = R;
     const int nranges = (ntiles + R - 1) / R;
     const int grid = (nranges + FW_WARPS - 1) / FW_WARPS;
     AgcCtl ctl;
@@ -912,7 +916,7 @@ long Demod::process(const void *d_raw, long n, int8_t *soft_dst)
     }
     B200_CUDA(cudaEventRecord(ev[1], stream));
     float2 *fir_out = bufA.p + 16, *cos_out = bufB.p + 16;
-    if (dump)
+    if (dump || keep_front)
         B200_CUDA(cudaMemcpyAsync(fir_dump.p, fir_out, n * sizeof(float2), cudaMemcpyDeviceToDevice, stream));
 
     const int L = choose_L(n);
@@ -1159,6 +1163,7 @@ void Demod::stats(b200_demod_stats *o)
     o->peak_snr = snr_peak;
     o->pll_freq = (pm || cfg.has_carrier) ? h_state.p->pll[parity][1] : 0.f;
     o->pll_unconverged = (pm || cfg.has_carrier) ? h_state.p->pll_unconv : 0;
+    o->last_range_tiles = last_R;
 }
 
 } // namespace b200
@@ -1290,7 +1295,8 @@ int b200_demod_debug_stage(b200_demod *h, int stage, float *out, long cap_sample
     return guarded([&] {
         B200_REQUIRE(h && out, B200_EINVAL, "NULL argument");
         Demod &d = *h->d;
-        B200_REQUIRE(d.cfg.keep_stages, B200_ESTATE, "create the demodulator with keep_stages=1 to read stage outputs");
+        B200_REQUIRE(d.cfg.keep_stages || (d.keep_front && stage == B200_STAGE_FIR), B200_ESTATE,
+                     "create the demodulator with keep_stages=1 to read stage outputs (or set keep_front for the RRC output)");
         // pm_demod: the first AGC, the carrier PLL and PMToBPSK run on last_pm samples (the input rate with resample_after_pll)
         const bool at_pll = d.pm && (stage == B200_STAGE_AGC || stage == B200_STAGE_PLL || stage == B200_STAGE_PM);
         const long count = stage == B200_STAGE_DC ? d.last_in : (at_pll ? d.last_pm : d.last_n);
@@ -1391,6 +1397,25 @@ int b200_demod_debug_repair_merge(b200_demod *h, int enable)
     return guarded([&] {
         B200_REQUIRE(h, B200_EINVAL, "NULL argument");
         h->d->repair_merge = enable != 0;
+    });
+}
+int b200_demod_debug_shape(b200_demod *h, int range_tiles, int seg_len, int keep_front)
+{
+    return guarded([&] {
+        B200_REQUIRE(range_tiles >= 0, B200_EINVAL, "range_tiles %d: a range has at least one tile (0 = the production rule)", range_tiles);
+        B200_REQUIRE(seg_len == 0 || (seg_len >= 4096 && seg_len <= 16384 && seg_len % 16 == 0), B200_EINVAL,
+                     "seg_len %d: the loop kernels take a multiple of 16 in [4096, 16384] (0 = the production rule)", seg_len);
+        B200_REQUIRE(h, B200_EINVAL, "NULL argument");
+        Demod &d = *h->d;
+        B200_REQUIRE(!(keep_front && d.cfg.keep_stages), B200_EINVAL,
+                     "keep_front copies the production front kernel's output, which a keep_stages handle does not run");
+        if (keep_front && !d.fir_dump.p) {
+            DeviceGuard g(d.cfg.device);
+            d.fir_dump.alloc(d.max_work);
+        }
+        d.dbg_range_tiles = range_tiles;
+        d.dbg_seg_len = seg_len;
+        d.keep_front = keep_front != 0;
     });
 }
 int b200_demod_debug_loop_cycles(unsigned long long *out, int cap)

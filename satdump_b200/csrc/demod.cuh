@@ -489,7 +489,14 @@ __device__ __forceinline__ float fast_mag(float s2)
 // not hit). Inside a tile a composed map is carried as the float pair (E, B): g -> g*(1 - E) + B. Keeping E = 1 - a rather than
 // a keeps the *relative* precision of the decay for weak signals (e ~ 1e-5), so float is enough here: the composition depth on
 // any path is ~20 and a seed error decays by (1 - e) per sample anyway. Across tiles the maps are composed in fp64.
+// Strong input (cf32 above full scale, rate|x| ~ 0.1 per sample) is the opposite case: a composed decay 1 - E falls below the float
+// resolution of E, and a gain far above the new level (the chunks right after a step up) would be weighted by a decay that is off by
+// up to 6e-8 absolute, 1e-5 of the gain that follows. The decay is therefore also carried as the product a of the steps' (1 - e), which
+// keeps its relative precision, and replaces 1 - E below AGC_A_SMALL. Inputs within full scale (rate|x| <= 0.0142, so a chunk decays by
+// no less than 0.026 and a lane's prefix by more) never reach it, and their arithmetic is the (E, B) one alone.
 struct EB { float E, B; };
+constexpr float AGC_A_SMALL = 1.0f / 64;
+constexpr float AGC_E_LANE = 0.12f; // a lane's E at most this: its decay >= 0.88, and 0.88^32 = 0.0167 > AGC_A_SMALL
 __device__ __forceinline__ EB eb_compose(const EB first, const EB second)
 {
     EB r;
@@ -532,6 +539,16 @@ __device__ __forceinline__ EB agc_map8(const float2 (&x)[8], float rate, float (
         m.E = fmaf(-m.E, e[i], m.E + e[i]);
     }
     return m;
+}
+
+// the decay of a lane's steps as a product (AGC_A_SMALL); e[q] = 0 for samples beyond the stream
+__device__ __forceinline__ float decay8(const float (&e)[8])
+{
+    float a = 1.f;
+#pragma unroll
+    for (int q = 0; q < 8; q++)
+        a = fmaf(-e[q], a, a);
+    return a;
 }
 
 // Control block of the AGC seeding. need[epoch & 1] is raised by the fast pass when some range cannot prove its seed; the exact
@@ -667,6 +684,7 @@ __device__ __forceinline__ void fw_chunk(FwState<FMT> &st, RawRegs<FMT> &rr, int
             }
         }
     }
+    const bool strong = inc.E > AGC_E_LANE; // (the lane's own map, before the scan)
 #pragma unroll
     for (int off = 1; off < 32; off <<= 1) {
         EB p;
@@ -685,9 +703,23 @@ __device__ __forceinline__ void fw_chunk(FwState<FMT> &st, RawRegs<FMT> &rr, int
     excl.B = __shfl_up_sync(0xffffffffu, inc.B, 1);
     excl.E = lane > 0 ? excl.E : 0.f; // identity map in lane 0
     excl.B = lane > 0 ? excl.B : 0.f;
+    // the decays as products (AGC_A_SMALL), scanned only when some lane's own E exceeds AGC_E_LANE: otherwise every prefix of the 32
+    // lanes decays by more than AGC_A_SMALL and the (E, B) form is the one used anyway
+    float exclA = 1.f, totA = 1.f;
+    if (__any_sync(0xffffffffu, strong)) {
+        float incA = decay8(e);
+#pragma unroll
+        for (int off = 1; off < 32; off <<= 1) {
+            const float pA = __shfl_up_sync(0xffffffffu, incA, off);
+            incA = lane >= off ? pA * incA : incA;
+        }
+        totA = __shfl_sync(0xffffffffu, incA, 31);
+        exclA = __shfl_up_sync(0xffffffffu, incA, 1);
+        exclA = lane > 0 ? exclA : 1.f;
+    }
     const float Gf = (float)st.G;
-    float g = fmaf(-excl.E, Gf, Gf) + excl.B;
-    st.G = fma(1.0 - (double)totE, st.G, (double)totB);
+    float g = exclA < AGC_A_SMALL ? fmaf(exclA, Gf, excl.B) : fmaf(-excl.E, Gf, Gf) + excl.B;
+    st.G = fma(totA < AGC_A_SMALL ? (double)totA : 1.0 - (double)totE, st.G, (double)totB);
     if (CLAMP) {
         const float totC = __shfl_sync(0xffffffffu, incC, 31);
         float exclC = __shfl_up_sync(0xffffffffu, incC, 1);
@@ -824,6 +856,7 @@ __global__ void __launch_bounds__(32 * FW_WARPS, 8) k_agc_fir_w(const void *__re
             load8<FMT>(raw, (long)j * FW_CH + 8 * lane, N, x);
             float e[8];
             EB m = agc_map8(x, rate, e);
+            const bool strong = __any_sync(0xffffffffu, m.E > AGC_E_LANE);
 #pragma unroll
             for (int off = 1; off < 32; off <<= 1) { // lane l <- groups [l, l + 2*off)
                 EB o;
@@ -833,8 +866,17 @@ __global__ void __launch_bounds__(32 * FW_WARPS, 8) k_agc_fir_w(const void *__re
                     m = eb_compose(m, o);
             }
             const float tE = __shfl_sync(0xffffffffu, m.E, 0), tB = __shfl_sync(0xffffffffu, m.B, 0);
+            double decay = 1.0 - (double)tE;
+            if (strong) { // the chunk's decay as a product (AGC_A_SMALL)
+                float a = decay8(e);
+#pragma unroll
+                for (int off = 1; off < 32; off <<= 1)
+                    a *= __shfl_xor_sync(0xffffffffu, a, off);
+                if (a < AGC_A_SMALL)
+                    decay = (double)a;
+            }
             Bc = fma(A, (double)tB, Bc);
-            A *= 1.0 - (double)tE;
+            A *= decay;
             // anything older enters as A * gain with gain <= max_gain (2^16 for the demodulator's AGC): done once that is below float resolution of the seed
             if (A * (double)ctl.max_gain <= Bc * 0x1p-30) {
                 ok = true;

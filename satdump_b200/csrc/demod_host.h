@@ -93,6 +93,11 @@ class Demod
     // junction tolerance itself 5 of 510 repairs of successors no longer happen, with 1/2 and 1/4 one, from 1/8 on none).
     static constexpr float MERGE_TIGHTER = 16.0f;
     bool repair_merge = true;  // test hook (b200_demod_debug_repair_merge): false = tolerance 0, every repair runs its whole segment
+    // test hook (b200_demod_debug_shape): forced range length of k_agc_fir_w / segment length of the loop kernels (0: production
+    // rules), and a copy of the production front kernel's RRC output into fir_dump
+    int dbg_range_tiles = 0, dbg_seg_len = 0;
+    bool keep_front = false;
+    int last_R = 0; // range length of the last launch_front
 
     b200_demod_cfg cfg;
     cudaStream_t stream = nullptr;

@@ -108,3 +108,17 @@ def test_bench_reference_arm_contract(built):
         assert set(cb["variants"]) == {"generic_O2", "native_O3_fma"}
         for v in cb["variants"].values():
             assert len(v["one_stream_MSps_runs"]) >= 3 and v["stage_single_thread_MSps"]["fir"] > 0
+
+
+def test_debug_shape_validates_its_arguments(built):
+    """b200_demod_debug_shape checks its values before it looks at the handle: a segment length the loop kernels cannot run (not a
+    multiple of 16, outside [4096, 16384]) and a negative range length are refused by name, valid ones get as far as the NULL handle."""
+    from satdump_b200 import capi
+    L = capi.lib()
+    for seg_len in (4095, 4100, 16400, 16392, -16, 1):
+        assert L.b200_demod_debug_shape(None, 0, seg_len, 0) == -1
+        assert "seg_len" in capi.last_error(), (seg_len, capi.last_error())
+    assert L.b200_demod_debug_shape(None, -1, 0, 0) == -1 and "range_tiles" in capi.last_error()
+    for range_tiles, seg_len in ((0, 0), (1, 4096), (64, 4112), (3, 15888), (0, 16384)):
+        assert L.b200_demod_debug_shape(None, range_tiles, seg_len, 1) == -1
+        assert "NULL" in capi.last_error(), (range_tiles, seg_len, capi.last_error())

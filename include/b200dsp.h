@@ -53,7 +53,7 @@ enum { B200_CF32 = 0, B200_CS16 = 1, B200_CS8 = 2 };
 /* decoder kind */
 enum { B200_FEC_METOP = 0, B200_FEC_CCSDS = 1, B200_FEC_SIMPLE = 2, B200_FEC_LDPC = 3, B200_FEC_TURBO = 4, B200_FEC_METOP_DUMP = 5,
        B200_FEC_METEOR_LRPT = 6, B200_FEC_NOAA_HRPT = 7 /* noaa_hrpt_decoder */, B200_FEC_METEOR_HRPT = 8 /* meteor_hrpt_decoder */,
-       B200_FEC_AQUA_DB = 9 /* aqua_db_decoder */ };
+       B200_FEC_AQUA_DB = 9 /* aqua_db_decoder */, B200_FEC_NOAA_GAC = 10 /* noaa_gac_decoder */, B200_FEC_DMSP_RTD = 11 /* dmsp_rtd_decoder */ };
 /* debug stage ids for b200_demod_debug_stage */
 enum { B200_STAGE_AGC = 0, B200_STAGE_FIR = 1, B200_STAGE_COSTAS = 2, B200_STAGE_RESAMP = 3, B200_STAGE_DC = 4, B200_STAGE_MM = 5,
        B200_STAGE_PLL = 6 /* pm_demod: PLLCarrierTrackingBlock output */, B200_STAGE_PM = 7 /* pm_demod: PMToBPSK output */,
@@ -193,6 +193,17 @@ typedef struct b200_fec_cfg
        deframer_state reports 2 / 6 / 10. A push that ends inside a symbol keeps its odd byte for the next push. Only device and max_soft
        are read; max_soft <= 2^30. Device memory: about 1.4 bytes per max_soft byte (soft FIFO, bit FIFO, room for two pushes of CADUs). */
     int deframer_thresold;    /* "deframer_thresold" of noaa_hrpt_decoder (required by the module): 0 .. 60                              */
+    /* kind B200_FEC_NOAA_GAC = noaa_gac_decoder (module_noaa_gac_decoder.cpp): hard bits soft > 0 -> BPSK_CCSDS_Deframer(33270, 0xA116FD71,
+       backward: 0x33C3E4A6) with states 2 / 6 / 12 and 6 bits of padding: a frame is 4159 bytes, the clean sync word, the payload XOR the
+       inversion, its last byte holding 6 bits right-aligned. backward reverses each frame's 33270 bits from that byte image, as the
+       module does (the last two data bits are lost, two zero bits enter). Then every frame is XORed byte by byte with the GAC PN sequence
+       (60 zero bits, then the 1023-bit sequence repeated). cadu_bytes 4159; backward playback's reversal of the frame ORDER is the file
+       writer's (the host layer). Only backward, device and max_soft are read.
+       kind B200_FEC_DMSP_RTD = dmsp_rtd_decoder (module_dmsp_rtd_decoder.cpp, dmsp_deframer.cpp): hard bits soft > 0 -> DMSP_Deframer(150, 2):
+       the 13-bit sync 0b1010110011111 (or its complement: inverted), states 0 / 2 / 6, each its own error threshold; a frame is 19 bytes,
+       the clean sync and 137 bits XOR the inversion, its last byte holding 6 bits right-aligned. Only device and max_soft are read.
+       Both: max_soft <= 2^30; b200_fec_frame_bits returns the stream bit at which each pulled frame completed. */
+    int backward;             /* "backward" of noaa_gac_decoder (required by the module): backward tape playback                         */
 } b200_fec_cfg;
 
 typedef struct b200_demod_stats
@@ -222,7 +233,8 @@ typedef struct b200_fec_stats
     int viterbi_state;        /* 0 NOSYNC 1 SYNCED  (Viterbi3_4::getState)                       */
     float viterbi_ber;
     int deframer_state;       /* 2 NOSYNC / 6 SYNCING / 12|18 SYNCED (BPSK_CCSDS_Deframer; aqua_db_decoder: 10); meteor_hrpt_decoder: its own state
-                                 numbers 0 (NOSYNC) / 2, 6 (SYNCING) / 12 (SYNCED, "deframer_lock"); noaa_hrpt_decoder: 0           */
+                                 numbers 0 (NOSYNC) / 2, 6 (SYNCING) / 12 (SYNCED, "deframer_lock"); noaa_hrpt_decoder: 0;
+                                 noaa_gac_decoder: 2 / 6 / 12; dmsp_rtd_decoder: 0 (NOSYNC) / 2 (SYNCING) / 6 (SYNCED)                */
     long rs_corrected, rs_failed;
     long replays;             /* slow-path re-decodes (lock changes, start-state mis-speculation) */
     long kernel_launches;
@@ -396,6 +408,10 @@ typedef struct b200_hrpt_frame
     int state;                /* the state that accepted it: METEOR 0 / 2 / 6 / 12; NOAA 0                                            */
 } b200_hrpt_frame;
 int b200_fec_debug_hrpt_frames(b200_fec *f, b200_hrpt_frame *out, long cap, long *n_out);
+/* noaa_gac_decoder / dmsp_rtd_decoder: for each frame the last b200_fec_pull_frames returned, in order, the stream bit index (soft bytes
+   since create / reset) of the bit that completed it. dmsp_rtd_decoder's "_timestamps.txt" needs it: the module stamps a frame with the
+   number of 8192-byte reads that produced frames, up to the one holding that bit. Other kinds: B200_EINVAL. */
+int b200_fec_frame_bits(b200_fec *f, long *out, long cap, long *n_out);
 
 /* ---- fused chain: raw IQ -> CADUs, soft stream stays in HBM ---------------------------------------- */
 b200_chain *b200_chain_create(const b200_demod_cfg *dcfg, const b200_fec_cfg *fcfg);

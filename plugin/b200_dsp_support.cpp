@@ -6,7 +6,7 @@
 //
 //   loader()                          the one symbol SatDump dlsym()s (core/plugin.cpp:15-33)
 //   B200DSPSupport::init()            on SatDumpStartedEvent (fired after every plugin registered its modules, init.cpp:163) the
-//                                     entries "psk_demod", "pm_demod", "terra_db_demod", "fsk_demod", "metop_ahrpt_decoder", "ccsds_conv_concat_decoder", "ccsds_simple_psk_decoder", "ccsds_ldpc_decoder", "ccsds_turbo_decoder", "metop_dump_decoder", "meteor_lrpt_decoder", "noaa_hrpt_decoder", "meteor_hrpt_decoder" and "aqua_db_decoder" of
+//                                     entries "psk_demod", "pm_demod", "terra_db_demod", "fsk_demod", "metop_ahrpt_decoder", "ccsds_conv_concat_decoder", "ccsds_simple_psk_decoder", "ccsds_ldpc_decoder", "ccsds_turbo_decoder", "metop_dump_decoder", "meteor_lrpt_decoder", "noaa_hrpt_decoder", "meteor_hrpt_decoder", "aqua_db_decoder", "noaa_gac_decoder" and "dmsp_rtd_decoder" of
 //                                     satdump::pipeline::modules_registry (module.h:210, looked up first-match by id, module.cpp:129-135)
 //                                     get their factory replaced, so existing pipelines instantiate the CUDA modules.
 //                                     Set B200_DSP_REGISTER_ONLY=1 to register "<id>_b200" ids instead and leave the originals alone.
@@ -259,6 +259,17 @@ namespace b200plugin
                 v["frame_count"] = stage->frames_written.load();
                 return v;
             }
+            if (stage->getID() == "noaa_gac_decoder") // NOAAGACDecoderModule::getModuleStats (module_noaa_gac_decoder.cpp:144-150): the
+            {                                         // HRPT module's divisor, as the module has it
+                v["frame_count"] = stage->frames_written.load() / 11090;
+                return v;
+            }
+            if (stage->getID() == "dmsp_rtd_decoder") // DMSPRTDDecoderModule::getModuleStats (module_dmsp_rtd_decoder.cpp:76-82)
+            {
+                const int ds = stage->deframer_state.load();
+                v["deframer_state"] = ds == 0 ? "NOSYNC" : (ds == 2 ? "SYNCING" : "SYNCED");
+                return v;
+            }
             if (stage->getID() == "aqua_db_decoder") // AquaDBDecoderModule::getModuleStats (module_aqua_db_decoder.cpp:83-93): SYNCED is state 10
             {
                 const int ds = stage->deframer_state.load();
@@ -312,7 +323,7 @@ public:
     {
         for (const char *id : {"psk_demod", "pm_demod", "terra_db_demod", "fsk_demod", "metop_ahrpt_decoder", "ccsds_conv_concat_decoder", "ccsds_simple_psk_decoder", "ccsds_ldpc_decoder",
                                "ccsds_turbo_decoder", "metop_dump_decoder", "meteor_lrpt_decoder", "noaa_hrpt_decoder", "meteor_hrpt_decoder",
-                               "aqua_db_decoder"})
+                               "aqua_db_decoder", "noaa_gac_decoder", "dmsp_rtd_decoder"})
             evt.modules_registry.push_back({std::string(id) + "_b200", nlohmann::json(), factory(id)});
     }
 
@@ -322,7 +333,7 @@ public:
             if (e.id == "psk_demod" || e.id == "pm_demod" || e.id == "terra_db_demod" || e.id == "fsk_demod" || e.id == "metop_ahrpt_decoder" || e.id == "ccsds_conv_concat_decoder" || e.id == "ccsds_simple_psk_decoder" ||
                 e.id == "ccsds_ldpc_decoder" || e.id == "ccsds_turbo_decoder" || e.id == "metop_dump_decoder" ||
                 e.id == "meteor_lrpt_decoder" || e.id == "noaa_hrpt_decoder" || e.id == "meteor_hrpt_decoder" ||
-                e.id == "aqua_db_decoder")
+                e.id == "aqua_db_decoder" || e.id == "noaa_gac_decoder" || e.id == "dmsp_rtd_decoder")
             {
                 e.inst = factory(e.id);
                 logger->info("b200_dsp_support: module " + e.id + " now runs on the B200 path");

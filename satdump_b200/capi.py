@@ -26,7 +26,7 @@ SYMBOLS = [
     "b200_fec_create", "b200_fec_destroy", "b200_fec_push_soft", "b200_fec_push_soft_device", "b200_fec_pull_frames",
     "b200_fec_debug_bits", "b200_fec_get_stats", "b200_fec_cadu_bytes", "b200_fec_chunk_size", "b200_fec_debug_ldpc_frames", "b200_fec_ldpc_timing",
     "b200_fec_debug_turbo_frames", "b200_fec_debug_turbo_llr", "b200_fec_turbo_timing", "b200_fec_debug_dump_frames", "b200_fec_debug_meteor_frames",
-    "b200_fec_debug_hrpt_frames",
+    "b200_fec_debug_hrpt_frames", "b200_fec_frame_bits",
     "b200_chain_create", "b200_chain_destroy", "b200_chain_push_iq", "b200_chain_push_iq_device", "b200_chain_prefetch_iq", "b200_chain_pull_frames",
     "b200_chain_frames_device", "b200_chain_get_stats", "b200_chain_last_timing", "b200_chain_reset",
     "b200_chain_set_pipelined", "b200_chain_sync", "b200_chain_span_begin", "b200_chain_span_end",
@@ -55,7 +55,8 @@ class FecCfg(C.Structure):
                 ("device", C.c_int), ("max_soft", C.c_long), ("qpsk_swap_iq", C.c_int), ("qpsk_swap_diff", C.c_int), ("oqpsk_delay", C.c_int), ("conv_rate", C.c_int),
                 ("ldpc_rate", C.c_int), ("ldpc_block_size", C.c_int), ("ldpc_iterations", C.c_int), ("ldpc2", C.c_int), ("internal_stream", C.c_int),
                 ("internal_cadu_size", C.c_int), ("turbo_rate", C.c_int), ("turbo_base", C.c_int), ("turbo_iters", C.c_int),
-                ("diff_decode", C.c_int), ("m2x_mode", C.c_int), ("interleaved", C.c_int), ("deframer_thresold", C.c_int)]
+                ("diff_decode", C.c_int), ("m2x_mode", C.c_int), ("interleaved", C.c_int), ("deframer_thresold", C.c_int),
+                ("backward", C.c_int)]
 
 
 class DemuxCfg(C.Structure):
@@ -167,6 +168,7 @@ def lib():
         L.b200_fec_debug_dump_frames.argtypes = [vp, C.POINTER(DumpFrame), cl, C.POINTER(cl)]
         L.b200_fec_debug_meteor_frames.argtypes = [vp, C.POINTER(MeteorFrame), cl, C.POINTER(cl)]
         L.b200_fec_debug_hrpt_frames.argtypes = [vp, C.POINTER(HrptFrame), cl, C.POINTER(cl)]
+        L.b200_fec_frame_bits.argtypes = [vp, vp, cl, C.POINTER(cl)]
         L.b200_chain_create.restype = vp
         L.b200_chain_create.argtypes = [C.POINTER(DemodCfg), C.POINTER(FecCfg)]
         L.b200_chain_destroy.argtypes = [vp]
@@ -413,6 +415,40 @@ def aqua_db_cfg(device=0, max_soft=1 << 24):
     return cfg
 
 
+def noaa_gac_cfg(backward=None, device=0, max_soft=1 << 24):
+    """noaa_gac_decoder (module_noaa_gac_decoder.cpp:17): backward is required, as the module reads it without a default. 4159-byte
+    frames; with backward each frame's bits come out reversed (the reversal of the frame order is the file writer's)."""
+    if backward is None:
+        raise ValueError("noaa_gac_decoder: backward is required")
+    cfg = FecCfg()
+    cfg.kind, cfg.constellation, cfg.cadu_size, cfg.device, cfg.max_soft = 10, CONST["bpsk"], 33270, device, max_soft
+    cfg.backward = int(bool(backward))
+    return cfg
+
+
+def dmsp_rtd_cfg(device=0, max_soft=1 << 24):
+    """dmsp_rtd_decoder (module_dmsp_rtd_decoder.cpp): no decoder parameters (start_timestamp is the file writer's); 19-byte frames."""
+    cfg = FecCfg()
+    cfg.kind, cfg.constellation, cfg.cadu_size, cfg.device, cfg.max_soft = 11, CONST["bpsk"], 150, device, max_soft
+    return cfg
+
+
+def dmsp_timestamps(bits, start_timestamp, read_bits_seen=None):
+    """dmsp_rtd_decoder's "_timestamps.txt" values for frames completed at stream bits `bits` (b200_fec_frame_bits): start +
+    8192 * (reads of 8192 soft bytes from the stream's start that produced frames, up to the frame's) / 1.024e6. read_bits_seen carries
+    the count and the last read across calls: a dict, updated."""
+    st = read_bits_seen if read_bits_seen is not None else {}
+    n, last = st.get("n", 0), st.get("last", -1)
+    out = []
+    for b in np.asarray(bits, np.int64).tolist():
+        r = b // 8192
+        if r != last:
+            n, last = n + 1, r
+        out.append(start_timestamp + float(n * 8192) / 1.024e6)
+    st["n"], st["last"] = n, last
+    return out
+
+
 def fec_cfg_for(sig, max_soft, device=0):
     """The decoder configuration that goes with a satdump_b200.synth.SignalCfg (metop_ahrpt_decoder / ccsds_conv_concat_decoder /
     ccsds_simple_psk_decoder parameters of the shipped pipeline JSONs)."""
@@ -428,6 +464,10 @@ def fec_cfg_for(sig, max_soft, device=0):
         return meteor_hrpt_cfg(device=device, max_soft=max_soft)
     if sig.decoder == "aqua_db":
         return aqua_db_cfg(device=device, max_soft=max_soft)
+    if sig.decoder == "noaa_gac":
+        return noaa_gac_cfg(sig.backward, device=device, max_soft=max_soft)
+    if sig.decoder == "dmsp_rtd":
+        return dmsp_rtd_cfg(device=device, max_soft=max_soft)
     if sig.decoder == "turbo":
         return turbo_cfg(sig.turbo_rate, sig.turbo_base, sig.turbo_iters, device=device, max_soft=max_soft)
     if sig.decoder == "ldpc":
@@ -695,6 +735,14 @@ class Fec:
         _chk(lib().b200_fec_debug_hrpt_frames(self.h, recs, cap, C.byref(n)))
         return np.array([[recs[k].bit, recs[k].inverted, recs[k].state] for k in range(n.value)], np.int64).reshape(-1, 3)
 
+    def frame_bits(self):
+        """noaa_gac_decoder / dmsp_rtd_decoder: the stream bit that completed each frame of the last frames() pull, as int64"""
+        cap = int(getattr(self, "_n", 0)) // 100 + 1024
+        out = np.zeros(cap, np.int64)
+        n = C.c_long(0)
+        _chk(lib().b200_fec_frame_bits(self.h, out.ctypes.data, cap, C.byref(n)))
+        return out[:n.value].copy()
+
     def turbo_llr(self, frame, K):
         """ccsds_turbo_decoder: the a-priori arrays (input 0, input 1) of a frame of the last push after its last iteration."""
         a0, a1 = np.zeros(K), np.zeros(K)
@@ -724,6 +772,8 @@ class Chain:
         if not self.h:
             raise B200Error(-1 if "device" not in last_error().lower() else -2, last_error())
         self.cadu_bytes = (fcfg.cadu_size + 7) // 8 if fcfg.kind in (1, 3, 7) else (fcfg.turbo_base + 4 if fcfg.kind == 4 else 1024)
+        if fcfg.kind in (10, 11):  # noaa_gac_decoder, dmsp_rtd_decoder: (cadu_size + padding) / 8
+            self.cadu_bytes = 4159 if fcfg.kind == 10 else 19
 
     def close(self):
         if getattr(self, "h", None):

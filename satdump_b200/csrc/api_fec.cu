@@ -94,7 +94,7 @@ Fec::Fec(const b200_fec_cfg &in) : cfg(meteor_m2x_as_ccsds(in))
     const b200_fec_cfg c = cfg;
     B200_REQUIRE(c.kind == B200_FEC_METOP || c.kind == B200_FEC_CCSDS || c.kind == B200_FEC_SIMPLE || c.kind == B200_FEC_LDPC || c.kind == B200_FEC_TURBO ||
                      c.kind == B200_FEC_METOP_DUMP || c.kind == B200_FEC_METEOR_LRPT || c.kind == B200_FEC_NOAA_HRPT || c.kind == B200_FEC_METEOR_HRPT ||
-                     c.kind == B200_FEC_AQUA_DB,
+                     c.kind == B200_FEC_AQUA_DB || c.kind == B200_FEC_NOAA_GAC || c.kind == B200_FEC_DMSP_RTD,
                  B200_EINVAL, "unknown decoder kind %d", c.kind);
     B200_REQUIRE(c.max_soft >= 65536, B200_EINVAL, "max_soft must be >= 65536");
     memset(&geom, 0, sizeof(geom));
@@ -110,6 +110,10 @@ Fec::Fec(const b200_fec_cfg &in) : cfg(meteor_m2x_as_ccsds(in))
         framed = hrpt_decoder(*this);
     else if (c.kind == B200_FEC_AQUA_DB)
         framed = aqua_decoder(*this);
+    else if (c.kind == B200_FEC_NOAA_GAC)
+        framed = gac_decoder(*this);
+    else if (c.kind == B200_FEC_DMSP_RTD)
+        framed = dmsp_decoder(*this);
     if (framed)
         return;
     if (c.kind != B200_FEC_METOP) {
@@ -1117,6 +1121,9 @@ long Fec::pull(uint8_t *host_out, long cap)
         B200_CUDA(cudaMemcpyAsync(host_out, frames_out.p, nb, cudaMemcpyDeviceToHost, stream));
         B200_CUDA(cudaStreamSynchronize(stream));
     }
+    const long kb = std::min<long>((long)done_bits.size(), out_frames);
+    pulled_bits.assign(done_bits.end() - kb, done_bits.end());
+    done_bits.clear();
     out_frames = 0;
     return nb;
 }
@@ -1268,6 +1275,13 @@ int b200_fec_debug_hrpt_frames(b200_fec *h, b200_hrpt_frame *out, long cap, long
     return guarded([&] {
         B200_REQUIRE(h && out && n_out, B200_EINVAL, "NULL argument");
         *n_out = h->f->hrpt_frames(out, cap);
+    });
+}
+int b200_fec_frame_bits(b200_fec *h, long *out, long cap, long *n_out)
+{
+    return guarded([&] {
+        B200_REQUIRE(h && out && n_out, B200_EINVAL, "NULL argument");
+        *n_out = h->f->frame_bits(out, cap);
     });
 }
 int b200_fec_turbo_timing(b200_fec *h, float *ms_out, int n)

@@ -51,7 +51,9 @@ std::unique_ptr<Framed> turbo_decoder(Fec &f);
 std::unique_ptr<Framed> dump_decoder(Fec &f);
 std::unique_ptr<Framed> meteor_decoder(Fec &f);
 std::unique_ptr<Framed> hrpt_decoder(Fec &f); // noaa_hrpt_decoder, meteor_hrpt_decoder (api_hrpt.cu)
-std::unique_ptr<Framed> aqua_decoder(Fec &f); // aqua_db_decoder (api_aqua.cu): the deframer and frame stage behind its own bit stage
+std::unique_ptr<Framed> aqua_decoder(Fec &f);
+std::unique_ptr<Framed> gac_decoder(Fec &f);  // noaa_gac_decoder (api_hrpt.cu): the deframer and frame stage behind its own bit stage
+std::unique_ptr<Framed> dmsp_decoder(Fec &f); // dmsp_rtd_decoder (api_hrpt.cu) // aqua_db_decoder (api_aqua.cu): the deframer and frame stage behind its own bit stage
 
 class Fec
 {
@@ -94,6 +96,10 @@ class Fec
     long dump_frames(b200_dump_frame *out, long cap); // records of the last push
     long meteor_frames(b200_meteor_frame *out, long cap); // records of the last push
     long hrpt_frames(b200_hrpt_frame *out, long cap); // records of the last push
+    // noaa_gac_decoder / dmsp_rtd_decoder: the stream bit that completed each frame waiting in frames_out, and each frame of the last pull
+    std::vector<long> done_bits, pulled_bits;
+    void note_frame_bits(long out0, const std::vector<long> &bits); // the bits of the frames a push wrote from frames_out index out0
+    long frame_bits(long *out, long cap);
 
     // device storage
     DevBuf<int8_t> softbuf;
@@ -175,6 +181,8 @@ class Fec
     friend struct Meteor;
     friend struct Hrpt;
     friend struct Aqua;
+    friend struct Gac;
+    friend struct Dmsp;
     // the main deframer and the frame counters at a point a pass may have to roll back to
     struct Mark { DefrState h_dstate; long fifo_bits, out_frames, total_frames, rs_corrected, rs_failed; int defr_state_now; };
     Mark mark();

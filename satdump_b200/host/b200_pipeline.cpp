@@ -11,6 +11,11 @@ using namespace b200host;
 // module_aqua_db_decoder.cpp:83-93); frames: output units
 static void print_hrpt_stats(const std::string &dec, long frames, int state)
 {
+    // module_noaa_gac_decoder.cpp:144-150 (the HRPT module's divisor, as the module has it), module_dmsp_rtd_decoder.cpp:76-82
+    if (dec == "noaa_gac_decoder")
+        printf("frame_count %ld\n", frames / 11090);
+    if (dec == "dmsp_rtd_decoder")
+        printf("deframer_state %s\n", state == 0 ? "NOSYNC" : (state == 2 ? "SYNCING" : "SYNCED"));
     if (dec == "aqua_db_decoder")
         printf("deframer_state %s\n", state == 2 ? "NOSYNC" : (state == 6 ? "SYNCING" : "SYNCED"));
     if (dec == "noaa_hrpt_decoder")
@@ -23,7 +28,7 @@ static void print_hrpt_stats(const std::string &dec, long frames, int state)
 int main(int argc, char **argv)
 {
     if (argc < 5) {
-        fprintf(stderr, "usage: %s <metop_ahrpt|jpss_hrd|npp_hrd|simple_bpsk|simple_qpsk|pm_bpsk|ldpc_qpsk|landsat|turbo_pm|turbo_bpsk|metop_dump|meteor_lrpt|noaa_hrpt|meteor_hrpt|aqua_db|aura_db|terra_db|bluewalker3_wide|bluewalker3_narrow> baseband <input> <output_hint> [--fused] [--key value ...]\n", argv[0]);
+        fprintf(stderr, "usage: %s <metop_ahrpt|jpss_hrd|npp_hrd|simple_bpsk|simple_qpsk|pm_bpsk|ldpc_qpsk|landsat|turbo_pm|turbo_bpsk|metop_dump|meteor_lrpt|noaa_hrpt|meteor_hrpt|noaa_gac|dmsp_rtd|aqua_db|aura_db|terra_db|bluewalker3_wide|bluewalker3_narrow> baseband <input> <output_hint> [--fused] [--key value ...]\n", argv[0]);
         return 2;
     }
     const std::string pipe = argv[1], level = argv[2], in = argv[3], out = argv[4];
@@ -40,6 +45,15 @@ int main(int argc, char **argv)
         dp = Params{{"constellation", "qpsk"}, {"symbolrate", "72000"}, {"rrc_alpha", "0.5"}, {"pll_bw", "0.002"}};
         fp = Params{{"diff_decode", "false"}};
         dec = "meteor_lrpt_decoder";
+    } else if (pipe == "noaa_gac" || pipe == "dmsp_rtd") { // resources/pipelines/NOAA.json "noaa_gac", DMSP.json "dmsp_rtd": psk_demod BPSK
+        if (pipe == "noaa_gac") {
+            dp = Params{{"constellation", "bpsk"}, {"symbolrate", "2661600"}, {"rrc_alpha", "0.5"}, {"pll_bw", "0.004"}, {"post_costas_dc", "true"}};
+            fp = Params{{"backward", "false"}};
+            dec = "noaa_gac_decoder";
+        } else {
+            dp = Params{{"constellation", "bpsk"}, {"symbolrate", "1024000"}, {"rrc_alpha", "0.5"}, {"pll_bw", "0.005"}};
+            dec = "dmsp_rtd_decoder";
+        }
     } else if (pipe == "noaa_hrpt" || pipe == "meteor_hrpt") { // resources/pipelines/NOAA.json "noaa_hrpt", Meteor-M.json "meteor_hrpt":
         // pm_demod at 665 400 sym/s (pll_bw 0.01, rrc_alpha 0.6 | 0.5, clock_omega_relative_limit 0.001), 3 MS/s by default
         const bool noaa = pipe == "noaa_hrpt";

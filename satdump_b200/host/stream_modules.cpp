@@ -394,6 +394,23 @@ b200_fec_cfg fec_cfg_from_params(const std::string &id, const Params &p)
             throw ModuleError("noaa_hrpt_decoder: deframer_thresold must be 0..60 (got " + std::to_string(c.deframer_thresold) + ")");
         return c;
     }
+    if (id == "noaa_gac_decoder") { // module_noaa_gac_decoder.cpp:17: backward read with no default; 4159-byte frames
+        c.kind = B200_FEC_NOAA_GAC;
+        c.device = (int)p.num("b200_device", 0);
+        c.constellation = B200_BPSK;
+        c.cadu_size = 33270;
+        if (!p.has("backward"))
+            throw ModuleError("noaa_gac_decoder: backward is required");
+        c.backward = p.flag("backward", false);
+        return c;
+    }
+    if (id == "dmsp_rtd_decoder") { // module_dmsp_rtd_decoder.cpp:16-24: DMSP_Deframer(150, 2), 19-byte frames
+        c.kind = B200_FEC_DMSP_RTD;
+        c.device = (int)p.num("b200_device", 0);
+        c.constellation = B200_BPSK;
+        c.cadu_size = 150;
+        return c;
+    }
     if (id == "aqua_db_decoder") { // module_aqua_db_decoder.cpp:16-22: no parameters; 1024-byte CADUs (Aqua and Aura DB)
         c.kind = B200_FEC_AQUA_DB;
         c.device = (int)p.num("b200_device", 0);
@@ -697,6 +714,38 @@ void PskDemodStage::process()
 }
 
 // ------------------------------------------------------------------------------------------------ FecStage
+// noaa_gac_decoder with backward writes hint + ".frm.tmp" and at the end rewrites ".frm" in reverse frame order, then removes the
+// ".tmp" file (module_noaa_gac_decoder.cpp:41-46,113-133); every other decoder writes its output file directly
+static std::string frame_file(const b200_fec_cfg &c, const std::string &hint, bool ccsds)
+{
+    if (c.kind == B200_FEC_NOAA_GAC)
+        return hint + (c.backward ? ".frm.tmp" : ".frm");
+    if (c.kind == B200_FEC_DMSP_RTD)
+        return hint + ".frm";
+    return hint + (c.kind == B200_FEC_NOAA_HRPT ? ".raw16" : (ccsds ? ".cadu" : ".frm"));
+}
+static void finish_backward(const b200_fec_cfg &c, const std::string &hint)
+{
+    if (c.kind != B200_FEC_NOAA_GAC || !c.backward)
+        return;
+    const std::string tmp = hint + ".frm.tmp";
+    FILE *in = fopen(tmp.c_str(), "rb");
+    FILE *out = fopen((hint + ".frm").c_str(), "wb");
+    if (!in || !out)
+        throw std::runtime_error("cannot reverse " + tmp);
+    std::vector<uint8_t> fr(4159);
+    fseek(in, 0, SEEK_END);
+    for (long pos = ftell(in) - 4159; pos >= 0; pos -= 4159) {
+        fseek(in, pos, SEEK_SET);
+        if (fread(fr.data(), 1, fr.size(), in) != fr.size())
+            throw std::runtime_error("cannot read " + tmp);
+        fwrite(fr.data(), 1, fr.size(), out);
+    }
+    fclose(in);
+    fclose(out);
+    remove(tmp.c_str());
+}
+
 FecStage::FecStage(const std::string &module_id, std::string in, std::string hint, Params p)
     : StageBase(std::move(in), std::move(hint), std::move(p)), id(module_id)
 {
@@ -725,10 +774,16 @@ void FecStage::process()
     }
     if (out_type == DataType::FILE) {
         const bool ccsds = params.flag("ccsds", true);
-        output_file = output_hint + (cfg.kind == B200_FEC_NOAA_HRPT ? ".raw16" : (ccsds ? ".cadu" : ".frm")); // filestream_to_filestream.cpp:27-36,
-        // ccsds decoder :131, module_noaa_hrpt_decoder.cpp:20
+        output_file = frame_file(cfg, output_hint, ccsds); // filestream_to_filestream.cpp:27-36, ccsds decoder :131, module_noaa_hrpt_decoder.cpp:20
         fout = fopen(output_file.c_str(), "wb");
+        if (cfg.kind == B200_FEC_NOAA_GAC)
+            output_file = output_hint + ".frm";
     }
+    // dmsp_rtd_decoder's start_timestamp (module_dmsp_rtd_decoder.cpp:36-42,60-66): getValueOrDefault(..., -1)
+    const double start_ts = cfg.kind == B200_FEC_DMSP_RTD ? params.num("start_timestamp", -1) : -1;
+    FILE *fts = start_ts != -1 ? fopen((output_hint + "_timestamps.txt").c_str(), "wb") : nullptr;
+    long ts_reads = 0, ts_last = -1;
+    std::vector<long> fbits;
     const int chunk = b200_fec_chunk_size(h);
     while (!should_stop) {
         size_t got;
@@ -752,6 +807,20 @@ void FecStage::process()
             else if (output_fifo->write(out.data(), (int)nb) < 0)
                 break;
         }
+        if (fts && nb > 0) { // one line per frame: start + 8192 * (the 8192-byte reads that produced frames, up to its own) / 1.024e6
+            fbits.resize((size_t)nb / 19 + 1);
+            long n = 0;
+            check(b200_fec_frame_bits(h, fbits.data(), (long)fbits.size(), &n), "b200_fec_frame_bits");
+            for (long k = 0; k < n; k++) {
+                const long r = fbits[k] / 8192;
+                if (r != ts_last) {
+                    ts_reads++;
+                    ts_last = r;
+                }
+                const std::string line = std::to_string(start_ts + double(ts_reads * 8192) / 1.024e6) + "\n";
+                fwrite(line.data(), 1, line.size(), fts);
+            }
+        }
         if (cfg.kind == B200_FEC_TURBO) { // "CRC Check": the CRC of the last frame decoded
             std::vector<b200_turbo_frame> recs(got / 1024 + 4);
             long nrec = 0;
@@ -772,8 +841,12 @@ void FecStage::process()
     }
     if (fin)
         fclose(fin);
-    if (fout)
+    if (fts)
+        fclose(fts);
+    if (fout) {
         fclose(fout);
+        finish_backward(cfg, output_hint);
+    }
 }
 
 // ------------------------------------------------------------------------------------------------ FusedStage
@@ -783,6 +856,8 @@ FusedStage::FusedStage(const std::string &decoder_id, std::string in, std::strin
     bool bpsk;
     dcfg = demod_cfg_from_params(dparams, bpsk, dparams.str("b200_demod_module", "psk_demod")); // "pm_demod": PMDemodModule's chain in front
     fcfg = fec_cfg_from_params(dec_id, params);
+    if (fcfg.kind == B200_FEC_DMSP_RTD && params.has("start_timestamp")) // (the pipelined chain does not keep the frames' completion bits)
+        throw ModuleError("dmsp_rtd_decoder: start_timestamp is not built in the fused chain; run the decoder as its own stage");
     batch_samples = (long)dparams.num("b200_batch_samples", (double)batch_samples);
     dcfg.max_batch = batch_samples;
     fcfg.max_soft = batch_samples + (1 << 20);
@@ -809,8 +884,11 @@ void FusedStage::process()
     const uint64_t fsz = file_size(input_file);
     if (data_offset)
         fseek(fin, (long)data_offset, SEEK_SET);
-    output_file = output_hint + (fcfg.kind == B200_FEC_NOAA_HRPT ? ".raw16" : ".cadu");
+    output_file = (fcfg.kind == B200_FEC_NOAA_GAC || fcfg.kind == B200_FEC_DMSP_RTD) ? frame_file(fcfg, output_hint, true)
+                                                                                   : output_hint + (fcfg.kind == B200_FEC_NOAA_HRPT ? ".raw16" : ".cadu");
     FILE *fout = fopen(output_file.c_str(), "wb");
+    if (fcfg.kind == B200_FEC_NOAA_GAC)
+        output_file = output_hint + ".frm";
     uint64_t done = 0;
     size_t have = 0;
     const long min_batch = dcfg.final_samplerate > 0 ? 256 : 64;
@@ -862,6 +940,7 @@ void FusedStage::process()
     }
     fclose(fin);
     fclose(fout);
+    finish_backward(fcfg, output_hint);
 }
 
 // ------------------------------------------------------------------------------------------------ two-module wiring

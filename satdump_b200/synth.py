@@ -216,6 +216,8 @@ class SignalCfg:
     post_costas_dc: bool = False
     # noaa_hrpt_decoder's "deframer_thresold" (NOAA.json: 10)
     deframer_thresold: int = 10
+    # noaa_gac_decoder's "backward" (NOAA.json "noaa_gac": false)
+    backward: bool = False
 
     @property
     def cadu_bytes(self):
@@ -331,6 +333,12 @@ CONFIGS = {
     # terra_db_demod -> ccsds_conv_concat_decoder, EOS Terra DB (EOS.json "terra_db"): 13.125 Msym/s recorded at 45 MS/s. The demodulator
     # runs BPSK loops at twice the symbol rate (1.714 samples per half-symbol), so the signal is BPSK at 26.25 Mbaud carrying the r=1/2 code
     # (terra_db_frames). The receiver's parameters are the module's (capi.terra_db_demod_kwargs); clock_alpha only stands in for them here.
+    # psk_demod BPSK -> noaa_gac_decoder / dmsp_rtd_decoder (NOAA.json "noaa_gac", DMSP.json "dmsp_rtd"): bit streams without FEC at
+    # 2.6616 Msym/s (6 MS/s, post_costas_dc) and 1.024 Msym/s (2 MS/s)
+    "noaa_gac": SignalCfg(name="noaa_gac", samplerate=6e6, symbolrate=2661600, constellation="bpsk", conv="none", rrc_alpha=0.5, pll_bw=0.004,
+                          fmt="cs16", decoder="noaa_gac", esn0_db=15.0, carrier_rad=1e-4, phase0=0.1, post_costas_dc=True),
+    "dmsp_rtd": SignalCfg(name="dmsp_rtd", samplerate=2e6, symbolrate=1024000, constellation="bpsk", conv="none", rrc_alpha=0.5, pll_bw=0.005,
+                          fmt="cs16", decoder="dmsp_rtd", esn0_db=15.0, carrier_rad=1e-4, phase0=0.1),
     "terra_db": SignalCfg(name="terra_db", samplerate=45e6, symbolrate=26250000, constellation="bpsk", conv="none", interleave=4, rrc_alpha=0.5,
                           pll_bw=0.004, fmt="cs16", decoder="terra_db", esn0_db=12.0, carrier_rad=1e-4, phase0=0.1, clock_alpha=0.001),
 }
@@ -373,6 +381,12 @@ def make_bitstream(cfg: SignalCfg, nframes, seed):
     if cfg.decoder == "noaa_hrpt":  # nframes NOAA HRPT minor frames (10-bit words, no FEC); clear: the words
         bits, words = noaa_hrpt_frames(nframes, seed)
         return bits.reshape(-1), words
+    if cfg.decoder == "noaa_gac":  # nframes GAC frames (no FEC); clear: the frames the decoder writes
+        bits, frames = gac_frames(nframes, seed, cfg.backward)
+        return bits.reshape(-1), frames
+    if cfg.decoder == "dmsp_rtd":  # nframes DMSP RTD frames (no FEC)
+        bits, frames = dmsp_frames(nframes, seed)
+        return bits.reshape(-1), frames
     if cfg.decoder == "meteor_hrpt":  # nframes METEOR HRPT CADUs (no FEC)
         bits, cadu = meteor_hrpt_frames(nframes, seed)
         return bits.reshape(-1), cadu
@@ -506,6 +520,8 @@ def frames_for_samples(cfg: SignalCfg, nsamples):
         return int(nsamples * bps / (cfg.samplerate / cfg.symbolrate) / 16384) + 2
     if cfg.decoder in ("noaa_hrpt", "meteor_hrpt"):  # bits on air: 110900 per NOAA minor frame, 8192 per METEOR CADU
         return int(nsamples / (cfg.samplerate / cfg.symbolrate) / (NOAA_WORDS * 10 if cfg.decoder == "noaa_hrpt" else 8192)) + 2
+    if cfg.decoder in ("noaa_gac", "dmsp_rtd"):  # bits on air: 33270 per GAC frame, 150 per DMSP frame
+        return int(nsamples / (cfg.samplerate / cfg.symbolrate) / (GAC_BITS if cfg.decoder == "noaa_gac" else DMSP_BITS)) + 2
     if cfg.decoder == "terra_db":  # 16384 code symbols per CADU, one per sample period of the half-symbol rate
         return int(nsamples / (cfg.samplerate / cfg.symbolrate) / 16384) + 2
     if cfg.decoder in ("ldpc", "dump", "aqua_db"):  # LDPC frames / MetOp dump and Aqua DB CADUs of 8192 bits
@@ -857,6 +873,63 @@ def hrpt_soft(bits, inverted=False, amp=60.0, sigma=0.0, seed=0, slips=(), gaps=
         a = at
     pieces.append(s[a:][keep[a:]])
     return np.clip(np.round(np.concatenate(pieces)), -127, 127).astype(np.int8)
+
+
+# ---- NOAA GAC and DMSP RTD (noaa_gac_decoder, dmsp_rtd_decoder): bit streams without FEC ------------------------------------------------
+GAC_BITS, GAC_BYTES = 33270, 4159
+GAC_SYNC, GAC_SYNC_BACKWARD = 0xA116FD71, 0x33C3E4A6
+DMSP_BITS, DMSP_BYTES, DMSP_ASM = 150, 19, 0b1010110011111
+
+
+def gac_pn_bits():
+    """The GAC PN sequence (1023 bits): b[i] = b[i-1] ^ b[i-5] ^ b[i-6] ^ b[i-8] ^ b[i-11] from 0 0 0 0 0 1 1 1 0 1 0"""
+    b = [0, 0, 0, 0, 0, 1, 1, 1, 0, 1, 0]
+    for i in range(11, 1023):
+        b.append(b[i - 1] ^ b[i - 5] ^ b[i - 6] ^ b[i - 8] ^ b[i - 11])
+    return np.array(b, np.uint8)
+
+
+def gac_pn_bytes():
+    """The 4159 bytes noaa_gac_decoder XORs onto each frame: 60 zero bits, then the PN bits repeated, MSB first"""
+    bits = np.concatenate([np.zeros(60, np.uint8), np.resize(gac_pn_bits(), GAC_BYTES * 8 - 60)])
+    return np.packbits(bits)
+
+
+def frame_image(bits, nbytes):
+    """The byte image write_bit leaves of frames of len(bits) bits: MSB first, the partial last byte right-aligned. bits [n, nbits]"""
+    bits = np.asarray(bits, np.uint8)
+    full = bits.shape[1] // 8 * 8
+    img = np.zeros((bits.shape[0], nbytes), np.uint8)
+    img[:, :full // 8] = np.packbits(bits[:, :full], axis=1)
+    if full < bits.shape[1]:
+        img[:, full // 8] = (bits[:, full:] << np.arange(bits.shape[1] - full - 1, -1, -1, dtype=np.uint8)).sum(axis=1)
+    return img
+
+
+def gac_post(img, backward):
+    """noaa_gac_decoder after the deframer (module_noaa_gac_decoder.cpp:84-98): with backward, output bit ii = bit 33269 - ii of the byte
+    image read MSB first (written back with write_bit's right-aligned last byte); then the PN bytes. img uint8 [n, 4159]"""
+    img = np.asarray(img, np.uint8)
+    if backward:
+        rd = np.unpackbits(img, axis=1)[:, GAC_BITS - 1::-1]
+        img = frame_image(rd, GAC_BYTES)
+    return img ^ gac_pn_bytes()
+
+
+def gac_frames(nframes, seed=0, backward=False):
+    """(bits uint8 [n, 33270] as sent; frames uint8 [n, 4159] as noaa_gac_decoder writes them): the sync word (0x33C3E4A6 when backward)
+    and 33238 random bits per frame"""
+    bits = np.random.default_rng(seed).integers(0, 2, size=(nframes, GAC_BITS)).astype(np.uint8)
+    sync = GAC_SYNC_BACKWARD if backward else GAC_SYNC
+    bits[:, :32] = (sync >> np.arange(31, -1, -1)) & 1
+    return bits, gac_post(frame_image(bits, GAC_BYTES), backward)
+
+
+def dmsp_frames(nframes, seed=0):
+    """(bits uint8 [n, 150] as sent; frames uint8 [n, 19] as dmsp_rtd_decoder writes them): the 13-bit sync and 137 random bits"""
+    bits = np.random.default_rng(seed).integers(0, 2, size=(nframes, DMSP_BITS)).astype(np.uint8)
+    bits[:, :13] = (DMSP_ASM >> np.arange(12, -1, -1)) & 1
+    return bits, frame_image(bits, DMSP_BYTES)
 
 
 # ---- EOS Aqua / Aura DB (aqua_db_decoder): randomised CADUs on two NRZ-M rails -----------------------------------------------------------

@@ -6,13 +6,14 @@
 namespace b200
 {
 
-struct Dump : Framed
+struct Dump : Correlated
 {
     DumpSync sw{};
     DevBuf<uint32_t> hw;
 
     explicit Dump(Fec &f);
     void process(Fec &f) override;
+    long records(const Fec &f, b200_dump_frame *out, long cap) const; // of the last push
 };
 
 namespace
@@ -84,10 +85,7 @@ void Dump::process(Fec &f)
         B200_CUDA(cudaMemcpyAsync(f.h_rs_err.p, f.rs_err.p, sizeof(int) * nf * DUMP_RS_I, cudaMemcpyDeviceToHost, stream));
     }
     f.keep_soft_tail(h_walk.p->next);
-    B200_CUDA(cudaEventRecord(f.ev[1], stream));
-    B200_CUDA(cudaStreamSynchronize(stream));
-    B200_CUDA(cudaGetLastError());
-    cudaEventElapsedTime(&f.t_vit, f.ev[0], f.ev[1]);
+    end(f);
     finish(nf, f.soft_have);
     for (int i = 0; i < nf * DUMP_RS_I; i++) {
         const int e = f.h_rs_err.p[i];
@@ -102,12 +100,11 @@ void Dump::process(Fec &f)
     f.total_bits += (long)nf * DUMP_CADU * 8;
 }
 
-long Fec::dump_frames(b200_dump_frame *out, long cap)
+long Dump::records(const Fec &f, b200_dump_frame *out, long cap) const
 {
-    const Dump &D = framed_as<Dump>("not a MetOp dump decoder");
-    B200_REQUIRE(D.last_nf <= cap, B200_ESTATE, "output buffer too small: need %ld records", D.last_nf);
-    for (long k = 0; k < D.last_nf; k++) {
-        const WalkFrame &r = D.h_frames.p[k];
+    B200_REQUIRE(last_nf <= cap, B200_ESTATE, "output buffer too small: need %ld records", last_nf);
+    for (long k = 0; k < last_nf; k++) {
+        const WalkFrame &r = h_frames.p[k];
         b200_dump_frame &d = out[k];
         d.offset = (long)r.off;
         d.pos = r.pos;
@@ -115,9 +112,20 @@ long Fec::dump_frames(b200_dump_frame *out, long cap)
         d.phase = r.phase;
         d.swap = r.swap;
         for (int i = 0; i < DUMP_RS_I; i++)
-            d.rs[i] = h_rs_err.p[k * DUMP_RS_I + i];
+            d.rs[i] = f.h_rs_err.p[k * DUMP_RS_I + i];
     }
-    return D.last_nf;
+    return last_nf;
 }
 
 } // namespace b200
+
+using namespace b200;
+
+extern "C" int b200_fec_debug_dump_frames(b200_fec *h, b200_dump_frame *out, long cap, long *n_out)
+{
+    return guarded([&] {
+        B200_REQUIRE(h && out && n_out, B200_EINVAL, "NULL argument");
+        Fec &f = *h->f;
+        *n_out = f.framed_as<Dump>("not a MetOp dump decoder").records(f, out, cap);
+    });
+}

@@ -92,30 +92,23 @@ static b200_fec_cfg meteor_m2x_as_ccsds(const b200_fec_cfg &c)
 Fec::Fec(const b200_fec_cfg &in) : cfg(meteor_m2x_as_ccsds(in))
 {
     const b200_fec_cfg c = cfg;
-    B200_REQUIRE(c.kind == B200_FEC_METOP || c.kind == B200_FEC_CCSDS || c.kind == B200_FEC_SIMPLE || c.kind == B200_FEC_LDPC || c.kind == B200_FEC_TURBO ||
-                     c.kind == B200_FEC_METOP_DUMP || c.kind == B200_FEC_METEOR_LRPT || c.kind == B200_FEC_NOAA_HRPT || c.kind == B200_FEC_METEOR_HRPT ||
-                     c.kind == B200_FEC_AQUA_DB || c.kind == B200_FEC_NOAA_GAC || c.kind == B200_FEC_DMSP_RTD,
-                 B200_EINVAL, "unknown decoder kind %d", c.kind);
+    std::unique_ptr<Framed> (*decoder)(Fec &) = nullptr; // (none: the Viterbi / simple-PSK path below)
+    switch (c.kind) {
+    case B200_FEC_METOP: case B200_FEC_CCSDS: case B200_FEC_SIMPLE: break;
+    case B200_FEC_LDPC: decoder = ldpc_decoder; break;
+    case B200_FEC_TURBO: decoder = turbo_decoder; break;
+    case B200_FEC_METOP_DUMP: decoder = dump_decoder; break;
+    case B200_FEC_METEOR_LRPT: decoder = meteor_decoder; break;
+    case B200_FEC_NOAA_HRPT: case B200_FEC_METEOR_HRPT: case B200_FEC_DMSP_RTD: decoder = sync_walk_decoder; break;
+    case B200_FEC_AQUA_DB: case B200_FEC_NOAA_GAC: decoder = bit_stage_decoder; break;
+    default: B200_REQUIRE(false, B200_EINVAL, "unknown decoder kind %d", c.kind);
+    }
     B200_REQUIRE(c.max_soft >= 65536, B200_EINVAL, "max_soft must be >= 65536");
     memset(&geom, 0, sizeof(geom));
-    if (c.kind == B200_FEC_LDPC)
-        framed = ldpc_decoder(*this);
-    else if (c.kind == B200_FEC_TURBO)
-        framed = turbo_decoder(*this);
-    else if (c.kind == B200_FEC_METOP_DUMP)
-        framed = dump_decoder(*this);
-    else if (c.kind == B200_FEC_METEOR_LRPT)
-        framed = meteor_decoder(*this);
-    else if (c.kind == B200_FEC_NOAA_HRPT || c.kind == B200_FEC_METEOR_HRPT)
-        framed = hrpt_decoder(*this);
-    else if (c.kind == B200_FEC_AQUA_DB)
-        framed = aqua_decoder(*this);
-    else if (c.kind == B200_FEC_NOAA_GAC)
-        framed = gac_decoder(*this);
-    else if (c.kind == B200_FEC_DMSP_RTD)
-        framed = dmsp_decoder(*this);
-    if (framed)
+    if (decoder) {
+        framed = decoder(*this);
         return;
+    }
     if (c.kind != B200_FEC_METOP) {
         B200_REQUIRE(c.cadu_size >= 64 && c.cadu_size <= 65536, B200_EINVAL, "cadu_size out of range");
         B200_REQUIRE(c.cadu_size % 8 == 0, B200_EINVAL, "cadu_size must be a multiple of 8 (frame padding is not built)");
@@ -719,35 +712,15 @@ void Fec::framed_storage(int F, long frames_per_push)
     }
 }
 
-void Framed::alloc(long positions, long frames_cap)
-{
-    score.alloc((size_t)positions);
-    bsync.alloc((size_t)positions);
-    bval.alloc((size_t)positions / 32 + 2);
-    bidx.alloc((size_t)positions / 32 + 2);
-    max_frames = frames_cap;
-    frames.alloc((size_t)max_frames);
-    walk.alloc(1);
-    h_walk.alloc(1);
-    h_frames.alloc((size_t)max_frames);
-}
-
 void Framed::reset(Fec &f)
 {
     f.soft_have = 0;
     f.out_frames = 0;
+    f.done_bits.clear();
+    f.pulled_bits.clear();
     tail_seen = -1;
     base_off = 0;
     last_nf = 0;
-    lock = 0;
-    cor = 0.f;
-}
-
-void Framed::stats(b200_fec_stats *o)
-{
-    o->correlator_lock = lock;
-    o->correlator_corr = cor;
-    o->ldpc_resyncs = resyncs;
 }
 
 // A push's records, timings and debug bits start empty, unless it brought no new bytes (then it changes nothing).
@@ -767,7 +740,42 @@ bool Framed::begin(Fec &f, int F)
     return true;
 }
 
-int Framed::walked(cudaStream_t stream)
+void Framed::end(Fec &f)
+{
+    B200_CUDA(cudaEventRecord(f.ev[1], f.stream));
+    B200_CUDA(cudaStreamSynchronize(f.stream));
+    B200_CUDA(cudaGetLastError());
+    cudaEventElapsedTime(&f.t_vit, f.ev[0], f.ev[1]);
+}
+
+void Correlated::alloc(long positions, long frames_cap)
+{
+    score.alloc((size_t)positions);
+    bsync.alloc((size_t)positions);
+    bval.alloc((size_t)positions / 32 + 2);
+    bidx.alloc((size_t)positions / 32 + 2);
+    max_frames = frames_cap;
+    frames.alloc((size_t)max_frames);
+    walk.alloc(1);
+    h_walk.alloc(1);
+    h_frames.alloc((size_t)max_frames);
+}
+
+void Correlated::reset(Fec &f)
+{
+    Framed::reset(f);
+    lock = 0;
+    cor = 0.f;
+}
+
+void Correlated::stats(b200_fec_stats *o)
+{
+    o->correlator_lock = lock;
+    o->correlator_corr = cor;
+    o->ldpc_resyncs = resyncs;
+}
+
+int Correlated::walked(cudaStream_t stream)
 {
     B200_CUDA(cudaMemcpyAsync(h_walk.p, walk.p, sizeof(WalkOut), cudaMemcpyDeviceToHost, stream));
     B200_CUDA(cudaStreamSynchronize(stream));
@@ -775,7 +783,7 @@ int Framed::walked(cudaStream_t stream)
 }
 
 // after keep_soft_tail: `soft_have` is what the FIFO keeps
-void Framed::finish(int nf, long soft_have)
+void Correlated::finish(int nf, long soft_have)
 {
     for (int k = 0; k < nf; k++) {
         WalkFrame &r = h_frames.p[k];
@@ -1154,10 +1162,6 @@ void Fec::stats(b200_fec_stats *o)
 } // namespace b200
 
 using namespace b200;
-struct b200_fec
-{
-    Fec *f;
-};
 
 extern "C" {
 b200_fec *b200_fec_create(const b200_fec_cfg *cfg)
@@ -1227,68 +1231,11 @@ int b200_fec_get_stats(b200_fec *h, b200_fec_stats *out)
 }
 int b200_fec_cadu_bytes(b200_fec *h) { return h ? h->f->cadu_bytes : B200_EINVAL; }
 int b200_fec_chunk_size(b200_fec *h) { return h ? h->f->geom.chunk : B200_EINVAL; }
-int b200_fec_debug_ldpc_frames(b200_fec *h, b200_ldpc_frame *out, long cap, long *n_out)
-{
-    return guarded([&] {
-        B200_REQUIRE(h && out && n_out, B200_EINVAL, "NULL argument");
-        *n_out = h->f->ldpc_frames(out, cap);
-    });
-}
-int b200_fec_ldpc_timing(b200_fec *h, float *ms_out, int n)
-{
-    return guarded([&] {
-        B200_REQUIRE(h && ms_out, B200_EINVAL, "NULL argument");
-        h->f->ldpc_timing(ms_out, n);
-    });
-}
-int b200_fec_debug_turbo_frames(b200_fec *h, b200_turbo_frame *out, long cap, long *n_out)
-{
-    return guarded([&] {
-        B200_REQUIRE(h && out && n_out, B200_EINVAL, "NULL argument");
-        *n_out = h->f->turbo_frames(out, cap);
-    });
-}
-int b200_fec_debug_turbo_llr(b200_fec *h, long frame, double *app0, double *app1, long cap, long *n_out)
-{
-    return guarded([&] {
-        B200_REQUIRE(h && app0 && app1 && n_out, B200_EINVAL, "NULL argument");
-        DeviceGuard g(h->f->cfg.device);
-        *n_out = h->f->turbo_llr(frame, app0, app1, cap);
-    });
-}
-int b200_fec_debug_dump_frames(b200_fec *h, b200_dump_frame *out, long cap, long *n_out)
-{
-    return guarded([&] {
-        B200_REQUIRE(h && out && n_out, B200_EINVAL, "NULL argument");
-        *n_out = h->f->dump_frames(out, cap);
-    });
-}
-int b200_fec_debug_meteor_frames(b200_fec *h, b200_meteor_frame *out, long cap, long *n_out)
-{
-    return guarded([&] {
-        B200_REQUIRE(h && out && n_out, B200_EINVAL, "NULL argument");
-        *n_out = h->f->meteor_frames(out, cap);
-    });
-}
-int b200_fec_debug_hrpt_frames(b200_fec *h, b200_hrpt_frame *out, long cap, long *n_out)
-{
-    return guarded([&] {
-        B200_REQUIRE(h && out && n_out, B200_EINVAL, "NULL argument");
-        *n_out = h->f->hrpt_frames(out, cap);
-    });
-}
 int b200_fec_frame_bits(b200_fec *h, long *out, long cap, long *n_out)
 {
     return guarded([&] {
         B200_REQUIRE(h && out && n_out, B200_EINVAL, "NULL argument");
         *n_out = h->f->frame_bits(out, cap);
-    });
-}
-int b200_fec_turbo_timing(b200_fec *h, float *ms_out, int n)
-{
-    return guarded([&] {
-        B200_REQUIRE(h && ms_out, B200_EINVAL, "NULL argument");
-        h->f->turbo_timing(ms_out, n);
     });
 }
 }

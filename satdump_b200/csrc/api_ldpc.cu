@@ -108,7 +108,7 @@ int syncwords(int constellation, LdpcSync &sw)
 }
 } // namespace
 
-struct Ldpc : Framed
+struct Ldpc : Correlated
 {
     int constellation = 0, nsync = 0, nlevels = 0;
     bool derandomize = true, internal = false;
@@ -125,6 +125,8 @@ struct Ldpc : Framed
     void process(Fec &f) override;
     void reset(Fec &f) override;
     void stats(b200_fec_stats *o) override;
+    long records(b200_ldpc_frame *out, long cap) const; // of the last push
+    void timing(float *ms, int n) const;
 };
 
 // Everything this build does not cover is refused by name before the device is touched.
@@ -197,7 +199,7 @@ void Ldpc::reset(Fec &f)
         f.start_stream(64); // the bit FIFO and the deframer
         B200_CUDA(cudaStreamSynchronize(f.stream));
     }
-    Framed::reset(f);
+    Correlated::reset(f);
     corr = 0;
 }
 
@@ -265,26 +267,43 @@ void Ldpc::process(Fec &f)
 
 void Ldpc::stats(b200_fec_stats *o)
 {
-    Framed::stats(o);
+    Correlated::stats(o);
     o->ldpc_corr = corr;
 }
 
-long Fec::ldpc_frames(b200_ldpc_frame *out, long cap)
+long Ldpc::records(b200_ldpc_frame *out, long cap) const
 {
-    const Ldpc &L = framed_as<Ldpc>("not an LDPC decoder");
-    B200_REQUIRE(L.last_nf <= cap, B200_ESTATE, "output buffer too small: need %ld records", L.last_nf);
-    for (long k = 0; k < L.last_nf; k++) {
-        const WalkFrame &r = L.h_frames.p[k];
+    B200_REQUIRE(last_nf <= cap, B200_ESTATE, "output buffer too small: need %ld records", last_nf);
+    for (long k = 0; k < last_nf; k++) {
+        const WalkFrame &r = h_frames.p[k];
         out[k] = b200_ldpc_frame{(long)r.off, r.pos, r.cor, r.phase, r.swap, r.corr};
     }
-    return L.last_nf;
+    return last_nf;
 }
 
-void Fec::ldpc_timing(float *ms, int n)
+void Ldpc::timing(float *ms, int n) const
 {
-    const Ldpc &L = framed_as<Ldpc>("not an LDPC decoder (kind B200_FEC_LDPC)");
     for (int k = 0; k < n && k < 5; k++)
-        ms[k] = L.t_ms[k];
+        ms[k] = t_ms[k];
 }
 
 } // namespace b200
+
+using namespace b200;
+
+extern "C" {
+int b200_fec_debug_ldpc_frames(b200_fec *h, b200_ldpc_frame *out, long cap, long *n_out)
+{
+    return guarded([&] {
+        B200_REQUIRE(h && out && n_out, B200_EINVAL, "NULL argument");
+        *n_out = h->f->framed_as<Ldpc>("not an LDPC decoder").records(out, cap);
+    });
+}
+int b200_fec_ldpc_timing(b200_fec *h, float *ms_out, int n)
+{
+    return guarded([&] {
+        B200_REQUIRE(h && ms_out, B200_EINVAL, "NULL argument");
+        h->f->framed_as<Ldpc>("not an LDPC decoder (kind B200_FEC_LDPC)").timing(ms_out, n);
+    });
+}
+}

@@ -8,7 +8,7 @@
 namespace b200
 {
 
-struct Meteor : Framed
+struct Meteor : Correlated
 {
     MeteorSync sw{};
     DevBuf<uint32_t> hw;
@@ -19,6 +19,7 @@ struct Meteor : Framed
     explicit Meteor(Fec &f);
     void process(Fec &f) override;
     void reset(Fec &f) override;
+    long records(const Fec &f, b200_meteor_frame *out, long cap) const; // of the last push
 };
 
 namespace
@@ -106,7 +107,7 @@ std::unique_ptr<Framed> meteor_decoder(Fec &f) { return std::make_unique<Meteor>
 
 void Meteor::reset(Fec &f)
 {
-    Framed::reset(f);
+    Correlated::reset(f);
     f.main_next_start = -1; // a fresh CCDecoder starts unbiased, its encoder from 0
     f.enc_state = 0;
     f.nrzm_last = 0;
@@ -146,10 +147,7 @@ void Meteor::process(Fec &f)
         f.nrzm_last = nrzm_next;
     }
     f.keep_soft_tail(h_walk.p->next);
-    B200_CUDA(cudaEventRecord(f.ev[1], stream));
-    B200_CUDA(cudaStreamSynchronize(stream));
-    B200_CUDA(cudaGetLastError());
-    cudaEventElapsedTime(&f.t_vit, f.ev[0], f.ev[1]);
+    end(f);
     finish(nf, f.soft_have);
     if (nf > 0) {
         kept = f.h_counters.p[2];
@@ -170,12 +168,11 @@ void Meteor::process(Fec &f)
     f.total_bits += (long)nf * METEOR_BITS;
 }
 
-long Fec::meteor_frames(b200_meteor_frame *out, long cap)
+long Meteor::records(const Fec &f, b200_meteor_frame *out, long cap) const
 {
-    const Meteor &D = framed_as<Meteor>("not a METEOR LRPT decoder in m2x_mode false");
-    B200_REQUIRE(D.last_nf <= cap, B200_ESTATE, "output buffer too small: need %ld records", D.last_nf);
-    for (long k = 0; k < D.last_nf; k++) {
-        const WalkFrame &r = D.h_frames.p[k];
+    B200_REQUIRE(last_nf <= cap, B200_ESTATE, "output buffer too small: need %ld records", last_nf);
+    for (long k = 0; k < last_nf; k++) {
+        const WalkFrame &r = h_frames.p[k];
         b200_meteor_frame &d = out[k];
         d.offset = (long)r.off;
         d.pos = r.pos;
@@ -183,10 +180,21 @@ long Fec::meteor_frames(b200_meteor_frame *out, long cap)
         d.phase = r.phase;
         d.swap = r.swap;
         for (int i = 0; i < METEOR_RS_I; i++)
-            d.rs[i] = h_rs_err.p[k * METEOR_RS_I + i];
-        d.ber = ((float)D.h_ber.p[k] / 1024.0f) * 4.0f;
+            d.rs[i] = f.h_rs_err.p[k * METEOR_RS_I + i];
+        d.ber = ((float)h_ber.p[k] / 1024.0f) * 4.0f;
     }
-    return D.last_nf;
+    return last_nf;
 }
 
 } // namespace b200
+
+using namespace b200;
+
+extern "C" int b200_fec_debug_meteor_frames(b200_fec *h, b200_meteor_frame *out, long cap, long *n_out)
+{
+    return guarded([&] {
+        B200_REQUIRE(h && out && n_out, B200_EINVAL, "NULL argument");
+        Fec &f = *h->f;
+        *n_out = f.framed_as<Meteor>("not a METEOR LRPT decoder in m2x_mode false").records(f, out, cap);
+    });
+}

@@ -12,7 +12,7 @@ namespace b200
 
 constexpr int TURBO_BATCH = 1024; // frames decoded at once: their BCJR metrics take 2 (K + 4) x 16 doubles each (2.3 MB at base 1115)
 
-struct Turbo : Framed
+struct Turbo : Correlated
 {
     TurboGeom G{};
     TurboCode upper{}, lower{};
@@ -33,6 +33,9 @@ struct Turbo : Framed
     void process(Fec &f) override;
     void reset(Fec &f) override;
     void stats(b200_fec_stats *o) override;
+    long records(b200_turbo_frame *out, long cap) const; // of the last push
+    long llr(cudaStream_t stream, long frame, double *app0, double *app1, long cap) const;
+    void timing(float *ms, int n) const;
 };
 
 namespace
@@ -205,7 +208,7 @@ std::unique_ptr<Framed> turbo_decoder(Fec &f) { return std::make_unique<Turbo>(f
 
 void Turbo::reset(Fec &f)
 {
-    Framed::reset(f);
+    Correlated::reset(f);
     near_ties = 0;
     ties.zero(f.stream);
     B200_CUDA(cudaStreamSynchronize(f.stream));
@@ -294,42 +297,66 @@ void Turbo::process(Fec &f)
 
 void Turbo::stats(b200_fec_stats *o)
 {
-    Framed::stats(o);
+    Correlated::stats(o);
     o->crc_ok = crc_ok;
     o->crc_fail = crc_fail;
     o->turbo_near_ties = near_ties;
 }
 
-long Fec::turbo_frames(b200_turbo_frame *out, long cap)
+long Turbo::records(b200_turbo_frame *out, long cap) const
 {
-    const Turbo &T = framed_as<Turbo>("not a turbo decoder");
-    B200_REQUIRE(T.last_nf <= cap, B200_ESTATE, "output buffer too small: need %ld records", T.last_nf);
-    for (long k = 0; k < T.last_nf; k++) {
-        const WalkFrame &r = T.h_frames.p[k];
+    B200_REQUIRE(last_nf <= cap, B200_ESTATE, "output buffer too small: need %ld records", last_nf);
+    for (long k = 0; k < last_nf; k++) {
+        const WalkFrame &r = h_frames.p[k];
         out[k] = b200_turbo_frame{(long)r.off, r.pos, r.cor, r.swap, r.corr};
     }
-    return T.last_nf;
+    return last_nf;
 }
 
-long Fec::turbo_llr(long frame, double *app0, double *app1, long cap)
+long Turbo::llr(cudaStream_t stream, long frame, double *app0, double *app1, long cap) const
 {
-    const Turbo &T = framed_as<Turbo>("not a turbo decoder");
-    const int K = T.G.K;
-    B200_REQUIRE(frame >= T.last_b0 && frame < T.last_nf, B200_ESTATE, "frame %ld is not in the last decoding batch [%ld, %ld) of the last push",
-                 frame, T.last_b0, T.last_nf);
+    const int K = G.K;
+    B200_REQUIRE(frame >= last_b0 && frame < last_nf, B200_ESTATE, "frame %ld is not in the last decoding batch [%ld, %ld) of the last push",
+                 frame, last_b0, last_nf);
     B200_REQUIRE(cap >= K, B200_ESTATE, "output buffer too small: need %d values", K);
-    const double *m = T.msg.p + (size_t)(frame - T.last_b0) * 2 * K;
+    const double *m = msg.p + (size_t)(frame - last_b0) * 2 * K;
     B200_CUDA(cudaMemcpyAsync(app0, m, sizeof(double) * K, cudaMemcpyDeviceToHost, stream));
     B200_CUDA(cudaMemcpyAsync(app1, m + K, sizeof(double) * K, cudaMemcpyDeviceToHost, stream));
     B200_CUDA(cudaStreamSynchronize(stream));
     return K;
 }
 
-void Fec::turbo_timing(float *ms, int n)
+void Turbo::timing(float *ms, int n) const
 {
-    const Turbo &T = framed_as<Turbo>("not a turbo decoder (kind B200_FEC_TURBO)");
     for (int k = 0; k < n && k < 6; k++)
-        ms[k] = T.t_ms[k];
+        ms[k] = t_ms[k];
 }
 
 } // namespace b200
+
+using namespace b200;
+
+extern "C" {
+int b200_fec_debug_turbo_frames(b200_fec *h, b200_turbo_frame *out, long cap, long *n_out)
+{
+    return guarded([&] {
+        B200_REQUIRE(h && out && n_out, B200_EINVAL, "NULL argument");
+        *n_out = h->f->framed_as<Turbo>("not a turbo decoder").records(out, cap);
+    });
+}
+int b200_fec_debug_turbo_llr(b200_fec *h, long frame, double *app0, double *app1, long cap, long *n_out)
+{
+    return guarded([&] {
+        B200_REQUIRE(h && app0 && app1 && n_out, B200_EINVAL, "NULL argument");
+        DeviceGuard g(h->f->cfg.device);
+        *n_out = h->f->framed_as<Turbo>("not a turbo decoder").llr(h->f->stream, frame, app0, app1, cap);
+    });
+}
+int b200_fec_turbo_timing(b200_fec *h, float *ms_out, int n)
+{
+    return guarded([&] {
+        B200_REQUIRE(h && ms_out, B200_EINVAL, "NULL argument");
+        h->f->framed_as<Turbo>("not a turbo decoder (kind B200_FEC_TURBO)").timing(ms_out, n);
+    });
+}
+}

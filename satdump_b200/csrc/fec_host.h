@@ -15,11 +15,30 @@ namespace b200
 struct DefrEvent { long pos; int state; int pad; };
 class Fec;
 
-// The stream state of a correlator-driven decoder (ccsds_ldpc_decoder, ccsds_turbo_decoder, metop_dump_decoder, meteor_lrpt_decoder): a correlator scores
-// every position of the soft FIFO, k_frame_walk (walk.cuh) goes o -> o + pos + F over its windows, the frames are decoded, and the
-// FIFO keeps the bytes behind the walk's next window. Each decoder derives from it (Ldpc, Turbo, Dump, Meteor in api_ldpc.cu, api_turbo.cu,
-// api_dump.cu, api_meteor.cu); its process() reads begin -> correlate -> walk -> walked -> decode -> keep_soft_tail -> timings -> finish.
+// A decoder that replaces the Viterbi path (Fec::framed): its own kernels consume the soft FIFO of Fec, and the deframer and frame stage
+// of the convolutional decoders serve it where it needs them. Every push reads begin -> the decoder's kernels -> keep_soft_tail -> end
+// (or the decoder's own timing).
 struct Framed
+{
+    long tail_seen = -1;              // FIFO bytes left by the last pass (a second process() without new bytes changes nothing)
+    long base_off = 0;                // stream offset of the FIFO's first byte
+    long last_nf = 0;                 // records of the last push
+    float t_ms[6]{};                  // device ms of the last push's stages, as the decoder's timing getter lists them
+
+    virtual ~Framed() = default;
+    virtual void process(Fec &f) = 0;
+    virtual void reset(Fec &f);       // a new stream: the FIFO, its stream offset, the frame bits (the counters carry over)
+    virtual void stats(b200_fec_stats *) {}
+
+    bool begin(Fec &f, int F);        // false when there is nothing to do: no new bytes, or fewer than F in the FIFO
+    void end(Fec &f);                 // waits for the push, checks it, and puts its device time ev[0] .. ev[1] in t_vit
+};
+
+// The decoders driven by a correlator (ccsds_ldpc_decoder, ccsds_turbo_decoder, metop_dump_decoder, meteor_lrpt_decoder in api_ldpc.cu,
+// api_turbo.cu, api_dump.cu, api_meteor.cu): the correlator scores every position of the soft FIFO, k_frame_walk (walk.cuh) goes
+// o -> o + pos + F over its windows, the frames are decoded, and the FIFO keeps the bytes behind the walk's next window. Their process()
+// reads begin -> correlate -> walk -> walked -> decode -> keep_soft_tail -> timings -> finish.
+struct Correlated : Framed
 {
     DevBuf<float> score, bval;        // the correlator's score at every position, the maxima of 32-position blocks
     DevBuf<int> bidx;                 // ... and their positions
@@ -28,21 +47,14 @@ struct Framed
     DevBuf<WalkOut> walk;
     PinnedBuf<WalkOut> h_walk;
     PinnedBuf<WalkFrame> h_frames;    // records of the last push (offsets made absolute)
-    long max_frames = 0;
-    long tail_seen = -1;              // FIFO bytes left by the last pass (a second process() without new bytes changes nothing)
-    long base_off = 0;                // stream offset of the FIFO's first byte
-    long last_nf = 0, resyncs = 0;
+    long max_frames = 0, resyncs = 0;
     int lock = 0;
     float cor = 0.f;
-    float t_ms[6]{};                  // device ms of the last push's stages, as the decoder's timing getter lists them
 
-    virtual ~Framed() = default;
-    virtual void process(Fec &f) = 0;
-    virtual void reset(Fec &f);       // a new stream: the FIFO, the walk's position and the lock (the counters carry over)
-    virtual void stats(b200_fec_stats *o); // correlator_lock, correlator_corr and ldpc_resyncs
+    void reset(Fec &f) override;      // ... and the lock
+    void stats(b200_fec_stats *o) override; // correlator_lock, correlator_corr and ldpc_resyncs
 
     void alloc(long positions, long frames_cap); // the correlator's outputs for `positions` scores, the walk's records
-    bool begin(Fec &f, int F);        // false when there is nothing to do: no new bytes, or fewer than F in the FIFO
     int walked(cudaStream_t stream);  // waits for the walk; its frame count
     void finish(int nf, long soft_have); // records made absolute, resyncs, lock and cor of the last frame, the next pass's start
 };
@@ -50,10 +62,8 @@ std::unique_ptr<Framed> ldpc_decoder(Fec &f);
 std::unique_ptr<Framed> turbo_decoder(Fec &f);
 std::unique_ptr<Framed> dump_decoder(Fec &f);
 std::unique_ptr<Framed> meteor_decoder(Fec &f);
-std::unique_ptr<Framed> hrpt_decoder(Fec &f); // noaa_hrpt_decoder, meteor_hrpt_decoder (api_hrpt.cu)
-std::unique_ptr<Framed> aqua_decoder(Fec &f);
-std::unique_ptr<Framed> gac_decoder(Fec &f);  // noaa_gac_decoder (api_hrpt.cu): the deframer and frame stage behind its own bit stage
-std::unique_ptr<Framed> dmsp_decoder(Fec &f); // dmsp_rtd_decoder (api_hrpt.cu) // aqua_db_decoder (api_aqua.cu): the deframer and frame stage behind its own bit stage
+std::unique_ptr<Framed> sync_walk_decoder(Fec &f); // noaa_hrpt_decoder, meteor_hrpt_decoder, dmsp_rtd_decoder (api_hrpt.cu)
+std::unique_ptr<Framed> bit_stage_decoder(Fec &f); // aqua_db_decoder, noaa_gac_decoder (api_hrpt.cu)
 
 class Fec
 {
@@ -71,7 +81,7 @@ class Fec
 
     b200_fec_cfg cfg;
     VitGeom geom;
-    int cadu_bytes, nphases, ph0, ph1, nswap, st_synced, spec_steps;
+    int cadu_bytes = 0, nphases = 0, ph0 = 0, ph1 = 0, nswap = 0, st_synced = 0, spec_steps = 0; // (a Framed decoder sets only what it uses)
     int fr_smem = 0; // dynamic shared memory of k_frames
     cudaStream_t stream = nullptr;
     cudaEvent_t ev[2];
@@ -79,8 +89,7 @@ class Fec
     cudaEvent_t evm[2], evf[2];
     long last_main_chunks = 0;
     void reset();
-    // the correlator-driven decoders (B200_FEC_LDPC, B200_FEC_TURBO, B200_FEC_METOP_DUMP): set up by the constructor instead of the
-    // Viterbi / deframer storage (ccsds_ldpc_decoder's internal_stream adds the deframer stage)
+    // every kind but METOP, CCSDS and SIMPLE: set up by the constructor instead of the Viterbi / deframer storage
     std::unique_ptr<Framed> framed;
     template <class D> D &framed_as(const char *what) // the decoder as a D, or B200_EINVAL with `what`
     {
@@ -88,14 +97,6 @@ class Fec
         B200_REQUIRE(d, B200_EINVAL, "%s", what);
         return *d;
     }
-    long ldpc_frames(b200_ldpc_frame *out, long cap); // records of the last push
-    void ldpc_timing(float *ms, int n);
-    long turbo_frames(b200_turbo_frame *out, long cap); // records of the last push
-    long turbo_llr(long frame, double *app0, double *app1, long cap);
-    void turbo_timing(float *ms, int n);
-    long dump_frames(b200_dump_frame *out, long cap); // records of the last push
-    long meteor_frames(b200_meteor_frame *out, long cap); // records of the last push
-    long hrpt_frames(b200_hrpt_frame *out, long cap); // records of the last push
     // noaa_gac_decoder / dmsp_rtd_decoder: the stream bit that completed each frame waiting in frames_out, and each frame of the last pull
     std::vector<long> done_bits, pulled_bits;
     void note_frame_bits(long out0, const std::vector<long> &bits); // the bits of the frames a push wrote from frames_out index out0
@@ -152,6 +153,12 @@ class Fec
     bool two_deframers() const { return cfg.kind == B200_FEC_SIMPLE && cfg.constellation == B200_QPSK && !cfg.nrzm; }
     void swap_unit();
     void compact_fifo(bool sync);
+    void start_stream(size_t fifo_bytes);
+    int last_raw_bit(long q, int nbits);
+    void keep_soft_tail(long used);
+    void deframe_and_rs(long new_bits);
+    void framed_storage(int F, long frames_per_push); // what every Framed decoder needs of the decoder object
+    void deframer_storage(long max_new_bits); // the bit FIFO, deframer and frame stage behind a Framed decoder's own stages
     // pinned host mirrors
     PinnedBuf<VitRec> h_rec;
     PinnedBuf<VitIdleOut> h_idle;
@@ -175,26 +182,12 @@ class Fec
     long total_soft = 0, total_chunks = 0, total_bits = 0, total_frames = 0, rs_corrected = 0, rs_failed = 0, replays = 0, launches = 0;
 
   private:
-    friend struct Ldpc;
-    friend struct Turbo;
-    friend struct Dump;
-    friend struct Meteor;
-    friend struct Hrpt;
-    friend struct Aqua;
-    friend struct Gac;
-    friend struct Dmsp;
     // the main deframer and the frame counters at a point a pass may have to roll back to
     struct Mark { DefrState h_dstate; long fifo_bits, out_frames, total_frames, rs_corrected, rs_failed; int defr_state_now; };
     Mark mark();
     void rewind(const Mark &m);
-    void start_stream(size_t fifo_bytes);
     void decode_simple(long nch);
     void decode_conv(long nch);
-    int last_raw_bit(long q, int nbits);
-    void keep_soft_tail(long used);
-    void deframe_and_rs(long new_bits);
-    void framed_storage(int F, long frames_per_push); // what every Framed decoder needs of the decoder object (api_fec.cu)
-    void deframer_storage(long max_new_bits); // bit FIFO, deframer and frame stage of LDPC's internal_stream (api_fec.cu)
 };
 
 // Viterbi27 (meteor_lrpt_decoder): the n chunks at src (geom.chunk bytes apart, already rotated) decoded as consecutive calls of ONE chained
@@ -209,3 +202,9 @@ void build_rs_tables(RsTables &T);
 void ccsds_pn_bits(unsigned char *pn);
 
 } // namespace b200
+
+// the handle of the C ABI (each decoder's file defines the entry points that read its records)
+struct b200_fec
+{
+    b200::Fec *f;
+};

@@ -61,8 +61,7 @@ __global__ void __launch_bounds__(256) k_gac_post(uint8_t *__restrict__ frames, 
 }
 
 // ---------------------------------------------------------------- DMSP
-struct DmspRec { long long bit; int inverted, state; }; // the sync's last bit (FIFO bits in a walk, stream bits on the host)
-struct DmspOut { int nrec, nseg; };
+// The walk reports through hrpt.cuh's HrptRec (a sync's last bit, in FIFO bits) and HrptOut (units = nseg: one unit per frame).
 // The machine between pushes (stream bits)
 struct DmspState
 {
@@ -79,8 +78,8 @@ __device__ __forceinline__ unsigned dmsp_win(const uint32_t *__restrict__ hw, lo
 // within 1 bit (< 2), a failure tests the next bit; SYNCED tests 128 frames ahead at once, within 5 bits (< 6), and one failure drops to
 // NOSYNC at the next bit. Every accepted sync is a record and, once complete, a frame. One warp; every lane runs the same control flow.
 __global__ void __launch_bounds__(32) k_dmsp_walk(const uint32_t *__restrict__ hw, const uint32_t *__restrict__ cand, long long have, long long base,
-                                                  DmspState *__restrict__ st, DmspRec *__restrict__ recs, DmspRec *__restrict__ segs,
-                                                  DmspOut *__restrict__ out)
+                                                  DmspState *__restrict__ st, HrptRec *__restrict__ recs, HrptRec *__restrict__ segs,
+                                                  HrptOut *__restrict__ out)
 {
     const int lane = threadIdx.x & 31;
     DmspState S = *st;
@@ -91,7 +90,7 @@ __global__ void __launch_bounds__(32) k_dmsp_walk(const uint32_t *__restrict__ h
         if (s + DMSP_PAY >= have) // (p stays on the test after it)
             goto done;
         if (lane == 0)
-            segs[nseg] = DmspRec{s, S.open_inv, 0};
+            segs[nseg] = HrptRec{s, S.open_inv, 0};
         nseg++;
         S.open = HRPT_NONE;
     }
@@ -128,9 +127,9 @@ __global__ void __launch_bounds__(32) k_dmsp_walk(const uint32_t *__restrict__ h
                 const int f = lane + 32 * g;
                 const long long e = p + (long long)f * DMSP_BITS;
                 if (f < n)
-                    recs[nrec + f] = DmspRec{e, S.inv, 6};
+                    recs[nrec + f] = HrptRec{e, S.inv, 6};
                 if (f < m)
-                    segs[nseg + f] = DmspRec{e, S.inv, 6};
+                    segs[nseg + f] = HrptRec{e, S.inv, 6};
             }
             nrec += n;
             nseg += m;
@@ -187,11 +186,11 @@ __global__ void __launch_bounds__(32) k_dmsp_walk(const uint32_t *__restrict__ h
                 break;
         }
         if (lane == 0)
-            recs[nrec] = DmspRec{hit, S.inv, from};
+            recs[nrec] = HrptRec{hit, S.inv, from};
         nrec++;
         if (hit + DMSP_PAY < have) {
             if (lane == 0)
-                segs[nseg] = DmspRec{hit, S.inv, 0};
+                segs[nseg] = HrptRec{hit, S.inv, 0};
             nseg++;
         } else {
             S.open = hit + base;
@@ -203,20 +202,20 @@ done:
     if (lane == 0) {
         S.next = max(p, have) + base;
         *st = S;
-        *out = DmspOut{nrec, nseg};
+        *out = HrptOut{nrec, nseg, nseg};
     }
 }
 
 // One thread per frame byte: frame bit k < 13 is the clean sync's, bit k >= 13 the stream bit sync + k - 12 XOR the inversion; bytes
 // MSB first, the last one holding bits 144 .. 149 right-aligned.
-__global__ void __launch_bounds__(256) k_dmsp_gather(const uint32_t *__restrict__ hw, const DmspRec *__restrict__ segs, long nseg, uint8_t *__restrict__ out)
+__global__ void __launch_bounds__(256) k_dmsp_gather(const uint32_t *__restrict__ hw, const HrptRec *__restrict__ segs, long nseg, uint8_t *__restrict__ out)
 {
     const long t = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= nseg * DMSP_BYTES)
         return;
     const long f = t / DMSP_BYTES;
     const int j = (int)(t - f * DMSP_BYTES);
-    const DmspRec g = segs[f];
+    const HrptRec g = segs[f];
     const int n = min(8, DMSP_BITS - 8 * j);
     unsigned v = 0;
     for (int k = 8 * j; k < 8 * j + n; k++) {

@@ -53,7 +53,8 @@ enum { B200_CF32 = 0, B200_CS16 = 1, B200_CS8 = 2 };
 /* decoder kind */
 enum { B200_FEC_METOP = 0, B200_FEC_CCSDS = 1, B200_FEC_SIMPLE = 2, B200_FEC_LDPC = 3, B200_FEC_TURBO = 4, B200_FEC_METOP_DUMP = 5,
        B200_FEC_METEOR_LRPT = 6, B200_FEC_NOAA_HRPT = 7 /* noaa_hrpt_decoder */, B200_FEC_METEOR_HRPT = 8 /* meteor_hrpt_decoder */,
-       B200_FEC_AQUA_DB = 9 /* aqua_db_decoder */, B200_FEC_NOAA_GAC = 10 /* noaa_gac_decoder */, B200_FEC_DMSP_RTD = 11 /* dmsp_rtd_decoder */ };
+       B200_FEC_AQUA_DB = 9 /* aqua_db_decoder */, B200_FEC_NOAA_GAC = 10 /* noaa_gac_decoder */, B200_FEC_DMSP_RTD = 11 /* dmsp_rtd_decoder */,
+       B200_FEC_METEOR_XBAND = 12 /* meteor_xband_decoder */ };
 /* debug stage ids for b200_demod_debug_stage */
 enum { B200_STAGE_AGC = 0, B200_STAGE_FIR = 1, B200_STAGE_COSTAS = 2, B200_STAGE_RESAMP = 3, B200_STAGE_DC = 4, B200_STAGE_MM = 5,
        B200_STAGE_PLL = 6 /* pm_demod: PLLCarrierTrackingBlock output */, B200_STAGE_PM = 7 /* pm_demod: PMToBPSK output */,
@@ -204,6 +205,18 @@ typedef struct b200_fec_cfg
        the clean sync and 137 bits XOR the inversion, its last byte holding 6 bits right-aligned. Only device and max_soft are read.
        Both: max_soft <= 2^30; b200_fec_frame_bits returns the stream bit at which each pulled frame completed. */
     int backward;             /* "backward" of noaa_gac_decoder (required by the module): backward tape playback                         */
+    /* kind B200_FEC_METEOR_XBAND = meteor_xband_decoder (module_meteor_xband_decoder.cpp): hard bits soft > 0 -> NRZMDiff::decode_bits
+       carried across pushes, then by instrument_type:
+         0 "mtvza": MTVZA_ExtDeframer (3072-bit records, four patterns) -> eight 46-byte packets XOR 0xAA per record ->
+           SimpleDeframer(0x38FB456A, 32, 3040): one output unit is one 380-byte frame (cadu_bytes 380).
+         1 "kmss_bpsk": RepackBitsByte -> KMSS_BPSK_ExtDeframer (1536-byte records) -> eight 188-byte packets per record -> three
+           SimpleDeframers (syncs 0xAF5FFF50AA5AA0, 0xAE5EEC61BB7982, 0xAB5BB394EED628, 481280-bit frames) -> kmssFrameProcessor: one
+           output unit is the four 15040-byte lanes of one frame (cadu_bytes 60160).
+       Inner frames cut by the next sync are filled with zeros, as SimpleDeframer does. The decoder works in the module's 8192-byte reads
+       counted from the stream's start: a push decodes every read it completes and keeps the rest, and the frames come out in the module's
+       order (by read, then deframer, then position). Only instrument_type, device and max_soft are read; another instrument_type is
+       refused ("Invalid METEOR instrument type!") before the device is looked at. max_soft <= 2^30. */
+    int instrument_type;      /* "instrument_type": 0 "mtvza", 1 "kmss_bpsk"                                                              */
 } b200_fec_cfg;
 
 typedef struct b200_demod_stats

@@ -6,7 +6,7 @@
 //
 //   loader()                          the one symbol SatDump dlsym()s (core/plugin.cpp:15-33)
 //   B200DSPSupport::init()            on SatDumpStartedEvent (fired after every plugin registered its modules, init.cpp:163) the
-//                                     entries "psk_demod", "pm_demod", "terra_db_demod", "fsk_demod", "metop_ahrpt_decoder", "ccsds_conv_concat_decoder", "ccsds_simple_psk_decoder", "ccsds_ldpc_decoder", "ccsds_turbo_decoder", "metop_dump_decoder", "meteor_lrpt_decoder", "noaa_hrpt_decoder", "meteor_hrpt_decoder", "aqua_db_decoder", "noaa_gac_decoder" and "dmsp_rtd_decoder" of
+//                                     entries "psk_demod", "pm_demod", "terra_db_demod", "fsk_demod", "metop_ahrpt_decoder", "ccsds_conv_concat_decoder", "ccsds_simple_psk_decoder", "ccsds_ldpc_decoder", "ccsds_turbo_decoder", "metop_dump_decoder", "meteor_lrpt_decoder", "noaa_hrpt_decoder", "meteor_hrpt_decoder", "aqua_db_decoder", "noaa_gac_decoder", "dmsp_rtd_decoder" and "meteor_xband_decoder" of
 //                                     satdump::pipeline::modules_registry (module.h:210, looked up first-match by id, module.cpp:129-135)
 //                                     get their factory replaced, so existing pipelines instantiate the CUDA modules.
 //                                     Set B200_DSP_REGISTER_ONLY=1 to register "<id>_b200" ids instead and leave the originals alone.
@@ -239,8 +239,8 @@ namespace b200plugin
                 v["lock_state"] = stage->correlator_lock.load() ? "SYNCED" : "NOSYNC";
                 return v;
             }
-            if (stage->getID() == "ccsds_turbo_decoder") // CCSDSTurboDecoderModule has no getModuleStats: ProcessingModule's empty one
-                return v;
+            if (stage->getID() == "ccsds_turbo_decoder" || stage->getID() == "meteor_xband_decoder") // neither module has getModuleStats:
+                return v;                                                                          // ProcessingModule's empty one
             if (stage->getID() == "metop_dump_decoder") // MetOpDumpDecoderModule::getModuleStats (module_metop_dump_decoder.cpp:84-90)
             {
                 v["lock_state"] = stage->correlator_lock.load() ? "SYNCED" : "NOSYNC";
@@ -323,7 +323,7 @@ public:
     {
         for (const char *id : {"psk_demod", "pm_demod", "terra_db_demod", "fsk_demod", "metop_ahrpt_decoder", "ccsds_conv_concat_decoder", "ccsds_simple_psk_decoder", "ccsds_ldpc_decoder",
                                "ccsds_turbo_decoder", "metop_dump_decoder", "meteor_lrpt_decoder", "noaa_hrpt_decoder", "meteor_hrpt_decoder",
-                               "aqua_db_decoder", "noaa_gac_decoder", "dmsp_rtd_decoder"})
+                               "aqua_db_decoder", "noaa_gac_decoder", "dmsp_rtd_decoder", "meteor_xband_decoder"})
             evt.modules_registry.push_back({std::string(id) + "_b200", nlohmann::json(), factory(id)});
     }
 
@@ -333,7 +333,7 @@ public:
             if (e.id == "psk_demod" || e.id == "pm_demod" || e.id == "terra_db_demod" || e.id == "fsk_demod" || e.id == "metop_ahrpt_decoder" || e.id == "ccsds_conv_concat_decoder" || e.id == "ccsds_simple_psk_decoder" ||
                 e.id == "ccsds_ldpc_decoder" || e.id == "ccsds_turbo_decoder" || e.id == "metop_dump_decoder" ||
                 e.id == "meteor_lrpt_decoder" || e.id == "noaa_hrpt_decoder" || e.id == "meteor_hrpt_decoder" ||
-                e.id == "aqua_db_decoder" || e.id == "noaa_gac_decoder" || e.id == "dmsp_rtd_decoder")
+                e.id == "aqua_db_decoder" || e.id == "noaa_gac_decoder" || e.id == "dmsp_rtd_decoder" || e.id == "meteor_xband_decoder")
             {
                 e.inst = factory(e.id);
                 logger->info("b200_dsp_support: module " + e.id + " now runs on the B200 path");

@@ -56,7 +56,7 @@ class FecCfg(C.Structure):
                 ("ldpc_rate", C.c_int), ("ldpc_block_size", C.c_int), ("ldpc_iterations", C.c_int), ("ldpc2", C.c_int), ("internal_stream", C.c_int),
                 ("internal_cadu_size", C.c_int), ("turbo_rate", C.c_int), ("turbo_base", C.c_int), ("turbo_iters", C.c_int),
                 ("diff_decode", C.c_int), ("m2x_mode", C.c_int), ("interleaved", C.c_int), ("deframer_thresold", C.c_int),
-                ("backward", C.c_int)]
+                ("backward", C.c_int), ("instrument_type", C.c_int)]
 
 
 class DemuxCfg(C.Structure):
@@ -433,6 +433,20 @@ def dmsp_rtd_cfg(device=0, max_soft=1 << 24):
     return cfg
 
 
+METEOR_XBAND_TYPES = {"mtvza": 0, "kmss_bpsk": 1}
+
+
+def meteor_xband_cfg(instrument_type=None, device=0, max_soft=1 << 24):
+    """meteor_xband_decoder (module_meteor_xband_decoder.cpp, meteor_xband_types.h): instrument_type "mtvza" (380-byte frames) or
+    "kmss_bpsk" (60160-byte frames: the four lanes of one frame) is required, as the module refuses anything else."""
+    if instrument_type not in METEOR_XBAND_TYPES:
+        raise ValueError("Invalid METEOR instrument type!")
+    cfg = FecCfg()
+    cfg.kind, cfg.constellation, cfg.device, cfg.max_soft = 12, CONST["bpsk"], device, max_soft
+    cfg.instrument_type = METEOR_XBAND_TYPES[instrument_type]
+    return cfg
+
+
 def dmsp_timestamps(bits, start_timestamp, read_bits_seen=None):
     """dmsp_rtd_decoder's "_timestamps.txt" values for frames completed at stream bits `bits` (b200_fec_frame_bits): start +
     8192 * (reads of 8192 soft bytes from the stream's start that produced frames, up to the frame's) / 1.024e6. read_bits_seen carries
@@ -468,6 +482,8 @@ def fec_cfg_for(sig, max_soft, device=0):
         return noaa_gac_cfg(sig.backward, device=device, max_soft=max_soft)
     if sig.decoder == "dmsp_rtd":
         return dmsp_rtd_cfg(device=device, max_soft=max_soft)
+    if sig.decoder in ("meteor_mtvza", "meteor_kmss_bpsk"):
+        return meteor_xband_cfg("mtvza" if sig.decoder == "meteor_mtvza" else "kmss_bpsk", device=device, max_soft=max_soft)
     if sig.decoder == "turbo":
         return turbo_cfg(sig.turbo_rate, sig.turbo_base, sig.turbo_iters, device=device, max_soft=max_soft)
     if sig.decoder == "ldpc":
@@ -656,7 +672,7 @@ class Fec:
         return self
 
     def frames(self):
-        cap = int(self._n) + 65536
+        cap = int(self._n) + 65536 + 4 * self.cadu_bytes  # (meteor_xband_decoder: a byte that completes a read may release its frames)
         out = np.zeros(cap, np.uint8)
         n = C.c_long(0)
         _chk(lib().b200_fec_pull_frames(self.h, out.ctypes.data, cap, C.byref(n)))
@@ -774,6 +790,8 @@ class Chain:
         self.cadu_bytes = (fcfg.cadu_size + 7) // 8 if fcfg.kind in (1, 3, 7) else (fcfg.turbo_base + 4 if fcfg.kind == 4 else 1024)
         if fcfg.kind in (10, 11):  # noaa_gac_decoder, dmsp_rtd_decoder: (cadu_size + padding) / 8
             self.cadu_bytes = 4159 if fcfg.kind == 10 else 19
+        if fcfg.kind == 12:  # meteor_xband_decoder
+            self.cadu_bytes = 60160 if fcfg.instrument_type == 1 else 380
 
     def close(self):
         if getattr(self, "h", None):

@@ -101,6 +101,7 @@ Fec::Fec(const b200_fec_cfg &in) : cfg(meteor_m2x_as_ccsds(in))
     case B200_FEC_METEOR_LRPT: decoder = meteor_decoder; break;
     case B200_FEC_NOAA_HRPT: case B200_FEC_METEOR_HRPT: case B200_FEC_DMSP_RTD: decoder = sync_walk_decoder; break;
     case B200_FEC_AQUA_DB: case B200_FEC_NOAA_GAC: decoder = bit_stage_decoder; break;
+    case B200_FEC_METEOR_XBAND: decoder = xband_decoder; break;
     default: B200_REQUIRE(false, B200_EINVAL, "unknown decoder kind %d", c.kind);
     }
     B200_REQUIRE(c.max_soft >= 65536, B200_EINVAL, "max_soft must be >= 65536");

@@ -7,8 +7,12 @@
 //   The bit stages: aqua_db_decoder (B200_FEC_AQUA_DB) and noaa_gac_decoder (B200_FEC_NOAA_GAC), that is AquaDBDecoderModule::process
 //   (plugins/eos_support/aqua/module_aqua_db_decoder.cpp:27-83) and NOAAGACDecoderModule::process (module_noaa_gac_decoder.cpp:65-102).
 //   Every push: its bits into the bit FIFO, then the deframer and frame stage of the convolutional decoders.
+//   The METEOR-M X-band dump decoder: meteor_xband_decoder (B200_FEC_METEOR_XBAND), that is MeteorXBandDecoderModule::process
+//   (plugins/meteor_support/meteor/module_meteor_xband_decoder.cpp:62-212), two-level: a record walk and packet gather, then the inner
+//   deframers' walk over the packet FIFO and the frame gather (xband.cuh).
 #include "hrpt.cuh"
 #include "gac.cuh"
+#include "xband.cuh"
 #include "fec_host.h"
 #include <algorithm>
 
@@ -336,6 +340,196 @@ void BitStage::process(Fec &f)
     }
     tail_seen = f.soft_have;
     f.total_bits += nbits;
+}
+
+// ---------------------------------------------------------------- meteor_xband_decoder
+
+// The soft FIFO starts with the byte before the first bit not decoded yet (its hard bit is NRZMDiff::lastBit); FIFO bit q >= 1 is padded
+// stream bit q + pos0 - 1 (xband.cuh). At a stream's start the FIFO holds that byte and PAD zero bytes: the zeroed shift buffers, lastBit 0.
+// A push decodes the module's whole 8192-byte reads: the record walk tests the window starts [next, R) with R the soft bytes of those
+// reads, its records' packets enter the packet FIFO (32-bit words MSB first, whole records, each with its read), and the inner deframers
+// walk the new packet bits. The inner frames come out ordered by (read, deframer, position), as the module writes them.
+struct XBand : Framed
+{
+    bool kmss;
+    int pad, npb, ndef, frm_bytes;
+    long rec_cap = 0, frm_cap = 0, pk_cap = 0;
+    long long pos0 = 0, pbase = 0;    // padded bit of FIFO bit 1; packet-stream bit of packet FIFO bit 0
+    long pk_bytes = 0;                // bytes in the packet FIFO
+    DevBuf<uint32_t> hw, db, cand, pk, pcand, pk_read, pk_tmp;
+    DevBuf<XbRec> recs;
+    DevBuf<XbFrame> frm;
+    DevBuf<int> order;
+    DevBuf<XbState> st;
+    DevBuf<XbInner> inner;
+    DevBuf<XbOut> out;
+    PinnedBuf<XbOut> h_out;
+    PinnedBuf<XbState> h_st;
+    PinnedBuf<XbInner> h_inner;
+    PinnedBuf<XbFrame> h_frm;
+    PinnedBuf<int> h_order;
+
+    explicit XBand(Fec &f);
+    void process(Fec &f) override;
+    void reset(Fec &f) override;
+};
+
+XBand::XBand(Fec &f)
+    : kmss(f.cfg.instrument_type == 1), pad(kmss ? KMSS_PAD : MTVZA_PAD), npb(8 * (kmss ? KMSS_PKT : MTVZA_PKT)), ndef(kmss ? 3 : 1),
+      frm_bytes(kmss ? KMSS_FRM : MTVZA_FRM)
+{
+    B200_REQUIRE(f.cfg.instrument_type == 0 || f.cfg.instrument_type == 1, B200_EINVAL, "Invalid METEOR instrument type!");
+    B200_REQUIRE(f.cfg.max_soft <= (1L << 30), B200_EINVAL, "max_soft must be <= 2^30 for meteor_xband_decoder");
+    f.cadu_bytes = frm_bytes;
+    f.geom.chunk = XB_READ;
+    const int F = pad + XB_READ + 64;    // what the FIFO keeps: the carried byte, the windows' reach and a partial read
+    const long fifo = f.cfg.max_soft + 2L * F;
+    // records a push can accept: kmss_bpsk one per 12288 tests; mtvza one per 3072 tests when locked (the cap allows 8 times that)
+    rec_cap = kmss ? fifo / KMSS_REC + 4 : fifo / 384 + 8;
+    // inner frames: one per 481280 / 3040 packet bits when locked, plus the open ones (the cap allows about 7 times that)
+    const long pk_new = rec_cap * npb;
+    frm_cap = kmss ? pk_new / 8192 + 8 : pk_new / 64 + 8;
+    pk_cap = pk_new + (kmss ? KMSS_FRM : MTVZA_FRM) + 2L * npb + 64;
+    check_device(f.cfg.device);
+    DeviceGuard g(f.cfg.device);
+    f.framed_storage(F, frm_cap * ndef);
+    const size_t words = (size_t)fifo / 32 + 8, pwords = (size_t)pk_cap / 4 + 8;
+    hw.alloc(words);
+    db.alloc(words);
+    cand.alloc(words);
+    pk.alloc(pwords);
+    pk_tmp.alloc(pwords);
+    pcand.alloc((pwords + 8) * ndef);
+    pk_read.alloc((size_t)pk_cap / npb + 8);
+    recs.alloc((size_t)rec_cap);
+    frm.alloc((size_t)frm_cap * ndef);
+    order.alloc((size_t)frm_cap * ndef);
+    st.alloc(1);
+    inner.alloc(3);
+    out.alloc(1);
+    h_out.alloc(1);
+    h_st.alloc(1);
+    h_inner.alloc(3);
+    h_frm.alloc((size_t)frm_cap * ndef);
+    h_order.alloc((size_t)frm_cap * ndef);
+    reset(f);
+}
+
+std::unique_ptr<Framed> xband_decoder(Fec &f) { return std::make_unique<XBand>(f); }
+
+// a fresh module: lastBit 0, zeroed shift buffers, not synced, runs_since_sync and skip_bits 0, no open inner frame
+void XBand::reset(Fec &f)
+{
+    Framed::reset(f);
+    B200_CUDA(cudaMemsetAsync(f.softbuf.p, 0, (size_t)pad + 1, f.stream));
+    f.soft_have = pad + 1;
+    pos0 = pbase = 0;
+    pk_bytes = 0;
+    *h_st.p = XbState{0, 0, 0};
+    for (int d = 0; d < 3; d++)
+        h_inner.p[d] = XbInner{0, HRPT_NONE};
+    B200_CUDA(cudaMemcpyAsync(st.p, h_st.p, sizeof(XbState), cudaMemcpyHostToDevice, f.stream));
+    B200_CUDA(cudaMemcpyAsync(inner.p, h_inner.p, 3 * sizeof(XbInner), cudaMemcpyHostToDevice, f.stream));
+    B200_CUDA(cudaStreamSynchronize(f.stream));
+}
+
+void XBand::process(Fec &f)
+{
+    if (!begin(f, 1))
+        return;
+    cudaStream_t stream = f.stream;
+    const long have = f.soft_have;
+    const long long R = (pos0 + have - 1 - pad) / XB_READ * XB_READ; // (pos0 + have - 1: the padded bits in the FIFO)
+    if (R <= pos0) {
+        tail_seen = have;
+        return;
+    }
+    const long long base = pos0 - 1, qend = R - base;
+    const long nwords = (have + 31) / 32 + 2;
+    B200_CUDA(cudaEventRecord(f.ev[0], stream));
+    k_hard_pack<1><<<(unsigned)((nwords * 32 + 255) / 256), 256, 0, stream>>>(f.softbuf.p, have, nwords, hw.p);
+    k_nrzm_words<<<(unsigned)((nwords + 255) / 256), 256, 0, stream>>>(hw.p, nwords, db.p);
+    k_xband_cand<<<(unsigned)((qend + 255) / 256), 256, 0, stream>>>(db.p, qend, kmss, cand.p);
+    k_xband_rec_walk<<<1, 32, 0, stream>>>(db.p, cand.p, base, R, kmss, st.p, recs.p, (int)rec_cap, out.p);
+    f.launches += 4;
+    B200_CUDA(cudaMemcpyAsync(h_out.p, out.p, sizeof(XbOut), cudaMemcpyDeviceToHost, stream));
+    B200_CUDA(cudaStreamSynchronize(stream));
+    const int nrec = h_out.p->nrec;
+    B200_REQUIRE(nrec <= rec_cap && pk_bytes + (long)nrec * npb <= pk_cap, B200_ESTATE,
+                 "meteor_xband_decoder: %d records in one push (at most %ld): push less at a time", nrec, rec_cap);
+    if (nrec > 0) {
+        k_xband_packets<<<(unsigned)(((long)nrec * npb + 255) / 256), 256, 0, stream>>>(db.p, base, recs.p, nrec, kmss, (uint8_t *)pk.p,
+                                                                                       pk_bytes, pk_read.p, pk_bytes / npb);
+        f.launches++;
+    }
+    pk_bytes += (long)nrec * npb;
+    const long long pbits = 8LL * pk_bytes;
+    const long cwords = (long)(pbits / 32) + 2;
+    for (int d = 0; d < ndef && pbits > 0; d++)
+        k_sync_cand<<<(unsigned)((pbits + 255) / 256), 256, 0, stream>>>(pk.p, pbits, kmss ? kmss_sync(d) : MTVZA_SYNC,
+                                                                       kmss ? (1ull << 56) - 1 : 0xFFFFFFFFull, 0, pcand.p + d * cwords);
+    k_xband_inner_walk<<<ndef, 32, 0, stream>>>(pk.p, pcand.p, cwords, pbits, pbase, kmss, pk_read.p, inner.p, frm.p, (int)frm_cap, out.p);
+    f.launches += (pbits > 0 ? ndef : 0) + 1;
+    B200_CUDA(cudaMemcpyAsync(h_out.p, out.p, sizeof(XbOut), cudaMemcpyDeviceToHost, stream));
+    B200_CUDA(cudaMemcpyAsync(h_inner.p, inner.p, 3 * sizeof(XbInner), cudaMemcpyDeviceToHost, stream));
+    B200_CUDA(cudaStreamSynchronize(stream));
+    long nf = 0;
+    for (int d = 0; d < ndef; d++) {
+        B200_REQUIRE(h_out.p->nfrm[d] <= frm_cap, B200_ESTATE, "meteor_xband_decoder: %d frames in one push (at most %ld): push less at a time",
+                     h_out.p->nfrm[d], frm_cap);
+        nf += h_out.p->nfrm[d];
+    }
+    if (nf > 0) {
+        B200_REQUIRE((size_t)(f.out_frames + nf) * f.cadu_bytes <= f.frames_out.n, B200_ESTATE,
+                     "%ld frames not pulled yet: pull the frames between pushes", f.out_frames);
+        uint8_t *dst = f.frames_out.p + f.out_frames * f.cadu_bytes;
+        if (kmss) {
+            // the module runs deframer 1, 2, 3 over each read's packets and writes their frames in that order
+            for (int d = 0; d < 3; d++)
+                if (h_out.p->nfrm[d] > 0)
+                    B200_CUDA(cudaMemcpyAsync(h_frm.p + d * frm_cap, frm.p + d * frm_cap, sizeof(XbFrame) * h_out.p->nfrm[d],
+                                              cudaMemcpyDeviceToHost, stream));
+            B200_CUDA(cudaStreamSynchronize(stream));
+            long k = 0, at[3] = {0, 0, 0};
+            while (k < nf) {
+                int best = -1;
+                for (int d = 0; d < 3; d++)
+                    if (at[d] < h_out.p->nfrm[d] && (best < 0 || h_frm.p[d * frm_cap + at[d]].read < h_frm.p[best * frm_cap + at[best]].read))
+                        best = d;
+                h_order.p[k++] = (int)(best * frm_cap + at[best]++);
+            }
+            B200_CUDA(cudaMemcpyAsync(order.p, h_order.p, sizeof(int) * nf, cudaMemcpyHostToDevice, stream));
+            k_kmss_frames<<<(unsigned)((nf * KMSS_FRM + 255) / 256), 256, 0, stream>>>(pk.p, pbase, frm.p, order.p, nf, dst);
+        } else {
+            k_mtvza_frames<<<(unsigned)((nf * MTVZA_FRM + 255) / 256), 256, 0, stream>>>(pk.p, pbase, frm.p, nf, dst);
+        }
+        f.launches++;
+    }
+    // the packet FIFO keeps whole records from the first open frame's sync, else from 64 bits before the next test
+    long long keep = pbits;
+    for (int d = 0; d < ndef; d++)
+        keep = std::min(keep, (h_inner.p[d].open != HRPT_NONE ? h_inner.p[d].open : h_inner.p[d].next) - 64 - pbase);
+    const long drop_recs = (long)(std::max(0LL, keep) / 8 / npb);
+    if (drop_recs > 0) {
+        const long drop = drop_recs * npb, kept = pk_bytes - drop, nrecs = kept / npb;
+        if (kept > 0) {
+            B200_CUDA(cudaMemcpyAsync(pk_tmp.p, (uint8_t *)pk.p + drop, kept, cudaMemcpyDeviceToDevice, stream));
+            B200_CUDA(cudaMemcpyAsync(pk.p, pk_tmp.p, kept, cudaMemcpyDeviceToDevice, stream));
+            B200_CUDA(cudaMemcpyAsync(pk_tmp.p, pk_read.p + drop_recs, nrecs * 4, cudaMemcpyDeviceToDevice, stream));
+            B200_CUDA(cudaMemcpyAsync(pk_read.p, pk_tmp.p, nrecs * 4, cudaMemcpyDeviceToDevice, stream));
+        }
+        pk_bytes = kept;
+        pbase += 8LL * drop;
+    }
+    const long used = (long)(R - pos0);
+    f.keep_soft_tail(used);
+    end(f);
+    pos0 = R;
+    tail_seen = f.soft_have;
+    last_nf = nrec;
+    f.out_frames += nf;
+    f.total_frames += nf;
+    f.total_bits += used;
 }
 
 // frames in frames_out [0, out0) keep their bits; what left frames_out without a pull (b200_chain) is forgotten

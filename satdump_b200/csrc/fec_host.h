@@ -64,6 +64,7 @@ std::unique_ptr<Framed> dump_decoder(Fec &f);
 std::unique_ptr<Framed> meteor_decoder(Fec &f);
 std::unique_ptr<Framed> sync_walk_decoder(Fec &f); // noaa_hrpt_decoder, meteor_hrpt_decoder, dmsp_rtd_decoder (api_hrpt.cu)
 std::unique_ptr<Framed> bit_stage_decoder(Fec &f); // aqua_db_decoder, noaa_gac_decoder (api_hrpt.cu)
+std::unique_ptr<Framed> xband_decoder(Fec &f);     // meteor_xband_decoder (api_hrpt.cu)
 
 class Fec
 {

@@ -16,6 +16,8 @@ static void print_hrpt_stats(const std::string &dec, long frames, int state)
         printf("frame_count %ld\n", frames / 11090);
     if (dec == "dmsp_rtd_decoder")
         printf("deframer_state %s\n", state == 0 ? "NOSYNC" : (state == 2 ? "SYNCING" : "SYNCED"));
+    if (dec == "meteor_xband_decoder")
+        printf("frame_count %ld\n", frames);
     if (dec == "aqua_db_decoder")
         printf("deframer_state %s\n", state == 2 ? "NOSYNC" : (state == 6 ? "SYNCING" : "SYNCED"));
     if (dec == "noaa_hrpt_decoder")
@@ -28,7 +30,7 @@ static void print_hrpt_stats(const std::string &dec, long frames, int state)
 int main(int argc, char **argv)
 {
     if (argc < 5) {
-        fprintf(stderr, "usage: %s <metop_ahrpt|jpss_hrd|npp_hrd|simple_bpsk|simple_qpsk|pm_bpsk|ldpc_qpsk|landsat|turbo_pm|turbo_bpsk|metop_dump|meteor_lrpt|noaa_hrpt|meteor_hrpt|noaa_gac|dmsp_rtd|aqua_db|aura_db|terra_db|bluewalker3_wide|bluewalker3_narrow> baseband <input> <output_hint> [--fused] [--key value ...]\n", argv[0]);
+        fprintf(stderr, "usage: %s <metop_ahrpt|jpss_hrd|npp_hrd|simple_bpsk|simple_qpsk|pm_bpsk|ldpc_qpsk|landsat|turbo_pm|turbo_bpsk|metop_dump|meteor_lrpt|noaa_hrpt|meteor_hrpt|noaa_gac|dmsp_rtd|meteor_mtvza|meteor_kmss_bpsk|aqua_db|aura_db|terra_db|bluewalker3_wide|bluewalker3_narrow> baseband <input> <output_hint> [--fused] [--key value ...]\n", argv[0]);
         return 2;
     }
     const std::string pipe = argv[1], level = argv[2], in = argv[3], out = argv[4];
@@ -54,6 +56,14 @@ int main(int argc, char **argv)
             dp = Params{{"constellation", "bpsk"}, {"symbolrate", "1024000"}, {"rrc_alpha", "0.5"}, {"pll_bw", "0.005"}};
             dec = "dmsp_rtd_decoder";
         }
+    } else if (pipe == "meteor_mtvza" || pipe == "meteor_kmss_bpsk") { // resources/pipelines/Meteor-M.json "meteor_m_mtvza_dump",
+        // "meteor_m_kmss_bpsk_db": psk_demod BPSK at 15.36 | 61.44 Msym/s (rrc_alpha 0.6, pll_bw 0.004, rrc_taps 31); the pipelines name no
+        // samplerate: it comes from the command line
+        const bool kmss = pipe == "meteor_kmss_bpsk";
+        dp = Params{{"constellation", "bpsk"}, {"symbolrate", kmss ? "61440000" : "15360000"}, {"rrc_alpha", "0.6"}, {"pll_bw", "0.004"},
+                    {"rrc_taps", "31"}};
+        fp = Params{{"instrument_type", kmss ? "kmss_bpsk" : "mtvza"}};
+        dec = "meteor_xband_decoder";
     } else if (pipe == "noaa_hrpt" || pipe == "meteor_hrpt") { // resources/pipelines/NOAA.json "noaa_hrpt", Meteor-M.json "meteor_hrpt":
         // pm_demod at 665 400 sym/s (pll_bw 0.01, rrc_alpha 0.6 | 0.5, clock_omega_relative_limit 0.001), 3 MS/s by default
         const bool noaa = pipe == "noaa_hrpt";

@@ -411,6 +411,20 @@ b200_fec_cfg fec_cfg_from_params(const std::string &id, const Params &p)
         c.cadu_size = 150;
         return c;
     }
+    if (id == "meteor_xband_decoder") { // module_meteor_xband_decoder.cpp:14-32, meteor_xband_types.h: instrument_type "mtvza" | "kmss_bpsk"
+        c.kind = B200_FEC_METEOR_XBAND;
+        c.device = (int)p.num("b200_device", 0);
+        c.constellation = B200_BPSK;
+        const std::string t = p.has("instrument_type") ? p.str("instrument_type") : "";
+        if (t != "mtvza" && t != "kmss_bpsk")
+            throw ModuleError("Invalid METEOR instrument type!");
+        c.instrument_type = t == "kmss_bpsk";
+        c.cadu_size = c.instrument_type ? 481280 : 3040; // one output unit = one .frm record: 60160 | 380 bytes
+        // SoftSymbolReader's hard_symbols path starts from an uninitialised buffer (DESIGN §10.5)
+        if (p.flag("hard_symbols", false))
+            throw ModuleError("meteor_xband_decoder: hard_symbols input is not supported by the B200 path");
+        return c;
+    }
     if (id == "aqua_db_decoder") { // module_aqua_db_decoder.cpp:16-22: no parameters; 1024-byte CADUs (Aqua and Aura DB)
         c.kind = B200_FEC_AQUA_DB;
         c.device = (int)p.num("b200_device", 0);
@@ -720,7 +734,7 @@ static std::string frame_file(const b200_fec_cfg &c, const std::string &hint, bo
 {
     if (c.kind == B200_FEC_NOAA_GAC)
         return hint + (c.backward ? ".frm.tmp" : ".frm");
-    if (c.kind == B200_FEC_DMSP_RTD)
+    if (c.kind == B200_FEC_DMSP_RTD || c.kind == B200_FEC_METEOR_XBAND)
         return hint + ".frm";
     return hint + (c.kind == B200_FEC_NOAA_HRPT ? ".raw16" : (ccsds ? ".cadu" : ".frm"));
 }
@@ -884,7 +898,8 @@ void FusedStage::process()
     const uint64_t fsz = file_size(input_file);
     if (data_offset)
         fseek(fin, (long)data_offset, SEEK_SET);
-    output_file = (fcfg.kind == B200_FEC_NOAA_GAC || fcfg.kind == B200_FEC_DMSP_RTD) ? frame_file(fcfg, output_hint, true)
+    output_file = (fcfg.kind == B200_FEC_NOAA_GAC || fcfg.kind == B200_FEC_DMSP_RTD || fcfg.kind == B200_FEC_METEOR_XBAND)
+                      ? frame_file(fcfg, output_hint, true)
                                                                                    : output_hint + (fcfg.kind == B200_FEC_NOAA_HRPT ? ".raw16" : ".cadu");
     FILE *fout = fopen(output_file.c_str(), "wb");
     if (fcfg.kind == B200_FEC_NOAA_GAC)

@@ -339,6 +339,13 @@ CONFIGS = {
                           fmt="cs16", decoder="noaa_gac", esn0_db=15.0, carrier_rad=1e-4, phase0=0.1, post_costas_dc=True),
     "dmsp_rtd": SignalCfg(name="dmsp_rtd", samplerate=2e6, symbolrate=1024000, constellation="bpsk", conv="none", rrc_alpha=0.5, pll_bw=0.005,
                           fmt="cs16", decoder="dmsp_rtd", esn0_db=15.0, carrier_rad=1e-4, phase0=0.1),
+    # psk_demod BPSK -> meteor_xband_decoder (Meteor-M.json "meteor_m_mtvza_dump", "meteor_m_kmss_bpsk_db"): NRZ-M record streams at
+    # 15.36 and 61.44 Msym/s, recorded at two samples per symbol
+    "meteor_mtvza": SignalCfg(name="meteor_mtvza", samplerate=30.72e6, symbolrate=15360000, constellation="bpsk", conv="none", rrc_alpha=0.6,
+                              pll_bw=0.004, fmt="cs16", decoder="meteor_mtvza", esn0_db=15.0, carrier_rad=1e-4, phase0=0.1),
+    "meteor_kmss_bpsk": SignalCfg(name="meteor_kmss_bpsk", samplerate=122.88e6, symbolrate=61440000, constellation="bpsk", conv="none",
+                                  rrc_alpha=0.6, pll_bw=0.004, fmt="cs16", decoder="meteor_kmss_bpsk", esn0_db=15.0, carrier_rad=1e-4,
+                                  phase0=0.1),
     "terra_db": SignalCfg(name="terra_db", samplerate=45e6, symbolrate=26250000, constellation="bpsk", conv="none", interleave=4, rrc_alpha=0.5,
                           pll_bw=0.004, fmt="cs16", decoder="terra_db", esn0_db=12.0, carrier_rad=1e-4, phase0=0.1, clock_alpha=0.001),
 }
@@ -399,6 +406,8 @@ def make_bitstream(cfg: SignalCfg, nframes, seed):
         return coded, clear
     if cfg.decoder == "terra_db":  # nframes CADUs, NRZ-M, r=1/2: one BPSK symbol per code symbol
         return terra_db_frames(nframes, seed)
+    if cfg.decoder in ("meteor_mtvza", "meteor_kmss_bpsk"):  # nframes inner frames in records, NRZ-M
+        return meteor_xband_frames(cfg.decoder == "meteor_kmss_bpsk", nframes, seed)
     if cfg.decoder == "ldpc":  # nframes LDPC frames
         if cfg.internal_cadu_size:
             info, clear = ldpc_inner_frames(nframes, cfg.internal_cadu_size, cfg.internal_asm, seed)
@@ -522,6 +531,9 @@ def frames_for_samples(cfg: SignalCfg, nsamples):
         return int(nsamples / (cfg.samplerate / cfg.symbolrate) / (NOAA_WORDS * 10 if cfg.decoder == "noaa_hrpt" else 8192)) + 2
     if cfg.decoder in ("noaa_gac", "dmsp_rtd"):  # bits on air: 33270 per GAC frame, 150 per DMSP frame
         return int(nsamples / (cfg.samplerate / cfg.symbolrate) / (GAC_BITS if cfg.decoder == "noaa_gac" else DMSP_BITS)) + 2
+    if cfg.decoder in ("meteor_mtvza", "meteor_kmss_bpsk"):  # bits on air per inner frame: its share of the records
+        per = MTVZA_FRM * 8 * 384 / 368 if cfg.decoder == "meteor_mtvza" else KMSS_FRM * 8 * 1536 / 1504
+        return int(nsamples / (cfg.samplerate / cfg.symbolrate) / per) + 2
     if cfg.decoder == "terra_db":  # 16384 code symbols per CADU, one per sample period of the half-symbol rate
         return int(nsamples / (cfg.samplerate / cfg.symbolrate) / 16384) + 2
     if cfg.decoder in ("ldpc", "dump", "aqua_db"):  # LDPC frames / MetOp dump and Aqua DB CADUs of 8192 bits
@@ -930,6 +942,70 @@ def dmsp_frames(nframes, seed=0):
     bits = np.random.default_rng(seed).integers(0, 2, size=(nframes, DMSP_BITS)).astype(np.uint8)
     bits[:, :13] = (DMSP_ASM >> np.arange(12, -1, -1)) & 1
     return bits, frame_image(bits, DMSP_BYTES)
+
+
+# ---- METEOR-M X-band dumps (meteor_xband_decoder) -------------------------------------------------------------------------------------
+MTVZA_FRM, KMSS_FRM = 380, 60160
+MTVZA_SYNC = bytes.fromhex("38FB456A")
+KMSS_SYNCS = [bytes.fromhex("AF5FFF50AA5AA0"), bytes.fromhex("AE5EEC61BB7982"), bytes.fromhex("AB5BB394EED628")]
+
+
+def kmss_frame_process(frame, d):
+    """kmssFrameProcessor (module_meteor_xband_decoder.cpp:44-53) on one 60160-byte frame of deframer d (0, 1, 2), with the module's lane
+    moves for deframers 2 and 3: the 60160 bytes the module writes"""
+    b = np.unpackbits(np.asarray(frame, np.uint8) ^ 0xF0).reshape(KMSS_FRM // 4, 4, 2, 4)  # [c, byte i, nibble, bit in nibble]
+    lanes = np.packbits(b.transpose(3, 0, 1, 2).reshape(4, -1), axis=1)  # lane o: bits o and 4 + o of bytes 4c .. 4c + 3
+    if d:
+        mv = [2, 3] if d == 1 else [0, 1]
+        lanes[mv, 1:] = lanes[mv, :-1].copy()
+    return lanes.reshape(-1)
+
+
+def meteor_xband_records(kmss, packets, rng):
+    """Records carrying the packet stream `packets` (a whole number of records' worth): MTVZA 384 bytes with its four patterns and eight
+    46-byte packets XOR 0xAA at byte 2 + 48k; KMSS 1536 bytes with 0x0035 at its start, zeros at byte 382 and eight 188-byte packets at
+    byte 2 + 192k. The bytes between the packets are random where no pattern lies."""
+    P, stride, size = (188, 192, 1536) if kmss else (46, 48, 384)
+    pk = np.asarray(packets, np.uint8).reshape(-1, 8, P)
+    rec = rng.integers(0, 256, size=(pk.shape[0], size), dtype=np.uint8)
+    for k in range(8):
+        rec[:, 2 + stride * k:2 + stride * k + P] = pk[:, k] if kmss else pk[:, k] ^ 0xAA
+    if kmss:
+        rec[:, 0], rec[:, 1], rec[:, 382:386] = 0x00, 0x35, 0
+    else:
+        rec[:, 0], rec[:, 48], rec[:, 96], rec[:, 240] = 0xB3, 0xE3, 0x75, 0
+        rec[:, 241] &= 0x7F
+    return rec
+
+
+def meteor_xband_frames(kmss, nframes, seed=0, cut=None):
+    """(bits on air uint8: the records NRZ-M encoded; the frames meteor_xband_decoder writes, [n, 380] | [n, 60160]). Inner frames are the
+    sync and random bytes (KMSS: the three deframers' syncs in turn). cut = (k, nbytes): frame k is sent only up to nbytes, so the next
+    sync cuts it and the decoder writes it filled with zeros after that sync."""
+    rng = np.random.default_rng(seed)
+    F = KMSS_FRM if kmss else MTVZA_FRM
+    frames = rng.integers(0, 256, size=(nframes, F), dtype=np.uint8)
+    ds = [i % 3 if kmss else 0 for i in range(nframes)]
+    if kmss and cut is not None and cut[0] + 1 < nframes:  # (the cut frame is followed by one of the same deframer)
+        ds = ds[:cut[0] + 1] + [(d + 2) % 3 for d in ds[cut[0] + 1:]]
+    syncs = [KMSS_SYNCS[d] if kmss else MTVZA_SYNC for d in ds]
+    for i in range(nframes):
+        frames[i, :len(syncs[i])] = np.frombuffer(syncs[i], np.uint8)
+    sent, written = [], []
+    for i in range(nframes):
+        f = w = frames[i]
+        if cut is not None and cut[0] == i and i + 1 < nframes:
+            f = f[:cut[1]]
+            w = np.zeros(F, np.uint8)
+            w[:cut[1]] = f
+            w[cut[1]:cut[1] + len(syncs[i + 1])] = np.frombuffer(syncs[i + 1], np.uint8)
+        sent.append(f)
+        written.append(kmss_frame_process(w, ds[i]) if kmss else w)
+    stream = np.concatenate(sent)
+    npb = 1504 if kmss else 368
+    stream = np.concatenate([stream, rng.integers(0, 256, size=(-stream.size) % npb + npb, dtype=np.uint8)])
+    rec = meteor_xband_records(kmss, stream, rng)
+    return nrzm_encode(np.unpackbits(rec.reshape(-1))), np.stack(written)
 
 
 # ---- EOS Aqua / Aura DB (aqua_db_decoder): randomised CADUs on two NRZ-M rails -----------------------------------------------------------

@@ -89,6 +89,15 @@ static b200_fec_cfg meteor_m2x_as_ccsds(const b200_fec_cfg &c)
     return r;
 }
 
+// Most deframer state changes (k_deframe's event list) a walk over `max_bits` FIFO bits can record. Every NOSYNC -> SYNCING change
+// opens a frame whose cadu_size - 32 payload bits the walk skips before it tests again, and at most two changes follow it (SYNCING ->
+// SYNCED -> NOSYNC, or SYNCING -> NOSYNC); the state a push starts in adds at most two more. A noisy stream that loses and finds the
+// ASM every few frames stays within this, at any push size.
+static long defr_event_cap(long max_bits, int cadu_size)
+{
+    return 3 * (max_bits / std::max(1, cadu_size - 32) + 2);
+}
+
 Fec::Fec(const b200_fec_cfg &in) : cfg(meteor_m2x_as_ccsds(in))
 {
     const b200_fec_cfg c = cfg;
@@ -217,7 +226,8 @@ Fec::Fec(const b200_fec_cfg &in) : cfg(meteor_m2x_as_ccsds(in))
     h_idle2.alloc(1);
     B200_CUDA(cudaFuncSetAttribute(k_vit_idle2, cudaFuncAttributeMaxDynamicSharedMemorySize, 8 * VIT_IDLE_WARP_BYTES));
     dstate.alloc(2);
-    devents.alloc(4096);
+    max_events = defr_event_cap(32L * (long)fifo.n, cfg.cadu_size);
+    devents.alloc((size_t)max_events);
     if (simple) {
         chunk_bits2.alloc((size_t)max_chunks * geom.bit_words + 4);
         fifo2.alloc(fifo.n);
@@ -236,7 +246,7 @@ Fec::Fec(const b200_fec_cfg &in) : cfg(meteor_m2x_as_ccsds(in))
     h_idle.alloc(1);
     h_counters.alloc(8);
     h_dstate.alloc(2);
-    h_events.alloc(4096);
+    h_events.alloc((size_t)max_events);
     h_rs_err.alloc((size_t)(max_frames_push + 4) * std::max(1, cfg.rs_i));
     RsTables T;
     build_rs_tables(T);
@@ -595,16 +605,17 @@ void Fec::deframe_and_rs(long new_bits)
     const long nbits = fifo_bits + new_bits;
     B200_CUDA(cudaEventRecord(evf[0], stream));
     k_deframe<<<1, 32, 0, stream>>>(fifo.p, nbits, cfg.cadu_size, st_synced, cfg.asm_sync, dstate.p, frames.p, (int)max_frames_push,
-                                   reinterpret_cast<DefrEventDev *>(devents.p), 4096, counters.p);
+                                   reinterpret_cast<DefrEventDev *>(devents.p), (int)max_events, counters.p);
     launches++;
     B200_CUDA(cudaMemcpyAsync(h_counters.p, counters.p, sizeof(int) * 2, cudaMemcpyDeviceToHost, stream));
     B200_CUDA(cudaMemcpyAsync(h_dstate.p, dstate.p, sizeof(DefrState), cudaMemcpyDeviceToHost, stream));
-    B200_CUDA(cudaMemcpyAsync(h_events.p, devents.p, sizeof(DefrEvent) * 4096, cudaMemcpyDeviceToHost, stream));
     B200_CUDA(cudaStreamSynchronize(stream));
-    const int nf = h_counters.p[0];
+    const int nf = h_counters.p[0], ne = h_counters.p[1];
     last_nf = nf;
     B200_REQUIRE(nf <= max_frames_push, B200_ESTATE, "internal: frame list overflow");
-    B200_REQUIRE(h_counters.p[1] <= 4096, B200_EUNSUPPORTED, "deframer changed state more than 4096 times in one push (noise input?): push smaller batches");
+    B200_REQUIRE(ne <= max_events, B200_ESTATE, "internal: %d deframer state changes in one push, more than the %ld its bits allow", ne, max_events);
+    if (ne > 0) // (complete at the event synchronise below)
+        B200_CUDA(cudaMemcpyAsync(h_events.p, devents.p, sizeof(DefrEvent) * ne, cudaMemcpyDeviceToHost, stream));
     if (nf > 0) {
         B200_REQUIRE((size_t)(out_frames + nf) * cadu_bytes <= frames_out.n, B200_ESTATE, "frame output buffer full: call pull_frames");
         FrameCfg fc;
@@ -807,7 +818,8 @@ void Fec::deframer_storage(long max_new_bits)
 {
     fifo.alloc((size_t)((max_new_bits + 2L * cfg.cadu_size + 4096) / 32 + 8));
     dstate.alloc(2);
-    devents.alloc(4096);
+    max_events = defr_event_cap(32L * (long)fifo.n, cfg.cadu_size);
+    devents.alloc((size_t)max_events);
     max_frames_push = max_new_bits / cfg.cadu_size + 4;
     frames.alloc(max_frames_push);
     frames_out.alloc((size_t)(2 * max_frames_push + 4) * cadu_bytes);
@@ -818,7 +830,7 @@ void Fec::deframer_storage(long max_new_bits)
     tables.alloc(1);
     h_counters.alloc(8);
     h_dstate.alloc(2);
-    h_events.alloc(4096);
+    h_events.alloc((size_t)max_events);
     h_rs_err.alloc((size_t)(max_frames_push + 4) * std::max(1, cfg.rs_i));
     RsTables T;
     build_rs_tables(T);

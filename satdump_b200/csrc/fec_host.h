@@ -170,6 +170,7 @@ class Fec
 
     // stream state
     long soft_have = 0, max_chunks = 0, fifo_bits = 32, max_frames_push = 0;
+    long max_events = 0; // deframer state changes one push can make (defr_event_cap)
     long swapped = 0; // bpsk_90 / iq_invert: FIFO bytes whose pairs are already swapped
     int vit_state = 0, invalid = 0, main_next_start = -1, enc_state = 0, nrzm_last = 0, nosync_runs = 0;
     VitHyp hyp{0, 0, 0};

@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE ONLY — ctypes bindings of the checkers of the MetOp X-band dump decoder (metop_dump_decoder):
 
-  impl "ref"   oracle/_ref/libsatref_dump.so: the unmodified reference translation units + oracle/dump_harness.cpp (oracle/dump.mk)
+  impl "ref"   oracle/_ref/libsatref_dump.so: the unmodified reference translation units + oracle/dump_harness.cpp (oracle/Makefile)
   impl "port"  oracle/libdump_port.so: our own C restatement (oracle/dump_port.c), pinned to "ref" by tests/test_metop_dump_oracle.py
 
 Both export the same C ABI (prefix ref_ / orc_). impl=None means "ref". Where "ref" was not built (the reference is absent) the tests read
@@ -11,47 +11,24 @@ import os
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_PATHS = {"ref": (os.path.join(_HERE, "_ref", "libsatref_dump.so"), "ref_"), "port": (os.path.join(_HERE, "libdump_port.so"), "orc_")}
+from . import _checker
+from ._checker import HERE, Handle, Library, ref_path
+
 F = 8192
 CADU = 1024
 REC = ("offset", "pos", "corr", "phase", "swap", "rs0", "rs1", "rs2", "rs3")
 
-
-def available(impl="ref"):
-    return os.path.exists(_PATHS[impl][0])
-
-
-_libs = {}
+vp, cl = C.c_void_p, C.c_long
+lib = Library({"ref": (ref_path("dump"), "ref_"), "port": (os.path.join(HERE, "libdump_port.so"), "orc_")},
+              [("dump_create", vp, []), ("dump_destroy", None, [vp]), ("dump_run", cl, [vp, vp, cl, vp, cl, C.POINTER(cl), vp, cl])])
+available = lib.available
 
 
-def lib(impl="ref"):
-    """{name without prefix: function}"""
-    if impl not in _libs:
-        path, pfx = _PATHS[impl]
-        L = C.CDLL(path)
-        vp, cl = C.c_void_p, C.c_long
-        fn = {}
-        for name, res, args in [("dump_create", vp, []), ("dump_destroy", None, [vp]),
-                                ("dump_run", cl, [vp, vp, cl, vp, cl, C.POINTER(cl), vp, cl])]:
-            f = getattr(L, pfx + name)
-            f.restype, f.argtypes = res, args
-            fn[name] = f
-        _libs[impl] = fn
-    return _libs[impl]
-
-
-class Dump:
+class Dump(Handle):
     """The module loop over a soft stream; run() may be called repeatedly (the stream continues, like ragged pushes)."""
 
     def __init__(self, impl="ref"):
-        self.L = lib(impl)
-        self.h = self.L["dump_create"]()
-
-    def __del__(self):
-        if getattr(self, "h", None):
-            self.L["dump_destroy"](self.h)
-            self.h = None
+        super().__init__(lib(impl), "dump")
 
     def run(self, soft):
         """Returns cadu (uint8 [frames, 1024], every frame) and recs (int64 [n, 9], columns REC)."""
@@ -67,10 +44,4 @@ class Dump:
 
 def run_pieces(soft, cuts=(), impl="ref"):
     """One decoder over soft pushed in the pieces cut at `cuts`; the concatenated results."""
-    d = Dump(impl)
-    cadu, recs = [], []
-    for a, b in zip([0, *cuts], [*cuts, soft.size]):
-        r = d.run(soft[a:b])
-        cadu.append(r["cadu"])
-        recs.append(r["recs"])
-    return dict(cadu=np.concatenate(cadu), recs=np.concatenate(recs))
+    return _checker.run_pieces(Dump(impl), soft, cuts)

@@ -3,7 +3,7 @@
  *
  * oracle/_ref MetOp dump harness: wires the UNMODIFIED reference translation units of the MetOp X-band dump decoder's parts
  * (correlator32.cpp, rotation.cpp, randomization.cpp, reedsolomon.cpp and libcorrect's Reed-Solomon, compiled from the reference tree by
- * oracle/dump.mk) the way
+ * oracle/Makefile) the way
  *   metop::MetOpDumpDecoderModule::process   plugins/noaa_metop_support/metop/module_metop_dump_decoder.cpp:27-83
  * runs them, and exposes them through a small C ABI for the Python tests (oracle/dump.py).
  *

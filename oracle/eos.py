@@ -1,51 +1,31 @@
 """TEST INFRASTRUCTURE ONLY — ctypes bindings of the checker of the Aqua / Aura DB decoder (aqua_db_decoder):
 
-  oracle/_ref/libsatref_eos.so: the unmodified reference blocks + oracle/eos_harness.cpp (oracle/eos.mk)
+  oracle/_ref/libsatref_eos.so: the unmodified reference blocks + oracle/eos_harness.cpp (oracle/Makefile)
 
 Where it was not built (the reference is absent) the tests read tests/golden/eos_pins.json.
 """
 import ctypes as C
-import os
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-PATH = os.path.join(_HERE, "_ref", "libsatref_eos.so")
+from . import _checker
+from ._checker import Handle, Library, ref_path
+
 CADU = 1024
 READ = 65536
 
-
-def available():
-    return os.path.exists(PATH)
-
-
-_lib = None
+vp, cl = C.c_void_p, C.c_long
+lib = Library({"ref": (ref_path("eos"), "ref_")}, [("aqua_create", vp, []), ("aqua_destroy", None, [vp]),
+                                                  ("aqua_run", C.c_int, [vp, vp, cl, vp, cl, C.POINTER(cl), vp, cl, vp])])
+available = lib.available
 
 
-def lib():
-    global _lib
-    if _lib is None:
-        L = C.CDLL(PATH)
-        vp, cl = C.c_void_p, C.c_long
-        for name, res, args in [("ref_aqua_create", vp, []), ("ref_aqua_destroy", None, [vp]),
-                                ("ref_aqua_run", C.c_int, [vp, vp, cl, vp, cl, C.POINTER(cl), vp, cl, vp])]:
-            f = getattr(L, name)
-            f.restype, f.argtypes = res, args
-        _lib = L
-    return _lib
-
-
-class Aqua:
+class Aqua(Handle):
     """The module loop of aqua_db_decoder over 65 536-byte reads; run() may be called repeatedly (the stream continues, and bytes short of
     a whole read wait for the next call)."""
 
     def __init__(self):
-        self.h = lib().ref_aqua_create()
-
-    def __del__(self):
-        if getattr(self, "h", None):
-            lib().ref_aqua_destroy(self.h)
-            self.h = None
+        super().__init__(lib(), "aqua")
 
     def run(self, soft):
         """Returns cadu (uint8 [frames, 1024]), rs (int32 [frames, 4]: decode_interlaved's errors[]) and stats (frames written so far,
@@ -56,7 +36,7 @@ class Aqua:
         rs = np.zeros(nf * 4, np.int32)
         st = np.zeros(5, np.int64)
         nb = C.c_long(0)
-        assert lib().ref_aqua_run(self.h, soft.ctypes.data, soft.size, out.ctypes.data, out.size, C.byref(nb), rs.ctypes.data, rs.size,
+        assert self.L["aqua_run"](self.h, soft.ctypes.data, soft.size, out.ctypes.data, out.size, C.byref(nb), rs.ctypes.data, rs.size,
                                   st.ctypes.data) == 0
         k = nb.value // CADU
         return dict(cadu=out[:nb.value].reshape(-1, CADU).copy(), rs=rs[:4 * k].reshape(-1, 4).copy(),
@@ -65,11 +45,4 @@ class Aqua:
 
 def run_pieces(soft, cuts=()):
     """One decoder over soft pushed in the pieces cut at `cuts`: the concatenated CADUs and RS results, and the stats after every piece."""
-    d = Aqua()
-    cadu, rs, stats = [], [], []
-    for a, b in zip([0, *cuts], [*cuts, soft.size]):
-        r = d.run(soft[a:b])
-        cadu.append(r["cadu"])
-        rs.append(r["rs"])
-        stats.append(r["stats"])
-    return dict(cadu=np.concatenate(cadu), rs=np.concatenate(rs), stats=stats)
+    return _checker.run_pieces(Aqua(), soft, cuts)

@@ -2,7 +2,7 @@
  * TEST INFRASTRUCTURE ONLY — never linked into or called from the product path.
  *
  * oracle/_ref EOS harness: wires the UNMODIFIED reference blocks dsp::constellation_t (QPSK soft_demod), diff::NRZMDiff,
- * deframing::BPSK_CCSDS_Deframer, derand_ccsds and reedsolomon::ReedSolomon, compiled from the reference tree by oracle/eos.mk, the way
+ * deframing::BPSK_CCSDS_Deframer, derand_ccsds and reedsolomon::ReedSolomon, compiled from the reference tree by oracle/Makefile, the way
  *   aqua::AquaDBDecoderModule::process  plugins/eos_support/aqua/module_aqua_db_decoder.cpp:27-83
  * runs them: 65 536-byte reads, the deframer with STATE_SYNCING 6 and STATE_SYNCED 10, every frame derandomised, RS-decoded and written.
  * The module file pulls in ImGui and the pipeline base, so its loop is restated here as wiring. The stream reader hands the loop whole

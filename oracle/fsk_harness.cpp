@@ -2,7 +2,7 @@
  * TEST INFRASTRUCTURE ONLY — never linked into or called from the product path.
  *
  * oracle/_ref/libsatref_fsk.so harness: wires the UNMODIFIED reference blocks of fsk_demod (compiled from the reference tree by
- * oracle/fsk.mk) the way FSKDemodModule does, behind BaseDemodModule's AGC:
+ * oracle/Makefile) the way FSKDemodModule does, behind BaseDemodModule's AGC:
  *   FSKDemodModule::init / process    src-core/pipeline/modules/demod/module_fsk_demod.cpp:59-158
  *   BaseDemodModule::initb (AGC)      src-core/pipeline/modules/demod/module_demod_base.cpp:207
  * and exposes every stage's output, the symbols, the soft bytes and the per-read SNR through a small C ABI.

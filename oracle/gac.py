@@ -1,59 +1,39 @@
 """TEST INFRASTRUCTURE ONLY — ctypes bindings of the checker of the NOAA GAC and DMSP RTD decoders (noaa_gac_decoder, dmsp_rtd_decoder):
 
-  oracle/_ref/libsatref_gac.so: the unmodified reference deframers + oracle/gac_harness.cpp (oracle/gac.mk)
+  oracle/_ref/libsatref_gac.so: the unmodified reference deframers + oracle/gac_harness.cpp (oracle/Makefile)
 
 Where it was not built (the reference is absent) the tests read tests/golden/gac_pins.json.
 """
 import ctypes as C
-import os
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-PATH = os.path.join(_HERE, "_ref", "libsatref_gac.so")
+from . import _checker
+from ._checker import Handle, Library, ref_path
+
 GAC_BYTES, DMSP_BYTES = 4159, 19
 
-
-def available():
-    return os.path.exists(PATH)
-
-
-_lib = None
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        L = C.CDLL(PATH)
-        vp, cl = C.c_void_p, C.c_long
-        for name, res, args in [("ref_gac_pn_table", None, [vp]), ("ref_gac_create", vp, [C.c_int, C.c_int, C.c_double]),
-                                ("ref_gac_destroy", None, [vp]),
-                                ("ref_gac_run", C.c_int, [vp, vp, cl, vp, cl, C.POINTER(cl), vp, cl, C.POINTER(cl), vp])]:
-            f = getattr(L, name)
-            f.restype, f.argtypes = res, args
-        _lib = L
-    return _lib
+vp, cl = C.c_void_p, C.c_long
+lib = Library({"ref": (ref_path("gac"), "ref_")},
+              [("gac_pn_table", None, [vp]), ("gac_create", vp, [C.c_int, C.c_int, C.c_double]), ("gac_destroy", None, [vp]),
+               ("gac_run", C.c_int, [vp, vp, cl, vp, cl, C.POINTER(cl), vp, cl, C.POINTER(cl), vp])])
+available = lib.available
 
 
 def pn_table():
     """the reference's gac_rand_bits (1023 entries, 0 / 1)"""
     out = np.zeros(1023, np.uint8)
-    lib().ref_gac_pn_table(out.ctypes.data)
+    lib()["gac_pn_table"](out.ctypes.data)
     return out
 
 
-class Ref:
+class Ref(Handle):
     """The module loop of noaa_gac_decoder (dmsp False, `backward`) or dmsp_rtd_decoder (dmsp True, start_timestamp, -1: none); run() may
     be called repeatedly (the stream continues; only whole 8192-byte reads from the stream's start are decoded)."""
 
     def __init__(self, dmsp, backward=False, start_timestamp=-1.0):
         self.dmsp = bool(dmsp)
-        self.h = lib().ref_gac_create(int(self.dmsp), int(bool(backward)), float(start_timestamp))
-
-    def __del__(self):
-        if getattr(self, "h", None):
-            lib().ref_gac_destroy(self.h)
-            self.h = None
+        super().__init__(lib(), "gac", int(self.dmsp), int(bool(backward)), float(start_timestamp))
 
     def run(self, soft):
         """frames uint8 [n, 4159 | 19] in decode order, ts (DMSP timestamps, float64) and stats (frames so far, state)"""
@@ -64,7 +44,7 @@ class Ref:
         ts = np.zeros(soft.size // 100 + 128, np.float64)
         st = np.zeros(2, np.int64)
         nb, nt = C.c_long(0), C.c_long(0)
-        rc = lib().ref_gac_run(self.h, soft.ctypes.data, soft.size, out.ctypes.data, cap, C.byref(nb), ts.ctypes.data, ts.size, C.byref(nt),
+        rc = self.L["gac_run"](self.h, soft.ctypes.data, soft.size, out.ctypes.data, cap, C.byref(nb), ts.ctypes.data, ts.size, C.byref(nt),
                                st.ctypes.data)
         assert rc == 0
         return dict(out=out[:nb.value].reshape(-1, nbytes).copy(), ts=ts[:nt.value].copy(), stats=dict(frames=int(st[0]), state=int(st[1])))
@@ -72,11 +52,4 @@ class Ref:
 
 def run_pieces(soft, cuts=(), dmsp=False, backward=False, start_timestamp=-1.0):
     """One decoder over soft pushed in the pieces cut at `cuts`: the concatenated frames and timestamps, and the stats after every piece."""
-    d = Ref(dmsp, backward, start_timestamp)
-    out, ts, stats = [], [], []
-    for a, b in zip([0, *cuts], [*cuts, soft.size]):
-        r = d.run(soft[a:b])
-        out.append(r["out"])
-        ts.append(r["ts"])
-        stats.append(r["stats"])
-    return dict(out=np.concatenate(out), ts=np.concatenate(ts), stats=stats)
+    return _checker.run_pieces(Ref(dmsp, backward, start_timestamp), soft, cuts)

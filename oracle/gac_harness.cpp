@@ -3,7 +3,7 @@
  *
  * oracle/_ref GAC / DMSP harness: wires the UNMODIFIED reference deframers deframing::BPSK_CCSDS_Deframer
  * (src-core/common/codings/deframing/bpsk_ccsds_deframer.cpp) and dmsp::DMSP_Deframer (plugins/dmsp_support/dmsp/dmsp_deframer.cpp),
- * compiled from the reference tree by oracle/gac.mk, the way
+ * compiled from the reference tree by oracle/Makefile, the way
  *   noaa::NOAAGACDecoderModule::process   plugins/noaa_metop_support/noaa/module_noaa_gac_decoder.cpp:30-133
  *   dmsp::DMSPRTDDecoderModule::process   plugins/dmsp_support/dmsp/module_dmsp_rtd_decoder.cpp:34-70
  * run them, and exposes them through a small C ABI for the Python tests (oracle/gac.py). The module files pull in ImGui and the pipeline

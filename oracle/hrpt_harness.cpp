@@ -2,7 +2,7 @@
  * TEST INFRASTRUCTURE ONLY — never linked into or called from the product path.
  *
  * oracle/_ref HRPT harness: wires the UNMODIFIED reference deframers noaa::NOAADeframer (noaa_metop_support/noaa/noaa_deframer.cpp) and
- * meteor::CADUDeframer (meteor_support/meteor/deframer.cpp), compiled from the reference tree by oracle/hrpt.mk, the way
+ * meteor::CADUDeframer (meteor_support/meteor/deframer.cpp), compiled from the reference tree by oracle/Makefile, the way
  *   noaa::NOAAHRPTDecoderModule::process      plugins/noaa_metop_support/noaa/module_noaa_hrpt_decoder.cpp:26-45
  *   meteor::METEORHRPTDecoderModule::process  plugins/meteor_support/meteor/module_meteor_hrpt_decoder.cpp:24-50
  * run them (8192-byte reads, the last read of a piece shorter), and exposes them through a small C ABI for the Python tests

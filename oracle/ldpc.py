@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE ONLY — ctypes bindings of the checkers of the CCSDS LDPC decoder (ccsds_ldpc_decoder, rate 7/8 C2 code):
 
-  impl "ref"   oracle/_ref/libsatref_ldpc.so: the unmodified reference translation units + oracle/ldpc_harness.cpp (oracle/ldpc.mk)
+  impl "ref"   oracle/_ref/libsatref_ldpc.so: the unmodified reference translation units + oracle/ldpc_harness.cpp (oracle/Makefile)
   impl "port"  oracle/libldpc_port.so: our own C restatement (oracle/ldpc_port.c), pinned to "ref" by tests/test_ldpc_oracle.py
 
 Both export the same C ABI (prefix ref_ / orc_). impl=None picks "ref" when it was built, else "port" — like tests.common.oracle().
@@ -11,41 +11,28 @@ from dataclasses import dataclass
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_PATHS = {"ref": (os.path.join(_HERE, "_ref", "libsatref_ldpc.so"), "ref_"), "port": (os.path.join(_HERE, "libldpc_port.so"), "orc_")}
+from ._checker import HERE, Handle, Library, ref_path
+
 CONST = {"bpsk": 0, "qpsk": 1, "oqpsk": 2}
 F = 8192      # soft bytes per frame: 32-bit ASM + 8160 code bits
 CW = 8160     # code bits sent per frame (8176 minus the 18 shortened positions, plus 2 fill bits)
 REC = ("offset", "pos", "cor_bits", "phase", "swap", "ldpc_corr", "locked", "deframer_state")
 
 
-def available(impl="ref"):
-    return os.path.exists(_PATHS[impl][0])
+_lib = Library({"ref": (ref_path("ldpc"), "ref_"), "port": (os.path.join(HERE, "libldpc_port.so"), "orc_")},
+               [("ldpc_create", C.c_void_p, [C.c_int] * 4 + [C.c_uint]), ("ldpc_destroy", None, [C.c_void_p]),
+                ("ldpc_run", C.c_long, [C.c_void_p, C.c_void_p, C.c_long, C.c_void_p, C.c_long, C.POINTER(C.c_long), C.c_void_p, C.c_long]),
+                ("ldpc_decode", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]), ("ldpc_matrix", C.c_int, [C.c_void_p, C.c_int])])
+available = _lib.available
 
 
 def default_impl():
     return "ref" if available("ref") else "port"
 
 
-_libs = {}
-
-
 def lib(impl=None):
-    impl = impl or default_impl()
-    if impl not in _libs:
-        path, pfx = _PATHS[impl]
-        L = C.CDLL(path)
-        fn = {}
-        for name, res, args in [("ldpc_create", C.c_void_p, [C.c_int] * 4 + [C.c_uint]), ("ldpc_destroy", None, [C.c_void_p]),
-                                ("ldpc_run", C.c_long, [C.c_void_p, C.c_void_p, C.c_long, C.c_void_p, C.c_long, C.POINTER(C.c_long), C.c_void_p,
-                                                        C.c_long]),
-                                ("ldpc_decode", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
-                                ("ldpc_matrix", C.c_int, [C.c_void_p, C.c_int])]:
-            f = getattr(L, pfx + name)
-            f.restype, f.argtypes = res, args
-            fn[name] = f
-        _libs[impl] = fn
-    return _libs[impl]
+    """{name without prefix: function}"""
+    return _lib(impl or default_impl())
 
 
 @dataclass(frozen=True)
@@ -64,19 +51,14 @@ def ldpc_cfg(constellation, iterations=10, derandomize=True, internal_cadu_size=
     return LdpcCfg(constellation, int(iterations), bool(derandomize), int(internal_cadu_size), int(internal_asm))
 
 
-class Fec:
+class Fec(Handle):
     """The module loop over a soft stream; run() may be called repeatedly (the stream continues, like ragged pushes)."""
 
     def __init__(self, cfg, impl=None):
         self.cfg, self.impl = cfg, impl or default_impl()
-        self.L = lib(self.impl)
         self.cadu_bytes = cfg.internal_cadu_size // 8 if cfg.internal_cadu_size else 1024
-        self.h = self.L["ldpc_create"](CONST[cfg.constellation], cfg.iterations, int(cfg.derandomize), cfg.internal_cadu_size, cfg.internal_asm)
-
-    def __del__(self):
-        if getattr(self, "h", None):
-            self.L["ldpc_destroy"](self.h)
-            self.h = None
+        super().__init__(lib(self.impl), "ldpc", CONST[cfg.constellation], cfg.iterations, int(cfg.derandomize), cfg.internal_cadu_size,
+                         cfg.internal_asm)
 
     def run(self, soft):
         """Returns cadu (uint8 [frames, cadu_bytes]: the CADUs, or with internal_stream the inner frames) and recs (int64 [n, 8], columns

@@ -2,7 +2,7 @@
  * TEST INFRASTRUCTURE ONLY — never linked into or called from the product path.
  *
  * oracle/_ref LDPC harness: wires the UNMODIFIED reference translation units of the CCSDS LDPC decoder (compiled from the reference
- * tree by oracle/ldpc.mk, with oracle/ldpc_shim + oracle/shim standing in for VOLK and the logger) the way
+ * tree by oracle/Makefile, with oracle/ldpc_shim + oracle/shim standing in for VOLK and the logger) the way
  *   CCSDSLDPCDecoderModule::process   src-core/pipeline/modules/ccsds/module_ccsds_ldpc_decoder.cpp:134-277 (ldpc_rate "7/8", with and
  *                                     without internal_stream)
  * runs them, and exposes them through a small C ABI for the Python tests (oracle/ldpc.py).

@@ -3,7 +3,7 @@
  *
  * oracle/_ref METEOR LRPT harness: wires the UNMODIFIED reference translation units of the METEOR-M LRPT decoder's parts (correlator.cpp,
  * viterbi27.cpp with cc_decoder.cpp / cc_encoder.cpp, viterbi_1_2.cpp, nrzm.cpp, rotation.cpp, randomization.cpp, bpsk_ccsds_deframer.cpp,
- * reedsolomon.cpp and libcorrect's Reed-Solomon, compiled from the reference tree by oracle/meteor.mk) the way
+ * reedsolomon.cpp and libcorrect's Reed-Solomon, compiled from the reference tree by oracle/Makefile) the way
  *   meteor::METEORLRPTDecoderModule::process   plugins/meteor_support/meteor/module_meteor_lrpt_decoder.cpp:101-262
  * runs them in its two working modes (m2x_mode false: :198-262; m2x_mode without "interleaved": :103-197), and exposes them through a
  * small C ABI for the Python tests (oracle/meteor.py). The module file itself pulls in ImGui and the pipeline base, so its two loops are

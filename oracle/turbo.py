@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE ONLY — ctypes bindings of the checkers of the CCSDS turbo decoder (ccsds_turbo_decoder):
 
-  impl "ref"   oracle/_ref/libsatref_turbo.so: the unmodified reference translation units + oracle/turbo_harness.cpp (oracle/turbo.mk)
+  impl "ref"   oracle/_ref/libsatref_turbo.so: the unmodified reference translation units + oracle/turbo_harness.cpp (oracle/Makefile)
   impl "port"  oracle/libturbo_port.so: our own C restatement (oracle/turbo_port.c), pinned to "ref" by tests/test_turbo_oracle.py
 
 Both export the same C ABI (prefix ref_ / orc_; the encoder only in "ref"). impl=None means "ref". Where "ref" was not built (the reference
@@ -11,51 +11,26 @@ import os
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_PATHS = {"ref": (os.path.join(_HERE, "_ref", "libsatref_turbo.so"), "ref_"), "port": (os.path.join(_HERE, "libturbo_port.so"), "orc_")}
+from ._checker import HERE, Handle, Library, ref_path
+
 RATES = {"1/2": 2, "1/3": 3, "1/4": 4, "1/6": 6}
 REC = ("offset", "pos", "cor_bits", "swapped", "crc_ok", "locked")
 
-
-def available(impl="ref"):
-    return os.path.exists(_PATHS[impl][0])
-
-
-_libs = {}
-
-
-def lib(impl="ref"):
-    """{name without prefix: function}"""
-    if impl not in _libs:
-        path, pfx = _PATHS[impl]
-        L = C.CDLL(path)
-        vp, ci, cl = C.c_void_p, C.c_int, C.c_long
-        fn = {}
-        for name, res, args in [("turbo_create", vp, [ci, ci, ci]), ("turbo_destroy", None, [vp]), ("turbo_frame_size", ci, [vp]),
-                                ("turbo_run", cl, [vp, vp, cl, vp, cl, C.POINTER(cl), vp, cl]),
-                                ("turbo_encode", ci, [ci, ci, vp, vp]), ("turbo_perm", ci, [ci, vp]),
-                                ("turbo_half", None, [ci, ci, ci, vp, vp, vp, ci, vp])]:
-            if hasattr(L, pfx + name):
-                f = getattr(L, pfx + name)
-                f.restype, f.argtypes = res, args
-                fn[name] = f
-        _libs[impl] = fn
-    return _libs[impl]
+vp, ci, cl = C.c_void_p, C.c_int, C.c_long
+lib = Library({"ref": (ref_path("turbo"), "ref_"), "port": (os.path.join(HERE, "libturbo_port.so"), "orc_")},
+              [("turbo_create", vp, [ci, ci, ci]), ("turbo_destroy", None, [vp]), ("turbo_frame_size", ci, [vp]),
+               ("turbo_run", cl, [vp, vp, cl, vp, cl, C.POINTER(cl), vp, cl]), ("turbo_encode", ci, [ci, ci, vp, vp]),
+               ("turbo_perm", ci, [ci, vp]), ("turbo_half", None, [ci, ci, ci, vp, vp, vp, ci, vp])], optional=("turbo_encode",))
+available = lib.available
 
 
-class Turbo:
+class Turbo(Handle):
     """The module loop over a soft stream; run() may be called repeatedly (the stream continues, like ragged pushes)."""
 
     def __init__(self, rate, base, iters, impl="ref"):
         self.rate, self.base, self.iters = RATES[rate], int(base), int(iters)
-        self.L = lib(impl)
-        self.h = self.L["turbo_create"](self.rate, self.base, self.iters)
+        super().__init__(lib(impl), "turbo", self.rate, self.base, self.iters)
         self.F = self.L["turbo_frame_size"](self.h)
-
-    def __del__(self):
-        if getattr(self, "h", None):
-            self.L["turbo_destroy"](self.h)
-            self.h = None
 
     def run(self, soft):
         """Returns cadu (uint8 [frames, base + 4], the frames whose CRC passes) and recs (int64 [n, 6], columns REC) of every frame."""

@@ -2,7 +2,7 @@
  * TEST INFRASTRUCTURE ONLY — never linked into or called from the product path.
  *
  * oracle/_ref turbo harness: wires the UNMODIFIED reference translation units of the CCSDS turbo decoder (ccsds_turbo.cpp, the
- * deepspace-turbo library, crc_generic.cpp and randomization.cpp, compiled from the reference tree by oracle/turbo.mk, with oracle/shim
+ * deepspace-turbo library, crc_generic.cpp and randomization.cpp, compiled from the reference tree by oracle/Makefile, with oracle/shim
  * standing in for VOLK) the way
  *   CCSDSTurboDecoderModule::process   src-core/pipeline/modules/ccsds/module_ccsds_turbo_decoder.cpp:137-235
  * runs them, and exposes them through a small C ABI for the Python tests (oracle/turbo.py).

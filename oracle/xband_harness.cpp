@@ -4,7 +4,7 @@
  * oracle/_ref METEOR X-band harness: wires the UNMODIFIED reference blocks meteor::MTVZA_ExtDeframer and meteor::KMSS_BPSK_ExtDeframer
  * (plugins/meteor_support/meteor/meteor_rec_deframer.h, with meteor_rec_deframer.cpp), diff::NRZMDiff (common/codings/differential/nrzm.cpp),
  * RepackBitsByte (common/repack_bits_byte.cpp) and def::SimpleDeframer (common/simple_deframer.h), compiled from the reference tree by
- * oracle/xband.mk, the way
+ * oracle/Makefile, the way
  *   meteor::MeteorXBandDecoderModule::process   plugins/meteor_support/meteor/module_meteor_xband_decoder.cpp:62-212
  * runs them ("mtvza" and "kmss_bpsk"), and exposes them through a small C ABI for the Python tests (oracle/xband.py). The module file
  * pulls in ImGui and the pipeline base, so its loop is restated here as wiring.

@@ -1,6 +1,10 @@
 """Shared helpers of the test-suite: config plumbing between the synthetic transmitter, the oracle and the C ABI."""
+import copy
 import functools
+import hashlib
+import json
 import os
+import subprocess
 import sys
 
 import numpy as np
@@ -9,6 +13,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
+from oracle._checker import pieces  # noqa: E402,F401  (the (start, end) of each push, shared with the checkers)
 from satdump_b200 import synth  # noqa: E402
 
 
@@ -19,6 +24,77 @@ def oracle():
         return ref
     from oracle import port
     return port
+
+
+def reference(O):
+    """The checker module O (oracle.hrpt, ...) when its library was built from the reference, else skip: without the reference the
+    tests compare with the pins."""
+    if not O.available():
+        import pytest
+        pytest.skip(f"{O.__name__}: oracle/_ref not built (the reference is absent): the tests compare with the pins")
+    return O
+
+
+def digest(a, dtype=None, hexlen=None):
+    """sha256 of the array's bytes (cast to dtype first when given) in hex, its first hexlen digits when given"""
+    return hashlib.sha256(np.ascontiguousarray(a, dtype).tobytes()).hexdigest()[:hexlen]
+
+
+@functools.cache
+def _read_json(path):
+    with open(path) as f:
+        return json.load(f)
+
+
+def load_pins(path):
+    """A golden JSON file, read from disk once; each caller gets its own copy."""
+    return copy.deepcopy(_read_json(path))
+
+
+def assert_pin(pin, golden, **live):
+    """The reference's results now (live: field -> value) equal the pinned ones (pin[field]). The pins stand in for the reference where it
+    is absent: otherwise the golden file `golden` is stale."""
+    stale = sorted(k for k, v in live.items() if pin[k] != v)
+    assert not stale, f"{golden} is stale: {stale}"
+
+
+def after_lock(frames, clear, prefix=None):
+    """The frames from the third one whose data (its first `prefix` bytes when given) is a transmitted frame's on: the first ones are
+    read while the demodulator's loops acquire, where its soft bytes sit on the float floor (DESIGN §5)"""
+    for i, row in enumerate(frames):
+        if any(np.array_equal(row[:prefix], c[:prefix]) for c in clear):
+            return frames[i + 2:]
+    return frames[:0]
+
+
+def run_chain(dcfg, fcfg, raw, fmt, pipelined):
+    """raw IQ through a capi.Chain of the two configs in three pushes (the second ends off a third of the stream), synchronous or
+    pipelined: the frames concatenated, and the decoder's stats"""
+    from satdump_b200 import capi
+    per = 1 if fmt == "cf32" else 2
+    n = raw.size // per
+    ch = capi.Chain(dcfg, fcfg)
+    if pipelined:
+        ch.set_pipelined(True)
+    out = []
+    for a, b in [(0, n // 3), (n // 3, 2 * n // 3 + 1001), (2 * n // 3 + 1001, n)]:
+        ch.push(raw[per * a:per * b])
+        out.append(ch.frames())
+    if pipelined:
+        ch.sync()
+        out.append(ch.frames())
+    _, fs = ch.stats()
+    ch.close()
+    return np.concatenate(out), fs
+
+
+def run_cli(pipe, inp, hint, *args, fused=False, timeout=300):
+    """b200_pipeline <pipe> baseband <inp> <hint> <args>, two-stage or --fused; the completed process, which must have exited 0"""
+    tool = os.path.join(ROOT, "satdump_b200", "host", "b200_pipeline")
+    r = subprocess.run([tool, pipe, "baseband", str(inp), hint, *args] + (["--fused"] if fused else []), capture_output=True, text=True,
+                       timeout=timeout)
+    assert r.returncode == 0, r.stderr
+    return r
 
 
 def rx_const(cfg):

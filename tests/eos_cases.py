@@ -3,13 +3,13 @@ output for each of them in tests/golden/eos_pins.json, which the tests read wher
 
 A case edits the DECODED bit stream (the CADUs as the deframer sees them) before its two rails are NRZ-M encoded, so an ASM gets an exact
 number of bit errors, a frame its exact RS errors, and a bit slip stays one bit; a symbol slip drops one soft pair."""
-import hashlib
-import json
+import functools
 import os
 
 import numpy as np
 
 from satdump_b200 import synth
+from tests.common import after_lock as _after_lock, digest, load_pins
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 PINS = os.path.join(HERE, "golden", "eos_pins.json")
@@ -35,13 +35,7 @@ RAGGED = (1, 3, 65535, 65537)  # piece sizes of the ragged pushes
 LARGE_FRAMES = 8320            # >= 2^26 soft bytes in one push
 
 
-def digest(a):
-    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
-
-
-def pins():
-    with open(PINS) as f:
-        return json.load(f)
+pins = functools.partial(load_pins, PINS)
 
 
 def _noise(rng, n):
@@ -131,12 +125,8 @@ def chain_reference(name):
     return O.Aqua().run(soft[:soft.size // READ * READ])["cadu"], clear
 
 
-def after_lock(cadus, clear):
-    """The CADUs from the third one whose data is a sent frame's on: the first ones are read while the demodulator's loops acquire"""
-    for i, row in enumerate(cadus):
-        if any(np.array_equal(row[:896], c[:896]) for c in clear):
-            return cadus[i + 2:]
-    return cadus[:0]
+# a CADU's data: its first 896 bytes
+after_lock = functools.partial(_after_lock, prefix=896)
 
 
 def stats_rows(stats):

@@ -2,13 +2,13 @@
 the reference on each stream and stores a digest of its frames and timestamps, its frame count and final state in
 tests/golden/gac_pins.json, which the tests read where the reference is absent. Every stream is a whole number of the modules' 8192-byte
 reads, so the reference decodes all of it."""
-import hashlib
-import json
+import functools
 import os
 
 import numpy as np
 
 from satdump_b200 import synth
+from tests import common
 
 PINS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "gac_pins.json")
 START_TS = 1700000000.25  # dmsp_rtd_decoder's start_timestamp in the DMSP cases
@@ -83,8 +83,7 @@ def cuts_for(name, n, sizes):
     return sorted(c for c in cuts | extra if 0 < c < n)
 
 
-def digest(a):
-    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()[:24]
+digest = functools.partial(common.digest, hexlen=24)
 
 
 def ts_digest(ts):
@@ -92,15 +91,7 @@ def ts_digest(ts):
     return digest(np.frombuffer("".join("%f\n" % t for t in ts).encode(), np.uint8))
 
 
-_pins = None
-
-
-def pins():
-    global _pins
-    if _pins is None:
-        with open(PINS) as f:
-            _pins = json.load(f)
-    return _pins
+pins = functools.partial(common.load_pins, PINS)
 
 
 def ref_result(name):

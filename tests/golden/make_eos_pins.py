@@ -1,4 +1,4 @@
-"""Writes tests/golden/eos_pins.json from the reference's own Aqua DB decoder blocks (oracle/_ref/libsatref_eos.so, built by oracle/eos.mk):
+"""Writes tests/golden/eos_pins.json from the reference's own Aqua DB decoder blocks (oracle/_ref/libsatref_eos.so, built by oracle/Makefile):
 for every stream of tests/eos_cases.CASES the CADUs' digest and count, every frame's RS results and the stats after every push, pushed in
 whole reads and in the ragged pieces of ragged_cuts (the stats of the last piece there); the same for the large push; and for the IQ
 streams of CHAIN (reference psk_demod + decoder) and the Terra DB signal (reference terra_db_demod chain + ccsds_conv_concat_decoder) the
@@ -22,7 +22,7 @@ def pin(soft, cuts):
 
 
 def main():
-    assert O.available(), "build oracle/_ref/libsatref_eos.so first (make -C oracle -f eos.mk ref)"
+    assert O.available(), "build oracle/_ref/libsatref_eos.so first (make -C oracle ref)"
     out = {"cases": {}, "ragged": {}, "large": {}, "chain": {}}
     for name in CASES:
         soft, _ = stream(name)

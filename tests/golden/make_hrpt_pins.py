@@ -1,4 +1,4 @@
-"""Writes tests/golden/hrpt_pins.json from the reference's own HRPT deframers (oracle/_ref/libsatref_hrpt.so, built by oracle/hrpt.mk): for
+"""Writes tests/golden/hrpt_pins.json from the reference's own HRPT deframers (oracle/_ref/libsatref_hrpt.so, built by oracle/Makefile): for
 every stream of tests/hrpt_cases.NOAA and METEOR the records, a digest of the output and the stats after every push, pushed whole and in
 the ragged pieces of piece_cuts (stats as a digest there: one entry per piece), and the same for the large pushes of LARGE; for the IQ streams of CHAIN (reference pm_demod + deframer)
 the output size and a digest of the frames after the lock. Run from the
@@ -22,7 +22,7 @@ def pin(soft, cuts, meteor, thr):
 
 
 def main():
-    assert O.available(), "build oracle/_ref/libsatref_hrpt.so first (make -C oracle -f hrpt.mk ref)"
+    assert O.available(), "build oracle/_ref/libsatref_hrpt.so first (make -C oracle ref)"
     out = {"cases": {}, "pieces": {}, "large": {}, "chain": {}}
     for name in [*NOAA, *METEOR]:
         soft, cuts = stream(name)

@@ -1,5 +1,5 @@
 """Writes tests/golden/meteor_lrpt_pins.json from the reference's own METEOR LRPT decoder parts (oracle/_ref/libsatref_meteor.so, built by
-oracle/meteor.mk): for every stream of tests/meteor_lrpt_cases.CASES the frame records, the stats and a digest of the written CADUs, whole
+oracle/Makefile): for every stream of tests/meteor_lrpt_cases.CASES the frame records, the stats and a digest of the written CADUs, whole
 and in the pieces of piece_cuts for PIECES; for M2X the CADU digest and stats; for the IQ streams of CHAIN (reference demodulator + decoder)
 the number of CADUs and a digest of those after the lock. Run from the repository root: python tests/golden/make_meteor_lrpt_pins.py"""
 import json
@@ -29,7 +29,7 @@ def m2x_pin(name):
 
 
 def main():
-    assert O.available(), "build oracle/_ref/libsatref_meteor.so first (make -C oracle -f meteor.mk ref)"
+    assert O.available(), "build oracle/_ref/libsatref_meteor.so first (make -C oracle ref)"
     out = {"cases": {}, "pieces": {}, "m2x": {}, "chain": {}}
     for name in CASES:
         out["cases"][name] = case_pin(name)

@@ -8,7 +8,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspa
 from oracle import xband  # noqa: E402
 from tests import xband_cases as X  # noqa: E402
 
-assert xband.available(), "build oracle/_ref first (oracle/xband.mk)"
+assert xband.available(), "build oracle/_ref first (oracle/Makefile)"
 pins = {name: X.reference(name) for name in X.CASES + X.LARGE}
 with open(X.PINS, "w") as f:
     json.dump(pins, f, indent=1, sort_keys=True)

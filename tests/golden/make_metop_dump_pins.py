@@ -1,5 +1,5 @@
 """Writes tests/golden/metop_dump_pins.json from the reference's own MetOp dump decoder parts (oracle/_ref/libsatref_dump.so, built by
-oracle/dump.mk): for every stream of tests/metop_dump_cases.CASES the frame records and a digest of the written CADUs, and for the IQ
+oracle/Makefile): for every stream of tests/metop_dump_cases.CASES the frame records and a digest of the written CADUs, and for the IQ
 streams of tests/metop_dump_cases.CHAIN (reference demodulator + decoder) the number of CADUs and a digest of those after the lock. Run
 from the repository root: python tests/golden/make_metop_dump_pins.py"""
 import json
@@ -14,7 +14,7 @@ from tests.metop_dump_cases import CASES, CHAIN, PINS, after_lock, chain_referen
 
 
 def main():
-    assert O.available(), "build oracle/_ref/libsatref_dump.so first (make -C oracle -f dump.mk ref)"
+    assert O.available(), "build oracle/_ref/libsatref_dump.so first (make -C oracle ref)"
     out = {"cases": {}, "chain": {}}
     for name, case in CASES.items():
         soft, _, _ = stream(case)

@@ -1,4 +1,4 @@
-"""Writes tests/golden/turbo_pins.json from the reference's own turbo decoder (oracle/_ref/libsatref_turbo.so, built by oracle/turbo.mk):
+"""Writes tests/golden/turbo_pins.json from the reference's own turbo decoder (oracle/_ref/libsatref_turbo.so, built by oracle/Makefile):
 for every stream of tests/turbo_cases.CASES the frame records and a digest of the written CADUs, the interleaver of each base and the
 encoder output of each rate and base, and the CADUs of the IQ streams of tests/turbo_cases.CHAIN (reference demodulator + decoder); and
 tests/golden/turbo_llr.npz: the a-priori arrays after the last iteration of the frames of tests/turbo_cases.LLR_CASES. Run from the repository root: python tests/golden/make_turbo_pins.py"""
@@ -13,15 +13,12 @@ sys.path.insert(0, ROOT)
 
 from oracle import turbo as O  # noqa: E402
 from satdump_b200 import synth  # noqa: E402
-from tests.turbo_cases import CASES, CHAIN, LLR, LLR_CASES, PINS, RATE_NAME, chain_reference, digest, llr_frames, reference_llr, stream  # noqa: E402
-
-
-def encoder_info(rate, base):
-    return np.random.default_rng(rate * 7 + base).integers(0, 256, base, dtype=np.uint8)
+from tests.turbo_cases import (CASES, CHAIN, LLR, LLR_CASES, PINS, RATE_NAME, chain_reference, digest, encoder_info, llr_frames,  # noqa: E402
+                               reference_llr, stream)
 
 
 def main():
-    assert O.available(), "build oracle/_ref/libsatref_turbo.so first (make -C oracle -f turbo.mk ref)"
+    assert O.available(), "build oracle/_ref/libsatref_turbo.so first (make -C oracle ref)"
     out = {"perm": {}, "encode": {}, "cases": {}}
     for base in synth.TURBO_BASES:
         out["perm"][str(base)] = digest(O.perm(base).astype(np.int32))

@@ -1,13 +1,13 @@
 """Soft streams of the noaa_hrpt_decoder and meteor_hrpt_decoder tests, rebuilt from seeds on any machine. tests/golden/make_hrpt_pins.py
 runs the reference on each stream and stores its records, per-push stats and a digest of its output in tests/golden/hrpt_pins.json, which
 the tests read where the reference is absent."""
-import hashlib
-import json
+import functools
 import os
 
 import numpy as np
 
 from satdump_b200 import synth
+from tests.common import after_lock, digest, load_pins  # noqa: F401
 
 PINS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "hrpt_pins.json")
 NOAA_BITS = synth.NOAA_WORDS * 10
@@ -128,13 +128,7 @@ def boundary_cuts(name):
     return [600, 3000 + 17, 3000 + 32 + 8 * 400 + 5, 3000 + MH_BITS + 20]
 
 
-def digest(a):
-    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
-
-
-def pins():
-    with open(PINS) as f:
-        return json.load(f)
+pins = functools.partial(load_pins, PINS)
 
 
 def stats_rows(stats):
@@ -187,15 +181,6 @@ def frames_of(out, meteor):
         else:
             i += 1
     return np.array([w[s:s + synth.NOAA_WORDS] for s in starts], np.uint16).reshape(-1, synth.NOAA_WORDS)
-
-
-def after_lock(frames, clear):
-    """The frames from the third one that is a transmitted frame on: the first ones are read while the demodulator's loops acquire, where
-    its soft bytes sit on the float floor (DESIGN §5)"""
-    for i, row in enumerate(frames):
-        if any(np.array_equal(row, c) for c in clear):
-            return frames[i + 2:]
-    return frames[:0]
 
 
 def chain_reference(name):

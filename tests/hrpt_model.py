@@ -4,6 +4,8 @@ the CPU: per push, the hard bits of the soft FIFO, the candidate bitmap (windows
 frame, METEOR's windows of mixed inversion after a state-2 timeout), the gathered output, and the FIFO keeping an open frame or 63 bits."""
 import numpy as np
 
+from oracle._checker import pieces
+
 NOAA_WORDS, NOAA_DATA_BITS, NOAA_SYNC, NOAA_MASK = 11090, 11084 * 10, 0x0A116FD719D83C95, (1 << 60) - 1
 NOAA_FIXED = np.array([0x284, 0x16F, 0x35C, 0x19D, 0x20F, 0x095], np.uint16)
 MH_ASM, MH_DATA_BITS, MH_PERIOD, MH_S2_LIMIT = 0x1ACFFC1D, 8160, 8192, 5 * 1024 * 8
@@ -205,7 +207,7 @@ def run_pieces(soft, cuts=(), meteor=False, thr=0):
     """As oracle.hrpt.run_pieces"""
     m = Model(meteor, thr)
     out, recs, stats = [], [], []
-    for a, b in zip([0, *cuts], [*cuts, soft.size]):
+    for a, b in pieces(soft.size, cuts):
         r = m.push(soft[a:b])
         out.append(r["out"])
         recs.append(r["recs"])

@@ -1,13 +1,13 @@
 """Soft and IQ streams of the meteor_lrpt_decoder tests, rebuilt from seeds on any machine. tests/golden/make_meteor_lrpt_pins.py runs the
 reference on each of them and stores its records, stats and digests of its output in tests/golden/meteor_lrpt_pins.json, which the tests
 read where the reference is absent."""
-import hashlib
-import json
+import functools
 import os
 
 import numpy as np
 
 from satdump_b200 import synth
+from tests.common import after_lock, digest, load_pins  # noqa: F401
 
 PINS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "meteor_lrpt_pins.json")
 F = 16384
@@ -77,13 +77,7 @@ M2X_PARAMS = dict(viterbi_ber_thresold=0.3, viterbi_outsync_after=20)
 CHAIN = {"meteor_lrpt_cs16": ("meteor_lrpt", "cs16", 20, 5), "meteor_lrpt_1m_cs16": ("meteor_lrpt_1m", "cs16", 21, 6)}
 
 
-def digest(a):
-    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
-
-
-def pins():
-    with open(PINS) as f:
-        return json.load(f)
+pins = functools.partial(load_pins, PINS)
 
 
 def chain_signal(name):
@@ -93,15 +87,6 @@ def chain_signal(name):
     cfg = dataclasses.replace(synth.CONFIGS[cfg_name], fmt=fmt)
     raw, clear = synth.make_signal(cfg, 1 << log2n, seed=seed, device="cpu")
     return cfg, raw.numpy(), clear
-
-
-def after_lock(cadu, clear):
-    """The CADUs from the third one that is a transmitted frame on: the first frames are read while the demodulator's loops acquire, where
-    its soft bytes sit on the float floor (DESIGN §5)"""
-    for i, row in enumerate(cadu):
-        if any(np.array_equal(row, c) for c in clear):
-            return cadu[i + 2:]
-    return cadu[:0]
 
 
 def chain_reference(name):

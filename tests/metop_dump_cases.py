@@ -1,12 +1,12 @@
 """Soft streams of the metop_dump_decoder tests, rebuilt from seeds on any machine. tests/golden/make_metop_dump_pins.py runs the reference
 on each of them and stores digests of its output in tests/golden/metop_dump_pins.json, which the tests read where the reference is absent."""
-import hashlib
-import json
+import functools
 import os
 
 import numpy as np
 
 from satdump_b200 import synth
+from tests.common import after_lock, digest, load_pins  # noqa: F401
 
 PINS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "metop_dump_pins.json")
 F = 8192
@@ -115,13 +115,7 @@ PIECES = ("noise_signal_noise", "shift_small", "shift_large", "tail_8162", "rs_e
 CHAIN = {"metop_dump_cs16": ("metop_dump", "cs16", 20, 5), "metop_dump_cs8": ("metop_dump", "cs8", 20, 6)}
 
 
-def digest(a):
-    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
-
-
-def pins():
-    with open(PINS) as f:
-        return json.load(f)
+pins = functools.partial(load_pins, PINS)
 
 
 def chain_signal(name):
@@ -131,15 +125,6 @@ def chain_signal(name):
     cfg = dataclasses.replace(synth.CONFIGS[cfg_name], fmt=fmt)
     raw, clear = synth.make_signal(cfg, 1 << log2n, seed=seed, device="cpu")
     return cfg, raw.numpy(), clear
-
-
-def after_lock(cadu, clear):
-    """The CADUs from the third one that is a transmitted frame on: the first frames are read while the demodulator's loops acquire, where
-    its soft bytes sit on the float floor (DESIGN §5)"""
-    for i, row in enumerate(cadu):
-        if any(np.array_equal(row, c) for c in clear):
-            return cadu[i + 2:]
-    return cadu[:0]
 
 
 def chain_reference(name):

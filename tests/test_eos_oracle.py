@@ -9,14 +9,9 @@ import subprocess
 import numpy as np
 import pytest
 
+from oracle import eos as O
+from tests.common import reference
 from tests.eos_cases import CASES, after_lock, digest, pins, ragged_cuts, read_cuts, stats_rows, stream
-
-
-def _ref():
-    from oracle import eos as O
-    if not O.available():
-        pytest.skip("oracle/_ref/libsatref_eos.so not built (the reference is absent): the tests compare with the pins")
-    return O
 
 
 def _same(r, pin):
@@ -27,7 +22,7 @@ def _same(r, pin):
 
 @pytest.mark.parametrize("name", sorted(CASES))
 def test_reference_equals_pins(name):
-    O = _ref()
+    reference(O)
     soft, _ = stream(name)
     _same(O.run_pieces(soft, read_cuts(soft.size)), pins()["cases"][name])
     _same(O.run_pieces(soft, ragged_cuts(soft.size, CASES[name]["lead"])), pins()["ragged"][name])
@@ -35,7 +30,7 @@ def test_reference_equals_pins(name):
 
 def test_synthesised_streams_come_out_as_sent():
     """The decoded stream's rails NRZ-M encoded on Q (A) and I (B): the reference writes the sent CADUs; on swapped rails it never syncs"""
-    O = _ref()
+    reference(O)
     from satdump_b200 import synth
     bits, sent = synth.aqua_db_frames(16, seed=3)
     soft = synth.aqua_db_soft(bits, sigma=10.0, seed=4)
@@ -46,7 +41,7 @@ def test_synthesised_streams_come_out_as_sent():
 
 def test_iq_signal_decodes_through_the_reference_chain():
     """psk_demod OQPSK at 15 MS/s (EOS.json's parameters) -> the module loop: after the lock every CADU is a sent one"""
-    _ref()
+    reference(O)
     from tests.eos_cases import chain_reference
     o, clear = chain_reference("cs16")
     tail = after_lock(o, clear)
@@ -87,7 +82,7 @@ def test_terra_refuses_too_few_samples_per_half_symbol(built, tmp_path, fused):
 def test_terra_omega_and_taps_equal_the_reference():
     """The mapping runs psk_demod's BPSK chain at 2 x symbolrate. Its M&M omega fs / (2 rs) in float is bitwise TerraDBDemodModule's
     ((float)fs / (float)rs) / 2 at every rate of the window (halving is exact), and its RRC is firdes' RRC at the same arguments."""
-    _ref()
+    reference(O)
     from oracle import ref as R
     from satdump_b200 import capi
     for fs in (15e6, 26.5e6, 30e6, 45e6, 52.5e6):
@@ -101,7 +96,7 @@ def test_terra_omega_and_taps_equal_the_reference():
 
 
 def test_terra_signal_decodes_through_the_reference_chain():
-    _ref()
+    reference(O)
     from tests.eos_cases import terra_chain_reference, terra_signal
     o = terra_chain_reference()
     clear = terra_signal()[1]

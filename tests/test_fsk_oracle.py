@@ -3,14 +3,13 @@ import numpy as np
 import pytest
 
 from satdump_b200 import capi, synth
+from tests.common import reference
 
 
 @pytest.fixture(scope="module")
 def O():
     from oracle import fsk
-    if not fsk.available():
-        pytest.skip("oracle/_ref/libsatref_fsk.so was not built (the reference is absent)")
-    return fsk
+    return reference(fsk)
 
 
 def test_correctly_rounded_arm_is_within_one_ulp_of_glibc(O):

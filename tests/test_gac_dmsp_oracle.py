@@ -5,16 +5,11 @@ reference (or its pins) on every case; the timestamp rule follows the reference'
 import numpy as np
 import pytest
 
+from oracle import gac as O
 from satdump_b200 import capi, synth
+from tests.common import reference
 from tests import gac_cases as G
 from tests import gac_model as M
-
-
-def _ref():
-    from oracle import gac as O
-    if not O.available():
-        pytest.skip("oracle/_ref/libsatref_gac.so not built (the reference is absent): the tests compare with the pins")
-    return O
 
 
 def test_pn_table_equals_the_reference():
@@ -35,7 +30,7 @@ def test_pn_recurrence_has_period_1023():
 
 @pytest.mark.parametrize("name", G.CASES)
 def test_reference_equals_pins(name):
-    O = _ref()
+    reference(O)
     dmsp, backward = G.params(name)
     r = O.Ref(dmsp, backward, G.START_TS if dmsp else -1.0).run(G.stream(name))
     pin = G.pins()["cases"][name]
@@ -54,7 +49,7 @@ def test_model_equals_the_reference(name):
 
 @pytest.mark.parametrize("backward", [False, True])
 def test_synthesised_gac_frames_come_out_as_sent(backward):
-    O = _ref()
+    reference(O)
     bits, sent = synth.gac_frames(13, seed=3, backward=backward)
     soft = synth.hrpt_soft(np.concatenate([np.zeros(999, np.uint8), bits.reshape(-1)]), inverted=True, sigma=10.0, seed=4)
     soft = np.concatenate([soft, np.zeros((-soft.size) % 8192, np.int8)])
@@ -63,7 +58,7 @@ def test_synthesised_gac_frames_come_out_as_sent(backward):
 
 
 def test_synthesised_dmsp_frames_come_out_as_sent():
-    O = _ref()
+    reference(O)
     bits, sent = synth.dmsp_frames(500, seed=3)
     soft = synth.hrpt_soft(bits.reshape(-1), sigma=10.0, seed=4)
     soft = np.concatenate([soft, np.zeros((-soft.size) % 8192, np.int8)])

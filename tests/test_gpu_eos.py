@@ -4,6 +4,7 @@ where it was built, else against tests/golden/eos_pins.json."""
 import numpy as np
 import pytest
 
+from tests.common import assert_pin, pieces, run_chain, run_cli
 from tests.eos_cases import (CASES, CHAIN, READ, TERRA_FEC, TERRA_RATE, after_lock, aqua_demod_kwargs, chain_reference, chain_signal, digest,
                              large_stream, pins, ragged_cuts, read_cuts, stats_rows, stream, terra_chain_reference, terra_demod_kwargs,
                              terra_floor, terra_reference, terra_signal)
@@ -16,7 +17,7 @@ def run_gpu(soft, cuts):
     from satdump_b200 import capi
     g = capi.Fec(capi.aqua_db_cfg(max_soft=max(1 << 17, soft.size)))
     out, rows = [], []
-    for a, b in zip([0, *cuts], [*cuts, soft.size]):
+    for a, b in pieces(soft.size, cuts):
         g.push(soft[a:b])
         out.append(g.frames())
         s = g.stats()
@@ -28,7 +29,7 @@ def check(pin, soft, cuts, every_push=True):
     from oracle import eos as O
     if O.available():
         r = O.run_pieces(soft, cuts)
-        assert digest(r["cadu"]) == pin["cadu"] and stats_rows(r["stats"])[-1] == pin["stats"][-1], "eos_pins.json is stale"
+        assert_pin(dict(cadu=pin["cadu"], stats=pin["stats"][-1]), "eos_pins.json", cadu=digest(r["cadu"]), stats=stats_rows(r["stats"])[-1])
     got, rows = run_gpu(soft, cuts)
     assert got.shape[0] == pin["frames"] and digest(got) == pin["cadu"]
     if every_push:
@@ -99,7 +100,7 @@ def _chain_tail_matches(got, name, clear):
     if O.available():
         o, _ = chain_reference(name)
         t = after_lock(o, clear)
-        assert t.shape[0] == pin["ntail"] and digest(t) == pin["tail"], "eos_pins.json is stale"
+        assert_pin(pin, "eos_pins.json", ntail=t.shape[0], tail=digest(t))
     tail = after_lock(got, clear)
     # the reference decodes whole reads only, so the GPU, which decodes every byte, may write more frames at the end
     assert tail.shape[0] >= pin["ntail"] >= 100 and digest(tail[:pin["ntail"]]) == pin["tail"]
@@ -113,18 +114,9 @@ def test_fused_chain(built, name, pipelined):
     from satdump_b200 import capi
     cfg, raw, clear = chain_signal(name)
     n = raw.size // 2
-    ch = capi.Chain(capi.demod_cfg(max_batch=n, **aqua_demod_kwargs(cfg.fmt)), capi.aqua_db_cfg(max_soft=n + READ))
-    if pipelined:
-        ch.set_pipelined(True)
-    out = []
-    for a, b in [(0, n // 3), (n // 3, 2 * n // 3 + 1001), (2 * n // 3 + 1001, n)]:
-        ch.push(raw[2 * a:2 * b])
-        out.append(ch.frames())
-    if pipelined:
-        ch.sync()
-        out.append(ch.frames())
-    _chain_tail_matches(np.concatenate(out), name, clear)
-    _, fs = ch.stats()
+    got, fs = run_chain(capi.demod_cfg(max_batch=n, **aqua_demod_kwargs(cfg.fmt)), capi.aqua_db_cfg(max_soft=n + READ), raw, cfg.fmt,
+                        pipelined)
+    _chain_tail_matches(got, name, clear)
     assert fs["deframer_state"] == 10
 
 
@@ -133,17 +125,11 @@ def test_fused_chain(built, name, pipelined):
 def test_cli(built, tmp_path, pipe, mode):
     """b200_pipeline aqua_db | aura_db (EOS.json's psk_demod parameters) writes the reference chain's .cadu after the lock and reports
     deframer_state"""
-    import os
-    import subprocess
-    from tests.common import ROOT
     cfg, raw, clear = chain_signal("cs16")
     inp = tmp_path / "in.cs16"
     raw.tofile(inp)
     hint = str(tmp_path / "out")
-    tool = os.path.join(ROOT, "satdump_b200", "host", "b200_pipeline")
-    cmd = [tool, pipe, "baseband", str(inp), hint, "--samplerate", "15000000", "--baseband_format", "cs16"]
-    r = subprocess.run(cmd + (["--fused"] if mode == "fused" else []), capture_output=True, text=True, timeout=300)
-    assert r.returncode == 0, r.stderr
+    r = run_cli(pipe, inp, hint, "--samplerate", "15000000", "--baseband_format", "cs16", fused=mode == "fused")
     _chain_tail_matches(np.fromfile(hint + ".cadu", np.uint8).reshape(-1, 1024), "cs16", clear)
     assert "deframer_state SYNCED" in r.stdout
 
@@ -195,7 +181,7 @@ def _terra_tail_matches(got, clear):
     from oracle import ref
     if oracle() is ref:
         t = after_lock(terra_chain_reference(), clear)
-        assert t.shape[0] == pin["ntail"] and digest(t) == pin["tail"], "eos_pins.json is stale"
+        assert_pin(pin, "eos_pins.json", ntail=t.shape[0], tail=digest(t))
     tail = after_lock(got, clear)
     assert tail.shape[0] >= pin["ntail"] >= 50 and digest(tail[:pin["ntail"]]) == pin["tail"]
     assert all(any(np.array_equal(row[:896], c[:896]) for c in clear) for row in tail)
@@ -207,34 +193,19 @@ def test_terra_fused_chain(built, pipelined):
     from satdump_b200 import capi
     raw, clear = terra_signal()
     n = raw.size // 2
-    ch = capi.Chain(capi.demod_cfg(max_batch=n, **terra_demod_kwargs()),
-                    capi.ccsds_cfg("bpsk_90", 8192, 0.3, 20, max_soft=2 * n, **TERRA_FEC))
-    if pipelined:
-        ch.set_pipelined(True)
-    out = []
-    for a, b in [(0, n // 3), (n // 3, 2 * n // 3 + 1001), (2 * n // 3 + 1001, n)]:
-        ch.push(raw[2 * a:2 * b])
-        out.append(ch.frames())
-    if pipelined:
-        ch.sync()
-        out.append(ch.frames())
-    _terra_tail_matches(np.concatenate(out), clear)
+    got, _ = run_chain(capi.demod_cfg(max_batch=n, **terra_demod_kwargs()),
+                       capi.ccsds_cfg("bpsk_90", 8192, 0.3, 20, max_soft=2 * n, **TERRA_FEC), raw, "cs16", pipelined)
+    _terra_tail_matches(got, clear)
 
 
 @pytest.mark.parametrize("mode", ["two_stage", "fused"])
 def test_terra_cli(built, tmp_path, mode):
     """b200_pipeline terra_db (terra_db_demod, then EOS.json's decoder parameters) writes the reference chain's .cadu after the lock"""
-    import os
-    import subprocess
-    from tests.common import ROOT
     raw, clear = terra_signal()
     inp = tmp_path / "in.cs16"
     raw.tofile(inp)
     hint = str(tmp_path / "out")
-    tool = os.path.join(ROOT, "satdump_b200", "host", "b200_pipeline")
-    cmd = [tool, "terra_db", "baseband", str(inp), hint, "--samplerate", "45000000", "--baseband_format", "cs16"]
-    r = subprocess.run(cmd + (["--fused"] if mode == "fused" else []), capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stderr
+    run_cli("terra_db", inp, hint, "--samplerate", "45000000", "--baseband_format", "cs16", fused=mode == "fused", timeout=600)
     _terra_tail_matches(np.fromfile(hint + ".cadu", np.uint8).reshape(-1, 1024), clear)
 
 
@@ -261,7 +232,7 @@ def test_terra_decoder_equals_the_reference(built, cuts):
     soft = o["soft"][:o["soft"].size // 8192 * 8192]
     want = O.Fec(O.ccsds_cfg("bpsk_90", 8192, 0.3, 20, **TERRA_FEC)).run(soft)
     g = capi.Fec(capi.ccsds_cfg("bpsk_90", 8192, 0.3, 20, max_soft=soft.size, **TERRA_FEC))
-    got = np.concatenate([g.push(soft[a:b]).frames() for a, b in zip([0, *cuts], [*cuts, soft.size])])
+    got = np.concatenate([g.push(soft[a:b]).frames() for a, b in pieces(soft.size, cuts)])
     assert got.shape[0] >= 60 and np.array_equal(got.reshape(-1), want["cadu"])
     s = g.stats()
     e = want["rs_err"]

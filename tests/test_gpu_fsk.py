@@ -9,6 +9,8 @@
 import numpy as np
 import pytest
 
+from tests.common import pieces, reference, run_chain, run_cli
+
 
 pytestmark = pytest.mark.gpu
 
@@ -57,9 +59,7 @@ def _metrics(a, b, sa, sb):
 @pytest.fixture(scope="module")
 def oracle_fsk(built):
     from oracle import fsk as O
-    if not O.available():
-        pytest.skip("oracle/_ref/libsatref_fsk.so was not built (the reference is absent)")
-    return O
+    return reference(O)
 
 
 @pytest.mark.parametrize("sig", SIGNALS, ids=[s[0] for s in SIGNALS])
@@ -165,7 +165,7 @@ def test_snr_follows_the_reference(oracle_fsk, cuts):
     d = capi.Demod(_cfg(sig, max_batch=n))
     raw = _signal(sig, n)
     syms, got = [], []
-    for a, b in zip([0, *cuts], [*cuts, n]):
+    for a, b in pieces(n, cuts):
         d.push(raw[2 * a:2 * b])
         syms.append(d.symbols())
         got.append(d.stats()["snr"])
@@ -222,35 +222,19 @@ def test_fused_chain(oracle_fsk, chain, pipelined):
     if dcfg.final_samplerate == 0:
         soft = oracle_fsk.Fsk(dcfg).run(_as_cf32(raw, fmt))["soft"]
         want = ref.Fec(ref.ccsds_cfg("bpsk_90", cs, 0.3, 20, 0)).run(soft)["cadu"].reshape(-1, cs // 8)
-    ch = capi.Chain(dcfg, _fec_cfg(cs, 2 * n))
-    if pipelined:
-        ch.set_pipelined(True)
-    per = 1 if fmt == "cf32" else 2
-    out = []
-    for a, b in [(0, n // 3), (n // 3, 2 * n // 3 + 1001), (2 * n // 3 + 1001, n)]:
-        ch.push(raw[per * a:per * b])
-        out.append(ch.frames())
-    if pipelined:
-        ch.sync()
-        out.append(ch.frames())
-    _check_tail(np.concatenate(out).reshape(-1, cs // 8), clear, want)
+    got, _ = run_chain(dcfg, _fec_cfg(cs, 2 * n), raw, fmt, pipelined)
+    _check_tail(got.reshape(-1, cs // 8), clear, want)
 
 
 def test_cli_two_stage_and_fused_agree(oracle_fsk, tmp_path):
     """b200_pipeline bluewalker3_narrow, two-stage and --fused, write the same .cadu: the sent frames after the lock"""
-    import os
-    import subprocess
-    from tests.common import ROOT
     raw, clear = _chain_signal(500_000, 128_000, 2648, "cs16")
     inp = tmp_path / "in.cs16"
     raw.tofile(inp)
-    tool = os.path.join(ROOT, "satdump_b200", "host", "b200_pipeline")
     outs = []
     for mode in ("two_stage", "fused"):
         hint = str(tmp_path / mode)
-        cmd = [tool, "bluewalker3_narrow", "baseband", str(inp), hint, "--samplerate", "500000", "--baseband_format", "cs16"]
-        r = subprocess.run(cmd + (["--fused"] if mode == "fused" else []), capture_output=True, text=True, timeout=300)
-        assert r.returncode == 0, r.stderr
+        run_cli("bluewalker3_narrow", inp, hint, "--samplerate", "500000", "--baseband_format", "cs16", fused=mode == "fused")
         outs.append(np.fromfile(hint + ".cadu", np.uint8).reshape(-1, 331))
     assert np.array_equal(outs[0], outs[1])
     _check_tail(outs[0], clear)

@@ -8,6 +8,7 @@ import pytest
 from satdump_b200 import capi, synth
 from tests import gac_cases as G
 from tests import gac_model as M
+from tests.common import pieces, run_chain, run_cli
 
 pytestmark = pytest.mark.gpu
 
@@ -20,7 +21,7 @@ def _cfg(name, max_soft=1 << 20):
 def _decode(name, soft, cuts=()):
     f = capi.Fec(_cfg(name))
     out, bits = [], []
-    for a, b in zip([0, *cuts], [*cuts, soft.size]):
+    for a, b in pieces(soft.size, cuts):
         f.push(soft[a:b])
         out.append(f.frames())
         bits.append(f.frame_bits())
@@ -89,19 +90,7 @@ def test_other_kinds_refuse_frame_bits():
 
 def _chain(cfg, raw, pipelined):
     n = raw.size // 2
-    ch = capi.Chain(capi.demod_cfg_for(cfg, max_batch=n), capi.fec_cfg_for(cfg, max_soft=n))
-    if pipelined:
-        ch.set_pipelined(True)
-    out = []
-    for a, b in [(0, n // 3), (n // 3, 2 * n // 3 + 1001), (2 * n // 3 + 1001, n)]:
-        ch.push(raw[2 * a:2 * b])
-        out.append(ch.frames())
-    if pipelined:
-        ch.sync()
-        out.append(ch.frames())
-    _, fs = ch.stats()
-    ch.close()
-    return np.concatenate(out), fs
+    return run_chain(capi.demod_cfg_for(cfg, max_batch=n), capi.fec_cfg_for(cfg, max_soft=n), raw, cfg.fmt, pipelined)
 
 
 @pytest.mark.parametrize("name", ["noaa_gac", "dmsp_rtd"])
@@ -125,29 +114,22 @@ def test_cli(built, tmp_path, name, mode):
     """b200_pipeline noaa_gac | dmsp_rtd (the pipelines' psk_demod and decoder parameters) writes the sent frames to .frm after the lock;
     DMSP's two-stage run writes one timestamp per frame by the reference's rule; a backward GAC run leaves no .frm.tmp behind"""
     import os
-    import subprocess
-    from tests.common import ROOT
     cfg = synth.CONFIGS[name]
     raw, clear = synth.make_signal(cfg, 1 << 21, seed=5)
     inp = tmp_path / "in.cs16"
     raw.numpy().tofile(inp)
     hint = str(tmp_path / "out")
-    tool = os.path.join(ROOT, "satdump_b200", "host", "b200_pipeline")
-    cmd = [tool, name, "baseband", str(inp), hint, "--samplerate", str(int(cfg.samplerate)), "--baseband_format", "cs16"]
-    if mode == "fused":
-        cmd.append("--fused")
-    elif name == "dmsp_rtd":
-        cmd += ["--start_timestamp", "1700000000.5"]
-    r = subprocess.run(cmd, capture_output=True, text=True, timeout=300)
-    assert r.returncode == 0, r.stderr
+    args = ["--samplerate", str(int(cfg.samplerate)), "--baseband_format", "cs16"]
+    if mode == "two_stage" and name == "dmsp_rtd":
+        args += ["--start_timestamp", "1700000000.5"]
+    r = run_cli(name, inp, hint, *args, fused=mode == "fused")
     nb = 4159 if name == "noaa_gac" else 19
     got = np.fromfile(hint + ".frm", np.uint8).reshape(-1, nb)
     sent = {bytes(x) for x in np.asarray(clear).reshape(-1, nb)}
     assert got.shape[0] >= 5 and sum(bytes(x) in sent for x in got) >= got.shape[0] - 2
     if name == "noaa_gac":
         assert f"frame_count {got.shape[0] // 11090}\n" in r.stdout
-        rb = subprocess.run(cmd + ["--backward", "true"], capture_output=True, text=True, timeout=300)
-        assert rb.returncode == 0, rb.stderr
+        run_cli(name, inp, hint, *args, "--backward", "true", fused=mode == "fused")
         assert os.path.exists(hint + ".frm") and not os.path.exists(hint + ".frm.tmp")
     else:
         assert "deframer_state " in r.stdout

@@ -4,6 +4,7 @@ against oracle/_ref where it was built, else against tests/golden/hrpt_pins.json
 import numpy as np
 import pytest
 
+from tests.common import assert_pin, pieces, run_chain, run_cli
 from tests.hrpt_cases import (LARGE, METEOR, MIX_AT, NOAA, boundary_cuts, digest, large_stream, params, piece_cuts, pins, stats_rows,
                               stream)
 
@@ -17,7 +18,7 @@ def run_gpu(soft, cuts, meteor, thr):
     cfg = capi.meteor_hrpt_cfg(max_soft=max(1 << 16, soft.size)) if meteor else capi.noaa_hrpt_cfg(thr, max_soft=max(1 << 16, soft.size))
     g = capi.Fec(cfg)
     out, recs, rows = [], [], []
-    for a, b in zip([0, *cuts], [*cuts, soft.size]):
+    for a, b in pieces(soft.size, cuts):
         g.push(soft[a:b])
         f = g.frames()
         out.append(f.reshape(-1).view(np.uint16) if not meteor else f)
@@ -31,7 +32,7 @@ def check(pin, soft, cuts, meteor, thr):
     from oracle import hrpt as O
     if O.available():
         r = O.run_pieces(soft, cuts, meteor, thr)
-        assert digest(r["out"]) == pin["out"] and r["recs"].tolist() == pin["recs"], "hrpt_pins.json is stale"
+        assert_pin(pin, "hrpt_pins.json", out=digest(r["out"]), recs=r["recs"].tolist())
     got, recs, rows, s = run_gpu(soft, cuts, meteor, thr)
     assert recs.tolist() == pin["recs"]
     assert got.shape[0] == pin["units"] and digest(got) == pin["out"]
@@ -107,7 +108,7 @@ def same_as_reference(got, name, meteor, clear):
     from oracle import hrpt as O
     if O.available():
         o, _, _ = chain_reference(name)
-        assert o.shape[0] == pin["units"] and digest(after_lock(frames_of(o, meteor), clear)) == pin["tail"], "hrpt_pins.json is stale"
+        assert_pin(pin, "hrpt_pins.json", units=o.shape[0], tail=digest(after_lock(frames_of(o, meteor), clear)))
     tail = after_lock(frames_of(got, meteor), clear)
     assert got.shape[0] == pin["units"] and tail.shape[0] == pin["ntail"] and digest(tail) == pin["tail"]
     assert pin["ntail"] >= 5 and all(any(np.array_equal(row, c) for c in clear) for row in tail)
@@ -122,20 +123,10 @@ def test_fused_chain(built, name, pipelined):
     from tests.hrpt_cases import chain_signal, demod_kwargs
     cfg, raw, clear = chain_signal(name)
     n = raw.size // 2
-    ch = capi.Chain(capi.demod_cfg(max_batch=n, **demod_kwargs(cfg)), capi.fec_cfg_for(cfg, max_soft=n))
-    if pipelined:
-        ch.set_pipelined(True)
-    out = []
-    for a, b in [(0, n // 3), (n // 3, 2 * n // 3 + 1001), (2 * n // 3 + 1001, n)]:
-        ch.push(raw[2 * a:2 * b])
-        out.append(ch.frames())
-    if pipelined:
-        ch.sync()
-        out.append(ch.frames())
+    got, fs = run_chain(capi.demod_cfg(max_batch=n, **demod_kwargs(cfg)), capi.fec_cfg_for(cfg, max_soft=n), raw, cfg.fmt, pipelined)
     meteor = name == "meteor_hrpt"
-    got = np.concatenate([o.reshape(-1) for o in out])
+    got = got.reshape(-1)
     same_as_reference(got.reshape(-1, 1024) if meteor else got.view(np.uint16), name, meteor, clear)
-    _, fs = ch.stats()
     assert fs["deframer_state"] == (12 if meteor else 0)
 
 
@@ -144,18 +135,12 @@ def test_fused_chain(built, name, pipelined):
 def test_cli(built, tmp_path, name, mode):
     """b200_pipeline noaa_hrpt | meteor_hrpt (the pipelines' pm_demod and decoder parameters) writes the reference's .raw16 / .cadu after
     the lock and reports the module's stats"""
-    import os
-    import subprocess
-    from tests.common import ROOT
     from tests.hrpt_cases import chain_signal
     cfg, raw, clear = chain_signal(name)
     inp = tmp_path / "in.cs16"
     raw.tofile(inp)
     hint = str(tmp_path / "out")
-    tool = os.path.join(ROOT, "satdump_b200", "host", "b200_pipeline")
-    cmd = [tool, name, "baseband", str(inp), hint, "--samplerate", str(int(cfg.samplerate)), "--baseband_format", "cs16"]
-    r = subprocess.run(cmd + (["--fused"] if mode == "fused" else []), capture_output=True, text=True, timeout=300)
-    assert r.returncode == 0, r.stderr
+    r = run_cli(name, inp, hint, "--samplerate", str(int(cfg.samplerate)), "--baseband_format", "cs16", fused=mode == "fused")
     meteor = name == "meteor_hrpt"
     got = np.fromfile(hint + ".cadu", np.uint8).reshape(-1, 1024) if meteor else np.fromfile(hint + ".raw16", np.uint16)
     same_as_reference(got, name, meteor, clear)

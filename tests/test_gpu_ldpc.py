@@ -2,15 +2,12 @@
 exact: given a soft stream, the CUDA path must reproduce the reference's CADUs, every frame's (offset, pos, correlator_corr, phase, swap,
 ldpc_corr) and the module statistics bit for bit; with internal_stream the inner frames and the deframer state. End to end (IQ ->
 psk_demod -> LDPC) through the fused chain and the C++ module layer the CADUs equal the reference's and the transmitted ones."""
-import os
-import subprocess
-
 import numpy as np
 import pytest
 
 from oracle import ldpc as O
 from satdump_b200 import synth
-from tests.common import match_frames
+from tests.common import match_frames, run_chain, run_cli
 
 pytestmark = pytest.mark.gpu
 
@@ -185,17 +182,7 @@ def test_fused_chain_end_to_end(oracle_built, name, pipelined):
     cfg, raw, clear = signal(name, 20, seed=3)
     want = _oracle_chain(cfg, raw)
     n = raw.size // 2
-    ch = capi.Chain(capi.demod_cfg_for(cfg, max_batch=n), capi.fec_cfg_for(cfg, max_soft=4 * n))
-    if pipelined:
-        ch.set_pipelined(True)
-    out = []
-    for a, b in [(0, n // 3), (n // 3, 2 * n // 3 + 1001), (2 * n // 3 + 1001, n)]:
-        ch.push(raw[2 * a:2 * b])
-        out.append(ch.frames())
-    if pipelined:
-        ch.sync()
-        out.append(ch.frames())
-    got = np.concatenate(out)
+    got, _ = run_chain(capi.demod_cfg_for(cfg, max_batch=n), capi.fec_cfg_for(cfg, max_soft=4 * n), raw, cfg.fmt, pipelined)
     assert got.shape[0] >= 5 and got.shape == want.shape
     same_after_lock(got, want, clear)
 
@@ -214,17 +201,14 @@ def same_after_lock(got, want, clear):
 def test_cli_module_layer(oracle_built, tmp_path, pipe, name, mode):
     """The C++ module layer with module id ccsds_ldpc_decoder (parameters parsed as CCSDSLDPCDecoderModule's constructor), as the CLI
     runs it: the .cadu file holds the reference's frames."""
-    from tests.common import ROOT, signal
+    from tests.common import signal
     cfg, raw, clear = signal(name, 20, seed=4)
     inp = tmp_path / "in.raw"
     raw.tofile(inp)
     want = _oracle_chain(cfg, raw)
     hint = str(tmp_path / "out")
-    tool = os.path.join(ROOT, "satdump_b200", "host", "b200_pipeline")
-    cmd = [tool, pipe, "baseband", str(inp), hint, "--samplerate", str(cfg.samplerate), "--symbolrate", str(int(cfg.symbolrate)),
-           "--baseband_format", cfg.fmt] + (["--fused"] if mode == "fused" else [])
-    r = subprocess.run(cmd, capture_output=True, text=True, timeout=300)
-    assert r.returncode == 0, r.stderr
+    run_cli(pipe, inp, hint, "--samplerate", str(cfg.samplerate), "--symbolrate", str(int(cfg.symbolrate)), "--baseband_format", cfg.fmt,
+            fused=mode == "fused")
     got = np.fromfile(hint + ".cadu", np.uint8).reshape(-1, cfg.cadu_bytes)
     assert got.shape[0] >= 5 and got.shape == want.shape
     same_after_lock(got, want, clear)

@@ -1,12 +1,10 @@
 """GPU: meteor_lrpt_decoder parity. The decoder is all-integer (hard correlator, Viterbi27, byte stage, RS), so the CUDA path must
 reproduce the reference bit for bit: every frame's (offset, pos, corr, phase, swap, RS errors, BER) record, every CADU byte and the stats
 after every push, against oracle/_ref where it was built, else against tests/golden/meteor_lrpt_pins.json."""
-import os
-import subprocess
-
 import numpy as np
 import pytest
 
+from tests.common import assert_pin, pieces, run_chain, run_cli
 from tests.meteor_lrpt_cases import (CASES, CHAIN, M2X, M2X_PARAMS, MSG, PIECES, after_lock, chain_signal, digest, piece_cuts, pins,
                                      stream)
 
@@ -21,7 +19,7 @@ def expected(name, pieces=False):
         case = CASES[name]
         soft, _, cuts = stream(case)
         r = O.run_pieces(soft, piece_cuts(soft.size) if pieces else cuts, case.get("diff", False))
-        assert digest(r["cadu"]) == pin["cadu"] and r["recs"].tolist() == pin["recs"], "meteor_lrpt_pins.json is stale"
+        assert_pin(pin, "meteor_lrpt_pins.json", cadu=digest(r["cadu"]), recs=r["recs"].tolist())
     return pin
 
 
@@ -29,7 +27,7 @@ def run_gpu(soft, cuts, diff, max_soft=None):
     from satdump_b200 import capi
     g = capi.Fec(capi.meteor_lrpt_cfg(diff, max_soft=max_soft or max(1 << 16, soft.size)))
     frames, recs = [], []
-    for a, b in zip([0, *cuts], [*cuts, soft.size]):
+    for a, b in pieces(soft.size, cuts):
         g.push(soft[a:b])
         frames.append(g.frames())
         recs.append(g.meteor_frames())
@@ -127,7 +125,7 @@ def chain_expected(name):
     if O.available():
         from tests.meteor_lrpt_cases import chain_reference
         cadu, clear = chain_reference(name)
-        assert cadu.shape[0] == pin["ncadu"] and digest(after_lock(cadu, clear)) == pin["tail"], "meteor_lrpt_pins.json is stale"
+        assert_pin(pin, "meteor_lrpt_pins.json", ncadu=cadu.shape[0], tail=digest(after_lock(cadu, clear)))
     return pin["ncadu"], pin["ntail"], pin["tail"]
 
 
@@ -149,18 +147,8 @@ def test_fused_chain(built, name, pipelined):
     from tests.common import demod_kwargs
     cfg, raw, clear = chain_signal(name)
     n = raw.size // 2
-    ch = capi.Chain(capi.demod_cfg(max_batch=n, **demod_kwargs(cfg)), capi.fec_cfg_for(cfg, max_soft=4 * n))
-    if pipelined:
-        ch.set_pipelined(True)
-    out = []
-    for a, b in [(0, n // 3), (n // 3, 2 * n // 3 + 1001), (2 * n // 3 + 1001, n)]:
-        ch.push(raw[2 * a:2 * b])
-        out.append(ch.frames())
-    if pipelined:
-        ch.sync()
-        out.append(ch.frames())
-    same_as_reference(np.concatenate(out), name, clear)
-    _, fs = ch.stats()
+    got, fs = run_chain(capi.demod_cfg(max_batch=n, **demod_kwargs(cfg)), capi.fec_cfg_for(cfg, max_soft=4 * n), raw, cfg.fmt, pipelined)
+    same_as_reference(got, name, clear)
     assert fs["correlator_lock"] == 1
 
 
@@ -168,16 +156,12 @@ def test_fused_chain(built, name, pipelined):
 def test_cli_meteor_lrpt(built, tmp_path, mode):
     """b200_pipeline meteor_lrpt (the 72k pipeline's psk_demod parameters, module id meteor_lrpt_decoder, diff_decode false) at the
     pipeline's default 1 MS/s: the .cadu file holds the reference's frames and the module reports lock_state"""
-    from tests.common import ROOT
     name = "meteor_lrpt_1m_cs16"
     cfg, raw, clear = chain_signal(name)
     inp = tmp_path / "in.cs16"
     raw.tofile(inp)
     hint = str(tmp_path / "out")
-    tool = os.path.join(ROOT, "satdump_b200", "host", "b200_pipeline")
-    cmd = [tool, "meteor_lrpt", "baseband", str(inp), hint, "--samplerate", str(int(cfg.samplerate)), "--baseband_format", "cs16"]
-    r = subprocess.run(cmd + (["--fused"] if mode == "fused" else []), capture_output=True, text=True, timeout=300)
-    assert r.returncode == 0, r.stderr
+    r = run_cli("meteor_lrpt", inp, hint, "--samplerate", str(int(cfg.samplerate)), "--baseband_format", "cs16", fused=mode == "fused")
     assert "lock_state SYNCED" in r.stdout
     same_as_reference(np.fromfile(hint + ".cadu", np.uint8).reshape(-1, 1024), name, clear)
 

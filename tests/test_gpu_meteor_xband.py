@@ -8,6 +8,7 @@ import pytest
 
 from satdump_b200 import capi, synth
 from tests import xband_cases as X
+from tests.common import pieces, run_chain, run_cli
 
 pytestmark = pytest.mark.gpu
 
@@ -17,7 +18,7 @@ TYPES = {0: "mtvza", 1: "kmss_bpsk"}
 def _decode(name, soft, cuts=(), max_soft=1 << 22):
     f = capi.Fec(capi.meteor_xband_cfg(TYPES[X.kind(name)], max_soft=max_soft))
     out = []
-    for a, b in zip([0, *cuts], [*cuts, soft.size]):
+    for a, b in pieces(soft.size, cuts):
         f.push(soft[a:b])
         out.append(f.frames())
     st = f.stats()
@@ -93,19 +94,7 @@ def _signal(name, fmt):
 
 def _chain(cfg, raw, pipelined):
     n = raw.size // 2 if cfg.fmt != "cf32" else raw.size
-    ch = capi.Chain(capi.demod_cfg_for(cfg, max_batch=n), capi.fec_cfg_for(cfg, max_soft=n))
-    if pipelined:
-        ch.set_pipelined(True)
-    out = []
-    for a, b in [(0, n // 3), (n // 3, 2 * n // 3 + 1001), (2 * n // 3 + 1001, n)]:
-        ch.push(raw[2 * a:2 * b] if cfg.fmt != "cf32" else raw[a:b])
-        out.append(ch.frames())
-    if pipelined:
-        ch.sync()
-        out.append(ch.frames())
-    _, fs = ch.stats()
-    ch.close()
-    return np.concatenate(out), fs
+    return run_chain(capi.demod_cfg_for(cfg, max_batch=n), capi.fec_cfg_for(cfg, max_soft=n), raw, cfg.fmt, pipelined)
 
 
 @pytest.mark.parametrize("fmt", ["cs16", "cf32"])
@@ -137,22 +126,15 @@ def test_chain(name, fmt):
 def test_cli(built, tmp_path, name):
     """b200_pipeline meteor_mtvza | meteor_kmss_bpsk (the pipelines' psk_demod and decoder parameters), two-stage and fused, write the
     same .frm, the sent frames"""
-    import os
-    import subprocess
-    from tests.common import ROOT
     cfg, raw, clear = _signal(name, "cs16")
     inp = tmp_path / "in.cs16"
     raw.tofile(inp)
-    tool = os.path.join(ROOT, "satdump_b200", "host", "b200_pipeline")
     nb = clear.shape[1]
     got = {}
     for mode in ("two_stage", "fused"):
         hint = str(tmp_path / mode)
-        cmd = [tool, name, "baseband", str(inp), hint, "--samplerate", str(int(cfg.samplerate)), "--baseband_format", "cs16"]
-        if mode == "fused":
-            cmd.append("--fused")
-        r = subprocess.run(cmd, capture_output=True, text=True, timeout=600)
-        assert r.returncode == 0, r.stderr
+        r = run_cli(name, inp, hint, "--samplerate", str(int(cfg.samplerate)), "--baseband_format", "cs16", fused=mode == "fused",
+                    timeout=600)
         got[mode] = np.fromfile(hint + ".frm", np.uint8).reshape(-1, nb)
         assert f"frame_count {got[mode].shape[0]}\n" in r.stdout
     assert np.array_equal(got["two_stage"], got["fused"])

@@ -1,12 +1,10 @@
 """GPU: metop_dump_decoder parity. The decoder is all-integer, so the CUDA path must reproduce the reference bit for bit: every frame's
 (offset, pos, corr, phase, swap, RS errors) record and every CADU byte, against oracle/_ref where it was built, else against
 tests/golden/metop_dump_pins.json."""
-import os
-import subprocess
-
 import numpy as np
 import pytest
 
+from tests.common import assert_pin, pieces, run_chain, run_cli
 from tests.metop_dump_cases import CASES, CHAIN, PIECES, after_lock, chain_signal, digest, piece_cuts, pins, stream
 
 pytestmark = pytest.mark.gpu
@@ -20,7 +18,7 @@ def expected(name):
     if O.available():
         soft, _, _ = stream(CASES[name])
         r = O.Dump().run(soft)
-        assert digest(r["cadu"]) == pin["cadu"] and r["recs"].tolist() == pin["recs"], "metop_dump_pins.json is stale"
+        assert_pin(pin, "metop_dump_pins.json", cadu=digest(r["cadu"]), recs=r["recs"].tolist())
     return pin["cadu"], pin["ncadu"], np.array(pin["recs"], np.int64).reshape(-1, 9)
 
 
@@ -28,7 +26,7 @@ def run_gpu(soft, cuts, max_soft=None):
     from satdump_b200 import capi
     g = capi.Fec(capi.dump_cfg(max_soft=max_soft or max(1 << 16, soft.size)))
     frames, recs = [], []
-    for a, b in zip([0, *cuts], [*cuts, soft.size]):
+    for a, b in pieces(soft.size, cuts):
         g.push(soft[a:b])
         frames.append(g.frames())
         recs.append(g.dump_frames())
@@ -99,7 +97,7 @@ def chain_expected(name):
         from tests.metop_dump_cases import chain_reference
         cadu, clear = chain_reference(name)
         tail = after_lock(cadu, clear)
-        assert cadu.shape[0] == pin["ncadu"] and digest(tail) == pin["tail"], "metop_dump_pins.json is stale"
+        assert_pin(pin, "metop_dump_pins.json", ncadu=cadu.shape[0], tail=digest(tail))
     return pin["ncadu"], pin["ntail"], pin["tail"]
 
 
@@ -122,18 +120,8 @@ def test_fused_chain(built, name, pipelined):
     from tests.common import demod_kwargs
     cfg, raw, clear = chain_signal(name)
     n = raw.size // 2
-    ch = capi.Chain(capi.demod_cfg(max_batch=n, **demod_kwargs(cfg)), capi.fec_cfg_for(cfg, max_soft=4 * n))
-    if pipelined:
-        ch.set_pipelined(True)
-    out = []
-    for a, b in [(0, n // 3), (n // 3, 2 * n // 3 + 1001), (2 * n // 3 + 1001, n)]:
-        ch.push(raw[2 * a:2 * b])
-        out.append(ch.frames())
-    if pipelined:
-        ch.sync()
-        out.append(ch.frames())
-    same_as_reference(np.concatenate(out), name, clear)
-    _, fs = ch.stats()
+    got, fs = run_chain(capi.demod_cfg(max_batch=n, **demod_kwargs(cfg)), capi.fec_cfg_for(cfg, max_soft=4 * n), raw, cfg.fmt, pipelined)
+    same_as_reference(got, name, clear)
     assert fs["correlator_lock"] == 1
 
 
@@ -141,15 +129,11 @@ def test_fused_chain(built, name, pipelined):
 def test_cli_metop_dump(built, tmp_path, mode):
     """b200_pipeline metop_dump (MetOp.json's psk_demod parameters, module id metop_dump_decoder): the .cadu file holds the reference's
     frames and the module reports lock_state"""
-    from tests.common import ROOT
     name = "metop_dump_cs16"
     cfg, raw, clear = chain_signal(name)
     inp = tmp_path / "in.cs16"
     raw.tofile(inp)
     hint = str(tmp_path / "out")
-    tool = os.path.join(ROOT, "satdump_b200", "host", "b200_pipeline")
-    cmd = [tool, "metop_dump", "baseband", str(inp), hint, "--samplerate", str(int(cfg.samplerate)), "--baseband_format", "cs16"]
-    r = subprocess.run(cmd + (["--fused"] if mode == "fused" else []), capture_output=True, text=True, timeout=300)
-    assert r.returncode == 0, r.stderr
+    r = run_cli("metop_dump", inp, hint, "--samplerate", str(int(cfg.samplerate)), "--baseband_format", "cs16", fused=mode == "fused")
     assert "lock_state SYNCED" in r.stdout
     same_as_reference(np.fromfile(hint + ".cadu", np.uint8).reshape(-1, 1024), name, clear)

@@ -6,6 +6,7 @@ reported."""
 import numpy as np
 import pytest
 
+from tests.common import assert_pin, run_chain, run_cli
 from tests.turbo_cases import CASES, RATE_NAME, digest, frame_size, pins, stream
 
 pytestmark = pytest.mark.gpu
@@ -19,7 +20,7 @@ def expected(name):
     if O.available():
         soft, _, _ = stream(case)
         r = O.Turbo(RATE_NAME[case["rate"]], case["base"], case["iters"]).run(soft)
-        assert digest(r["cadu"]) == pin["cadu"] and r["recs"].tolist() == pin["recs"], "turbo_pins.json is stale"
+        assert_pin(pin, "turbo_pins.json", cadu=digest(r["cadu"]), recs=r["recs"].tolist())
     return pin["cadu"], pin["ncadu"], np.array(pin["recs"], np.int64).reshape(-1, 6)
 
 
@@ -116,7 +117,7 @@ def chain_expected(name):
     pin = pins()["chain"][name]
     if O.available():
         want = chain_reference(name)
-        assert digest(want[2:]) == pin["tail"] and want.shape[0] == pin["ncadu"], "turbo_pins.json is stale"
+        assert_pin(pin, "turbo_pins.json", tail=digest(want[2:]), ncadu=want.shape[0])
     return pin["tail"], pin["ncadu"]
 
 
@@ -141,17 +142,9 @@ def test_fused_chain_end_to_end(built, name, pipelined):
     log2n, seed = CHAIN[name]
     cfg, raw, clear = signal(name, log2n, seed=seed)
     n = raw.size // 2
-    ch = capi.Chain(capi.demod_cfg(max_batch=n, **chain_demod_kwargs(cfg)), capi.fec_cfg_for(cfg, max_soft=4 * n))
-    if pipelined:
-        ch.set_pipelined(True)
-    out = []
-    for a, b in [(0, n // 3), (n // 3, 2 * n // 3 + 1001), (2 * n // 3 + 1001, n)]:
-        ch.push(raw[2 * a:2 * b])
-        out.append(ch.frames())
-    if pipelined:
-        ch.sync()
-        out.append(ch.frames())
-    same_after_lock(np.concatenate(out), name, clear)
+    got, _ = run_chain(capi.demod_cfg(max_batch=n, **chain_demod_kwargs(cfg)), capi.fec_cfg_for(cfg, max_soft=4 * n), raw, cfg.fmt,
+                       pipelined)
+    same_after_lock(got, name, clear)
 
 
 @pytest.mark.parametrize("name", ["turbo_pm", "turbo_bpsk"])
@@ -159,22 +152,17 @@ def test_fused_chain_end_to_end(built, name, pipelined):
 def test_cli_module_layer(built, tmp_path, name, mode):
     """The C++ module layer with module id ccsds_turbo_decoder (parameters parsed as CCSDSTurboDecoderModule's constructor), as the
     b200_pipeline CLI runs it with the Juice / Psyche module parameters: the .cadu file holds the reference's frames."""
-    import os
-    import subprocess
-    from tests.common import ROOT, signal
+    from tests.common import signal
     from tests.turbo_cases import CHAIN
     log2n, seed = CHAIN[name]
     cfg, raw, clear = signal(name, log2n, seed=seed)
     inp = tmp_path / "in.raw"
     raw.tofile(inp)
     hint = str(tmp_path / "out")
-    tool = os.path.join(ROOT, "satdump_b200", "host", "b200_pipeline")
     # pm_demod's own clock-recovery defaults (0.01) differ from the psk_demod ones the checker's configuration carries: pass those
     extra = ["--clock_gain_omega", repr(float(np.float32(8.7e-3 ** 2 / 4.0))), "--clock_gain_mu", "0.0087"] if name == "turbo_pm" else []
-    cmd = [tool, name, "baseband", str(inp), hint, "--samplerate", str(int(cfg.samplerate)), "--symbolrate", str(int(cfg.symbolrate)),
-           "--baseband_format", cfg.fmt] + extra + (["--fused"] if mode == "fused" else [])
-    r = subprocess.run(cmd, capture_output=True, text=True, timeout=300)
-    assert r.returncode == 0, r.stderr
+    run_cli(name, inp, hint, "--samplerate", str(int(cfg.samplerate)), "--symbolrate", str(int(cfg.symbolrate)), "--baseband_format", cfg.fmt,
+            *extra, fused=mode == "fused")
     got = np.fromfile(hint + ".cadu", np.uint8).reshape(-1, cfg.cadu_bytes)
     same_after_lock(got, name, clear)
 

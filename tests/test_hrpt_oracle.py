@@ -5,16 +5,11 @@ every case, and a missing deframer_thresold is refused by name."""
 import numpy as np
 import pytest
 
+from oracle import hrpt as O
+from tests.common import reference
 from tests.hrpt_cases import METEOR, NOAA, boundary_cuts, digest, params, piece_cuts, pins, stats_rows, stream
 
 CASES = [*NOAA, *METEOR]
-
-
-def _ref():
-    from oracle import hrpt as O
-    if not O.available():
-        pytest.skip("oracle/_ref/libsatref_hrpt.so not built (the reference is absent): the tests compare with the pins")
-    return O
 
 
 def _same(r, pin):
@@ -25,7 +20,7 @@ def _same(r, pin):
 
 @pytest.mark.parametrize("name", CASES)
 def test_reference_equals_pins(name):
-    O = _ref()
+    reference(O)
     soft, cuts = stream(name)
     _same(O.run_pieces(soft, cuts, *params(name)), pins()["cases"][name])
     _same(O.run_pieces(soft, piece_cuts(soft.size, extra=boundary_cuts(name)), *params(name)), pins()["pieces"][name])
@@ -34,7 +29,7 @@ def test_reference_equals_pins(name):
 @pytest.mark.parametrize("name", CASES)
 def test_record_keeping_changes_nothing(name):
     """One work() call per byte (to see each accepted sync) writes what the module's 8192-byte reads write"""
-    O = _ref()
+    reference(O)
     soft, _ = stream(name)
     a, b = O.Hrpt(*params(name)).run(soft), O.Hrpt(*params(name)).run(soft, records=False)
     assert np.array_equal(a["out"], b["out"]) and a["stats"] == b["stats"]
@@ -42,7 +37,7 @@ def test_record_keeping_changes_nothing(name):
 
 @pytest.mark.parametrize("meteor", [False, True])
 def test_synthesised_frames_come_out_as_sent(meteor):
-    O = _ref()
+    reference(O)
     from satdump_b200 import synth
     bits, sent = (synth.meteor_hrpt_frames if meteor else synth.noaa_hrpt_frames)(12, seed=3)
     lead = np.random.default_rng(5).integers(0, 2, 1000).astype(np.uint8)

@@ -2,8 +2,8 @@
 reference's; the C restatement (oracle/ldpc_port.c) equals the reference's own decoder, correlator and module loop bit for bit (directly
 against oracle/_ref, or through the digests of tests/golden/ldpc_pins.json where it is absent); synthesised codewords satisfy H c = 0
 and decode to the transmitted frames; and the decoder's configuration refuses what is not built, by name."""
+import functools
 import hashlib
-import json
 import os
 
 import numpy as np
@@ -11,7 +11,7 @@ import pytest
 
 from oracle import ldpc as O
 from satdump_b200 import synth
-from tests.common import ROOT
+from tests.common import ROOT, load_pins
 
 PINS = os.path.join(ROOT, "tests", "golden", "ldpc_pins.json")
 # decoder alone: random LLRs (sigma) at 1, 10 and 50 iterations; module loop: soft streams (constellation, sigma, rotation, Q late, edit)
@@ -86,9 +86,7 @@ def digest_matrix(impl):
     return _h(O.matrix(impl).astype(np.int32))
 
 
-def pins():
-    with open(PINS) as f:
-        return json.load(f)
+pins = functools.partial(load_pins, PINS)
 
 
 def test_table_reproduces_the_reference_matrix(libs):

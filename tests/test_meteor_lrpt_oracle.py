@@ -4,19 +4,14 @@ configuration, and the decoder's refusals name their option before a device is t
 import numpy as np
 import pytest
 
+from oracle import meteor as O
+from tests.common import reference
 from tests.meteor_lrpt_cases import CASES, M2X, M2X_PARAMS, PIECES, digest, piece_cuts, pins, stream
-
-
-def _ref():
-    from oracle import meteor as O
-    if not O.available():
-        pytest.skip("oracle/_ref/libsatref_meteor.so not built (the reference is absent): the GPU tests compare with the pins")
-    return O
 
 
 @pytest.mark.parametrize("name", sorted(CASES))
 def test_reference_equals_pins(name):
-    O = _ref()
+    reference(O)
     case = CASES[name]
     soft, _, cuts = stream(case)
     r = O.run_pieces(soft, cuts, case.get("diff", False))
@@ -26,7 +21,7 @@ def test_reference_equals_pins(name):
 
 @pytest.mark.parametrize("name", PIECES)
 def test_reference_in_pieces_equals_pins(name):
-    O = _ref()
+    reference(O)
     case = CASES[name]
     soft, _, _ = stream(case)
     r = O.run_pieces(soft, piece_cuts(soft.size), case.get("diff", False))
@@ -42,7 +37,7 @@ def test_synthesised_frames_decode_to_the_transmitted_ones(diff):
     With NRZ-M the transmitted ASM is the syncword or its complement, depending on the parity before it; the correlator then also finds
     the table's IQ-swapped entries, whose frames the Viterbi decoder cannot decode and RS drops, so the frames written are transmitted ones,
     in order."""
-    O = _ref()
+    reference(O)
     from satdump_b200 import synth
     coded, written = synth.lrpt_frames(10, seed=5, nrzm=diff, inverted=(4,))
     r = O.Meteor(diff).run(synth.lrpt_soft(coded, sigma=25.0, seed=6))
@@ -60,7 +55,7 @@ def test_m2x_mode_is_the_conv_concat_oqpsk_configuration(name):
     rs_i 4, rs_dualbasis false, rs_usecheck): the same frames are written and the stats agree, so the decoder runs m2x_mode as that
     configuration. The stats keys are the same in both modules (deframer_lock, viterbi_ber, viterbi_lock, rs_avg, viterbi_state,
     deframer_state)."""
-    O = _ref()
+    reference(O)
     from oracle import ref
     if not ref.available():
         pytest.skip("oracle/_ref not built")

@@ -8,9 +8,7 @@ from oracle import xband
 from satdump_b200 import capi, synth
 from tests import xband_cases as X
 from tests import xband_model as M
-
-needs_ref = pytest.mark.skipif(not xband.available(), reason="oracle/_ref not built (reference absent)")
-
+from tests.common import load_pins, reference
 
 @pytest.mark.parametrize("name", X.CASES)
 def test_model_equals_reference(name):
@@ -22,17 +20,15 @@ def test_model_equals_reference(name):
 @pytest.mark.parametrize("name", X.CASES)
 def test_pins_are_current(name):
     """the pins hold what the reference computes (they stand in for it where it is absent)"""
-    import json
-    with open(X.PINS) as f:
-        pin = json.load(f)[name]
+    pin = load_pins(X.PINS)[name]
     if xband.available():
         assert pin == X.reference(name)
     assert pin["frames"] == pin["frame_count"]
 
 
-@needs_ref
 @pytest.mark.parametrize("kmss,cut", [(False, None), (False, (7, 200)), (True, None), (True, (1, 30000))])
 def test_synthesised_streams_decode_to_the_sent_frames(kmss, cut):
+    reference(xband)
     rng = np.random.default_rng(3)
     bits, sent = synth.meteor_xband_frames(kmss, 5 if kmss else 40, seed=11, cut=cut)
     bits = np.concatenate([[0], bits])  # (a clean first bit: the frame in the first record is then found too)
@@ -41,9 +37,9 @@ def test_synthesised_streams_decode_to_the_sent_frames(kmss, cut):
     assert np.array_equal(got, sent)
 
 
-@needs_ref
 def test_reference_in_pieces_equals_whole():
     """the harness decodes whole reads only, whatever the pieces"""
+    reference(xband)
     soft = X.stream("kmss_all_deframers_one_read")
     r = xband.Ref(1)
     out = np.concatenate([r.run(soft[a:a + 100003])["out"] for a in range(0, soft.size, 100003)])

@@ -6,18 +6,13 @@ import pytest
 
 from oracle import dump as O
 from satdump_b200 import synth
+from tests.common import reference
 from tests.metop_dump_cases import CASES, F, digest, pins, stream
-
-
-
-def _ref():
-    if not O.available():
-        pytest.skip("oracle/_ref/libsatref_dump.so not built (the reference is absent): the pins stand for it")
 
 
 @pytest.mark.parametrize("name", sorted(CASES))
 def test_pins_are_the_reference(name):
-    _ref()
+    reference(O)
     soft, _, _ = stream(CASES[name])
     r = O.Dump().run(soft)
     pin = pins()["cases"][name]

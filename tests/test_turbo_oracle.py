@@ -9,16 +9,13 @@ import numpy as np
 import pytest
 
 from satdump_b200 import synth
-from tests.turbo_cases import CASES, RATE_NAME, digest, frame_size, pins, stream
+from tests.common import reference
+from tests.turbo_cases import CASES, RATE_NAME, digest, encoder_info, frame_size, pins, stream
 
 
 def _ref():
     from oracle import turbo as O
     return O if O.available() else None
-
-
-def encoder_info(rate, base):
-    return np.random.default_rng(rate * 7 + base).integers(0, 256, base, dtype=np.uint8)
 
 
 @pytest.mark.parametrize("base", synth.TURBO_BASES)
@@ -53,9 +50,8 @@ def test_crc_matches_frame_layout():
 @pytest.mark.parametrize("name", ["combo_2_223", "combo_6_223", "swapped", "noise_signal_noise", "crc_failures"])
 def test_pins_are_the_reference(name):
     """Where the reference was built, it reproduces the pinned records and CADUs."""
-    O = _ref()
-    if not O:
-        pytest.skip("oracle/_ref/libsatref_turbo.so not built (the reference is absent): the pins stand for it")
+    from oracle import turbo
+    O = reference(turbo)
     case = CASES[name]
     soft, _, _ = stream(case)
     r = O.Turbo(RATE_NAME[case["rate"]], case["base"], case["iters"]).run(soft)
@@ -123,8 +119,8 @@ def test_missing_parameters(missing, text):
 def test_llr_golden_is_the_reference(name):
     """tests/golden/turbo_llr.npz holds what the reference's convcode_extrinsic computes, bit for bit, for the frames of the LLR cases."""
     from tests.turbo_cases import LLR, llr_frames, reference_llr
-    if not _ref():
-        pytest.skip("oracle/_ref/libsatref_turbo.so not built (the reference is absent)")
+    from oracle import turbo
+    reference(turbo)
     case = CASES[name]
     gold = np.load(LLR)
     frames = llr_frames(name)

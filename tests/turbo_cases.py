@@ -1,12 +1,12 @@
 """Soft streams of the ccsds_turbo_decoder tests, rebuilt from seeds on any machine. tests/golden/make_turbo_pins.py runs the reference on
 each of them and stores digests of its output in tests/golden/turbo_pins.json, which the tests read where the reference is absent."""
-import hashlib
-import json
+import functools
 import os
 
 import numpy as np
 
 from satdump_b200 import synth
+from tests.common import digest, load_pins  # noqa: F401
 
 PINS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "turbo_pins.json")
 LLR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "turbo_llr.npz")
@@ -70,13 +70,12 @@ CASES.update({
 })
 
 
-def digest(a):
-    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
+pins = functools.partial(load_pins, PINS)
 
 
-def pins():
-    with open(PINS) as f:
-        return json.load(f)
+def encoder_info(rate, base):
+    """the information bytes the encoder pins encode"""
+    return np.random.default_rng(rate * 7 + base).integers(0, 256, base, dtype=np.uint8)
 
 
 # IQ -> demodulator -> ccsds_turbo_decoder: satdump_b200.synth configurations, log2 of the sample count, seed

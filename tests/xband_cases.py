@@ -1,12 +1,13 @@
 """The meteor_xband_decoder case streams (soft bytes, a multiple of the module's 8192-byte reads) shared by the oracle, model and GPU
 tests, and the reference's result for each: oracle/_ref when built, else tests/golden/meteor_xband_pins.json."""
 import hashlib
-import json
+import functools
 import os
 
 import numpy as np
 
 from satdump_b200 import synth
+from tests import common
 
 PINS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "meteor_xband_pins.json")
 READ = 8192
@@ -91,8 +92,7 @@ def kind(name):
     return 1 if name.startswith("kmss") else 0
 
 
-def digest(frames):
-    return hashlib.sha256(np.ascontiguousarray(frames, np.uint8).tobytes()).hexdigest()
+digest = functools.partial(common.digest, dtype=np.uint8)
 
 
 def reference(name):
@@ -105,5 +105,4 @@ def ref_result(name):
     from oracle import xband
     if xband.available():
         return reference(name)
-    with open(PINS) as f:
-        return json.load(f)[name]
+    return common.load_pins(PINS)[name]

@@ -10,10 +10,11 @@ struct Dump : Correlated
 {
     DumpSync sw{};
     DevBuf<uint32_t> hw;
+    FrameStage fs;              // the RS tables and results of k_dump_frames
 
     explicit Dump(Fec &f);
     void process(Fec &f) override;
-    long records(const Fec &f, b200_dump_frame *out, long cap) const; // of the last push
+    long records(b200_dump_frame *out, long cap) const; // of the last push
 };
 
 namespace
@@ -36,10 +37,8 @@ uint32_t swap_iq(uint32_t w) { return ((w & 0xaaaaaaaau) >> 1) | ((w & 0x5555555
 Dump::Dump(Fec &f)
 {
     B200_REQUIRE(f.cfg.max_soft <= (1L << 30), B200_EINVAL, "max_soft must be <= 2^30 for the MetOp dump decoder");
-    f.geom.chunk = DUMP_F;
+    f.chunk = DUMP_F;
     f.cadu_bytes = DUMP_CADU;
-    f.cfg.cadu_size = DUMP_CADU * 8;
-    f.cfg.constellation = B200_QPSK;
     for (int p = 0; p < 4; p++) {
         sw.w[p] = rotate_64(0x1acffc1du, p);
         sw.w[4 + p] = rotate_64(swap_iq(0x1acffc1du) ^ 0xffffffffu, p); // (the module's 0xFFFFFFFFFF truncated to 32 bits)
@@ -48,18 +47,12 @@ Dump::Dump(Fec &f)
     DeviceGuard g(f.cfg.device);
     const long fifo = f.cfg.max_soft + 2L * DUMP_F;
     alloc(fifo / 2, fifo / DUMP_F + 2); // scores at the even positions
-    f.framed_storage(DUMP_F, max_frames);
+    f.open(DUMP_F, max_frames);
     hw.alloc((size_t)fifo / 32 + 8);
-    f.rs_err.alloc((size_t)max_frames * DUMP_RS_I);
-    f.h_rs_err.alloc((size_t)max_frames * DUMP_RS_I);
-    f.tables.alloc(1);
-    RsTables T;
-    build_rs_tables(T);
-    B200_CUDA(cudaMemcpyAsync(f.tables.p, &T, sizeof(T), cudaMemcpyHostToDevice, f.stream));
-    B200_CUDA(cudaStreamSynchronize(f.stream)); // (T dies here)
+    fs.alloc(f, max_frames, DUMP_RS_I, false);
 }
 
-std::unique_ptr<Framed> dump_decoder(Fec &f) { return std::make_unique<Dump>(f); }
+std::unique_ptr<Decoder> dump_decoder(Fec &f) { return std::make_unique<Dump>(f); }
 
 // The module loop over every frame the FIFO completes: hard bits, correlation at every even position, the frame walk, then all its frames
 // at once into frames_out (rs_err and h_rs_err: RS results of the last push's frames).
@@ -79,28 +72,22 @@ void Dump::process(Fec &f)
     if (nf > 0) {
         B200_REQUIRE((size_t)(f.out_frames + nf) * DUMP_CADU <= f.frames_out.n, B200_ESTATE,
                      "%ld frames not pulled yet: pull the frames between pushes", f.out_frames);
-        k_dump_frames<<<nf, 256, 0, stream>>>(f.softbuf.p, frames.p, f.tables.p, f.frames_out.p + f.out_frames * DUMP_CADU, f.rs_err.p);
+        k_dump_frames<<<nf, 256, 0, stream>>>(f.softbuf.p, frames.p, fs.tables.p, f.frames_out.p + f.out_frames * DUMP_CADU, fs.rs_err.p);
         f.launches++;
         B200_CUDA(cudaMemcpyAsync(h_frames.p, frames.p, sizeof(WalkFrame) * nf, cudaMemcpyDeviceToHost, stream));
-        B200_CUDA(cudaMemcpyAsync(f.h_rs_err.p, f.rs_err.p, sizeof(int) * nf * DUMP_RS_I, cudaMemcpyDeviceToHost, stream));
+        B200_CUDA(cudaMemcpyAsync(fs.h_rs_err.p, fs.rs_err.p, sizeof(int) * nf * DUMP_RS_I, cudaMemcpyDeviceToHost, stream));
     }
     f.keep_soft_tail(h_walk.p->next);
     end(f);
     finish(nf, f.soft_have);
-    for (int i = 0; i < nf * DUMP_RS_I; i++) {
-        const int e = f.h_rs_err.p[i];
-        if (e == -1)
-            f.rs_failed++;
-        else
-            f.rs_corrected += e;
-    }
+    fs.count_rs(f, nf, DUMP_RS_I);
     f.out_frames += nf;
     f.total_frames += nf;
     f.total_chunks += nf;
     f.total_bits += (long)nf * DUMP_CADU * 8;
 }
 
-long Dump::records(const Fec &f, b200_dump_frame *out, long cap) const
+long Dump::records(b200_dump_frame *out, long cap) const
 {
     B200_REQUIRE(last_nf <= cap, B200_ESTATE, "output buffer too small: need %ld records", last_nf);
     for (long k = 0; k < last_nf; k++) {
@@ -112,7 +99,7 @@ long Dump::records(const Fec &f, b200_dump_frame *out, long cap) const
         d.phase = r.phase;
         d.swap = r.swap;
         for (int i = 0; i < DUMP_RS_I; i++)
-            d.rs[i] = f.h_rs_err.p[k * DUMP_RS_I + i];
+            d.rs[i] = fs.h_rs_err.p[k * DUMP_RS_I + i];
     }
     return last_nf;
 }
@@ -125,7 +112,6 @@ extern "C" int b200_fec_debug_dump_frames(b200_fec *h, b200_dump_frame *out, lon
 {
     return guarded([&] {
         B200_REQUIRE(h && out && n_out, B200_EINVAL, "NULL argument");
-        Fec &f = *h->f;
-        *n_out = f.framed_as<Dump>("not a MetOp dump decoder").records(f, out, cap);
+        *n_out = h->f->decoder_as<Dump>("not a MetOp dump decoder").records(out, cap);
     });
 }

@@ -19,11 +19,12 @@
 namespace b200
 {
 
-struct SyncWalk : Framed
+struct SyncWalk : Decoder
 {
     enum Machine { NOAA, METEOR, DMSP } m;
     int thr = 0; // NOAA: deframer_thresold
     long max_seg = 0;
+    int dmsp_state = 0;               // DMSP: the state after its last complete push
     DevBuf<uint32_t> hw, cand;
     DevBuf<HrptRec> recs;             // every accepted sync
     DevBuf<HrptSeg> segs;             // NOAA / METEOR: what the gathers write
@@ -46,6 +47,7 @@ struct SyncWalk : Framed
 SyncWalk::SyncWalk(Fec &f)
     : m(f.cfg.kind == B200_FEC_NOAA_HRPT ? NOAA : (f.cfg.kind == B200_FEC_METEOR_HRPT ? METEOR : DMSP))
 {
+    keeps_frame_bits = m == DMSP;
     if (m == NOAA) {
         thr = f.cfg.deframer_thresold;
         B200_REQUIRE(thr >= 0 && thr <= 60, B200_EINVAL, "noaa_hrpt_decoder: deframer_thresold must be 0..60 (got %d)", thr);
@@ -53,14 +55,14 @@ SyncWalk::SyncWalk(Fec &f)
     B200_REQUIRE(f.cfg.max_soft <= (1L << 30), B200_EINVAL, "max_soft must be <= 2^30 for %s", m == DMSP ? "dmsp_rtd_decoder" : "the HRPT decoders");
     // one output unit per NOAA word / METEOR CADU / DMSP frame, so that frames_out and b200_chain work unchanged
     f.cadu_bytes = m == NOAA ? 2 : (m == METEOR ? MH_CADU : DMSP_BYTES);
-    f.geom.chunk = 8192; // the modules' read size: what a stream reader of the decoder hands over at a time (b200_fec_chunk_size)
+    f.chunk = 8192; // the modules' read size: what a stream reader of the decoder hands over at a time (b200_fec_chunk_size)
     const int frame_bits = m == NOAA ? NOAA_WORDS * 10 : (m == METEOR ? MH_PERIOD : DMSP_BITS);
     const long fifo = f.cfg.max_soft + 2L * frame_bits;
     // a push accepts at most one sync per frame length (NOAA: per frame's data bits), plus the frame left open by the push before
     max_seg = fifo / (m == NOAA ? NOAA_DATA_BITS : frame_bits) + 4;
     check_device(f.cfg.device);
     DeviceGuard g(f.cfg.device);
-    f.framed_storage(frame_bits, m == NOAA ? fifo / 10 + NOAA_WORDS * 2 : max_seg);
+    f.open(frame_bits, m == NOAA ? fifo / 10 + NOAA_WORDS * 2 : max_seg);
     hw.alloc((size_t)fifo / 32 + 8);
     cand.alloc((size_t)fifo / 32 + 8);
     recs.alloc((size_t)max_seg);
@@ -79,13 +81,13 @@ SyncWalk::SyncWalk(Fec &f)
     reset(f);
 }
 
-std::unique_ptr<Framed> sync_walk_decoder(Fec &f) { return std::make_unique<SyncWalk>(f); }
+std::unique_ptr<Decoder> sync_walk_decoder(Fec &f) { return std::make_unique<SyncWalk>(f); }
 
 // a fresh deframer: NOSYNC / IDLE / state 0, no inversion, the shifter 0 (the NOAA reference leaves it uninitialised: DESIGN §9)
 void SyncWalk::reset(Fec &f)
 {
-    Framed::reset(f);
-    f.defr_state_now = 0;
+    Decoder::reset(f);
+    dmsp_state = 0;
     if (m == DMSP) {
         memset(h_dmsp_st.p, 0, sizeof(DmspState));
         h_dmsp_st.p->open = HRPT_NONE;
@@ -99,12 +101,10 @@ void SyncWalk::reset(Fec &f)
     B200_CUDA(cudaStreamSynchronize(f.stream));
 }
 
-// NOAA / METEOR report the state the last walk left, also when its push failed after the walk; DMSP reports defr_state_now, the state
-// after its last complete push
+// NOAA / METEOR report the state the last walk left, also when its push failed after the walk; DMSP the state after its last complete push
 void SyncWalk::stats(b200_fec_stats *o)
 {
-    if (m != DMSP)
-        o->deframer_state = h_st.p->state;
+    o->deframer_state = m == DMSP ? dmsp_state : h_st.p->state;
 }
 
 void SyncWalk::process(Fec &f)
@@ -180,7 +180,8 @@ void SyncWalk::process(Fec &f)
     f.out_frames += o.units;
     f.total_frames += o.units;
     f.total_bits += have - f.soft_have;
-    f.defr_state_now = m == DMSP ? h_dmsp_st.p->state : h_st.p->state;
+    if (m == DMSP)
+        dmsp_state = h_dmsp_st.p->state;
 }
 
 long SyncWalk::records(b200_hrpt_frame *out, long cap) const
@@ -238,22 +239,27 @@ void gac_pn_bytes(uint8_t *pn)
 // Every push's bits enter the bit FIFO (aqua_db_decoder: k_aqua_bits, noaa_gac_decoder: k_gac_bits), the deframer and frame stage of the
 // convolutional decoders run with the decoder's settings, and noaa_gac_decoder's k_gac_post reverses (backward) and descrambles the frames
 // in the output.
-struct BitStage : Framed
+struct BitStage : Decoder
 {
     bool gac;
     int F;                            // the soft bytes a push needs (aqua_db_decoder: a complete symbol behind the carried one)
     long dropped = 0;                 // bit FIFO bits dropped by compaction: FIFO bit q is stream bit q - 32 + dropped
     DevBuf<uint8_t> pn;               // noaa_gac_decoder: the bytes XORed onto every frame ...
     PinnedBuf<FrameRec> h_fr;         // ... and the deframer's records of the last push
+    Deframer defr;
+    FrameStage fs;
 
     explicit BitStage(Fec &f);
     void process(Fec &f) override;
     void reset(Fec &f) override;
+    void stats(b200_fec_stats *o) override { o->deframer_state = defr.state_now; }
+    const Deframer *deframer() const override { return &defr; }
 };
 
 BitStage::BitStage(Fec &f) : gac(f.cfg.kind == B200_FEC_NOAA_GAC), F(gac ? 1 : 2 * AQUA_LEAD)
 {
     b200_fec_cfg &c = f.cfg;
+    keeps_frame_bits = gac;
     if (gac)
         B200_REQUIRE(c.backward == 0 || c.backward == 1, B200_EINVAL, "noaa_gac_decoder: backward must be 0 or 1 (got %d)", c.backward);
     B200_REQUIRE(c.max_soft <= (1L << 30), B200_EINVAL, "max_soft must be <= 2^30 for %s", gac ? "noaa_gac_decoder" : "aqua_db_decoder");
@@ -273,16 +279,18 @@ BitStage::BitStage(Fec &f) : gac(f.cfg.kind == B200_FEC_NOAA_GAC), F(gac ? 1 : 2
     c.rs_dualbasis = s.rs_dualbasis;
     c.nrzm = c.derand_after_rs = c.rs_type = c.rs_usecheck = 0;
     c.rs_fill_bytes = -1;
-    f.st_synced = s.st_synced;
     f.cadu_bytes = s.cadu_bytes;
-    f.geom.chunk = s.chunk;
+    f.chunk = s.chunk;
     check_device(c.device);
     DeviceGuard g(c.device);
-    f.framed_storage(F, 0);
-    f.deframer_storage(c.max_soft + (gac ? 0 : 2 * AQUA_LEAD)); // one bit per soft byte
+    const long max_bits = c.max_soft + (gac ? 0 : 2 * AQUA_LEAD); // one bit per soft byte
+    const long max_frames = Deframer::frames_cap(max_bits, c.cadu_size);
+    f.open(F, max_frames);
+    defr.alloc(f, max_bits, c.cadu_size, c.asm_sync, s.st_synced);
+    fs.alloc(f, max_frames, c.rs_i, false);
     if (gac) {
         pn.alloc(GAC_BYTES);
-        h_fr.alloc((size_t)f.max_frames_push);
+        h_fr.alloc((size_t)max_frames);
         std::vector<uint8_t> h_pn(GAC_BYTES);
         gac_pn_bytes(h_pn.data());
         B200_CUDA(cudaMemcpy(pn.p, h_pn.data(), GAC_BYTES, cudaMemcpyHostToDevice));
@@ -290,12 +298,12 @@ BitStage::BitStage(Fec &f) : gac(f.cfg.kind == B200_FEC_NOAA_GAC), F(gac ? 1 : 2
     reset(f);
 }
 
-std::unique_ptr<Framed> bit_stage_decoder(Fec &f) { return std::make_unique<BitStage>(f); }
+std::unique_ptr<Decoder> bit_stage_decoder(Fec &f) { return std::make_unique<BitStage>(f); }
 
 void BitStage::reset(Fec &f)
 {
-    f.start_stream(64); // the bit FIFO and the deframer
-    Framed::reset(f);
+    defr.start(f, 64);
+    Decoder::reset(f);
     dropped = 0;
     if (!gac) {
         B200_CUDA(cudaMemsetAsync(f.softbuf.p, 0, AQUA_LEAD, f.stream));
@@ -309,25 +317,24 @@ void BitStage::process(Fec &f)
     if (!begin(f, F))
         return;
     cudaStream_t stream = f.stream;
-    const long fb0 = f.fifo_bits;
-    f.compact_fifo(false);
-    dropped += fb0 - f.fifo_bits;
+    const long fb0 = defr.fifo_bits;
+    defr.compact(f);
+    dropped += fb0 - defr.fifo_bits;
     const long nbits = gac ? f.soft_have : (f.soft_have / 2 - 1) * 2;
-    B200_REQUIRE(((f.fifo_bits + nbits + 64) >> 5) + 2 < (long)f.fifo.n, B200_ESTATE, "internal: bit FIFO too small");
+    B200_REQUIRE(((defr.fifo_bits + nbits + 64) >> 5) + 2 < (long)defr.fifo.n, B200_ESTATE, "internal: bit FIFO too small");
     B200_CUDA(cudaEventRecord(f.ev[0], stream));
-    const long words = (f.fifo_bits + nbits + 31) / 32 - f.fifo_bits / 32;
+    const long words = (defr.fifo_bits + nbits + 31) / 32 - defr.fifo_bits / 32;
     const auto bits_kernel = gac ? k_gac_bits : k_aqua_bits;
-    bits_kernel<<<(unsigned)std::min<long>((words + 7) / 8, 132 * 32), 256, 0, stream>>>(f.softbuf.p, nbits, f.fifo.p, f.fifo_bits);
+    bits_kernel<<<(unsigned)std::min<long>((words + 7) / 8, 132 * 32), 256, 0, stream>>>(f.softbuf.p, nbits, defr.fifo.p, defr.fifo_bits);
     f.launches++;
-    f.last_bits0 = f.fifo_bits;
+    f.last_bits0 = defr.fifo_bits;
     f.last_nbits = nbits;
     const long out0 = f.out_frames;
-    f.deframe_and_rs(nbits); // (synchronises the stream)
-    const int nf = f.last_nf;
+    const int nf = defr.deframe(f, fs, nbits); // (synchronises the stream)
     if (gac && nf > 0) {
         k_gac_post<<<nf, 256, 0, stream>>>(f.frames_out.p + out0 * GAC_BYTES, f.cfg.backward, pn.p);
         f.launches++;
-        B200_CUDA(cudaMemcpyAsync(h_fr.p, f.frames.p, sizeof(FrameRec) * nf, cudaMemcpyDeviceToHost, stream));
+        B200_CUDA(cudaMemcpyAsync(h_fr.p, fs.frames.p, sizeof(FrameRec) * nf, cudaMemcpyDeviceToHost, stream));
     }
     f.keep_soft_tail(nbits); // (aqua_db_decoder: the last symbol, the next push's predecessor, and an odd byte stay)
     end(f);
@@ -349,7 +356,7 @@ void BitStage::process(Fec &f)
 // A push decodes the module's whole 8192-byte reads: the record walk tests the window starts [next, R) with R the soft bytes of those
 // reads, its records' packets enter the packet FIFO (32-bit words MSB first, whole records, each with its read), and the inner deframers
 // walk the new packet bits. The inner frames come out ordered by (read, deframer, position), as the module writes them.
-struct XBand : Framed
+struct XBand : Decoder
 {
     bool kmss;
     int pad, npb, ndef, frm_bytes;
@@ -381,7 +388,7 @@ XBand::XBand(Fec &f)
     B200_REQUIRE(f.cfg.instrument_type == 0 || f.cfg.instrument_type == 1, B200_EINVAL, "Invalid METEOR instrument type!");
     B200_REQUIRE(f.cfg.max_soft <= (1L << 30), B200_EINVAL, "max_soft must be <= 2^30 for meteor_xband_decoder");
     f.cadu_bytes = frm_bytes;
-    f.geom.chunk = XB_READ;
+    f.chunk = XB_READ;
     const int F = pad + XB_READ + 64;    // what the FIFO keeps: the carried byte, the windows' reach and a partial read
     const long fifo = f.cfg.max_soft + 2L * F;
     // records a push can accept: kmss_bpsk one per 12288 tests; mtvza one per 3072 tests when locked (the cap allows 8 times that)
@@ -392,7 +399,7 @@ XBand::XBand(Fec &f)
     pk_cap = pk_new + (kmss ? KMSS_FRM : MTVZA_FRM) + 2L * npb + 64;
     check_device(f.cfg.device);
     DeviceGuard g(f.cfg.device);
-    f.framed_storage(F, frm_cap * ndef);
+    f.open(F, frm_cap * ndef);
     const size_t words = (size_t)fifo / 32 + 8, pwords = (size_t)pk_cap / 4 + 8;
     hw.alloc(words);
     db.alloc(words);
@@ -415,12 +422,12 @@ XBand::XBand(Fec &f)
     reset(f);
 }
 
-std::unique_ptr<Framed> xband_decoder(Fec &f) { return std::make_unique<XBand>(f); }
+std::unique_ptr<Decoder> xband_decoder(Fec &f) { return std::make_unique<XBand>(f); }
 
 // a fresh module: lastBit 0, zeroed shift buffers, not synced, runs_since_sync and skip_bits 0, no open inner frame
 void XBand::reset(Fec &f)
 {
-    Framed::reset(f);
+    Decoder::reset(f);
     B200_CUDA(cudaMemsetAsync(f.softbuf.p, 0, (size_t)pad + 1, f.stream));
     f.soft_have = pad + 1;
     pos0 = pbase = 0;
@@ -532,24 +539,6 @@ void XBand::process(Fec &f)
     f.total_bits += used;
 }
 
-// frames in frames_out [0, out0) keep their bits; what left frames_out without a pull (b200_chain) is forgotten
-void Fec::note_frame_bits(long out0, const std::vector<long> &bits)
-{
-    if ((long)done_bits.size() > out0)
-        done_bits.erase(done_bits.begin(), done_bits.end() - out0);
-    done_bits.insert(done_bits.end(), bits.begin(), bits.end());
-}
-
-long Fec::frame_bits(long *out, long cap)
-{
-    B200_REQUIRE(cfg.kind == B200_FEC_NOAA_GAC || cfg.kind == B200_FEC_DMSP_RTD, B200_EINVAL,
-                 "frame completion bits are kept by noaa_gac_decoder and dmsp_rtd_decoder only");
-    const long n = (long)pulled_bits.size();
-    B200_REQUIRE(n <= cap, B200_ESTATE, "output buffer too small: need %ld", n);
-    std::copy(pulled_bits.begin(), pulled_bits.end(), out);
-    return n;
-}
-
 } // namespace b200
 
 using namespace b200;
@@ -558,6 +547,6 @@ extern "C" int b200_fec_debug_hrpt_frames(b200_fec *h, b200_hrpt_frame *out, lon
 {
     return guarded([&] {
         B200_REQUIRE(h && out && n_out, B200_EINVAL, "NULL argument");
-        *n_out = h->f->framed_as<SyncWalk>("not an HRPT decoder").records(out, cap);
+        *n_out = h->f->decoder_as<SyncWalk>("not an HRPT decoder").records(out, cap);
     });
 }

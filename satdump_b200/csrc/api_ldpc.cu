@@ -120,11 +120,14 @@ struct Ldpc : Correlated
     DevBuf<uint8_t> cadu_tmp; // internal_stream: the codewords' CADUs, whose info bits go to the bit FIFO
     DevBuf<uint16_t> cols, level_rows;
     Events<6> ev; // t_ms: correlation, walk, gather, decode + repack, and the whole push
+    Deframer defr;  // internal_stream: the bit FIFO of the info bits ...
+    FrameStage fs;  // ... and its frame stage
 
     explicit Ldpc(Fec &f);
     void process(Fec &f) override;
     void reset(Fec &f) override;
     void stats(b200_fec_stats *o) override;
+    const Deframer *deframer() const override { return &defr; }
     long records(b200_ldpc_frame *out, long cap) const; // of the last push
     void timing(float *ms, int n) const;
 };
@@ -147,7 +150,7 @@ Ldpc::Ldpc(Fec &f)
     B200_REQUIRE(c.ldpc_iterations >= 0 && c.ldpc_iterations <= 1000, B200_EINVAL, "ldpc_iterations out of range (0..1000)");
     B200_REQUIRE(c.max_soft <= (1L << 30), B200_EINVAL, "max_soft must be <= 2^30 for the LDPC decoder");
     derandomize = c.derandomize != 0; // (before internal_stream clears it for the deframer stage)
-    f.geom.chunk = LDPC_F;
+    f.chunk = LDPC_F;
     f.cadu_bytes = c.internal_stream ? c.internal_cadu_size / 8 : LDPC_CADU;
     f.cfg.cadu_size = c.internal_stream ? c.internal_cadu_size : LDPC_CADU * 8;
     if (c.internal_stream) { // BPSK_CCSDS_Deframer(internal_cadu_size, internal_asm) (:100-113): plain frames, no RS, no derandomiser
@@ -156,7 +159,6 @@ Ldpc::Ldpc(Fec &f)
         f.cfg.nrzm = 0;
         if (f.cfg.asm_sync == 0)
             f.cfg.asm_sync = 0x1ACFFC1D;
-        f.st_synced = 12;
     }
     constellation = c.constellation;
     internal = c.internal_stream != 0;
@@ -165,12 +167,14 @@ Ldpc::Ldpc(Fec &f)
     DeviceGuard g(c.device);
     const long fifo = c.max_soft + 2L * LDPC_F;
     alloc(fifo, fifo / LDPC_F + 2);
-    f.framed_storage(LDPC_F, internal ? 0 : max_frames);
+    const long max_bits = max_frames * (long)LDPC_INFO_BITS; // internal_stream: the bit FIFO's new bits a push
+    f.open(LDPC_F, internal ? Deframer::frames_cap(max_bits, f.cfg.cadu_size) : max_frames);
     ev.create();
     vn.alloc((size_t)max_frames * LDPC_VN);
     if (internal) {
         cadu_tmp.alloc((size_t)max_frames * LDPC_CADU);
-        f.deframer_storage(max_frames * (long)LDPC_INFO_BITS);
+        defr.alloc(f, max_bits, f.cfg.cadu_size, f.cfg.asm_sync, 12);
+        fs.alloc(f, Deframer::frames_cap(max_bits, f.cfg.cadu_size), 0, false);
     }
     const std::vector<uint16_t> cols_h = c2_rows();
     std::vector<int> ptr;
@@ -191,12 +195,12 @@ Ldpc::Ldpc(Fec &f)
     B200_CUDA(cudaStreamSynchronize(f.stream)); // (the host vectors above die here)
 }
 
-std::unique_ptr<Framed> ldpc_decoder(Fec &f) { return std::make_unique<Ldpc>(f); }
+std::unique_ptr<Decoder> ldpc_decoder(Fec &f) { return std::make_unique<Ldpc>(f); }
 
 void Ldpc::reset(Fec &f)
 {
     if (internal) {
-        f.start_stream(64); // the bit FIFO and the deframer
+        defr.start(f, 64);
         B200_CUDA(cudaStreamSynchronize(f.stream));
     }
     Correlated::reset(f);
@@ -210,7 +214,7 @@ void Ldpc::process(Fec &f)
     if (!begin(f, LDPC_F))
         return;
     if (internal)
-        f.compact_fifo(false);
+        defr.compact(f);
     cudaStream_t stream = f.stream;
     const long have = f.soft_have, npos = have - (LDPC_ASM - 1);
     B200_CUDA(cudaEventRecord(ev[0], stream));
@@ -234,11 +238,11 @@ void Ldpc::process(Fec &f)
         if (internal) { // :233-242: deframer->work(first 7136 decoded bits) of every codeword, in stream order
             const long new_bits = (long)nf * LDPC_INFO_BITS;
             const long words = (new_bits + 63) / 32;
-            k_ldpc_append<<<(unsigned)std::min<long>((words + 255) / 256, 132 * 8), 256, 0, stream>>>(cadu, nf, f.fifo.p, f.fifo_bits);
+            k_ldpc_append<<<(unsigned)std::min<long>((words + 255) / 256, 132 * 8), 256, 0, stream>>>(cadu, nf, defr.fifo.p, defr.fifo_bits);
             f.launches++;
-            f.last_bits0 = f.fifo_bits;
+            f.last_bits0 = defr.fifo_bits;
             f.last_nbits = new_bits;
-            f.deframe_and_rs(new_bits); // (synchronises the stream)
+            defr.deframe(f, fs, new_bits); // (synchronises the stream)
         }
         B200_CUDA(cudaEventRecord(ev[4], stream));
     }
@@ -257,7 +261,7 @@ void Ldpc::process(Fec &f)
     finish(nf, f.soft_have);
     if (nf > 0)
         corr = h_frames.p[nf - 1].corr;
-    if (!internal) { // (internal_stream: deframe_and_rs counted the inner frames)
+    if (!internal) { // (internal_stream: the frame stage counted the inner frames)
         f.out_frames += nf;
         f.total_frames += nf;
     }
@@ -269,6 +273,7 @@ void Ldpc::stats(b200_fec_stats *o)
 {
     Correlated::stats(o);
     o->ldpc_corr = corr;
+    o->deframer_state = defr.state_now;
 }
 
 long Ldpc::records(b200_ldpc_frame *out, long cap) const
@@ -296,14 +301,14 @@ int b200_fec_debug_ldpc_frames(b200_fec *h, b200_ldpc_frame *out, long cap, long
 {
     return guarded([&] {
         B200_REQUIRE(h && out && n_out, B200_EINVAL, "NULL argument");
-        *n_out = h->f->framed_as<Ldpc>("not an LDPC decoder").records(out, cap);
+        *n_out = h->f->decoder_as<Ldpc>("not an LDPC decoder").records(out, cap);
     });
 }
 int b200_fec_ldpc_timing(b200_fec *h, float *ms_out, int n)
 {
     return guarded([&] {
         B200_REQUIRE(h && ms_out, B200_EINVAL, "NULL argument");
-        h->f->framed_as<Ldpc>("not an LDPC decoder (kind B200_FEC_LDPC)").timing(ms_out, n);
+        h->f->decoder_as<Ldpc>("not an LDPC decoder (kind B200_FEC_LDPC)").timing(ms_out, n);
     });
 }
 }

@@ -165,14 +165,13 @@ Turbo::Turbo(Fec &f)
     const float var = sigma * sigma;
     two_nv = 2 * (double)var;
     ln_half = std::log(0.5);
-    f.geom.chunk = G.F;
+    f.chunk = G.F;
     f.cadu_bytes = c.turbo_base + 4;
-    f.cfg.cadu_size = f.cadu_bytes * 8;
     check_device(c.device);
     DeviceGuard g(c.device);
     const long fifo = c.max_soft + 2L * G.F;
     alloc(fifo, fifo / G.F + 2);
-    f.framed_storage(G.F, max_frames);
+    f.open(G.F, max_frames);
     ev.create();
     batch = (int)std::min<long>(max_frames, TURBO_BATCH);
     recv.alloc((size_t)batch * G.recv_stride);
@@ -204,7 +203,7 @@ Turbo::Turbo(Fec &f)
     B200_CUDA(cudaStreamSynchronize(f.stream)); // (the host vectors above die here)
 }
 
-std::unique_ptr<Framed> turbo_decoder(Fec &f) { return std::make_unique<Turbo>(f); }
+std::unique_ptr<Decoder> turbo_decoder(Fec &f) { return std::make_unique<Turbo>(f); }
 
 void Turbo::reset(Fec &f)
 {
@@ -341,7 +340,7 @@ int b200_fec_debug_turbo_frames(b200_fec *h, b200_turbo_frame *out, long cap, lo
 {
     return guarded([&] {
         B200_REQUIRE(h && out && n_out, B200_EINVAL, "NULL argument");
-        *n_out = h->f->framed_as<Turbo>("not a turbo decoder").records(out, cap);
+        *n_out = h->f->decoder_as<Turbo>("not a turbo decoder").records(out, cap);
     });
 }
 int b200_fec_debug_turbo_llr(b200_fec *h, long frame, double *app0, double *app1, long cap, long *n_out)
@@ -349,14 +348,14 @@ int b200_fec_debug_turbo_llr(b200_fec *h, long frame, double *app0, double *app1
     return guarded([&] {
         B200_REQUIRE(h && app0 && app1 && n_out, B200_EINVAL, "NULL argument");
         DeviceGuard g(h->f->cfg.device);
-        *n_out = h->f->framed_as<Turbo>("not a turbo decoder").llr(h->f->stream, frame, app0, app1, cap);
+        *n_out = h->f->decoder_as<Turbo>("not a turbo decoder").llr(h->f->stream, frame, app0, app1, cap);
     });
 }
 int b200_fec_turbo_timing(b200_fec *h, float *ms_out, int n)
 {
     return guarded([&] {
         B200_REQUIRE(h && ms_out, B200_EINVAL, "NULL argument");
-        h->f->framed_as<Turbo>("not a turbo decoder (kind B200_FEC_TURBO)").timing(ms_out, n);
+        h->f->decoder_as<Turbo>("not a turbo decoder (kind B200_FEC_TURBO)").timing(ms_out, n);
     });
 }
 }

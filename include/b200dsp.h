@@ -54,7 +54,7 @@ enum { B200_CF32 = 0, B200_CS16 = 1, B200_CS8 = 2 };
 enum { B200_FEC_METOP = 0, B200_FEC_CCSDS = 1, B200_FEC_SIMPLE = 2, B200_FEC_LDPC = 3, B200_FEC_TURBO = 4, B200_FEC_METOP_DUMP = 5,
        B200_FEC_METEOR_LRPT = 6, B200_FEC_NOAA_HRPT = 7 /* noaa_hrpt_decoder */, B200_FEC_METEOR_HRPT = 8 /* meteor_hrpt_decoder */,
        B200_FEC_AQUA_DB = 9 /* aqua_db_decoder */, B200_FEC_NOAA_GAC = 10 /* noaa_gac_decoder */, B200_FEC_DMSP_RTD = 11 /* dmsp_rtd_decoder */,
-       B200_FEC_METEOR_XBAND = 12 /* meteor_xband_decoder */ };
+       B200_FEC_METEOR_XBAND = 12 /* meteor_xband_decoder */, B200_FEC_FENGYUN_AHRPT = 13 /* fengyun_ahrpt_decoder */ };
 /* debug stage ids for b200_demod_debug_stage */
 enum { B200_STAGE_AGC = 0, B200_STAGE_FIR = 1, B200_STAGE_COSTAS = 2, B200_STAGE_RESAMP = 3, B200_STAGE_DC = 4, B200_STAGE_MM = 5,
        B200_STAGE_PLL = 6 /* pm_demod: PLLCarrierTrackingBlock output */, B200_STAGE_PM = 7 /* pm_demod: PMToBPSK output */,
@@ -217,6 +217,16 @@ typedef struct b200_fec_cfg
        order (by read, then deframer, then position). Only instrument_type, device and max_soft are read; another instrument_type is
        refused ("Invalid METEOR instrument type!") before the device is looked at. max_soft <= 2^30. */
     int instrument_type;      /* "instrument_type": 0 "mtvza", 1 "kmss_bpsk"                                                              */
+    /* kind B200_FEC_FENGYUN_AHRPT = fengyun_ahrpt_decoder (FengYun-3 AHRPT / DPT, module_fengyun_ahrpt_decoder.cpp): per 16384-byte read
+       counted from the stream's start, the I/Q pairs swapped, I and Q split with the read's `shift` (0 or 1 symbol; the bytes past the
+       read's end are 0) and Q complemented (~) when invert_second_viterbi, two Viterbi3_4 decoders in FengYun mode (8192 soft bytes ->
+       6144 bits each; outsync_after, ber_thresold), the FengYun 2-bit differential decoder joining the two branches (swapped when the
+       search machine says so), then, on reads where both Viterbis decoded, BPSK_CCSDS_Deframer(8192) with SYNCING 8 and SYNCED 16,
+       the derandomiser from byte 4 and RS(255,223) I=4 dual basis; every frame is written whatever RS returned (cadu_bytes 1024).
+       A push decodes every read it completes and keeps the rest. viterbi_state / viterbi_ber are viterbi1's, viterbi2_state /
+       viterbi2_ber viterbi2's, deframer_state 2 / 8 / 16, rs_avg the last frame's. b200_fec_debug_fengyun_reads gives one record per
+       read. max_soft <= 2^30. Device memory: about 7 bytes per max_soft byte (FIFO, the two branch streams, two Viterbi decisions). */
+    int invert_second_viterbi; /* "invert_second_viterbi"                                                                                */
 } b200_fec_cfg;
 
 typedef struct b200_demod_stats
@@ -271,6 +281,8 @@ typedef struct b200_fec_stats
        viterbi_ber (Viterbi27's BER of the last frame) and rs_corrected / rs_failed above; m2x_mode 1: the keys of
        ccsds_conv_concat_decoder above */
     int rs_avg;
+    int viterbi2_state;       /* fengyun_ahrpt_decoder: "viterbi2_lock" (viterbi_state above is "viterbi1_lock")                       */
+    float viterbi2_ber;       /* fengyun_ahrpt_decoder: "viterbi2_ber" (viterbi_ber above is "viterbi1_ber")                          */
 } b200_fec_stats;
 
 typedef struct b200_demod b200_demod;
@@ -425,6 +437,19 @@ int b200_fec_debug_hrpt_frames(b200_fec *f, b200_hrpt_frame *out, long cap, long
    since create / reset) of the bit that completed it. dmsp_rtd_decoder's "_timestamps.txt" needs it: the module stamps a frame with the
    number of 8192-byte reads that produced frames, up to the one holding that bit. Other kinds: B200_EINVAL. */
 int b200_fec_frame_bits(b200_fec *f, long *out, long cap, long *n_out);
+/* fengyun_ahrpt_decoder: one record per 16384-byte read the LAST push completed, the module's variables at the end of that read */
+typedef struct b200_fengyun_read
+{
+    long read;                /* read index since create / reset                                                                      */
+    int shift, invert_branches; /* the search machines after the read (shift toggles after 10 reads with a Viterbi in NOSYNC; the
+                                 branches swap after 10 deframer NOSYNC reads)                                                        */
+    int v1, v2;               /* bits each Viterbi returned (0 or 6144)                                                               */
+    int state1, state2;       /* Viterbi3_4::getState() after the read: 0 NOSYNC, 1 SYNCED                                             */
+    float ber1, ber2;         /* Viterbi3_4::ber() after the read                                                                     */
+    int deframer_state;       /* 2 / 8 / 16 after the read                                                                            */
+    int pad;
+} b200_fengyun_read;
+int b200_fec_debug_fengyun_reads(b200_fec *f, b200_fengyun_read *out, long cap, long *n_out);
 
 /* ---- fused chain: raw IQ -> CADUs, soft stream stays in HBM ---------------------------------------- */
 b200_chain *b200_chain_create(const b200_demod_cfg *dcfg, const b200_fec_cfg *fcfg);

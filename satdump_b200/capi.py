@@ -26,7 +26,7 @@ SYMBOLS = [
     "b200_fec_create", "b200_fec_destroy", "b200_fec_push_soft", "b200_fec_push_soft_device", "b200_fec_pull_frames",
     "b200_fec_debug_bits", "b200_fec_get_stats", "b200_fec_cadu_bytes", "b200_fec_chunk_size", "b200_fec_debug_ldpc_frames", "b200_fec_ldpc_timing",
     "b200_fec_debug_turbo_frames", "b200_fec_debug_turbo_llr", "b200_fec_turbo_timing", "b200_fec_debug_dump_frames", "b200_fec_debug_meteor_frames",
-    "b200_fec_debug_hrpt_frames", "b200_fec_frame_bits",
+    "b200_fec_debug_hrpt_frames", "b200_fec_frame_bits", "b200_fec_debug_fengyun_reads",
     "b200_chain_create", "b200_chain_destroy", "b200_chain_push_iq", "b200_chain_push_iq_device", "b200_chain_prefetch_iq", "b200_chain_pull_frames",
     "b200_chain_frames_device", "b200_chain_get_stats", "b200_chain_last_timing", "b200_chain_reset",
     "b200_chain_set_pipelined", "b200_chain_sync", "b200_chain_span_begin", "b200_chain_span_end",
@@ -56,7 +56,7 @@ class FecCfg(C.Structure):
                 ("ldpc_rate", C.c_int), ("ldpc_block_size", C.c_int), ("ldpc_iterations", C.c_int), ("ldpc2", C.c_int), ("internal_stream", C.c_int),
                 ("internal_cadu_size", C.c_int), ("turbo_rate", C.c_int), ("turbo_base", C.c_int), ("turbo_iters", C.c_int),
                 ("diff_decode", C.c_int), ("m2x_mode", C.c_int), ("interleaved", C.c_int), ("deframer_thresold", C.c_int),
-                ("backward", C.c_int), ("instrument_type", C.c_int)]
+                ("backward", C.c_int), ("instrument_type", C.c_int), ("invert_second_viterbi", C.c_int)]
 
 
 class DemuxCfg(C.Structure):
@@ -87,7 +87,8 @@ class FecStats(C.Structure):
                 ("rs_failed", C.c_long), ("replays", C.c_long), ("kernel_launches", C.c_long), ("start_redone", C.c_long), ("tb_serial", C.c_long),
                 ("spec_steps", C.c_int), ("tb_overlap", C.c_int),
                 ("correlator_lock", C.c_int), ("correlator_corr", C.c_float), ("ldpc_corr", C.c_int), ("ldpc_resyncs", C.c_long),
-                ("crc_ok", C.c_long), ("crc_fail", C.c_long), ("turbo_near_ties", C.c_long), ("rs_avg", C.c_int)]
+                ("crc_ok", C.c_long), ("crc_fail", C.c_long), ("turbo_near_ties", C.c_long), ("rs_avg", C.c_int),
+                ("viterbi2_state", C.c_int), ("viterbi2_ber", C.c_float)]
 
 
 class LdpcFrame(C.Structure):
@@ -109,6 +110,11 @@ class MeteorFrame(C.Structure):
 
 class HrptFrame(C.Structure):
     _fields_ = [("bit", C.c_long), ("inverted", C.c_int), ("state", C.c_int)]
+
+
+class FengyunRead(C.Structure):
+    _fields_ = [("read", C.c_long), ("shift", C.c_int), ("invert_branches", C.c_int), ("v1", C.c_int), ("v2", C.c_int), ("state1", C.c_int),
+                ("state2", C.c_int), ("ber1", C.c_float), ("ber2", C.c_float), ("deframer_state", C.c_int), ("pad", C.c_int)]
 
 
 class B200Error(RuntimeError):
@@ -169,6 +175,7 @@ def lib():
         L.b200_fec_debug_meteor_frames.argtypes = [vp, C.POINTER(MeteorFrame), cl, C.POINTER(cl)]
         L.b200_fec_debug_hrpt_frames.argtypes = [vp, C.POINTER(HrptFrame), cl, C.POINTER(cl)]
         L.b200_fec_frame_bits.argtypes = [vp, vp, cl, C.POINTER(cl)]
+        L.b200_fec_debug_fengyun_reads.argtypes = [vp, C.POINTER(FengyunRead), cl, C.POINTER(cl)]
         L.b200_chain_create.restype = vp
         L.b200_chain_create.argtypes = [C.POINTER(DemodCfg), C.POINTER(FecCfg)]
         L.b200_chain_destroy.argtypes = [vp]
@@ -447,6 +454,19 @@ def meteor_xband_cfg(instrument_type=None, device=0, max_soft=1 << 24):
     return cfg
 
 
+def fengyun_ahrpt_cfg(viterbi_outsync_after=None, viterbi_ber_thresold=None, invert_second_viterbi=None, device=0, max_soft=1 << 24):
+    """fengyun_ahrpt_decoder (module_fengyun_ahrpt_decoder.cpp:17-20): viterbi_outsync_after, viterbi_ber_thresold and
+    invert_second_viterbi are all required, as the module reads them with no default."""
+    for name, v in (("viterbi_outsync_after", viterbi_outsync_after), ("viterbi_ber_thresold", viterbi_ber_thresold),
+                    ("invert_second_viterbi", invert_second_viterbi)):
+        if v is None:
+            raise ValueError(f"fengyun_ahrpt_decoder: {name} is required")
+    cfg = FecCfg()
+    cfg.kind, cfg.constellation, cfg.device, cfg.max_soft = 13, CONST["qpsk"], device, max_soft
+    cfg.outsync_after, cfg.ber_thresold, cfg.invert_second_viterbi = int(viterbi_outsync_after), float(viterbi_ber_thresold), int(bool(invert_second_viterbi))
+    return cfg
+
+
 def dmsp_timestamps(bits, start_timestamp, read_bits_seen=None):
     """dmsp_rtd_decoder's "_timestamps.txt" values for frames completed at stream bits `bits` (b200_fec_frame_bits): start +
     8192 * (reads of 8192 soft bytes from the stream's start that produced frames, up to the frame's) / 1.024e6. read_bits_seen carries
@@ -482,6 +502,8 @@ def fec_cfg_for(sig, max_soft, device=0):
         return noaa_gac_cfg(sig.backward, device=device, max_soft=max_soft)
     if sig.decoder == "dmsp_rtd":
         return dmsp_rtd_cfg(device=device, max_soft=max_soft)
+    if sig.decoder == "fengyun_ahrpt":
+        return fengyun_ahrpt_cfg(sig.outsync_after, sig.ber_thresold, sig.invert_second_viterbi, device=device, max_soft=max_soft)
     if sig.decoder in ("meteor_mtvza", "meteor_kmss_bpsk"):
         return meteor_xband_cfg("mtvza" if sig.decoder == "meteor_mtvza" else "kmss_bpsk", device=device, max_soft=max_soft)
     if sig.decoder == "turbo":
@@ -671,6 +693,12 @@ class Fec:
         self._n = soft.size
         return self
 
+    def push_device(self, dev_ptr, n):
+        """n soft bytes already in device memory of the decoder's device"""
+        _chk(lib().b200_fec_push_soft_device(self.h, dev_ptr, n))
+        self._n = n
+        return self
+
     def frames(self):
         cap = int(self._n) + 65536 + 4 * self.cadu_bytes  # (meteor_xband_decoder: a byte that completes a read may release its frames)
         out = np.zeros(cap, np.uint8)
@@ -750,6 +778,16 @@ class Fec:
         n = C.c_long(0)
         _chk(lib().b200_fec_debug_hrpt_frames(self.h, recs, cap, C.byref(n)))
         return np.array([[recs[k].bit, recs[k].inverted, recs[k].state] for k in range(n.value)], np.int64).reshape(-1, 3)
+
+    def fengyun_reads(self):
+        """fengyun_ahrpt_decoder: one record per 16384-byte read the last push completed, as float64 [n, 9] = shift, invert_branches, v1,
+        v2, viterbi1 state, viterbi2 state, viterbi1 ber, viterbi2 ber, deframer state after the read (oracle.fengyun's records)"""
+        cap = int(self._n) // 16384 + 4
+        recs = (FengyunRead * cap)()
+        n = C.c_long(0)
+        _chk(lib().b200_fec_debug_fengyun_reads(self.h, recs, cap, C.byref(n)))
+        f = ("shift", "invert_branches", "v1", "v2", "state1", "state2", "ber1", "ber2", "deframer_state")
+        return np.array([[getattr(recs[k], x) for x in f] for k in range(n.value)], np.float64).reshape(-1, len(f))
 
     def frame_bits(self):
         """noaa_gac_decoder / dmsp_rtd_decoder: the stream bit that completed each frame of the last frames() pull, as int64"""

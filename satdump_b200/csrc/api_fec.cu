@@ -110,6 +110,7 @@ Fec::Fec(const b200_fec_cfg &in) : cfg(meteor_m2x_as_ccsds(in))
     case B200_FEC_NOAA_HRPT: case B200_FEC_METEOR_HRPT: case B200_FEC_DMSP_RTD: make = sync_walk_decoder; break;
     case B200_FEC_AQUA_DB: case B200_FEC_NOAA_GAC: make = bit_stage_decoder; break;
     case B200_FEC_METEOR_XBAND: make = xband_decoder; break;
+    case B200_FEC_FENGYUN_AHRPT: make = fengyun_decoder; break;
     default: B200_REQUIRE(false, B200_EINVAL, "unknown decoder kind %d", cfg.kind);
     }
     B200_REQUIRE(cfg.max_soft >= 65536, B200_EINVAL, "max_soft must be >= 65536");
@@ -135,11 +136,6 @@ struct Conv : Decoder
     VitIdleState idle_st{-1, 0};
     float last_ber = 10.f;
     long swapped = 0;                 // bpsk_90 / iq_invert: FIFO bytes whose pairs are already swapped
-    DevBuf<uint2> idle_dec;
-    DevBuf<VitIdleOut> idle_out;
-    DevBuf<VitIdle2Out> idle2_out;
-    PinnedBuf<VitIdleOut> h_idle;
-    PinnedBuf<VitIdle2Out> h_idle2;
     // Viterbi_Depunc (conv_rate 2/3 ... 7/8): the depunctured symbol stream the decoder windows read (leftover of the previous push in
     // front), the lock search's persistent test buffer, per-window count of real tail symbols, and the DepuncXX / ViterbiSlidingBuffer
     // state of viterbi_punc.cpp / depunc.h carried between pushes
@@ -266,12 +262,7 @@ Conv::Conv(Fec &f)
         slice_carry.alloc(4);
     } else {
         vit.alloc(f, geom, max_chunks);
-        idle_dec.alloc(VIT_TESTLEN + 64);
-        idle_out.alloc(1);
-        idle2_out.alloc(1);
-        h_idle.alloc(1);
-        h_idle2.alloc(1);
-        B200_CUDA(cudaFuncSetAttribute(k_vit_idle2, cudaFuncAttributeMaxDynamicSharedMemorySize, 8 * VIT_IDLE_WARP_BYTES));
+        vit.alloc_lock_search();
     }
     defr.alloc(f, max_new_bits, cfg.cadu_size, cfg.asm_sync, st_synced);
     if (two)
@@ -416,6 +407,42 @@ void Viterbi::chained(Fec &f, const int8_t *src, long n, int *ber_errors)
     }
 }
 
+void Viterbi::alloc_lock_search()
+{
+    idle_dec.alloc(VIT_TESTLEN + 64);
+    idle_out.alloc(1);
+    idle2_out.alloc(1);
+    h_idle.alloc(1);
+    h_idle2.alloc(1);
+    B200_CUDA(cudaFuncSetAttribute(k_vit_idle2<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8 * VIT_IDLE_WARP_BYTES));
+    B200_CUDA(cudaFuncSetAttribute(k_vit_idle2<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8 * VIT_IDLE_WARP_BYTES));
+}
+
+const VitIdleOut &Viterbi::lock_search(Fec &f, const int8_t *src, long c, int n, int nswap, int nphases, int ph0, int ph1, VitIdleState st, bool fy)
+{
+    // parallel search first (one warp per hypothesis); it hands over to the serial kernel at the first chunk whose chained 6-bit states
+    // its two-pass guess did not reproduce
+    const int nh = nswap * nphases * 2;
+    const float thr = f.cfg.ber_thresold;
+    auto idle2 = fy ? k_vit_idle2<true> : k_vit_idle2<false>;
+    idle2<<<1, 32 * nh, nh * VIT_IDLE_WARP_BYTES, f.stream>>>(src, c, n, geom, nswap, nphases, ph0, ph1, thr, st, idle2_out.p);
+    f.launches++;
+    B200_CUDA(cudaMemcpyAsync(h_idle2.p, idle2_out.p, sizeof(VitIdle2Out), cudaMemcpyDeviceToHost, f.stream));
+    B200_CUDA(cudaStreamSynchronize(f.stream));
+    *h_idle.p = h_idle2.p->o;
+    if (h_idle2.p->fallback_chunk >= 0) {
+        const long c2 = c + h_idle2.p->fallback_chunk;
+        auto idle1 = fy ? k_vit_idle<true> : k_vit_idle<false>;
+        idle1<<<1, 32, 0, f.stream>>>(src, c2, (int)(n - (c2 - c)), geom, nswap, nphases, ph0, ph1, thr, h_idle2.p->o.st, idle_dec.p, idle_out.p);
+        f.launches++;
+        B200_CUDA(cudaMemcpyAsync(h_idle.p, idle_out.p, sizeof(VitIdleOut), cudaMemcpyDeviceToHost, f.stream));
+        B200_CUDA(cudaStreamSynchronize(f.stream));
+        if (h_idle.p->lock_chunk >= 0)
+            h_idle.p->lock_chunk += (int)(c2 - c);
+    }
+    return *h_idle.p;
+}
+
 void Viterbi::alloc(Fec &f, const VitGeom &g, long max_chunks)
 {
     geom = g;
@@ -453,38 +480,18 @@ void Conv::viterbi_segment(Fec &f, long c0, long nch, std::vector<OutChunk> &out
     while (c < nch) {
         if (vit_state == 0) {
             idle_st.enc_state = vit.enc_state; // ONE chained CCEncoder serves the lock test and the SYNCED BER check (viterbi_3_4.cpp:126,157)
-            {
-                // parallel search first (one warp per hypothesis); it hands over to the serial kernel at the first chunk whose chained
-                // 6-bit states its two-pass guess did not reproduce
-                const int nh = nswap * nphases * 2;
-                k_vit_idle2<<<1, 32 * nh, nh * VIT_IDLE_WARP_BYTES, f.stream>>>(f.softbuf.p, c, (int)(nch - c), geom, nswap, nphases, ph0, ph1,
-                                                                               f.cfg.ber_thresold, idle_st, idle2_out.p);
-                f.launches++;
-                B200_CUDA(cudaMemcpyAsync(h_idle2.p, idle2_out.p, sizeof(VitIdle2Out), cudaMemcpyDeviceToHost, f.stream));
-                B200_CUDA(cudaStreamSynchronize(f.stream));
-                *h_idle.p = h_idle2.p->o;
-                if (h_idle2.p->fallback_chunk >= 0) {
-                    const long c2 = c + h_idle2.p->fallback_chunk;
-                    k_vit_idle<<<1, 32, 0, f.stream>>>(f.softbuf.p, c2, (int)(nch - c2), geom, nswap, nphases, ph0, ph1, f.cfg.ber_thresold,
-                                                      h_idle2.p->o.st, idle_dec.p, idle_out.p);
-                    f.launches++;
-                    B200_CUDA(cudaMemcpyAsync(h_idle.p, idle_out.p, sizeof(VitIdleOut), cudaMemcpyDeviceToHost, f.stream));
-                    B200_CUDA(cudaStreamSynchronize(f.stream));
-                    if (h_idle.p->lock_chunk >= 0)
-                        h_idle.p->lock_chunk += (int)(c2 - c);
-                }
-            }
-            idle_st = h_idle.p->st;
+            const VitIdleOut &o = vit.lock_search(f, f.softbuf.p, c, (int)(nch - c), nswap, nphases, ph0, ph1, idle_st, false);
+            idle_st = o.st;
             vit.enc_state = idle_st.enc_state;
             float bb = 10.f;
             for (int i = 0; i < 16; i++)
-                bb = std::min(bb, h_idle.p->bers[i]);
+                bb = std::min(bb, o.bers[i]);
             last_ber = bb;
-            if (h_idle.p->lock_chunk < 0)
+            if (o.lock_chunk < 0)
                 break;
-            c += h_idle.p->lock_chunk;
+            c += o.lock_chunk;
             vit_state = 1;
-            vit.hyp = VitHyp{h_idle.p->swap, h_idle.p->phase, h_idle.p->shift};
+            vit.hyp = VitHyp{o.swap, o.phase, o.shift};
             invalid = 0;
             vit.enc_state = idle_st.enc_state;
         }
@@ -539,7 +546,7 @@ void Conv::punc_segment(Fec &f, long c0, long ncalls, std::vector<OutChunk> &out
         if (vit_state == 0) {
             const VitIdleState st{pdec_start, vit.enc_state};
             k_punc_idle<<<1, 32, 0, f.stream>>>(f.softbuf.p, c, (int)(ncalls - c), size, P, nswap, nphases, ph0, ph1, f.cfg.ber_thresold, st, bdep.p,
-                                                idle_dec.p, punc_out.p);
+                                                vit.idle_dec.p, punc_out.p);
             f.launches++;
             B200_CUDA(cudaMemcpyAsync(h_punc.p, punc_out.p, sizeof(PuncIdleOut), cudaMemcpyDeviceToHost, f.stream));
             B200_CUDA(cudaStreamSynchronize(f.stream));
@@ -645,7 +652,7 @@ int Deframer::deframe(Fec &f, FrameStage &fs, long new_bits)
     cudaStream_t stream = f.stream;
     const long nbits = fifo_bits + new_bits;
     B200_CUDA(cudaEventRecord(f.evf[0], stream));
-    k_deframe<<<1, 32, 0, stream>>>(fifo.p, nbits, cadu_size, st_synced, asm_sync, dstate.p, fs.frames.p, (int)fs.max_frames,
+    k_deframe<<<1, 32, 0, stream>>>(fifo.p, nbits, cadu_size, st_syncing, st_synced, asm_sync, dstate.p, fs.frames.p, (int)fs.max_frames,
                                    reinterpret_cast<DefrEventDev *>(devents.p), (int)max_events, fs.counters.p);
     f.launches++;
     B200_CUDA(cudaMemcpyAsync(fs.h_counters.p, fs.counters.p, sizeof(int) * 2, cudaMemcpyDeviceToHost, stream));
@@ -857,11 +864,12 @@ void Correlated::finish(int nf, long soft_have)
     tail_seen = soft_have;
 }
 
-void Deframer::alloc(Fec &f, long max_new_bits, int cadu_size_, uint32_t asm_sync_, int st_synced_)
+void Deframer::alloc(Fec &f, long max_new_bits, int cadu_size_, uint32_t asm_sync_, int st_synced_, int st_syncing_)
 {
     cadu_size = cadu_size_;
     asm_sync = asm_sync_;
     st_synced = st_synced_;
+    st_syncing = st_syncing_;
     fifo.alloc((size_t)((max_new_bits + 2L * cadu_size + 4096) / 32 + 8));
     dstate.alloc(2);
     h_dstate.alloc(1);

@@ -667,6 +667,9 @@ __global__ void __launch_bounds__(32) k_punc_idle(const int8_t *__restrict__ sof
 struct VitIdleOut { int lock_chunk, swap, phase, shift; float ber; float bers[16]; VitIdleState st; int pad; };
 
 #ifdef B200_DEFINE_KERNELS
+// FY (fengyun_ahrpt_decoder, Viterbi3_4 with fymode): hypothesis (s = 0, shift) runs as VitHyp{shift, 0, shift}; with the branch stream
+// stored by k_fy_split (fengyun.cuh) that is FengYun's depuncture through the MetOp one (the stored bers and lswap keep s = 0).
+template <bool FY = false>
 __global__ void __launch_bounds__(32) k_vit_idle(const int8_t *__restrict__ soft, long chunk0, int nchunks, VitGeom g, int nswap, int nphases,
                                                   int ph0, int ph1, float thr, VitIdleState st_in, uint2 *__restrict__ scratch_dec,
                                                   VitIdleOut *__restrict__ out)
@@ -689,7 +692,7 @@ __global__ void __launch_bounds__(32) k_vit_idle(const int8_t *__restrict__ soft
         for (int s = 0; s < nswap; s++)
             for (int pi = 0; pi < nphases; pi++)
                 for (int shift = 0; shift < 2; shift++) {
-                    VitHyp h{s, pi == 0 ? ph0 : ph1, shift};
+                    VitHyp h{FY ? shift : s, pi == 0 ? ph0 : ph1, shift};
                     int xl, xh;
                     if (dec_start < 0) xl = xh = 31;
                     else { xl = (lane == dec_start) ? 0 : 63; xh = (lane + 32 == dec_start) ? 0 : 63; }
@@ -772,6 +775,7 @@ struct VitIdle2Out { VitIdleOut o; int fallback_chunk; int pad[3]; };
 constexpr int VIT_IDLE_ROWS = VIT_TESTLEN * 3 / 4 + 6 + 2;           // decision rows per hypothesis (r=3/4 is the larger: 1542)
 constexpr int VIT_IDLE_WARP_BYTES = VIT_IDLE_ROWS * 8 + 64 * 4;       // + 64 words of decoded bits
 #ifdef B200_DEFINE_KERNELS
+template <bool FY = false> // (as k_vit_idle)
 __global__ void __launch_bounds__(256) k_vit_idle2(const int8_t *__restrict__ soft, long chunk0, int nchunks, VitGeom g, int nswap, int nphases, int ph0,
                                                     int ph1, float thr, VitIdleState st_in, VitIdle2Out *__restrict__ out)
 {
@@ -787,7 +791,7 @@ __global__ void __launch_bounds__(256) k_vit_idle2(const int8_t *__restrict__ so
     const int steps = tg.F + 6, nsym = g.rate34 ? VIT_TESTLEN * 3 / 2 : VIT_TESTLEN;
     // hypothesis w in the reference's loop order: swap-major, then phase, then shift
     const int hs = w / (nphases * 2), hp = (w / 2) % nphases, hshift = w & 1;
-    const VitHyp h{hs, hp == 0 ? ph0 : ph1, hshift};
+    const VitHyp h{FY ? hshift : hs, hp == 0 ? ph0 : ph1, hshift};
     if (threadIdx.x == 0) { s_lock = -1; s_dec = st_in.dec_start; s_enc = st_in.enc_state; s_fallback = -1; }
     __syncthreads();
     float bers[16];
@@ -1070,7 +1074,7 @@ __global__ void k_slice(const int8_t *__restrict__ soft, long nchunks, SliceCfg 
 #endif // B200_DEFINE_KERNELS
 struct DefrState
 {
-    int state;       // 2 NOSYNC, 6 SYNCING, synced value (12 / 18): the numeric values double as thresholds
+    int state;       // 2 NOSYNC, SYNCING value (6; FengYun 8), SYNCED value (12 / 18; FengYun 16): the numeric values double as thresholds
     int inversion, good, bad;
     long pos;        // FIFO bit index of the next bit the machine examines with its shifter (when not inside a frame)
     long frame_pay;  // >= 0: a frame is open, payload starts at this FIFO bit index (its ASM ended at frame_pay-1)
@@ -1080,7 +1084,7 @@ struct DefrEventDev { long pos; int state; int pad; };
 
 // counters_out[0] = frames found, [1] = state-change events recorded (events[]: bit index at which the state changed)
 #ifdef B200_DEFINE_KERNELS
-__global__ void __launch_bounds__(32) k_deframe(const uint32_t *__restrict__ fifo, long nbits, int cadu_size, int st_synced, uint32_t sync,
+__global__ void __launch_bounds__(32) k_deframe(const uint32_t *__restrict__ fifo, long nbits, int cadu_size, int st_syncing, int st_synced, uint32_t sync,
                                                  DefrState *__restrict__ st_io, FrameRec *__restrict__ frames, int max_frames,
                                                  DefrEventDev *__restrict__ events, int max_events, int *__restrict__ counters_out)
 {
@@ -1130,12 +1134,12 @@ __global__ void __launch_bounds__(32) k_deframe(const uint32_t *__restrict__ fif
             const long e = p + found;
             S.inversion = inv;
             S.frame_pay = e + 1;
-            S.state = 6;
+            S.state = st_syncing;
             S.good = S.bad = 0;
-            note(e, 6);
+            note(e, st_syncing);
             continue;
         }
-        if (S.state != 6) {
+        if (S.state != st_syncing) {
             // SYNCED: 128 frames of lookahead per iteration (4 independent loads per lane, so their latencies overlap); lane l tests
             // the ASMs expected l, l+32, l+64, l+96 frames ahead. n = leading passes, m = how many of those are complete.
             constexpr int G = 4;
@@ -1185,7 +1189,7 @@ __global__ void __launch_bounds__(32) k_deframe(const uint32_t *__restrict__ fif
         {
             const uint32_t wv = fifo_window(fifo, S.pos - 31);
             const int diff = __popc(wv ^ (S.inversion ? ~sync : sync));
-            if (diff < 6) {
+            if (diff < st_syncing) {
                 S.frame_pay = S.pos + 1;
                 S.bad = 0;
                 S.good++;

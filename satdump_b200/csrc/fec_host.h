@@ -49,15 +49,16 @@ struct Deframer
     PinnedBuf<DefrEvent> h_events;
     long fifo_bits = 32, max_events = 0;
     int n_events = 0;                 // ... their number
-    int state_now = 2, st_synced = 12, cadu_size = 0;
+    int state_now = 2, st_syncing = 6, st_synced = 12, cadu_size = 0;
     uint32_t asm_sync = 0;
 
     // the machine and the frame counters of Fec at a point a pass may have to roll back to
     struct Mark { DefrState h_dstate; long fifo_bits, out_frames, total_frames, rs_corrected, rs_failed; int state_now; };
 
     static long frames_cap(long max_new_bits, int cadu_size) { return max_new_bits / cadu_size + 4; } // frames one push can complete
-    // room for max_new_bits new bits a push; the whole FIFO is cleared
-    void alloc(Fec &f, long max_new_bits, int cadu_size, uint32_t asm_sync, int st_synced);
+    // room for max_new_bits new bits a push; the whole FIFO is cleared. st_syncing / st_synced: the SYNCING and SYNCED state values,
+    // which are also the machine's error tolerances in those states (fengyun_ahrpt_decoder sets 8 and 16)
+    void alloc(Fec &f, long max_new_bits, int cadu_size, uint32_t asm_sync, int st_synced, int st_syncing = 6);
     void start(Fec &f, size_t clear_bytes); // a new stream: the machine and the FIFO's first clear_bytes
     void compact(Fec &f);             // keeps from the open frame's payload, or the 31 bits of shifter history
     Mark mark(const Fec &f);
@@ -99,6 +100,11 @@ struct Viterbi
     DevBuf<TbEdge> tb_edges;
     DevBuf<int> tb_list;              // [0] count of chunks redone serially in the last launch, [1..] their indices
     PinnedBuf<VitRec> h_rec;
+    DevBuf<uint2> idle_dec;           // the lock search's (alloc_lock_search)
+    DevBuf<VitIdleOut> idle_out;
+    DevBuf<VitIdle2Out> idle2_out;
+    PinnedBuf<VitIdleOut> h_idle;
+    PinnedBuf<VitIdle2Out> h_idle2;
     std::vector<int> h_redo, h_redo_ber, h_start;
     VitHyp hyp{0, 0, 0};
     int main_next_start = -1, enc_state = 0;
@@ -107,6 +113,10 @@ struct Viterbi
     long start_redone = 0, tb_serial_total = 0; // chunks decoded again from a corrected start state / chained back serially
 
     void alloc(Fec &f, const VitGeom &g, long max_chunks); // g's chunk, F and BER settings; the strides follow
+    void alloc_lock_search();
+    // Viterbi3_4 / Viterbi1_2::work in the IDLE state over the n chunks of src from chunk c, with the chained test decoder and encoder
+    // state st, until a hypothesis locks (lock_chunk relative to c, -1: none). fy: fengyun_ahrpt_decoder's hypotheses (k_vit_idle<true>)
+    const VitIdleOut &lock_search(Fec &f, const int8_t *src, long c, int n, int nswap, int nphases, int ph0, int ph1, VitIdleState st, bool fy);
     int decode_pass(Fec &f, const int8_t *src, long c, int nrange, long out_base, int n, const int *qlist, int nber, const int *ber_list);
     void decode_range(Fec &f, const int8_t *src, long c, int n, long out_base, int max_rounds);
     // Viterbi27 (meteor_lrpt_decoder): the n chunks at src (geom.chunk bytes apart, already rotated) decoded as consecutive calls of ONE
@@ -149,6 +159,7 @@ std::unique_ptr<Decoder> meteor_decoder(Fec &f);
 std::unique_ptr<Decoder> sync_walk_decoder(Fec &f); // noaa_hrpt_decoder, meteor_hrpt_decoder, dmsp_rtd_decoder (api_hrpt.cu)
 std::unique_ptr<Decoder> bit_stage_decoder(Fec &f); // aqua_db_decoder, noaa_gac_decoder (api_hrpt.cu)
 std::unique_ptr<Decoder> xband_decoder(Fec &f);     // meteor_xband_decoder (api_hrpt.cu)
+std::unique_ptr<Decoder> fengyun_decoder(Fec &f);   // fengyun_ahrpt_decoder (api_fengyun.cu)
 
 class Fec
 {

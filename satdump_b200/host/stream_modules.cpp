@@ -425,6 +425,21 @@ b200_fec_cfg fec_cfg_from_params(const std::string &id, const Params &p)
             throw ModuleError("meteor_xband_decoder: hard_symbols input is not supported by the B200 path");
         return c;
     }
+    if (id == "fengyun_ahrpt_decoder") { // module_fengyun_ahrpt_decoder.cpp:17-20: the three parameters are read with no default (nlohmann's
+        // get<>() on the null a missing key gives throws type_error 302); 1024-byte CADUs
+        c.kind = B200_FEC_FENGYUN_AHRPT;
+        c.device = (int)p.num("b200_device", 0);
+        c.constellation = B200_QPSK;
+        c.cadu_size = 8192;
+        for (const char *k : {"viterbi_outsync_after", "viterbi_ber_thresold", "invert_second_viterbi"})
+            if (!p.has(k))
+                throw ModuleError(std::string("fengyun_ahrpt_decoder: ") + k + " is required ([json.exception.type_error.302] type must be " +
+                                  (k[0] == 'i' ? "boolean" : "number") + ", but is null)");
+        c.outsync_after = (int)p.num("viterbi_outsync_after");
+        c.ber_thresold = (float)p.num("viterbi_ber_thresold");
+        c.invert_second_viterbi = p.flag("invert_second_viterbi", false);
+        return c;
+    }
     if (id == "aqua_db_decoder") { // module_aqua_db_decoder.cpp:16-22: no parameters; 1024-byte CADUs (Aqua and Aura DB)
         c.kind = B200_FEC_AQUA_DB;
         c.device = (int)p.num("b200_device", 0);
@@ -851,6 +866,8 @@ void FecStage::process()
             correlator_corr = st.correlator_corr;
             ldpc_corr = st.ldpc_corr;
             rs_avg = st.rs_avg;
+            viterbi2_lock = st.viterbi2_state;
+            viterbi2_ber = st.viterbi2_ber;
         }
     }
     if (fin)

@@ -218,6 +218,8 @@ class SignalCfg:
     deframer_thresold: int = 10
     # noaa_gac_decoder's "backward" (NOAA.json "noaa_gac": false)
     backward: bool = False
+    # fengyun_ahrpt_decoder's "invert_second_viterbi" (FengYun-3.json: false for A/B and C, true from D on)
+    invert_second_viterbi: bool = False
 
     @property
     def cadu_bytes(self):
@@ -339,6 +341,17 @@ CONFIGS = {
                           fmt="cs16", decoder="noaa_gac", esn0_db=15.0, carrier_rad=1e-4, phase0=0.1, post_costas_dc=True),
     "dmsp_rtd": SignalCfg(name="dmsp_rtd", samplerate=2e6, symbolrate=1024000, constellation="bpsk", conv="none", rrc_alpha=0.5, pll_bw=0.005,
                           fmt="cs16", decoder="dmsp_rtd", esn0_db=15.0, carrier_rad=1e-4, phase0=0.1),
+    # psk_demod QPSK -> fengyun_ahrpt_decoder (FengYun-3.json): "FengYun-3 A/B AHRPT" at 2.8 Msym/s, the D shape (30 Msym/s,
+    # invert_second_viterbi) and the E / F / H shape (38.4 Msym/s), recorded at about two samples per symbol
+    "fengyun_ahrpt": SignalCfg(name="fengyun_ahrpt", samplerate=6e6, symbolrate=2800000, constellation="qpsk", conv="3/4", rrc_alpha=0.5,
+                               pll_bw=0.003, fmt="cs16", decoder="fengyun_ahrpt", esn0_db=12.0, carrier_rad=1e-4, phase0=0.1,
+                               ber_thresold=0.26, outsync_after=20),
+    "fengyun_ahrpt_d": SignalCfg(name="fengyun_ahrpt_d", samplerate=60e6, symbolrate=30000000, constellation="qpsk", conv="3/4", rrc_alpha=0.35,
+                                 pll_bw=0.008, fmt="cs16", decoder="fengyun_ahrpt", esn0_db=12.0, carrier_rad=1e-4, phase0=0.1,
+                                 ber_thresold=0.26, outsync_after=20, invert_second_viterbi=True),
+    "fengyun_ahrpt_e": SignalCfg(name="fengyun_ahrpt_e", samplerate=76.8e6, symbolrate=38400000, constellation="qpsk", conv="3/4", rrc_alpha=0.35,
+                                 pll_bw=0.008, fmt="cs16", decoder="fengyun_ahrpt", esn0_db=12.0, carrier_rad=1e-4, phase0=0.1,
+                                 ber_thresold=0.26, outsync_after=20, invert_second_viterbi=True),
     # psk_demod BPSK -> meteor_xband_decoder (Meteor-M.json "meteor_m_mtvza_dump", "meteor_m_kmss_bpsk_db"): NRZ-M record streams at
     # 15.36 and 61.44 Msym/s, recorded at two samples per symbol
     "meteor_mtvza": SignalCfg(name="meteor_mtvza", samplerate=30.72e6, symbolrate=15360000, constellation="bpsk", conv="none", rrc_alpha=0.6,
@@ -406,6 +419,12 @@ def make_bitstream(cfg: SignalCfg, nframes, seed):
         return coded, clear
     if cfg.decoder == "terra_db":  # nframes CADUs, NRZ-M, r=1/2: one BPSK symbol per code symbol
         return terra_db_frames(nframes, seed)
+    if cfg.decoder == "fengyun_ahrpt":  # nframes CADUs on two punctured branches: the module swaps I and Q, so its I branch rides on Q
+        i_bits, q_bits, clear = fengyun_frames(nframes, seed)
+        n = min(i_bits.size, q_bits.size)
+        coded = np.empty(2 * n, np.uint8)
+        coded[0::2], coded[1::2] = (1 - q_bits[:n]) if cfg.invert_second_viterbi else q_bits[:n], i_bits[:n]
+        return coded, clear
     if cfg.decoder in ("meteor_mtvza", "meteor_kmss_bpsk"):  # nframes inner frames in records, NRZ-M
         return meteor_xband_frames(cfg.decoder == "meteor_kmss_bpsk", nframes, seed)
     if cfg.decoder == "ldpc":  # nframes LDPC frames
@@ -1009,6 +1028,53 @@ def meteor_xband_frames(kmss, nframes, seed=0, cut=None):
 
 
 # ---- EOS Aqua / Aura DB (aqua_db_decoder): randomised CADUs on two NRZ-M rails -----------------------------------------------------------
+# ---- FengYun-3 AHRPT / DPT (fengyun_ahrpt_decoder) ---------------------------------------------------------------------------------------
+def fengyun_diff_encode(bits):
+    """The inverse of FengyunDiff::work2 (diff.cpp:45-74) from Xin = Yin = 0: the branch bits (x, y) (x = in1 = the Q branch's, y = in2 =
+    the I branch's) of every pair, such that the decoder returns `bits` (even length). For output bits (h, l) and the previous pair
+    (xp, yp): x != y gives h = yp ^ y, l = xp ^ x, and x == y gives h = xp ^ x, l = yp ^ y; exactly one of the two is consistent."""
+    # Both branches give x ^ y = xp ^ yp ^ h ^ l, so d = x ^ y is the running XOR of h ^ l, and x steps by l where d = 1, else by h.
+    b = np.asarray(bits, np.uint8).reshape(-1, 2)
+    h, l = b[:, 0], b[:, 1]
+    d = np.bitwise_xor.accumulate(h ^ l)
+    x = np.bitwise_xor.accumulate(np.where(d == 1, l, h)).astype(np.uint8)
+    return x, (x ^ d).astype(np.uint8)
+
+
+def puncture_34_fengyun(coded):
+    """From each 6 coded symbols e0..e5 transmit e0, e1, e3, e4 (the inverse of Viterbi3_4::depuncture in fymode, shift 0: "110")."""
+    n = coded.size // 6 * 6
+    return coded[:n].reshape(-1, 6)[:, [0, 1, 3, 4]].reshape(-1)
+
+
+def fengyun_frames(nframes, seed=0, errors=()):
+    """The FengYun-3 AHRPT transmitter: (tx soft-symbol branches (I bits, Q bits) as uint8, the CADUs fengyun_ahrpt_decoder writes
+    [n, 1024]). Randomised CADUs with RS(255,223) I=4 dual basis (`errors`: (frame, codeword, nbytes) byte errors added on air), the
+    inverse of the differential decoder, then per branch the r=1/2 k=7 (79, 109) code punctured to 3/4 as FengYun does."""
+    tx_bits, clear = dump_frames(nframes, seed)
+    tx = np.packbits(tx_bits, axis=1)
+    rng = np.random.default_rng(seed + 1)
+    for fr, cw, nb in errors:  # codeword cw holds bytes 4 + cw, 4 + cw + 4, ... of the frame
+        pos = 4 + cw + 4 * rng.choice(255, nb, replace=False)
+        tx[fr, pos] ^= rng.integers(1, 256, nb, dtype=np.uint8)
+    x, y = fengyun_diff_encode(np.unpackbits(tx, axis=1).reshape(-1))
+    return puncture_34_fengyun(conv_encode(y)), puncture_34_fengyun(conv_encode(x)), clear
+
+
+def fengyun_soft(i_bits, q_bits, amp=60.0, sigma=0.0, seed=0, invert_second=False, swap_branches=False):
+    """int8 soft pairs that fengyun_ahrpt_decoder reads: bit 1 -> +amp; the module swaps I and Q of every pair first, so the Q branch goes
+    in byte 0 and the I branch in byte 1. invert_second: the Q branch sent negated (the module complements it back); swap_branches: the
+    two branches exchanged on air."""
+    I, Q = (q_bits, i_bits) if swap_branches else (i_bits, q_bits)
+    n = min(I.size, Q.size)
+    out = np.empty(2 * n, np.float32)
+    out[1::2] = (2.0 * I[:n] - 1.0) * amp
+    out[0::2] = (2.0 * Q[:n] - 1.0) * amp * (-1.0 if invert_second else 1.0)
+    if sigma:
+        out += np.random.default_rng(seed).normal(0, sigma, out.size).astype(np.float32)
+    return np.clip(np.round(out), -127, 127).astype(np.int8)
+
+
 def aqua_db_frames(nframes, seed=0):
     """(decoded bits uint8 [n, 8192]: randomised CADUs with RS(255,223) I=4 dual basis, the CADUs aqua_db_decoder writes for them
     [n, 1024]: the ASM and the derandomised codewords). The decoder's frame format is metop_dump_decoder's."""

@@ -54,7 +54,8 @@ enum { B200_CF32 = 0, B200_CS16 = 1, B200_CS8 = 2 };
 enum { B200_FEC_METOP = 0, B200_FEC_CCSDS = 1, B200_FEC_SIMPLE = 2, B200_FEC_LDPC = 3, B200_FEC_TURBO = 4, B200_FEC_METOP_DUMP = 5,
        B200_FEC_METEOR_LRPT = 6, B200_FEC_NOAA_HRPT = 7 /* noaa_hrpt_decoder */, B200_FEC_METEOR_HRPT = 8 /* meteor_hrpt_decoder */,
        B200_FEC_AQUA_DB = 9 /* aqua_db_decoder */, B200_FEC_NOAA_GAC = 10 /* noaa_gac_decoder */, B200_FEC_DMSP_RTD = 11 /* dmsp_rtd_decoder */,
-       B200_FEC_METEOR_XBAND = 12 /* meteor_xband_decoder */, B200_FEC_FENGYUN_AHRPT = 13 /* fengyun_ahrpt_decoder */ };
+       B200_FEC_METEOR_XBAND = 12 /* meteor_xband_decoder */, B200_FEC_FENGYUN_AHRPT = 13 /* fengyun_ahrpt_decoder */,
+       B200_FEC_FENGYUN_MPT = 14 /* fengyun_mpt_decoder */ };
 /* debug stage ids for b200_demod_debug_stage */
 enum { B200_STAGE_AGC = 0, B200_STAGE_FIR = 1, B200_STAGE_COSTAS = 2, B200_STAGE_RESAMP = 3, B200_STAGE_DC = 4, B200_STAGE_MM = 5,
        B200_STAGE_PLL = 6 /* pm_demod: PLLCarrierTrackingBlock output */, B200_STAGE_PM = 7 /* pm_demod: PMToBPSK output */,
@@ -225,8 +226,14 @@ typedef struct b200_fec_cfg
        the derandomiser from byte 4 and RS(255,223) I=4 dual basis; every frame is written whatever RS returned (cadu_bytes 1024).
        A push decodes every read it completes and keeps the rest. viterbi_state / viterbi_ber are viterbi1's, viterbi2_state /
        viterbi2_ber viterbi2's, deframer_state 2 / 8 / 16, rs_avg the last frame's. b200_fec_debug_fengyun_reads gives one record per
-       read. max_soft <= 2^30. Device memory: about 7 bytes per max_soft byte (FIFO, the two branch streams, two Viterbi decisions). */
-    int invert_second_viterbi; /* "invert_second_viterbi"                                                                                */
+       read. max_soft <= 2^30. Device memory: about 7 bytes per max_soft byte (FIFO, the two branch streams, two Viterbi decisions).
+       kind B200_FEC_FENGYUN_MPT = fengyun_mpt_decoder (FengYun-3 A/B/C MPT, module_fengyun_mpt_decoder.cpp): the same loop with two
+       Viterbi1_2 decoders (phases 0 / 90, no I/Q-swap search; 8192 soft bytes -> 4096 bits each) in place of Viterbi3_4. The split is
+       AHRPT's with Q always complemented, then each branch goes through rotate_soft(PHASE_0, swap): -128 -> -127 and the two bytes of
+       every branch pair exchanged. Only a read that leaves viterbi1 in NOSYNC counts towards the shift toggle (the module tests viterbi1
+       twice). The deframer has the default thresholds, deframer_state 2 / 6 / 12. The module has no invert_second_viterbi: a nonzero
+       value is refused before the device is looked at. Stats, records and max_soft as for AHRPT. */
+    int invert_second_viterbi; /* "invert_second_viterbi" (fengyun_ahrpt_decoder only; 0 for fengyun_mpt_decoder)                          */
 } b200_fec_cfg;
 
 typedef struct b200_demod_stats
@@ -281,8 +288,8 @@ typedef struct b200_fec_stats
        viterbi_ber (Viterbi27's BER of the last frame) and rs_corrected / rs_failed above; m2x_mode 1: the keys of
        ccsds_conv_concat_decoder above */
     int rs_avg;
-    int viterbi2_state;       /* fengyun_ahrpt_decoder: "viterbi2_lock" (viterbi_state above is "viterbi1_lock")                       */
-    float viterbi2_ber;       /* fengyun_ahrpt_decoder: "viterbi2_ber" (viterbi_ber above is "viterbi1_ber")                          */
+    int viterbi2_state;       /* fengyun_ahrpt / _mpt_decoder: "viterbi2_lock" (viterbi_state above is "viterbi1_lock")                */
+    float viterbi2_ber;       /* fengyun_ahrpt / _mpt_decoder: "viterbi2_ber" (viterbi_ber above is "viterbi1_ber")                   */
 } b200_fec_stats;
 
 typedef struct b200_demod b200_demod;
@@ -437,16 +444,17 @@ int b200_fec_debug_hrpt_frames(b200_fec *f, b200_hrpt_frame *out, long cap, long
    since create / reset) of the bit that completed it. dmsp_rtd_decoder's "_timestamps.txt" needs it: the module stamps a frame with the
    number of 8192-byte reads that produced frames, up to the one holding that bit. Other kinds: B200_EINVAL. */
 int b200_fec_frame_bits(b200_fec *f, long *out, long cap, long *n_out);
-/* fengyun_ahrpt_decoder: one record per 16384-byte read the LAST push completed, the module's variables at the end of that read */
+/* fengyun_ahrpt_decoder / fengyun_mpt_decoder: one record per 16384-byte read the LAST push completed, the module's variables at the end
+   of that read */
 typedef struct b200_fengyun_read
 {
     long read;                /* read index since create / reset                                                                      */
     int shift, invert_branches; /* the search machines after the read (shift toggles after 10 reads with a Viterbi in NOSYNC; the
                                  branches swap after 10 deframer NOSYNC reads)                                                        */
-    int v1, v2;               /* bits each Viterbi returned (0 or 6144)                                                               */
-    int state1, state2;       /* Viterbi3_4::getState() after the read: 0 NOSYNC, 1 SYNCED                                             */
-    float ber1, ber2;         /* Viterbi3_4::ber() after the read                                                                     */
-    int deframer_state;       /* 2 / 8 / 16 after the read                                                                            */
+    int v1, v2;               /* bits each Viterbi returned: 0 or 6144 (AHRPT) / 4096 (MPT)                                           */
+    int state1, state2;       /* Viterbi3_4 / Viterbi1_2::getState() after the read: 0 NOSYNC, 1 SYNCED                                */
+    float ber1, ber2;         /* Viterbi3_4 / Viterbi1_2::ber() after the read                                                        */
+    int deframer_state;       /* 2 / 8 / 16 (AHRPT) or 2 / 6 / 12 (MPT) after the read                                                */
     int pad;
 } b200_fengyun_read;
 int b200_fec_debug_fengyun_reads(b200_fec *f, b200_fengyun_read *out, long cap, long *n_out);

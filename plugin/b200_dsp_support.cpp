@@ -6,7 +6,7 @@
 //
 //   loader()                          the one symbol SatDump dlsym()s (core/plugin.cpp:15-33)
 //   B200DSPSupport::init()            on SatDumpStartedEvent (fired after every plugin registered its modules, init.cpp:163) the
-//                                     entries "psk_demod", "pm_demod", "terra_db_demod", "fsk_demod", "metop_ahrpt_decoder", "ccsds_conv_concat_decoder", "ccsds_simple_psk_decoder", "ccsds_ldpc_decoder", "ccsds_turbo_decoder", "metop_dump_decoder", "meteor_lrpt_decoder", "noaa_hrpt_decoder", "meteor_hrpt_decoder", "aqua_db_decoder", "noaa_gac_decoder", "dmsp_rtd_decoder", "meteor_xband_decoder" and "fengyun_ahrpt_decoder" of
+//                                     entries "psk_demod", "pm_demod", "terra_db_demod", "fsk_demod", "metop_ahrpt_decoder", "ccsds_conv_concat_decoder", "ccsds_simple_psk_decoder", "ccsds_ldpc_decoder", "ccsds_turbo_decoder", "metop_dump_decoder", "meteor_lrpt_decoder", "noaa_hrpt_decoder", "meteor_hrpt_decoder", "aqua_db_decoder", "noaa_gac_decoder", "dmsp_rtd_decoder", "meteor_xband_decoder", "fengyun_ahrpt_decoder" and "fengyun_mpt_decoder" of
 //                                     satdump::pipeline::modules_registry (module.h:210, looked up first-match by id, module.cpp:129-135)
 //                                     get their factory replaced, so existing pipelines instantiate the CUDA modules.
 //                                     Set B200_DSP_REGISTER_ONLY=1 to register "<id>_b200" ids instead and leave the originals alone.
@@ -241,10 +241,13 @@ namespace b200plugin
             }
             if (stage->getID() == "ccsds_turbo_decoder" || stage->getID() == "meteor_xband_decoder") // neither module has getModuleStats:
                 return v;                                                                          // ProcessingModule's empty one
-            if (stage->getID() == "fengyun_ahrpt_decoder") // FengyunAHRPTDecoderModule::getModuleStats (module_fengyun_ahrpt_decoder.cpp:138-152)
+            // FengyunAHRPTDecoderModule::getModuleStats (module_fengyun_ahrpt_decoder.cpp:138-152: deframer states 2 / 8 / 16) and
+            // FengyunMPTDecoderModule::getModuleStats (module_fengyun_mpt_decoder.cpp:137-153: 2 / 6 / 12)
+            if (stage->getID() == "fengyun_ahrpt_decoder" || stage->getID() == "fengyun_mpt_decoder")
             {
+                const bool mpt = stage->getID() == "fengyun_mpt_decoder";
                 const int ds = stage->deframer_state.load(), v1 = stage->viterbi_lock.load(), v2 = stage->viterbi2_lock.load();
-                v["deframer_lock"] = ds == 16;
+                v["deframer_lock"] = ds == (mpt ? 12 : 16);
                 v["viterbi1_ber"] = stage->viterbi_ber.load();
                 v["viterbi1_lock"] = v1;
                 v["viterbi2_ber"] = stage->viterbi2_ber.load();
@@ -252,7 +255,7 @@ namespace b200plugin
                 v["rs_avg"] = stage->rs_avg.load();
                 v["viterbi1_state"] = v1 == 0 ? "NOSYNC" : "SYNCED";
                 v["viterbi2_state"] = v2 == 0 ? "NOSYNC" : "SYNCED";
-                v["deframer_state"] = ds == 2 ? "NOSYNC" : (ds == 8 ? "SYNCING" : "SYNCED");
+                v["deframer_state"] = ds == 2 ? "NOSYNC" : (ds == (mpt ? 6 : 8) ? "SYNCING" : "SYNCED");
                 return v;
             }
             if (stage->getID() == "metop_dump_decoder") // MetOpDumpDecoderModule::getModuleStats (module_metop_dump_decoder.cpp:84-90)
@@ -337,7 +340,8 @@ public:
     {
         for (const char *id : {"psk_demod", "pm_demod", "terra_db_demod", "fsk_demod", "metop_ahrpt_decoder", "ccsds_conv_concat_decoder", "ccsds_simple_psk_decoder", "ccsds_ldpc_decoder",
                                "ccsds_turbo_decoder", "metop_dump_decoder", "meteor_lrpt_decoder", "noaa_hrpt_decoder", "meteor_hrpt_decoder",
-                               "aqua_db_decoder", "noaa_gac_decoder", "dmsp_rtd_decoder", "meteor_xband_decoder", "fengyun_ahrpt_decoder"})
+                               "aqua_db_decoder", "noaa_gac_decoder", "dmsp_rtd_decoder", "meteor_xband_decoder", "fengyun_ahrpt_decoder",
+                               "fengyun_mpt_decoder"})
             evt.modules_registry.push_back({std::string(id) + "_b200", nlohmann::json(), factory(id)});
     }
 
@@ -348,7 +352,7 @@ public:
                 e.id == "ccsds_ldpc_decoder" || e.id == "ccsds_turbo_decoder" || e.id == "metop_dump_decoder" ||
                 e.id == "meteor_lrpt_decoder" || e.id == "noaa_hrpt_decoder" || e.id == "meteor_hrpt_decoder" ||
                 e.id == "aqua_db_decoder" || e.id == "noaa_gac_decoder" || e.id == "dmsp_rtd_decoder" || e.id == "meteor_xband_decoder" ||
-                e.id == "fengyun_ahrpt_decoder")
+                e.id == "fengyun_ahrpt_decoder" || e.id == "fengyun_mpt_decoder")
             {
                 e.inst = factory(e.id);
                 logger->info("b200_dsp_support: module " + e.id + " now runs on the B200 path");

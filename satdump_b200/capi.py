@@ -467,6 +467,18 @@ def fengyun_ahrpt_cfg(viterbi_outsync_after=None, viterbi_ber_thresold=None, inv
     return cfg
 
 
+def fengyun_mpt_cfg(viterbi_outsync_after=None, viterbi_ber_thresold=None, device=0, max_soft=1 << 24):
+    """fengyun_mpt_decoder (module_fengyun_mpt_decoder.cpp:17-20): viterbi_outsync_after and viterbi_ber_thresold are both required, as
+    the module reads them with no default. The module has no invert_second_viterbi (its Q branch is always complemented)."""
+    for name, v in (("viterbi_outsync_after", viterbi_outsync_after), ("viterbi_ber_thresold", viterbi_ber_thresold)):
+        if v is None:
+            raise ValueError(f"fengyun_mpt_decoder: {name} is required")
+    cfg = FecCfg()
+    cfg.kind, cfg.constellation, cfg.device, cfg.max_soft = 14, CONST["qpsk"], device, max_soft
+    cfg.outsync_after, cfg.ber_thresold = int(viterbi_outsync_after), float(viterbi_ber_thresold)
+    return cfg
+
+
 def dmsp_timestamps(bits, start_timestamp, read_bits_seen=None):
     """dmsp_rtd_decoder's "_timestamps.txt" values for frames completed at stream bits `bits` (b200_fec_frame_bits): start +
     8192 * (reads of 8192 soft bytes from the stream's start that produced frames, up to the frame's) / 1.024e6. read_bits_seen carries
@@ -504,6 +516,8 @@ def fec_cfg_for(sig, max_soft, device=0):
         return dmsp_rtd_cfg(device=device, max_soft=max_soft)
     if sig.decoder == "fengyun_ahrpt":
         return fengyun_ahrpt_cfg(sig.outsync_after, sig.ber_thresold, sig.invert_second_viterbi, device=device, max_soft=max_soft)
+    if sig.decoder == "fengyun_mpt":
+        return fengyun_mpt_cfg(sig.outsync_after, sig.ber_thresold, device=device, max_soft=max_soft)
     if sig.decoder in ("meteor_mtvza", "meteor_kmss_bpsk"):
         return meteor_xband_cfg("mtvza" if sig.decoder == "meteor_mtvza" else "kmss_bpsk", device=device, max_soft=max_soft)
     if sig.decoder == "turbo":
@@ -780,8 +794,9 @@ class Fec:
         return np.array([[recs[k].bit, recs[k].inverted, recs[k].state] for k in range(n.value)], np.int64).reshape(-1, 3)
 
     def fengyun_reads(self):
-        """fengyun_ahrpt_decoder: one record per 16384-byte read the last push completed, as float64 [n, 9] = shift, invert_branches, v1,
-        v2, viterbi1 state, viterbi2 state, viterbi1 ber, viterbi2 ber, deframer state after the read (oracle.fengyun's records)"""
+        """fengyun_ahrpt_decoder / fengyun_mpt_decoder: one record per 16384-byte read the last push completed, as float64 [n, 9] = shift,
+        invert_branches, v1, v2, viterbi1 state, viterbi2 state, viterbi1 ber, viterbi2 ber, deframer state after the read (the records of
+        oracle.fengyun and oracle.fengyun_mpt)"""
         cap = int(self._n) // 16384 + 4
         recs = (FengyunRead * cap)()
         n = C.c_long(0)

@@ -110,7 +110,7 @@ Fec::Fec(const b200_fec_cfg &in) : cfg(meteor_m2x_as_ccsds(in))
     case B200_FEC_NOAA_HRPT: case B200_FEC_METEOR_HRPT: case B200_FEC_DMSP_RTD: make = sync_walk_decoder; break;
     case B200_FEC_AQUA_DB: case B200_FEC_NOAA_GAC: make = bit_stage_decoder; break;
     case B200_FEC_METEOR_XBAND: make = xband_decoder; break;
-    case B200_FEC_FENGYUN_AHRPT: make = fengyun_decoder; break;
+    case B200_FEC_FENGYUN_AHRPT: case B200_FEC_FENGYUN_MPT: make = fengyun_decoder; break;
     default: B200_REQUIRE(false, B200_EINVAL, "unknown decoder kind %d", cfg.kind);
     }
     B200_REQUIRE(cfg.max_soft >= 65536, B200_EINVAL, "max_soft must be >= 65536");
@@ -418,12 +418,21 @@ void Viterbi::alloc_lock_search()
     B200_CUDA(cudaFuncSetAttribute(k_vit_idle2<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8 * VIT_IDLE_WARP_BYTES));
 }
 
-const VitIdleOut &Viterbi::lock_search(Fec &f, const int8_t *src, long c, int n, int nswap, int nphases, int ph0, int ph1, VitIdleState st, bool fy)
+const VitIdleOut &Viterbi::lock_search(Fec &f, const int8_t *src, long c, int n, int nswap, int nphases, int ph0, int ph1, VitIdleState st, int mode,
+                                       unsigned head)
 {
+    const float thr = f.cfg.ber_thresold;
+    if (mode == VIT_IDLE_R12_EXACT) { // every trial reads the one before it: the serial kernel
+        k_vit_idle<VIT_IDLE_R12_EXACT><<<1, 32, 0, f.stream>>>(src, c, n, geom, nswap, nphases, ph0, ph1, thr, st, idle_dec.p, idle_out.p, head);
+        f.launches++;
+        B200_CUDA(cudaMemcpyAsync(h_idle.p, idle_out.p, sizeof(VitIdleOut), cudaMemcpyDeviceToHost, f.stream));
+        B200_CUDA(cudaStreamSynchronize(f.stream));
+        return *h_idle.p;
+    }
+    const bool fy = mode == VIT_IDLE_FY;
     // parallel search first (one warp per hypothesis); it hands over to the serial kernel at the first chunk whose chained 6-bit states
     // its two-pass guess did not reproduce
     const int nh = nswap * nphases * 2;
-    const float thr = f.cfg.ber_thresold;
     auto idle2 = fy ? k_vit_idle2<true> : k_vit_idle2<false>;
     idle2<<<1, 32 * nh, nh * VIT_IDLE_WARP_BYTES, f.stream>>>(src, c, n, geom, nswap, nphases, ph0, ph1, thr, st, idle2_out.p);
     f.launches++;
@@ -432,8 +441,8 @@ const VitIdleOut &Viterbi::lock_search(Fec &f, const int8_t *src, long c, int n,
     *h_idle.p = h_idle2.p->o;
     if (h_idle2.p->fallback_chunk >= 0) {
         const long c2 = c + h_idle2.p->fallback_chunk;
-        auto idle1 = fy ? k_vit_idle<true> : k_vit_idle<false>;
-        idle1<<<1, 32, 0, f.stream>>>(src, c2, (int)(n - (c2 - c)), geom, nswap, nphases, ph0, ph1, thr, h_idle2.p->o.st, idle_dec.p, idle_out.p);
+        auto idle1 = fy ? k_vit_idle<VIT_IDLE_FY> : k_vit_idle<VIT_IDLE_PLAIN>;
+        idle1<<<1, 32, 0, f.stream>>>(src, c2, (int)(n - (c2 - c)), geom, nswap, nphases, ph0, ph1, thr, h_idle2.p->o.st, idle_dec.p, idle_out.p, 0u);
         f.launches++;
         B200_CUDA(cudaMemcpyAsync(h_idle.p, idle_out.p, sizeof(VitIdleOut), cudaMemcpyDeviceToHost, f.stream));
         B200_CUDA(cudaStreamSynchronize(f.stream));
@@ -480,7 +489,7 @@ void Conv::viterbi_segment(Fec &f, long c0, long nch, std::vector<OutChunk> &out
     while (c < nch) {
         if (vit_state == 0) {
             idle_st.enc_state = vit.enc_state; // ONE chained CCEncoder serves the lock test and the SYNCED BER check (viterbi_3_4.cpp:126,157)
-            const VitIdleOut &o = vit.lock_search(f, f.softbuf.p, c, (int)(nch - c), nswap, nphases, ph0, ph1, idle_st, false);
+            const VitIdleOut &o = vit.lock_search(f, f.softbuf.p, c, (int)(nch - c), nswap, nphases, ph0, ph1, idle_st, VIT_IDLE_PLAIN);
             idle_st = o.st;
             vit.enc_state = idle_st.enc_state;
             float bb = 10.f;

@@ -1,11 +1,15 @@
-// Host driver of fengyun_ahrpt_decoder (B200_FEC_FENGYUN_AHRPT): FengyunAHRPTDecoderModule::process
-// (plugins/fengyun3_support/fengyun3/module_fengyun_ahrpt_decoder.cpp:42-136) over the soft FIFO of Fec, in the module's 16384-byte reads
-// counted from the stream's start. Every read: k_fy_split -> two Viterbi3_4 (fymode) -> FengyunDiff::work2 (k_fy_diff) -> when both
-// Viterbis decoded, the deframer and the frame stage of the convolutional decoders.
+// Host driver of the two FengYun-3 decoders over the soft FIFO of Fec, in the modules' 16384-byte reads counted from the stream's start:
+//   fengyun_ahrpt_decoder (B200_FEC_FENGYUN_AHRPT)  FengyunAHRPTDecoderModule::process
+//                                                    (plugins/fengyun3_support/fengyun3/module_fengyun_ahrpt_decoder.cpp:42-136)
+//   fengyun_mpt_decoder (B200_FEC_FENGYUN_MPT)      FengyunMPTDecoderModule::process
+//                                                    (plugins/fengyun3_support/fengyun3/module_fengyun_mpt_decoder.cpp:42-135)
+// Every read: k_fy_split -> two Viterbis (Viterbi3_4 fymode / Viterbi1_2) -> FengyunDiff::work2 (k_fy_diff) -> when both Viterbis
+// decoded, the deframer and the frame stage of the convolutional decoders. What differs between the two modules is data (FyKind).
 //
 // The module's search machines change only at read boundaries:
-//   * shift: after a read that leaves either Viterbi in NOSYNC, viterbiNoSyncRun++ (never reset); from 10 on, every such read toggles
-//     shift. It decides how the next reads are split, so the driver splits a run of reads with the current shift, decodes both branches,
+//   * shift: after a read that leaves a Viterbi in NOSYNC (AHRPT: either one; MPT: viterbi1 only, as the module's test names viterbi1
+//     twice), viterbiNoSyncRun++ (never reset); from 10 on, every such read toggles shift. It decides how the next reads are split,
+//     so the driver splits a run of reads with the current shift, decodes both branches,
 //     walks the reads on the host and, at the first toggle, rolls both Viterbis back to the end of that read and splits the rest again.
 //     While both Viterbis are SYNCED nothing toggles, so a locked push is split and decoded as one run. While one of them is in NOSYNC
 //     the driver steps read by read (the lock search reports the BERs of every read).
@@ -19,13 +23,36 @@
 namespace b200
 {
 
-// One Viterbi3_4(ber, outsync, 8192, fymode = true) and its lock machine (viterbi_3_4.cpp:106-173), decoding one branch of the reads
+// What distinguishes fengyun_mpt_decoder from fengyun_ahrpt_decoder
+struct FyKind
+{
+    const char *name;
+    int rate34;                       // the Viterbi: 1 Viterbi3_4(fymode), 0 Viterbi1_2 (VitGeom::rate34; its BER scale follows)
+    int F;                            // bits one Viterbi call returns per branch and read
+    int spec_steps;                   // k_vit_spec's initial window
+    int nphases, ph0, ph1;            // the lock search's phases (one I/Q-swap hypothesis, both shifts)
+    int idle_mode;                    // the lock search's VIT_IDLE_*: FY, FengYun's depuncture, VitHyp{shift, phase, shift}; else
+                                      // VitHyp{swap, phase, shift}
+    int st_syncing, st_synced;        // the deframer's STATE_SYNCING / STATE_SYNCED
+    bool v2_toggles;                  // a read leaving viterbi2 in NOSYNC counts towards the shift toggle
+    bool invert_q;                    // the module has invert_second_viterbi (else Q is always complemented and a nonzero one is refused)
+    void (*split)(const int8_t *, long, int, int, int8_t *, int8_t *);
+    void (*diff)(const uint32_t *, const uint32_t *, int, const int *, int, int, int, int, uint32_t *, long);
+};
+static const FyKind FY_AHRPT{"fengyun_ahrpt_decoder", 1, FY_BITS, VIT_SPEC_STEPS_34, 1, 0, 0, VIT_IDLE_FY, 8, 16, true, true, k_fy_split<false>,
+                             k_fy_diff<FY_BITS>};
+static const FyKind FY_MPT{"fengyun_mpt_decoder", 0, FY_MPT_BITS, VIT_SPEC_STEPS_12, 2, 0, 1, VIT_IDLE_R12_EXACT, 6, 12, false, false,
+                           k_fy_split<true>, k_fy_diff<FY_MPT_BITS>};
+
+// One Viterbi3_4(ber, outsync, 8192, fymode = true) (viterbi_3_4.cpp:106-173) or Viterbi1_2(ber, outsync, 8192, {PHASE_0, PHASE_90})
+// (viterbi_1_2.cpp:36-116) and its lock machine, decoding one branch of the reads
 struct FyVit
 {
     struct State
     {
         int vit_state = 0, invalid = 0;
         VitIdleState idle_st{-1, 0};
+        unsigned idle_head = 0;       // (Viterbi1_2) the first bits the last lock trial decoded
         VitHyp hyp{0, 0, 0};
         int main_next_start = -1, enc_state = 0;
         float ber = 10.f, search_ber = 10.f; // ber(): SYNCED the last BER check, else the least BER of the last lock search
@@ -61,9 +88,9 @@ struct FyVit
                 f.replays++;
                 break;
             }
-            const float ber = ((float)rec[i].ber_errors / (float)rec[i].ber_total) * 5.0f;
+            const float ber = ((float)rec[i].ber_errors / (float)rec[i].ber_total) * (vit.geom.rate34 ? 5.0f : 2.5f);
             bool lost = false;
-            if (ber > f.cfg.ber_thresold) { // viterbi_3_4.cpp:160-169
+            if (ber > f.cfg.ber_thresold) { // viterbi_3_4.cpp:160-169, viterbi_1_2.cpp:99-109
                 if (++s.invalid > f.cfg.outsync_after) {
                     s.vit_state = 0;
                     lost = true;
@@ -73,18 +100,19 @@ struct FyVit
             s.ber = lost ? s.search_ber : ber;
             vit.main_next_start = rec[i].next_start;
             vit.enc_state = rec[i].enc_tail;
-            outs.push_back(ReadOut{FY_BITS, now()});
+            outs.push_back(ReadOut{vit.geom.F, now()});
             if (lost)
                 break;
         }
     }
-    // one read: the lock search when in NOSYNC (phase 0, both puncturing shifts), and the read's decode when it locks or was SYNCED
-    void step(Fec &f, long j)
+    // one read: the lock search when in NOSYNC (the kind's phases, both shifts), and the read's decode when it locks or was SYNCED
+    void step(Fec &f, long j, const FyKind &kind)
     {
         if (s.vit_state == 0) {
             s.idle_st.enc_state = vit.enc_state; // ONE chained CCEncoder serves the lock test and the SYNCED BER check
-            const VitIdleOut &o = vit.lock_search(f, soft.p, j, 1, 1, 1, 0, 0, s.idle_st, true);
+            const VitIdleOut &o = vit.lock_search(f, soft.p, j, 1, 1, kind.nphases, kind.ph0, kind.ph1, s.idle_st, kind.idle_mode, s.idle_head);
             s.idle_st = o.st;
+            s.idle_head = o.head;
             vit.enc_state = o.st.enc_state;
             float bb = 10.f;
             for (int i = 0; i < 16; i++)
@@ -96,7 +124,8 @@ struct FyVit
             }
             s.vit_state = 1;
             s.invalid = 0;
-            vit.hyp = VitHyp{o.shift, 0, o.shift}; // (k_fy_split's storage: FengYun's depuncture of shift s is the MetOp one with swap s)
+            // (AHRPT, k_fy_split's storage: FengYun's depuncture of shift s is the MetOp one with swap s)
+            vit.hyp = VitHyp{kind.idle_mode == VIT_IDLE_FY ? o.shift : o.swap, o.phase, o.shift};
         }
         decode(f, j, 1);
     }
@@ -108,6 +137,7 @@ struct FyVit
 
 struct Fengyun : Decoder
 {
+    const FyKind &kind;
     FyVit v[2];                       // viterbi1 (I), viterbi2 (Q)
     Deframer defr;
     FrameStage fs;
@@ -119,7 +149,7 @@ struct Fengyun : Decoder
     long reads_done = 0;
     std::vector<b200_fengyun_read> recs; // the last push's
 
-    explicit Fengyun(Fec &f);
+    Fengyun(Fec &f, const FyKind &k);
     void process(Fec &f) override;
     void reset(Fec &f) override;
     void stats(b200_fec_stats *o) override;
@@ -128,10 +158,12 @@ struct Fengyun : Decoder
     void frames(Fec &f, int e);
 };
 
-Fengyun::Fengyun(Fec &f)
+Fengyun::Fengyun(Fec &f, const FyKind &k) : kind(k)
 {
     b200_fec_cfg &cfg = f.cfg;
-    B200_REQUIRE(cfg.max_soft <= (1L << 30), B200_EINVAL, "max_soft must be <= 2^30 for fengyun_ahrpt_decoder");
+    B200_REQUIRE(cfg.max_soft <= (1L << 30), B200_EINVAL, "max_soft must be <= 2^30 for %s", kind.name);
+    B200_REQUIRE(kind.invert_q || cfg.invert_second_viterbi == 0, B200_EINVAL,
+                 "%s has no invert_second_viterbi: its Q branch is always complemented", kind.name);
     // BPSK_CCSDS_Deframer (8192 bits), derand_ccsds(&cadu[4], 1020), decode_interlaved(&cadu[4], true, 4): RS223 I=4 dual basis
     cfg.cadu_size = 8192;
     cfg.rs_i = 4;
@@ -149,27 +181,30 @@ Fengyun::Fengyun(Fec &f)
     check_device(cfg.device);
     DeviceGuard g(cfg.device);
     const long max_reads = cfg.max_soft / FY_READ + 2;
-    const long max_new_bits = max_reads * 2L * FY_BITS;
+    const long max_new_bits = max_reads * 2L * kind.F;
     const long max_frames = Deframer::frames_cap(max_new_bits, cfg.cadu_size);
     f.open(FY_READ, max_frames);
     VitGeom geom{};
-    geom.rate34 = 1;
+    geom.rate34 = kind.rate34;
     geom.chunk = FY_BRANCH;
-    geom.F = FY_BITS;
+    geom.F = kind.F;
     for (FyVit &fv : v) {
-        fv.vit.spec_steps = VIT_SPEC_STEPS_34;
+        fv.vit.spec_steps = kind.spec_steps;
         fv.vit.alloc(f, geom, max_reads);
         fv.vit.alloc_lock_search();
         fv.soft.alloc((size_t)max_reads * FY_BRANCH);
         fv.outs.reserve(max_reads);
     }
     dreads.alloc(max_reads);
-    defr.alloc(f, max_new_bits, cfg.cadu_size, cfg.asm_sync, 16, 8); // deframer.STATE_SYNCING = 8, STATE_SYNCED = 16 (module :45-46)
+    defr.alloc(f, max_new_bits, cfg.cadu_size, cfg.asm_sync, kind.st_synced, kind.st_syncing); // AHRPT module :45-46; MPT the defaults
     fs.alloc(f, max_frames, cfg.rs_i, false);
     reset(f);
 }
 
-std::unique_ptr<Decoder> fengyun_decoder(Fec &f) { return std::make_unique<Fengyun>(f); }
+std::unique_ptr<Decoder> fengyun_decoder(Fec &f)
+{
+    return std::make_unique<Fengyun>(f, f.cfg.kind == B200_FEC_FENGYUN_MPT ? FY_MPT : FY_AHRPT);
+}
 
 void Fengyun::reset(Fec &f)
 {
@@ -189,8 +224,8 @@ void Fengyun::reset(Fec &f)
 int Fengyun::run_reads(Fec &f, long r, int n)
 {
     const long total = (long)n * FY_BRANCH;
-    k_fy_split<<<(unsigned)std::min<long>((total + 255) / 256, 132 * 16), 256, 0, f.stream>>>(f.softbuf.p + r * FY_READ, n, shift,
-                                                                                             f.cfg.invert_second_viterbi, v[0].soft.p, v[1].soft.p);
+    kind.split<<<(unsigned)std::min<long>((total + 255) / 256, 132 * 16), 256, 0, f.stream>>>(f.softbuf.p + r * FY_READ, n, shift,
+                                                                                              f.cfg.invert_second_viterbi, v[0].soft.p, v[1].soft.p);
     f.launches++;
     for (FyVit &fv : v)
         fv.outs.clear();
@@ -202,13 +237,13 @@ int Fengyun::run_reads(Fec &f, long r, int n)
             v[0].decode(f, j, n - j);
             v[1].decode(f, j, n - j);
         } else {
-            v[0].step(f, j);
-            v[1].step(f, j);
+            v[0].step(f, j, kind);
+            v[1].step(f, j, kind);
         }
         int e = (int)std::min(v[0].outs.size(), v[1].outs.size());
-        for (int k = j; k < e; k++) { // module :75-86
+        for (int k = j; k < e; k++) { // AHRPT module :75-86, MPT module :81-92
             const FyVit::State &a = v[0].outs[k].after, &b = v[1].outs[k].after;
-            if ((a.vit_state == 0 || b.vit_state == 0) && ++vit_nosync_runs >= 10) {
+            if ((a.vit_state == 0 || (kind.v2_toggles && b.vit_state == 0)) && ++vit_nosync_runs >= 10) {
                 shift ^= 1;
                 toggled = true;
                 e = k + 1;
@@ -250,7 +285,7 @@ int Fengyun::run_reads(Fec &f, long r, int n)
     return j;
 }
 
-// FengyunDiff::work2 and the deframer on the reads 0 .. e - 1 of the run where both Viterbis decoded (module :89-126)
+// FengyunDiff::work2 and the deframer on the reads 0 .. e - 1 of the run where both Viterbis decoded (AHRPT module :89-126, MPT :94-131)
 void Fengyun::frames(Fec &f, int e)
 {
     act.clear();
@@ -260,7 +295,7 @@ void Fengyun::frames(Fec &f, int e)
         if (v[0].outs[k].bits > 0 && v[1].outs[k].bits > 0)
             act.push_back(k);
     const int bw = v[0].vit.geom.bit_words;
-    const long rb = 2L * FY_BITS; // deframer bits per read
+    const long rb = 2L * kind.F; // deframer bits per read
     size_t k = 0;
     while (k < act.size()) {
         const int na = (int)(act.size() - k);
@@ -269,7 +304,7 @@ void Fengyun::frames(Fec &f, int e)
         const int rs_avg0 = f.rs_avg;
         B200_CUDA(cudaMemcpyAsync(dreads.p, act.data() + k, sizeof(int) * na, cudaMemcpyHostToDevice, f.stream));
         const long words = (na * rb + 64) / 32;
-        k_fy_diff<<<(unsigned)std::min<long>((words + 255) / 256, 132 * 16), 256, 0, f.stream>>>(v[0].vit.chunk_bits.p, v[1].vit.chunk_bits.p, bw,
+        kind.diff<<<(unsigned)std::min<long>((words + 255) / 256, 132 * 16), 256, 0, f.stream>>>(v[0].vit.chunk_bits.p, v[1].vit.chunk_bits.p, bw,
                                                                                                dreads.p, na, invert, xin, yin, defr.fifo.p,
                                                                                                defr.fifo_bits);
         f.launches++;
@@ -300,7 +335,7 @@ void Fengyun::frames(Fec &f, int e)
             defr.deframe(f, fs, done * rb);
         }
         const int q = act[k + done - 1];
-        const int b0 = last_raw_bit(f, v[0].vit.chunk_bits.p, bw, q, FY_BITS), b1 = last_raw_bit(f, v[1].vit.chunk_bits.p, bw, q, FY_BITS);
+        const int b0 = last_raw_bit(f, v[0].vit.chunk_bits.p, bw, q, kind.F), b1 = last_raw_bit(f, v[1].vit.chunk_bits.p, bw, q, kind.F);
         xin = invert ? b0 : b1; // in1 = viterbi2's bits unless the branches are swapped
         yin = invert ? b1 : b0;
         if (flip >= 0)
@@ -361,7 +396,7 @@ extern "C" int b200_fec_debug_fengyun_reads(b200_fec *h, b200_fengyun_read *out,
 {
     return guarded([&] {
         B200_REQUIRE(h && out && n_out, B200_EINVAL, "NULL argument");
-        const Fengyun &d = h->f->decoder_as<Fengyun>("not a fengyun_ahrpt_decoder");
+        const Fengyun &d = h->f->decoder_as<Fengyun>("not a fengyun_ahrpt_decoder or fengyun_mpt_decoder");
         const long n = (long)d.recs.size();
         B200_REQUIRE(n <= cap, B200_ESTATE, "output buffer too small: need %ld", n);
         std::copy(d.recs.begin(), d.recs.end(), out);

@@ -664,16 +664,24 @@ __global__ void __launch_bounds__(32) k_punc_idle(const int8_t *__restrict__ sof
 // Replays Viterbi3_4::work / Viterbi1_2::work in the IDLE state chunk by chunk until a hypothesis locks
 // (viterbi_3_4.cpp:112-144, viterbi_1_2.cpp:54-89), with the chained test decoder / encoder state.
 #endif // B200_DEFINE_KERNELS
-struct VitIdleOut { int lock_chunk, swap, phase, shift; float ber; float bers[16]; VitIdleState st; int pad; };
+// head (M = 2 only): the first 16 bits the test decoder's last trial decoded, bit j at (head >> j) & 1
+struct VitIdleOut { int lock_chunk, swap, phase, shift; float ber; float bers[16]; VitIdleState st; unsigned head; };
+constexpr int VIT_IDLE_PLAIN = 0, VIT_IDLE_FY = 1, VIT_IDLE_R12_EXACT = 2; // the lock search's modes (k_vit_idle)
 
 #ifdef B200_DEFINE_KERNELS
-// FY (fengyun_ahrpt_decoder, Viterbi3_4 with fymode): hypothesis (s = 0, shift) runs as VitHyp{shift, 0, shift}; with the branch stream
-// stored by k_fy_split (fengyun.cuh) that is FengYun's depuncture through the MetOp one (the stored bers and lswap keep s = 0).
-template <bool FY = false>
+// M (the lock search's mode, VIT_IDLE_*):
+//   FY (fengyun_ahrpt_decoder, Viterbi3_4 with fymode): hypothesis (s = 0, shift) runs as VitHyp{shift, 0, shift}; with the branch stream
+//   stored by k_fy_split (fengyun.cuh) that is FengYun's depuncture through the MetOp one (the stored bers and lswap keep s = 0).
+//   R12_EXACT (fengyun_mpt_decoder, r=1/2): the 12 symbols the test decoder reads past its 2048 test bytes are the first decoded bits (0 /
+//   1) of the trial before it, carried in head (head_in: the last trial of the previous call), as Viterbi1_2's member layout gives them.
+//   The other modes read them as 0.
+template <int M = VIT_IDLE_PLAIN>
 __global__ void __launch_bounds__(32) k_vit_idle(const int8_t *__restrict__ soft, long chunk0, int nchunks, VitGeom g, int nswap, int nphases,
                                                   int ph0, int ph1, float thr, VitIdleState st_in, uint2 *__restrict__ scratch_dec,
-                                                  VitIdleOut *__restrict__ out)
+                                                  VitIdleOut *__restrict__ out, unsigned head_in)
 {
+    constexpr bool FY = M == VIT_IDLE_FY;
+    unsigned head = head_in;
     const int lane = threadIdx.x;
     const AcsLane L = acs_lane_consts(lane);
     VitGeom tg = g;
@@ -702,7 +710,12 @@ __global__ void __launch_bounds__(32) k_vit_idle(const int8_t *__restrict__ soft
                         // r=1/2: the test decoder over-reads 12 bytes past the 2048 test bytes into the previous trial's decoded
                         // bits (viterbi_1_2.h:37-40); they only touch the last trellis steps. We feed erasure-neutral zeros/ones
                         // exactly like the reference layout would: previous decoded bits are 0/1 -> use 0.
-                        const int mine = tm < steps ? vit_symbols(c, tm, tg, h, VIT_TESTLEN, 0) : 0;
+                        int mine = tm < steps ? vit_symbols(c, tm, tg, h, VIT_TESTLEN, 0) : 0;
+                        if (M == VIT_IDLE_R12_EXACT && tm < steps) { // (r=1/2: symbol k of the test buffer is byte k)
+                            const int k0 = h.shift + 2 * tm - VIT_TESTLEN;
+                            if (k0 >= 0) mine = (mine & ~255) | ((head >> k0) & 1);
+                            if (k0 + 1 >= 0) mine = (mine & 255) | (((head >> (k0 + 1)) & 1) << 8);
+                        }
                         unsigned k0 = 0, k1 = 0;
                         const int nn = min(32, steps - t0);
                         for (int j = 0; j < nn; j++) {
@@ -747,6 +760,8 @@ __global__ void __launch_bounds__(32) k_vit_idle(const int8_t *__restrict__ soft
                     unsigned tail = 0;
                     for (int k = tg.F - 6; k < tg.F; k++) tail = (tail << 1) | ((tbits[k >> 5] >> (31 - (k & 31))) & 1u);
                     enc = tail;
+                    if (M == VIT_IDLE_R12_EXACT) // this trial's first bits: what the next trial's over-read sees
+                        head = __brev(tbits[0]) & 0xffffu;
                     const float b = ((float)errors / (float)total) * (g.rate34 ? 5.0f : 2.5f);
                     bers[(s * 4 + h.phase) * 2 + shift] = b;
                     if ((best == 10.f && b < thr) || (best < 10.f && b < best)) {
@@ -759,7 +774,7 @@ __global__ void __launch_bounds__(32) k_vit_idle(const int8_t *__restrict__ soft
         VitIdleOut o;
         o.lock_chunk = lock; o.swap = lswap; o.phase = lphase; o.shift = lshift; o.ber = best;
         for (int i = 0; i < 16; i++) o.bers[i] = bers[i];
-        o.st.dec_start = dec_start; o.st.enc_state = (int)enc; o.pad = 0;
+        o.st.dec_start = dec_start; o.st.enc_state = (int)enc; o.head = M == VIT_IDLE_R12_EXACT ? head : 0u;
         *out = o;
     }
 }
@@ -775,7 +790,7 @@ struct VitIdle2Out { VitIdleOut o; int fallback_chunk; int pad[3]; };
 constexpr int VIT_IDLE_ROWS = VIT_TESTLEN * 3 / 4 + 6 + 2;           // decision rows per hypothesis (r=3/4 is the larger: 1542)
 constexpr int VIT_IDLE_WARP_BYTES = VIT_IDLE_ROWS * 8 + 64 * 4;       // + 64 words of decoded bits
 #ifdef B200_DEFINE_KERNELS
-template <bool FY = false> // (as k_vit_idle)
+template <bool FY = false> // (as k_vit_idle; VIT_IDLE_R12_EXACT runs the serial kernel only)
 __global__ void __launch_bounds__(256) k_vit_idle2(const int8_t *__restrict__ soft, long chunk0, int nchunks, VitGeom g, int nswap, int nphases, int ph0,
                                                     int ph1, float thr, VitIdleState st_in, VitIdle2Out *__restrict__ out)
 {
@@ -901,7 +916,7 @@ __global__ void __launch_bounds__(256) k_vit_idle2(const int8_t *__restrict__ so
         VitIdle2Out r;
         r.o.lock_chunk = s_lock; r.o.swap = lswap; r.o.phase = lphase; r.o.shift = lshift; r.o.ber = best;
         for (int i = 0; i < 16; i++) r.o.bers[i] = bers[i];
-        r.o.st.dec_start = s_dec; r.o.st.enc_state = s_enc; r.o.pad = 0;
+        r.o.st.dec_start = s_dec; r.o.st.enc_state = s_enc; r.o.head = 0;
         r.fallback_chunk = s_fallback; r.pad[0] = r.pad[1] = r.pad[2] = 0;
         *out = r;
     }

@@ -115,8 +115,10 @@ struct Viterbi
     void alloc(Fec &f, const VitGeom &g, long max_chunks); // g's chunk, F and BER settings; the strides follow
     void alloc_lock_search();
     // Viterbi3_4 / Viterbi1_2::work in the IDLE state over the n chunks of src from chunk c, with the chained test decoder and encoder
-    // state st, until a hypothesis locks (lock_chunk relative to c, -1: none). fy: fengyun_ahrpt_decoder's hypotheses (k_vit_idle<true>)
-    const VitIdleOut &lock_search(Fec &f, const int8_t *src, long c, int n, int nswap, int nphases, int ph0, int ph1, VitIdleState st, bool fy);
+    // state st, until a hypothesis locks (lock_chunk relative to c, -1: none). mode: VIT_IDLE_PLAIN, VIT_IDLE_FY (fengyun_ahrpt_decoder's
+    // hypotheses) or VIT_IDLE_R12_EXACT (fengyun_mpt_decoder: the test decoder's over-read of the trial before, `head`; see k_vit_idle)
+    const VitIdleOut &lock_search(Fec &f, const int8_t *src, long c, int n, int nswap, int nphases, int ph0, int ph1, VitIdleState st, int mode,
+                                  unsigned head = 0);
     int decode_pass(Fec &f, const int8_t *src, long c, int nrange, long out_base, int n, const int *qlist, int nber, const int *ber_list);
     void decode_range(Fec &f, const int8_t *src, long c, int n, long out_base, int max_rounds);
     // Viterbi27 (meteor_lrpt_decoder): the n chunks at src (geom.chunk bytes apart, already rotated) decoded as consecutive calls of ONE
@@ -159,7 +161,7 @@ std::unique_ptr<Decoder> meteor_decoder(Fec &f);
 std::unique_ptr<Decoder> sync_walk_decoder(Fec &f); // noaa_hrpt_decoder, meteor_hrpt_decoder, dmsp_rtd_decoder (api_hrpt.cu)
 std::unique_ptr<Decoder> bit_stage_decoder(Fec &f); // aqua_db_decoder, noaa_gac_decoder (api_hrpt.cu)
 std::unique_ptr<Decoder> xband_decoder(Fec &f);     // meteor_xband_decoder (api_hrpt.cu)
-std::unique_ptr<Decoder> fengyun_decoder(Fec &f);   // fengyun_ahrpt_decoder (api_fengyun.cu)
+std::unique_ptr<Decoder> fengyun_decoder(Fec &f);   // fengyun_ahrpt_decoder, fengyun_mpt_decoder (api_fengyun.cu)
 
 class Fec
 {

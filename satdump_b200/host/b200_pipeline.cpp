@@ -22,6 +22,8 @@ static void print_hrpt_stats(const std::string &dec, long frames, int state)
         printf("deframer_state %s\n", state == 2 ? "NOSYNC" : (state == 6 ? "SYNCING" : "SYNCED"));
     if (dec == "fengyun_ahrpt_decoder") // module_fengyun_ahrpt_decoder.cpp:138-152: states 2 / 8 / 16
         printf("deframer_lock %d\ndeframer_state %s\n", state == 16, state == 2 ? "NOSYNC" : (state == 8 ? "SYNCING" : "SYNCED"));
+    if (dec == "fengyun_mpt_decoder") // module_fengyun_mpt_decoder.cpp:137-153: states 2 / 6 / 12
+        printf("deframer_lock %d\ndeframer_state %s\n", state == 12, state == 2 ? "NOSYNC" : (state == 6 ? "SYNCING" : "SYNCED"));
     if (dec == "noaa_hrpt_decoder")
         printf("frame_count %ld\n", frames / 11090);
     if (dec == "meteor_hrpt_decoder")
@@ -32,7 +34,7 @@ static void print_hrpt_stats(const std::string &dec, long frames, int state)
 int main(int argc, char **argv)
 {
     if (argc < 5) {
-        fprintf(stderr, "usage: %s <metop_ahrpt|jpss_hrd|npp_hrd|simple_bpsk|simple_qpsk|pm_bpsk|ldpc_qpsk|landsat|turbo_pm|turbo_bpsk|metop_dump|meteor_lrpt|noaa_hrpt|meteor_hrpt|noaa_gac|dmsp_rtd|meteor_mtvza|meteor_kmss_bpsk|fengyun_ahrpt|fengyun_ahrpt_d|aqua_db|aura_db|terra_db|bluewalker3_wide|bluewalker3_narrow> baseband <input> <output_hint> [--fused] [--key value ...]\n", argv[0]);
+        fprintf(stderr, "usage: %s <metop_ahrpt|jpss_hrd|npp_hrd|simple_bpsk|simple_qpsk|pm_bpsk|ldpc_qpsk|landsat|turbo_pm|turbo_bpsk|metop_dump|meteor_lrpt|noaa_hrpt|meteor_hrpt|noaa_gac|dmsp_rtd|meteor_mtvza|meteor_kmss_bpsk|fengyun_ahrpt|fengyun_ahrpt_d|fengyun_mpt|aqua_db|aura_db|terra_db|bluewalker3_wide|bluewalker3_narrow> baseband <input> <output_hint> [--fused] [--key value ...]\n", argv[0]);
         return 2;
     }
     const std::string pipe = argv[1], level = argv[2], in = argv[3], out = argv[4];
@@ -73,6 +75,12 @@ int main(int argc, char **argv)
         fp = Params{{"viterbi_outsync_after", "20"}, {"viterbi_ber_thresold", "0.26"},
                     {"invert_second_viterbi", pipe == "fengyun_ahrpt_d" ? "true" : "false"}};
         dec = "fengyun_ahrpt_decoder";
+    } else if (pipe == "fengyun_mpt") { // resources/pipelines/FengYun-3.json "FengYun-3 A/B/C MPT" (fengyun3_abc_mpt): psk_demod QPSK at
+        // 18.7 Msym/s (rrc_alpha 0.5, pll_bw 0.0063, costas_max_offset 1 MHz); the pipeline names no samplerate: it comes from the command line
+        dp = Params{{"constellation", "qpsk"}, {"symbolrate", "18700000"}, {"rrc_alpha", "0.5"}, {"pll_bw", "0.0063"},
+                    {"costas_max_offset", "1000000"}};
+        fp = Params{{"viterbi_outsync_after", "20"}, {"viterbi_ber_thresold", "0.300"}};
+        dec = "fengyun_mpt_decoder";
     } else if (pipe == "noaa_hrpt" || pipe == "meteor_hrpt") { // resources/pipelines/NOAA.json "noaa_hrpt", Meteor-M.json "meteor_hrpt":
         // pm_demod at 665 400 sym/s (pll_bw 0.01, rrc_alpha 0.6 | 0.5, clock_omega_relative_limit 0.001), 3 MS/s by default
         const bool noaa = pipe == "noaa_hrpt";

@@ -440,6 +440,20 @@ b200_fec_cfg fec_cfg_from_params(const std::string &id, const Params &p)
         c.invert_second_viterbi = p.flag("invert_second_viterbi", false);
         return c;
     }
+    if (id == "fengyun_mpt_decoder") { // module_fengyun_mpt_decoder.cpp:17-20: the two parameters are read with no default (as
+        // fengyun_ahrpt_decoder's); the module has no invert_second_viterbi. 1024-byte CADUs
+        c.kind = B200_FEC_FENGYUN_MPT;
+        c.device = (int)p.num("b200_device", 0);
+        c.constellation = B200_QPSK;
+        c.cadu_size = 8192;
+        for (const char *k : {"viterbi_outsync_after", "viterbi_ber_thresold"})
+            if (!p.has(k))
+                throw ModuleError(std::string("fengyun_mpt_decoder: ") + k +
+                                  " is required ([json.exception.type_error.302] type must be number, but is null)");
+        c.outsync_after = (int)p.num("viterbi_outsync_after");
+        c.ber_thresold = (float)p.num("viterbi_ber_thresold");
+        return c;
+    }
     if (id == "aqua_db_decoder") { // module_aqua_db_decoder.cpp:16-22: no parameters; 1024-byte CADUs (Aqua and Aura DB)
         c.kind = B200_FEC_AQUA_DB;
         c.device = (int)p.num("b200_device", 0);

@@ -136,7 +136,7 @@ class FecStage : public StageBase
     // noaa_hrpt_decoder: "frame_count" = frames_written (words) / 11090; meteor_hrpt_decoder: deframer_state (0 / 2 / 6 / 12), frame_count
     // aqua_db_decoder: deframer_state (2 / 6 / 10) above
     std::atomic<int> rs_avg{0};
-    std::atomic<int> viterbi2_lock{0};      // fengyun_ahrpt_decoder: "viterbi2_lock" / "viterbi2_ber" (viterbi_* above are viterbi1's)
+    std::atomic<int> viterbi2_lock{0};      // fengyun_ahrpt / _mpt_decoder: "viterbi2_lock" / "viterbi2_ber" (viterbi_* above are viterbi1's)
     std::atomic<float> viterbi2_ber{10.f};
     std::atomic<long> frames_written{0};
     b200_fec_cfg cfg{};

@@ -352,6 +352,11 @@ CONFIGS = {
     "fengyun_ahrpt_e": SignalCfg(name="fengyun_ahrpt_e", samplerate=76.8e6, symbolrate=38400000, constellation="qpsk", conv="3/4", rrc_alpha=0.35,
                                  pll_bw=0.008, fmt="cs16", decoder="fengyun_ahrpt", esn0_db=12.0, carrier_rad=1e-4, phase0=0.1,
                                  ber_thresold=0.26, outsync_after=20, invert_second_viterbi=True),
+    # psk_demod QPSK -> fengyun_mpt_decoder (FengYun-3.json "fengyun3_abc_mpt"): "FengYun-3 A/B/C MPT" at 18.7 Msym/s, recorded at
+    # 40 MS/s (2.14 samples per symbol)
+    "fengyun_mpt": SignalCfg(name="fengyun_mpt", samplerate=40e6, symbolrate=18700000, constellation="qpsk", conv="1/2", rrc_alpha=0.5,
+                             pll_bw=0.0063, fmt="cs16", decoder="fengyun_mpt", esn0_db=12.0, carrier_rad=1e-4, phase0=0.1,
+                             ber_thresold=0.3, outsync_after=20),
     # psk_demod BPSK -> meteor_xband_decoder (Meteor-M.json "meteor_m_mtvza_dump", "meteor_m_kmss_bpsk_db"): NRZ-M record streams at
     # 15.36 and 61.44 Msym/s, recorded at two samples per symbol
     "meteor_mtvza": SignalCfg(name="meteor_mtvza", samplerate=30.72e6, symbolrate=15360000, constellation="bpsk", conv="none", rrc_alpha=0.6,
@@ -424,6 +429,12 @@ def make_bitstream(cfg: SignalCfg, nframes, seed):
         n = min(i_bits.size, q_bits.size)
         coded = np.empty(2 * n, np.uint8)
         coded[0::2], coded[1::2] = (1 - q_bits[:n]) if cfg.invert_second_viterbi else q_bits[:n], i_bits[:n]
+        return coded, clear
+    if cfg.decoder == "fengyun_mpt":  # nframes CADUs on two r=1/2 branches, in the order of fengyun_mpt_pairs
+        i_bits, q_bits, clear = fengyun_mpt_frames(nframes, seed)
+        b0, b1 = fengyun_mpt_pairs(i_bits, q_bits)
+        coded = np.empty(2 * b0.size, np.uint8)
+        coded[0::2], coded[1::2] = b0, b1
         return coded, clear
     if cfg.decoder in ("meteor_mtvza", "meteor_kmss_bpsk"):  # nframes inner frames in records, NRZ-M
         return meteor_xband_frames(cfg.decoder == "meteor_kmss_bpsk", nframes, seed)
@@ -1047,10 +1058,10 @@ def puncture_34_fengyun(coded):
     return coded[:n].reshape(-1, 6)[:, [0, 1, 3, 4]].reshape(-1)
 
 
-def fengyun_frames(nframes, seed=0, errors=()):
-    """The FengYun-3 AHRPT transmitter: (tx soft-symbol branches (I bits, Q bits) as uint8, the CADUs fengyun_ahrpt_decoder writes
-    [n, 1024]). Randomised CADUs with RS(255,223) I=4 dual basis (`errors`: (frame, codeword, nbytes) byte errors added on air), the
-    inverse of the differential decoder, then per branch the r=1/2 k=7 (79, 109) code punctured to 3/4 as FengYun does."""
+def fengyun_diff_branches(nframes, seed=0, errors=()):
+    """What both FengYun-3 transmitters send before the convolutional code: (the I branch's bits y, the Q branch's bits x, the CADUs the
+    decoders write [n, 1024]). Randomised CADUs with RS(255,223) I=4 dual basis (`errors`: (frame, codeword, nbytes) byte errors added on
+    air), then the inverse of the differential decoder."""
     tx_bits, clear = dump_frames(nframes, seed)
     tx = np.packbits(tx_bits, axis=1)
     rng = np.random.default_rng(seed + 1)
@@ -1058,6 +1069,13 @@ def fengyun_frames(nframes, seed=0, errors=()):
         pos = 4 + cw + 4 * rng.choice(255, nb, replace=False)
         tx[fr, pos] ^= rng.integers(1, 256, nb, dtype=np.uint8)
     x, y = fengyun_diff_encode(np.unpackbits(tx, axis=1).reshape(-1))
+    return y, x, clear
+
+
+def fengyun_frames(nframes, seed=0, errors=()):
+    """The FengYun-3 AHRPT transmitter: (tx soft-symbol branches (I bits, Q bits) as uint8, the CADUs fengyun_ahrpt_decoder writes
+    [n, 1024]). fengyun_diff_branches, then per branch the r=1/2 k=7 (79, 109) code punctured to 3/4 as FengYun does."""
+    y, x, clear = fengyun_diff_branches(nframes, seed, errors)
     return puncture_34_fengyun(conv_encode(y)), puncture_34_fengyun(conv_encode(x)), clear
 
 
@@ -1070,6 +1088,43 @@ def fengyun_soft(i_bits, q_bits, amp=60.0, sigma=0.0, seed=0, invert_second=Fals
     out = np.empty(2 * n, np.float32)
     out[1::2] = (2.0 * I[:n] - 1.0) * amp
     out[0::2] = (2.0 * Q[:n] - 1.0) * amp * (-1.0 if invert_second else 1.0)
+    if sigma:
+        out += np.random.default_rng(seed).normal(0, sigma, out.size).astype(np.float32)
+    return np.clip(np.round(out), -127, 127).astype(np.int8)
+
+
+# ---- FengYun-3 MPT (fengyun_mpt_decoder) ------------------------------------------------------------------------------------------------
+def fengyun_mpt_frames(nframes, seed=0, errors=()):
+    """The FengYun-3 MPT transmitter: (the I and Q branches' code symbols as uint8, the CADUs fengyun_mpt_decoder writes [n, 1024]).
+    fengyun_diff_branches, then per branch the unpunctured r=1/2 k=7 (79, 109) code."""
+    y, x, clear = fengyun_diff_branches(nframes, seed, errors)
+    return conv_encode(y), conv_encode(x), clear
+
+
+def fengyun_mpt_pairs(i_bits, q_bits, phase90=False):
+    """The code symbols in the order fengyun_mpt_decoder reads them, as (byte 0 bits, byte 1 bits) of each soft pair. The module takes I
+    from byte 1 and the complement of byte 0 as Q, then exchanges the two symbols of every branch pair, so branch symbol k of a read
+    rides on pair k ^ 1. phase90: each branch pair (a, b) sent as (not b, a), which Viterbi1_2's PHASE_90 rotation undoes."""
+    n = min(i_bits.size, q_bits.size) & ~1
+
+    def rot(c):
+        c = np.asarray(c[:n], np.uint8)
+        if not phase90:
+            return c
+        r = np.empty_like(c)
+        r[0::2], r[1::2] = 1 - c[1::2], c[0::2]
+        return r
+    idx = np.arange(n) ^ 1
+    return 1 - rot(q_bits)[idx], rot(i_bits)[idx]
+
+
+def fengyun_mpt_soft(i_bits, q_bits, amp=60.0, sigma=0.0, seed=0, swap_branches=False, phase90=False):
+    """int8 soft pairs that fengyun_mpt_decoder reads (bit 1 -> +amp, see fengyun_mpt_pairs). swap_branches: the two branches exchanged
+    on air; phase90: see fengyun_mpt_pairs."""
+    b0, b1 = fengyun_mpt_pairs(*((q_bits, i_bits) if swap_branches else (i_bits, q_bits)), phase90=phase90)
+    out = np.empty(2 * b0.size, np.float32)
+    out[0::2] = (2.0 * b0 - 1.0) * amp
+    out[1::2] = (2.0 * b1 - 1.0) * amp
     if sigma:
         out += np.random.default_rng(seed).normal(0, sigma, out.size).astype(np.float32)
     return np.clip(np.round(out), -127, 127).astype(np.int8)
